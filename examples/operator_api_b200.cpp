@@ -1,6 +1,6 @@
 // examples/operator_api_b200.cpp -- the reference's operator-API call sequence
 // (examples/operator_api_batched_images_paf.example.cpp:58-74 and ..._pifpaf.example.cpp:48-64: engine.inference(batch),
-// then parser.process(packet[0], packet[1]) per image) against the B200 drop-in, using only the reference's
+// then parser.process(packet[0], packet[1]) per image) against the drop-in, using only the reference's
 // public headers.  Frames are synthetic (no OpenCV image I/O here); the model is an HPB2PACK file.
 //   usage: operator_api_b200 <model.pack> <width> <height> <batch> [save-as.pack|-] [iterations] [paf|pifpaf]
 #include <chrono>

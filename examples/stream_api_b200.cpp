@@ -1,8 +1,8 @@
 // examples/stream_api_b200.cpp -- the reference's STREAM API (examples/stream_api_video_paf.example.cpp:80-95:
-// hp::make_stream(engine, parser); stream.async() << input; stream.sync() >> writer) on the B200 drop-in.
+// hp::make_stream(engine, parser); stream.async() << input; stream.sync() >> writer) on the drop-in.
 // The scheduler is the reference's own: include/hyperpose/stream/stream.hpp is instantiated as it is and src/stream.cpp,
 // src/thread_pool.cpp, src/logging.cpp are compiled from the reference tree unchanged (hyperpose_b200/build.py::
-// build_stream_example); only the engine and the parser underneath are the B200 classes.  Input = in-memory frames
+// build_stream_example); only the engine and the parser underneath are the drop-in classes.  Input = in-memory frames
 // (std::vector<cv::Mat>, one of the stream's input types), output = a frame sink; the poses the stream hands to its drawing
 // stage are counted and compared with the operator-API sequence on the same frames.
 //   usage: stream_api_b200 <model.pack> <width> <height> <max_batch> <frames>

@@ -1,4 +1,4 @@
-"""In-tree build of libhyperpose_b200.so (nvcc, sm_100a only).  `python -m hyperpose_b200.build`."""
+"""In-tree build of libhyperpose_b200.so (nvcc, sm_90a only).  `python -m hyperpose_b200.build`."""
 from __future__ import annotations
 
 import os
@@ -10,7 +10,7 @@ ROOT = os.path.dirname(PKG)
 CSRC = os.path.join(PKG, "csrc")
 LIB = os.path.join(PKG, "libhyperpose_b200.so")
 
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC,-O2,-Wall", "-Xptxas", "-v"]
 # bit-exact fp32 kernels (parser): never let nvcc contract a*b+c
 EXACT_FLAGS = ["-fmad=false"]
@@ -68,7 +68,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
 def build_cpp_example(ref_root: str = "/root/reference") -> str | None:
     """Compiles the C++ drop-in (hyperpose_api/*.cpp) + examples/operator_api_b200.cpp against the reference's
     UNCHANGED public headers.  Needs the reference tree (headers are not copied into this repo); returns the
-    binary path, or None when the reference is absent (GPU box: the prebuilt binary travels with the snapshot)."""
+    binary path, or the prebuilt one / None when the reference is absent."""
     exe = os.path.join(ROOT, "examples", "operator_api_b200")
     if not os.path.isdir(os.path.join(ref_root, "include", "hyperpose")):
         return exe if os.path.exists(exe) else None
@@ -117,9 +117,9 @@ REFERENCE_EXAMPLES = ["operator_api_batched_images_paf.example", "operator_api_b
 def build_reference_examples(ref_root: str = "/root/reference") -> dict | None:
     """The reference's OWN example programs, compiled UNMODIFIED from <ref>/examples/*.cpp (+ examples/utils.cpp) against the drop-in:
     the reference's unchanged headers, its unchanged src/{stream,thread_pool,logging,human,data}.cpp (scheduler, drawing, batching
-    helpers), the B200 classes of hyperpose_api/*.cpp underneath, and the OpenCV / gflags stand-ins of csrc/shim (neither library
+    helpers), the drop-in classes of hyperpose_api/*.cpp underneath, and the OpenCV / gflags stand-ins of csrc/shim (neither library
     exists in this image).  Nothing of the reference is copied: every source is compiled where it lies.  Returns {name: binary} in
-    examples/ref_build/ (git-ignored, travels to the GPU box), or the prebuilt set / None where the reference tree is absent."""
+    examples/ref_build/ (git-ignored), or the prebuilt set / None where the reference tree is absent."""
     out_dir = os.path.join(ROOT, "examples", "ref_build")
     exes = {n: os.path.join(out_dir, n.replace(".example", "")) for n in REFERENCE_EXAMPLES}
     if not os.path.isdir(os.path.join(ref_root, "include", "hyperpose")):

@@ -16,7 +16,7 @@ const char* get_error() { return g_err; }
 
 extern "C" {
 const char* hp_last_error(void) { return hpb::get_error(); }
-const char* hp_version(void) { return "hyperpose_b200 0.1 (sm_100a)"; }
+const char* hp_version(void) { return "hyperpose_b200 0.1 (sm_90a)"; }
 int hp_device_count(void)
 {
     int n = 0;

@@ -1,276 +1,18 @@
-// conv_tf32.cuh -- the data_type::kFLOAT arithmetic of the reference engine API (include/hyperpose/operator/dnn/tensorrt.hpp:14-22,
-// 48,61) on the sm_100a tensor cores: fp32 activations in HBM, tcgen05.mma.kind::tf32, fp32 accumulation in TMEM.
+// conv_tf32.cuh -- the fp32 helper kernels of the data_type::kFLOAT engine (include/hyperpose/operator/dnn/tensorrt.hpp:14-22,
+// 48,61).  Its convolutions are conv_wgmma_kernel<float, ...> (conv_wgmma.cuh): fp32 activations in HBM, wgmma kind tf32, fp32
+// accumulation.
 //
 // TensorRT runs an "FP32" network on tensor-core GPUs exactly like this (TF32 is its default FP32 convolution math since
 // Ampere): tensors stay fp32 everywhere, the multiplier reads the 8-bit exponent and the top 10 mantissa bits of each operand.
 // The tensor core TRUNCATES the low 13 mantissa bits of what it reads; left alone that is a systematic toward-zero bias that
-// compounds over ~40 layers (measured: 7e-3 of max|activation| at a mid VGG layer against 2e-3 for the f16 engine).  So every
-// producer of a conv operand rounds to the TF32 grid with round-to-nearest (cvt.rna.tf32.f32) before it stores -- the weights
-// when the plan is built, the activations in the epilogue / helper kernel that writes them -- and the truncation on read is
-// then exact.  Bias, PReLU, residual adds, pools and the depthwise convs compute in full fp32; the network outputs handed to
-// the parser are NOT rounded.
-//
-// Same pipeline as conv_tcgen05_kernel (conv_tcgen05.cuh) with the element size doubled:
-//   D[128 pixels, BN out-channels] += A[128 pixels, 32 in-channels] * B[BN, 32]^T   per k-step (filter tap x 32-channel chunk)
-//   * A tile: ONE im2col-mode TMA load of 128 consecutive output pixels x 32 fp32 channels (128 B rows, 128B swizzle, 16 KiB);
-//   * B tile: 2-D TMA box {32, BN} of the fp32 K-major weight matrix;
-//   * four tcgen05.mma.kind::tf32 (M = 128, N = BN, K = 8) per k-step issued by one elected thread;
-//   * persistent CTAs, 4-8 stage mbarrier ring, double-buffered TMEM accumulators;
-//   * epilogue: tcgen05.ld -> bias (+ residual) + PReLU -> fp32 -> 128B-swizzled staging tile of 128 pixels x 32 channels ->
-//     TMA tensor store; the last layer writes the parser's fp32 NCHW planes directly.
+// compounds over ~40 layers.  So every producer of a conv operand rounds to the TF32 grid with round-to-nearest
+// (cvt.rna.tf32.f32) before it stores -- the weights when the plan is built, the activations in the epilogue / helper kernel
+// that writes them -- and the truncation on read is then exact.  Bias, PReLU, residual adds, pools and the depthwise convs
+// compute in full fp32; the network outputs handed to the parser are NOT rounded.
 #pragma once
-#include "conv_tcgen05.cuh"
+#include "conv_wgmma.cuh"
 
 namespace hpb {
-
-constexpr int TF32_BLOCK_K = 32;   // fp32 channels per k-step == one 128-byte swizzle row
-constexpr int TF32_UMMA_K = 8;     // K of one tcgen05.mma.kind::tf32
-
-namespace ptx {
-// instruction descriptor for kind::tf32: c_format = 1 (F32) | a_format = b_format = 2 (TF32), both K-major
-__host__ __device__ inline uint32_t make_idesc_tf32(int M, int N)
-{
-    return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-// round-to-nearest onto the TF32 grid (the value stays an fp32 bit pattern with 13 zero low mantissa bits)
-__device__ __forceinline__ float round_tf32(float x)
-{
-    uint32_t r;
-    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
-    return __uint_as_float(r);
-}
-__device__ __forceinline__ void umma_tf32(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate)
-{
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-} // namespace ptx
-
-// ConvParams is shared with the f16 kernels; here cin_g is a multiple of 32, `res` points to fp32, out_ld / offsets count fp32 elements,
-// tma_store needs BN % 32 == 0.
-template <bool kRes>
-__global__ void __launch_bounds__(CONV_THREADS, 1)
-conv_tf32_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
-                 const __grid_constant__ CUtensorMap tmap_o, const __grid_constant__ CUtensorMap tmap_r, const ConvParams p)
-{
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-    const int b_bytes = p.BN * 128;
-    const int stage_bytes = CONV_A_BYTES + b_bytes;
-    uint8_t* bar_base = smem + (size_t)p.num_stages * stage_bytes;
-    uint64_t* full_bar = (uint64_t*)bar_base;
-    uint64_t* empty_bar = full_bar + CONV_MAX_STAGES;
-    uint64_t* tfull_bar = empty_bar + CONV_MAX_STAGES;
-    uint64_t* tempty_bar = tfull_bar + 2;
-    uint64_t* res_bar = tempty_bar + 2;
-    uint32_t* tmem_slot = (uint32_t*)(res_bar + 2);
-    uint8_t* out_stage = (uint8_t*)(((uintptr_t)(tmem_slot + 4) + 1023) & ~(uintptr_t)1023);   // 2 x 16 KiB (128 px x 32 ch fp32)
-    uint8_t* res_stage = out_stage + 2 * CONV_A_BYTES;
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int n_tiles_g = p.cout_g_pad / p.BN;
-    const int total_tiles = p.m_tiles * p.groups * n_tiles_g;
-    const int chunks = p.cin_g / TF32_BLOCK_K;
-    const int ksteps = p.R * p.S * chunks;
-
-    if (warp == 0 && lane == 0) {
-        ptx::prefetch_tmap(&tmap_a);
-        ptx::prefetch_tmap(&tmap_b);
-        if (p.tma_store) ptx::prefetch_tmap(&tmap_o);
-    }
-    if (warp == 1 && lane == 0) {
-        for (int i = 0; i < p.num_stages; ++i) {
-            ptx::mbar_init(ptx::smem_u32(full_bar + i), 1);
-            ptx::mbar_init(ptx::smem_u32(empty_bar + i), 1);
-        }
-        for (int i = 0; i < 2; ++i) {
-            ptx::mbar_init(ptx::smem_u32(tfull_bar + i), 1);
-            ptx::mbar_init(ptx::smem_u32(tempty_bar + i), 4);
-            ptx::mbar_init(ptx::smem_u32(res_bar + i), 1);
-        }
-        ptx::fence_barrier_init();
-    }
-    if (warp == 2) ptx::tmem_alloc(ptx::smem_u32(tmem_slot), (uint32_t)p.tmem_cols);
-    ptx::tc_fence_before();
-    __syncthreads();
-    ptx::tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-
-    if (warp == 0) {
-        if (ptx::elect_one()) {
-            int stage = 0;
-            uint32_t phase = 0;
-            const int pad_h = p.R / 2, pad_w = p.S / 2;
-            for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-                const ConvTile t = decode_tile(p, tile, n_tiles_g);
-                const PixelPos q0 = unflatten(p, t.p0);
-                const int a_ch0 = p.in_ch_off + t.g * p.cin_g;
-                const int b_row = t.g * p.cout_g_pad + t.n0;
-                int kcol = 0;
-                for (int r = 0; r < p.R; ++r)
-                    for (int s = 0; s < p.S; ++s)
-                        for (int c = 0; c < chunks; ++c, kcol += TF32_BLOCK_K) {
-                            ptx::mbar_wait(ptx::smem_u32(empty_bar + stage), phase ^ 1);
-                            const uint32_t fb = ptx::smem_u32(full_bar + stage);
-                            uint8_t* sa = smem + (size_t)stage * stage_bytes;
-                            ptx::mbar_expect_tx(fb, (uint32_t)stage_bytes);
-                            ptx::tma_load_im2col_4d(ptx::smem_u32(sa), &tmap_a, fb, a_ch0 + c * TF32_BLOCK_K, q0.w - pad_w, q0.h - pad_h, q0.n, s, r);
-                            ptx::tma_load_2d(ptx::smem_u32(sa + CONV_A_BYTES), &tmap_b, fb, kcol, b_row);
-                            if (++stage == p.num_stages) { stage = 0; phase ^= 1; }
-                        }
-            }
-        }
-    } else if (warp == 1) {
-        if (ptx::elect_one()) {
-            const uint32_t idesc = ptx::make_idesc_tf32(CONV_BLOCK_M, p.BN);
-            int stage = 0;
-            uint32_t phase = 0;
-            int acc = 0;
-            uint32_t acc_phase = 0;
-            for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-                ptx::mbar_wait(ptx::smem_u32(tempty_bar + acc), acc_phase ^ 1);
-                ptx::tc_fence_after();
-                const uint32_t d_tmem = tmem_base + (uint32_t)(acc * p.BN);
-                for (int ks = 0; ks < ksteps; ++ks) {
-                    ptx::mbar_wait(ptx::smem_u32(full_bar + stage), phase);
-                    ptx::tc_fence_after();
-                    const uint32_t sa = ptx::smem_u32(smem + (size_t)stage * stage_bytes);
-                    const uint64_t da = ptx::make_sw128_kmajor_desc(sa);
-                    const uint64_t db = ptx::make_sw128_kmajor_desc(sa + CONV_A_BYTES);
-#pragma unroll
-                    for (int k = 0; k < TF32_BLOCK_K / TF32_UMMA_K; ++k) // K advances by 8 fp32 = 32 bytes: +2 in the (>>4) address field
-                        ptx::umma_tf32(d_tmem, da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), idesc, (ks | k) != 0 ? 1u : 0u);
-                    ptx::umma_commit(ptx::smem_u32(empty_bar + stage));
-                    if (++stage == p.num_stages) { stage = 0; phase ^= 1; }
-                }
-                ptx::umma_commit(ptx::smem_u32(tfull_bar + acc));
-                if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-            }
-        }
-    } else if (warp >= 4) {
-        const int ew = warp - 4;
-        const int row = ew * 32 + lane;
-        const int total_px = p.Nb * p.H * p.W;
-        int acc = 0;
-        uint32_t acc_phase = 0;
-        uint32_t stage_ctr = 0;
-        const bool res_tma = kRes && p.res_mode != 0 && p.tma_store != 0;
-        const int subs = p.BN / 32;
-        uint32_t res_issued = 0, res_used = 0;
-        int ri_tile = blockIdx.x, ri_sub = 0;
-        auto issue_residual = [&]() { // leader only
-            if (ri_tile >= total_tiles) return;
-            const ConvTile rt = decode_tile(p, ri_tile, n_tiles_g);
-            const uint32_t rb = ptx::smem_u32(res_bar + (res_issued & 1));
-            ptx::mbar_expect_tx(rb, (uint32_t)CONV_A_BYTES);
-            ptx::tma_load_2d(ptx::smem_u32(res_stage + (res_issued & 1) * CONV_A_BYTES), &tmap_r, rb,
-                             p.res_ch_off + rt.g * p.cout_g + rt.n0 + ri_sub * 32, rt.p0);
-            ++res_issued;
-            if (++ri_sub == subs) { ri_sub = 0; ri_tile += gridDim.x; }
-        };
-        if (kRes && res_tma && warp == 4 && lane == 0) { issue_residual(); issue_residual(); }
-        const float* resf = reinterpret_cast<const float*>(p.res);
-        for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-            const ConvTile t = decode_tile(p, tile, n_tiles_g);
-            const bool in_img = (t.p0 + row) < total_px;
-            const PixelPos q = unflatten(p, in_img ? t.p0 + row : 0);
-            ptx::mbar_wait(ptx::smem_u32(tfull_bar + acc), acc_phase);
-            ptx::tc_fence_after();
-            const uint32_t taddr = tmem_base + ((uint32_t)(ew * 32) << 16) + (uint32_t)(acc * p.BN);
-            const float* bias = p.bias + t.g * p.cout_g_pad + t.n0;
-            const float* alpha = p.alpha + t.g * p.cout_g_pad + t.n0;
-            const int n_valid = min(p.BN, p.cout_g - t.n0);
-            const size_t pix = (size_t)(t.p0 + row);
-            if (p.tma_store) {
-                const bool leader = (warp == 4 && lane == 0);
-                for (int sub = 0; sub < subs; ++sub, ++stage_ctr) {
-                    uint8_t* sbuf = out_stage + (stage_ctr & 1) * CONV_A_BYTES;
-                    if (leader) ptx::bulk_wait_group_read<1>();
-                    ptx::named_bar_sync(1, 128);
-                    const uint32_t srow = ptx::smem_u32(sbuf) + (uint32_t)row * 128u;
-                    const uint8_t* rrow = res_stage + (res_used & 1) * CONV_A_BYTES + row * 128;
-                    if (kRes && res_tma) ptx::mbar_wait(ptx::smem_u32(res_bar + (res_used & 1)), (res_used >> 1) & 1);
-#pragma unroll
-                    for (int h = 0; h < 2; ++h) {   // 16 channels at a time: four 16-byte chunks of the 128-byte row
-                        const int c0 = sub * 32 + h * 16;
-                        uint32_t v[16];
-                        ptx::tmem_ld_32x32b_x16(taddr + (uint32_t)c0, v);
-                        ptx::tmem_ld_wait();
-#pragma unroll
-                        for (int j4 = 0; j4 < 4; ++j4) {
-                            const float4 bv = __ldg((const float4*)(bias + c0) + j4);
-                            const float4 av = __ldg((const float4*)(alpha + c0) + j4);
-                            const int chunk = h * 4 + j4;
-                            float4 rv = make_float4(0.f, 0.f, 0.f, 0.f);
-                            if (kRes && res_tma) rv = *(const float4*)(rrow + ((chunk ^ (row & 7)) * 16));
-                            else if (kRes && p.res_mode && in_img) rv = __ldg((const float4*)(resf + pix * p.res_ld + p.res_ch_off + t.g * p.cout_g + t.n0 + c0) + j4);
-                            float a0 = __uint_as_float(v[4 * j4]) + bv.x, a1 = __uint_as_float(v[4 * j4 + 1]) + bv.y;
-                            float a2 = __uint_as_float(v[4 * j4 + 2]) + bv.z, a3 = __uint_as_float(v[4 * j4 + 3]) + bv.w;
-                            if (kRes && p.res_mode == 1) { a0 += rv.x; a1 += rv.y; a2 += rv.z; a3 += rv.w; }
-                            a0 = a0 > 0.f ? a0 : a0 * av.x; a1 = a1 > 0.f ? a1 : a1 * av.y;
-                            a2 = a2 > 0.f ? a2 : a2 * av.z; a3 = a3 > 0.f ? a3 : a3 * av.w;
-                            if (kRes && p.res_mode == 2) { a0 += rv.x; a1 += rv.y; a2 += rv.z; a3 += rv.w; }
-                            a0 = ptx::round_tf32(a0); a1 = ptx::round_tf32(a1); a2 = ptx::round_tf32(a2); a3 = ptx::round_tf32(a3);
-                            ptx::st_shared_v4(srow + (uint32_t)((chunk ^ (row & 7)) * 16),
-                                              make_uint4(__float_as_uint(a0), __float_as_uint(a1), __float_as_uint(a2), __float_as_uint(a3)));
-                        }
-                    }
-                    ptx::fence_proxy_async();
-                    ptx::named_bar_sync(1, 128);
-                    if (leader) {
-                        ptx::tma_store_2d(&tmap_o, ptx::smem_u32(sbuf), p.out_ch_off + t.g * p.cout_g + t.n0 + sub * 32, t.p0);
-                        ptx::bulk_commit_group();
-                        if (kRes && res_tma) issue_residual();
-                    }
-                    ++res_used;
-                }
-            } else
-            for (int c0 = 0; c0 < p.BN; c0 += 16) {
-                if (c0 >= n_valid) break;
-                uint32_t v[16];
-                ptx::tmem_ld_32x32b_x16(taddr + (uint32_t)c0, v);
-                ptx::tmem_ld_wait();
-                if (!in_img) continue;
-                const int nv = min(16, n_valid - c0);
-                for (int j = 0; j < nv; ++j) {
-                    float a = __uint_as_float(v[j]) + __ldg(bias + c0 + j);
-                    float r = 0.f;
-                    if (kRes && p.res_mode) r = resf[pix * p.res_ld + p.res_ch_off + t.g * p.cout_g + t.n0 + c0 + j];
-                    if (kRes && p.res_mode == 1) a += r;
-                    a = a > 0.f ? a : a * __ldg(alpha + c0 + j);
-                    if (kRes && p.res_mode == 2) a += r;
-                    const int ch = t.n0 + c0 + j;
-                    if (p.out_mode == OUT_F16_NHWC) {   // "NHWC activation buffer": fp32 elements on this path
-                        ((float*)p.out)[pix * p.out_ld + p.out_ch_off + t.g * p.cout_g + ch] = ptx::round_tf32(a);
-                    } else if (ch < p.split) {
-                        ((float*)p.out)[(((size_t)q.n * p.split + ch) * p.H + q.h) * p.W + q.w] = a;
-                    } else {
-                        const int c2 = ch - p.split, n2 = p.cout_g - p.split;
-                        ((float*)p.out2)[(((size_t)q.n * n2 + c2) * p.H + q.h) * p.W + q.w] = a;
-                    }
-                }
-            }
-            ptx::tc_fence_before();
-            __syncwarp();
-            if (lane == 0) ptx::mbar_arrive(ptx::smem_u32(tempty_bar + acc));
-            if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-        }
-        if (p.tma_store && warp == 4 && lane == 0) ptx::bulk_wait_group_read<0>();
-    }
-
-    ptx::tc_fence_before();
-    __syncthreads();
-    if (warp == 2) {
-        ptx::tc_fence_after();
-        ptx::tmem_dealloc(tmem_base, (uint32_t)p.tmem_cols);
-    }
-}
-
-// smem of a stage: 16 KiB of pixels + BN x 128 B of weights -- the same byte counts as the f16 kernel (conv_smem_bytes / conv_pick_stages)
 
 // ---- fp32 helper kernels of the tf32 engine (HBM-bound, off the critical path of the headline f16 configuration) -------------
 

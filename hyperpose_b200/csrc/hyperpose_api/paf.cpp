@@ -1,4 +1,4 @@
-// hyperpose_api/paf.cpp -- hyperpose::parser::paf implemented on the B200 C ABI.
+// hyperpose_api/paf.cpp -- hyperpose::parser::paf implemented on the hyperpose_b200 C ABI.
 //
 // Drop-in replacement for the reference's src/paf.cpp (the same seam src/fake/fake_paf.cpp uses,
 // cmake/hyperpose.fake.cmake:6-19): compiled against the reference's UNCHANGED

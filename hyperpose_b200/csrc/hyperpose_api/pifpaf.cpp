@@ -1,4 +1,4 @@
-// hyperpose_api/pifpaf.cpp -- hyperpose::parser::pifpaf::process implemented on the B200 C ABI.
+// hyperpose_api/pifpaf.cpp -- hyperpose::parser::pifpaf::process implemented on the hyperpose_b200 C ABI.
 // Drop-in replacement for the reference's src/pifpaf.cpp (+ src/pifpaf_decoder/*), compiled against the UNCHANGED
 // include/hyperpose/operator/parser/pifpaf.hpp.  The argument-order quirk is kept: the definition takes (paf, pif)
 // (src/pifpaf.cpp:6-7, "TODO: Name ORDER!") because the engine returns its outputs sorted by name.

@@ -1,4 +1,4 @@
-// hyperpose_api/pose_proposal.cpp -- hyperpose::parser::pose_proposal implemented on the B200 C ABI.
+// hyperpose_api/pose_proposal.cpp -- hyperpose::parser::pose_proposal implemented on the hyperpose_b200 C ABI.
 // Drop-in replacement for the reference's src/pose_proposal.cpp, compiled against the UNCHANGED
 // include/hyperpose/operator/parser/proposal_network.hpp.  The class holds only its parameters (no pimpl slot), so the
 // device handle lives per thread, like the reference's stateless process() allows (one parser copy per pool thread,

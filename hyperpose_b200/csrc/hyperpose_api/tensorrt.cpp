@@ -1,4 +1,4 @@
-// hyperpose_api/tensorrt.cpp -- hyperpose::dnn::tensorrt implemented on the B200 C ABI (no TensorRT).
+// hyperpose_api/tensorrt.cpp -- hyperpose::dnn::tensorrt implemented on the hyperpose_b200 C ABI (no TensorRT).
 //
 // Drop-in replacement for the reference's src/tensorrt.cpp (same seam as src/fake/fake_tensorrt.cpp),
 // compiled against the UNCHANGED include/hyperpose/operator/dnn/tensorrt.hpp.  All three constructors
@@ -28,8 +28,8 @@ namespace dnn {
             std::cerr << "[HyperPose::ERROR  ] " << what << ": " << hp_last_error() << '\n';
             std::exit(1);
         }
-        // data_type of the reference ctor (tensorrt.hpp:14-22,48,61): kFLOAT (the default every example uses) selects the tcgen05
-        // kind::tf32 engine (fp32 tensors, TF32 multiplies -- TensorRT's own FP32 convolution math on tensor-core GPUs), kHALF the
+        // data_type of the reference ctor (tensorrt.hpp:14-22,48,61): kFLOAT (the default every example uses) selects the wgmma
+        // kind tf32 engine (fp32 tensors, TF32 multiplies -- TensorRT's own FP32 convolution math on tensor-core GPUs), kHALF the
         // f16 engine.  A serialized engine carries no precision argument in the reference API (its plan was built with one): the pack
         // runs as kHALF unless HPB_DTYPE=tf32 says otherwise.
         int dtype_of(const data_type& t) { return t.val == data_type::kHALF ? HP_DTYPE_F16 : HP_DTYPE_TF32; }
@@ -143,7 +143,7 @@ namespace dnn {
         for (size_t i = 0; i < batch.size(); ++i) {
             const cv::Mat& m = batch[i];
             if (m.type() != CV_8UC3 || !m.isContinuous() || m.empty()) {
-                std::cerr << "[HyperPose::ERROR  ] B200 engine: frames must be continuous CV_8UC3\n";
+                std::cerr << "[HyperPose::ERROR  ] engine: frames must be continuous CV_8UC3\n";
                 std::exit(-1);
             }
             if (hp_engine_stage_frame_u8(m_cuda_dep->engine, (int)i, m.data, m.rows, m.cols, m_keep_ratio ? 1 : 0) != HP_OK) die("hp_engine_stage_frame_u8");
@@ -171,7 +171,7 @@ namespace dnn {
 
 // member-wise constructor + printer of feature_map_t (include/hyperpose/utility/data.hpp:22,28): in a full
 // integration these come from the reference's own src/data.cpp; they are repeated here only so that this
-// translation unit links stand-alone (tests, the B200 example) without OpenCV.
+// translation unit links stand-alone (tests, the drop-in example) without OpenCV.
 #ifdef HP_B200_STANDALONE
 feature_map_t::feature_map_t(std::string name, std::unique_ptr<char[]>&& tensor, std::vector<int> shape)
     : m_name(std::move(name)), m_data(std::move(tensor)), m_shape(std::move(shape))

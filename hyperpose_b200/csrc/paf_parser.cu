@@ -1,4 +1,4 @@
-// paf_parser.cu -- B200 (sm_100a) PAF post-processing: conf/PAF tensors -> human_t records.
+// paf_parser.cu -- H100 (sm_90a) PAF post-processing: conf/PAF tensors -> human_t records.
 //
 // Replaces the reference's CPU parser hyperpose::parser::paf
 //   src/paf.cpp:57-375, src/post_process.hpp:26-205, src/coco.hpp:6-52
@@ -35,6 +35,7 @@
 #include "../../include/hyperpose_b200.h"
 #include "common.h"
 #include "handoff.h"
+#include "pair_math.cuh"
 
 namespace {
 
@@ -77,13 +78,12 @@ __host__ __device__ inline int refl101(int p, int len)
 // ---------------------------------------------------------------------------------------------
 // K1: fused up-sample + Gaussian + NMS + peak emission
 // ---------------------------------------------------------------------------------------------
-// The kernel is ISSUE-bound (ncu, round 1: ~9.3k warp instructions per tile, 9504 tiles per 16-frame batch = 99 us), so this
+// The kernel is ISSUE-bound (~9.3k warp instructions per tile, 9504 tiles per 16-frame batch), so this
 // version is organised around instruction count: the horizontal lerp of the up-sampling is computed once per SOURCE row (the
 // default resolution stretches rows 7x: ~9 source rows feed 48 tile rows), both filter passes produce 16 outputs per thread
 // from one 32-value register window (1 shared load per 8.5 FMAs), every pass is exactly one round of the 192-thread CTA, and
 // the source bounds of a tile come from host tables instead of shared-memory atomics.
-// Both filter passes run on the packed fp32 pipe of sm_100 (FFMA2 / FADD2 / FMUL2 via __ffma2_rn & co: two IEEE fp32 operations
-// per instruction, each lane rounded exactly like the scalar instruction): the row pass pairs two ROWS (the up-sampled tile is
+// Both filter passes work on float2 pairs (pair_math.cuh: each lane rounded exactly like the scalar instruction): the row pass pairs two ROWS (the up-sampled tile is
 // stored as float2 {row 2r, row 2r+1}), the column pass pairs two COLUMNS (the row-pass output is row-major with an even stride).
 constexpr int K1_THREADS = 192;
 constexpr int TH = 30, TW = 62;          // interior tile of the up-map handled by one CTA
@@ -286,22 +286,22 @@ __global__ void __launch_bounds__(K1_THREADS) paf_peaks_kernel(const PeakParams 
         if (jlast < p.n4) {
             const float2 g0 = make_float2(c_g17[0], c_g17[0]);
 #pragma unroll
-            for (int o = 0; o < RUN; ++o) acc[o] = __fmul2_rn(g0, w[o]);
+            for (int o = 0; o < RUN; ++o) acc[o] = fmul2_rn(g0, w[o]);
 #pragma unroll
             for (int t = 1; t < 17; ++t) {
                 const float2 g = make_float2(c_g17[t], c_g17[t]);
 #pragma unroll
-                for (int o = 0; o < RUN; ++o) acc[o] = __ffma2_rn(g, w[o + t], acc[o]);
+                for (int o = 0; o < RUN; ++o) acc[o] = ffma2_rn(g, w[o + t], acc[o]);
             }
         } else {
 #pragma unroll
             for (int o = 0; o < RUN; ++o) {
                 const bool fma = (x0 - 1 + c0 + o) < p.n4;
-                float2 s2 = __fmul2_rn(make_float2(c_g17[0], c_g17[0]), w[o]);
+                float2 s2 = fmul2_rn(make_float2(c_g17[0], c_g17[0]), w[o]);
 #pragma unroll
                 for (int t = 1; t < 17; ++t) {
                     const float2 g = make_float2(c_g17[t], c_g17[t]);
-                    s2 = fma ? __ffma2_rn(g, w[o + t], s2) : __fadd2_rn(s2, __fmul2_rn(g, w[o + t]));
+                    s2 = fma ? ffma2_rn(g, w[o + t], s2) : fadd2_rn(s2, fmul2_rn(g, w[o + t]));
                 }
                 acc[o] = s2;
             }
@@ -331,32 +331,32 @@ __global__ void __launch_bounds__(K1_THREADS) paf_peaks_kernel(const PeakParams 
         const int jlo = x0 - 1, jhi = x0 - 1 + RT_W - 1;
         if (jhi < p.n8) {
 #pragma unroll
-            for (int o = 0; o < RUN; ++o) res[o] = __fmul2_rn(g8, w[o + 8]);
+            for (int o = 0; o < RUN; ++o) res[o] = fmul2_rn(g8, w[o + 8]);
 #pragma unroll
             for (int t = 1; t <= 8; ++t) {
                 const float2 g = make_float2(c_g17[8 + t], c_g17[8 + t]);
 #pragma unroll
-                for (int o = 0; o < RUN; ++o) res[o] = __ffma2_rn(g, __fadd2_rn(w[o + 8 + t], w[o + 8 - t]), res[o]);
+                for (int o = 0; o < RUN; ++o) res[o] = ffma2_rn(g, fadd2_rn(w[o + 8 + t], w[o + 8 - t]), res[o]);
             }
         } else if (jlo >= p.n8) {
 #pragma unroll
-            for (int o = 0; o < RUN; ++o) res[o] = __fmul2_rn(g8, w[o + 8]);
+            for (int o = 0; o < RUN; ++o) res[o] = fmul2_rn(g8, w[o + 8]);
 #pragma unroll
             for (int t = 1; t <= 8; ++t) {
                 const float2 g = make_float2(c_g17[8 + t], c_g17[8 + t]);
 #pragma unroll
-                for (int o = 0; o < RUN; ++o) res[o] = __fadd2_rn(res[o], __fmul2_rn(g, __fadd2_rn(w[o + 8 + t], w[o + 8 - t])));
+                for (int o = 0; o < RUN; ++o) res[o] = fadd2_rn(res[o], fmul2_rn(g, fadd2_rn(w[o + 8 + t], w[o + 8 - t])));
             }
         } else {   // the class boundary runs through this tile: both chains, each lane keeps its own
 #pragma unroll
             for (int o = 0; o < RUN; ++o) {
-                float2 sf = __fmul2_rn(g8, w[o + 8]), sn = sf;
+                float2 sf = fmul2_rn(g8, w[o + 8]), sn = sf;
 #pragma unroll
                 for (int t = 1; t <= 8; ++t) {
-                    const float2 a = __fadd2_rn(w[o + 8 + t], w[o + 8 - t]);
+                    const float2 a = fadd2_rn(w[o + 8 + t], w[o + 8 - t]);
                     const float2 g = make_float2(c_g17[8 + t], c_g17[8 + t]);
-                    sf = __ffma2_rn(g, a, sf);
-                    sn = __fadd2_rn(sn, __fmul2_rn(g, a));
+                    sf = ffma2_rn(g, a, sf);
+                    sn = fadd2_rn(sn, fmul2_rn(g, a));
                 }
                 res[o] = make_float2(fma0 ? sf.x : sn.x, fma1 ? sf.y : sn.y);
             }

@@ -1,4 +1,4 @@
-// pifpaf_decoder.cu -- B200 (sm_100a) OpenPifPaf decode: PIF / PAF fields -> human_t records.
+// pifpaf_decoder.cu -- H100 (sm_90a) OpenPifPaf decode: PIF / PAF fields -> human_t records.
 //
 // Replaces the reference's CPU decoder hyperpose::parser::pifpaf::process
 //   src/pifpaf.cpp:7-95  +  src/pifpaf_decoder/openpifpaf_postprocessor.cpp:142-926 (SURVEY 8a A12)

@@ -1,5 +1,5 @@
 /*
- * hyperpose_b200.h -- C ABI of the B200-native HyperPose inference path.
+ * hyperpose_b200.h -- C ABI of the H100-native HyperPose inference path.
  *
  * This is the drop-in boundary: the reference has no FFI, its seam is link-time
  * substitution of src/tensorrt.cpp + src/paf.cpp (CMakeLists.txt:28-34,
@@ -163,7 +163,7 @@ int hp_engine_create(hp_engine** out, const void* pack, size_t pack_bytes, int i
                      double factor, int flip_rgb, int device);
 /* The same with the arithmetic the reference's `data_type` ctor argument selects (tensorrt.hpp:14-22,48,61):
  *   HP_DTYPE_F16  (= data_type::kHALF):  fp16 operands and activations, fp32 accumulation -- what hp_engine_create builds;
- *   HP_DTYPE_TF32 (= data_type::kFLOAT, the reference default): fp32 activations in HBM, tcgen05.mma.kind::tf32 (fp32 operands
+ *   HP_DTYPE_TF32 (= data_type::kFLOAT, the reference default): fp32 activations in HBM, wgmma kind tf32 (fp32 operands
  *                 read with a 10-bit mantissa by the tensor core, fp32 accumulation) -- TensorRT's own FP32 mode on tensor-core GPUs. */
 #define HP_DTYPE_F16 0
 #define HP_DTYPE_TF32 1
@@ -242,7 +242,7 @@ int hp_pose_collect(hp_engine* e, int ticket, hp_human* out, int cap, int* n_out
 int hp_pose_stats(const hp_engine* e, long long* graph_captures, long long* graph_launches);
 /* The pipelined call for OpenPifPaf packs: engine.inference(batch) + pifpaf.process(packet[0], packet[1]) per image
  * (examples/operator_api_batched_images_pifpaf.example.cpp:48-64), two batches in flight.  The decoder's greedy growth is a
- * latency chain on one warp per frame (2 ms per batch of 16 while 16 of 148 SMs do anything at all), so it runs on the DECODER's
+ * latency chain on one warp per frame (milliseconds per batch of 16 while 16 of 132 SMs do anything at all), so it runs on the DECODER's
  * stream underneath the convolutions of the next batch: the engine's persistent kernels leave `reserve` SMs to it (default
  * min(max_batch, 16); env HPB_PIFPAF_RESERVE_SMS), and the next batch's head kernels wait only until the field tensors have
  * been consumed (decoder kernels P1-P3), not for the growth.  Tickets / hp_pose_collect as above. */

@@ -149,7 +149,23 @@ def main():
         pp[name + "_humans"] = oracle.ref_pifpaf_process(pif, paf, (h - 1) * 8 + 1, (w - 1) * 8 + 1, thr)
         pp[name + "_in_sha"] = np.array(sha(pif) + sha(paf))
     np.savez_compressed(os.path.join(HERE, "ref_pifpaf.npz"), **pp)
+    make_pifpaf_live()
     make_ppn()
+
+
+def make_pifpaf_live():
+    """the reference decoder on the inputs of test_gpu_decoder_batched_vs_live_reference (batched_i) and test_pifpaf_fields_hand_off
+    (handoff_i): those tests compare with these records where oracle/_ref is not built, and check them against it where it is"""
+    from hyperpose_b200 import synthetic as syn
+    import oracle
+    out = {}
+    for i in range(8):
+        pif, paf = syn.make_pifpaf_fields(100 + i, (1, 9), 49, 49)
+        out[f"batched_{i}"] = oracle.ref_pifpaf_process(pif, paf, 385, 385, 0.1)
+    for i in range(2):
+        pif, paf = syn.make_pifpaf_fields(20 + i, (2, 3), 49, 49)
+        out[f"handoff_{i}"] = oracle.ref_pifpaf_process(pif.astype(np.float32), paf.astype(np.float32), 385, 385, 0.1)
+    np.savez_compressed(os.path.join(HERE, "ref_pifpaf_live.npz"), **out)
 
 
 def make_ppn():

@@ -9,8 +9,7 @@ Every network of the BASELINE configs runs at its full input size through the en
         recorded in DESIGN.md section 4)
 
 Large-image behaviours this covers that the small-resolution tests cannot: im2col tiles wrapping over rows and images at
-W = 656, the NPX = 208 swapped-operand units at 46x82x16, the 16x8 halo grid at 368x656 / 184x328, the 3.19-wave merged
-7x7 layers, the u8 stem at 656 columns.
+W = 656, the 16x8 halo grid at 368x656, the many-wave 7x7 layers, the u8 stem at 656 columns.
 
 Pose-level check (what fp16 does to the OUTPUT of the path): the same frames through fp32 torch -> CPU oracle parser and
 through the engine -> GPU parser, thresholds at quantiles of the fp32 maps; peak-set and human-set agreement asserted."""
@@ -103,8 +102,8 @@ def test_pose_level_agreement_fp16_engine_vs_fp32_backbone():
     Random-init weights give structureless maps, so the thresholds sit at quantiles of the fp32 maps (as in
     test_end_to_end_pose_call...).  Parser parity on IDENTICAL tensors is bit-exact (test_paf_gpu.py); this measures what the
     fp16 operand rounding of the backbone does to the result: peaks that sit within the fp16 budget of the threshold or of a
-    neighbouring local maximum may flip.  Measured on B200 (round 2): Jaccard 0.897 of the peak sets on these structureless
-    maps (a worst case: every pixel is near a threshold or a tie; trained heat-maps have isolated peaks).  Asserted: >= 0.85
+    neighbouring local maximum may flip on these structureless maps (a worst case: every pixel is near a threshold or a
+    tie; trained heat-maps have isolated peaks).  Asserted: Jaccard of the peak sets >= 0.85
     and human counts within 10 % -- the measured values are printed."""
     g = models.openpose_vgg19(0)
     H, W, N = 368, 656, 2

@@ -56,25 +56,9 @@ def test_product_never_imports_oracle():
                 assert not re.search(r"^\s*(from|import)\s+oracle|#include\s+[\"<].*oracle", src, re.M), f
 
 
-def test_conv_traffic_json_is_the_fold_of_the_committed_launch_list():
-    """bench.py's roofline.traffic comes from profiles/conv_traffic.json; that file must be what tools/summarize_launches.py
-    computes from the committed ncu launch list (no hand-edited numbers)"""
-    import json
-    import subprocess
-    import sys
-    csv_path = os.path.join(ROOT, "profiles", "r02_final_launches_step.csv")
-    r = subprocess.run([sys.executable, os.path.join(ROOT, "tools", "summarize_launches.py"), csv_path, "2"], capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr
-    fold = json.loads(r.stdout[r.stdout.index("{"):])
-    committed = json.load(open(os.path.join(ROOT, "profiles", "conv_traffic.json")))
-    assert fold["conv_launches"] == committed["conv_launches"] == 52
-    assert abs(fold["dram_bytes_per_step"] - committed["dram_bytes_per_step"]) < 1.0
-    assert 0.85 < fold["conv_share_of_step_device_time"] < 0.99
-
-
 def test_docs_have_no_unfilled_number_placeholders():
-    """DESIGN.md / README.md take their headline numbers from the final bench line through tools/fill_doc_numbers.py; a placeholder
-    left in the text means the docs were not refreshed after the last measurement."""
+    """DESIGN.md / README.md quote measured numbers; a placeholder left in the text means the docs were not refreshed after the
+    last measurement."""
     import re
     for name in ("DESIGN.md", "README.md", "INTEGRATION.md"):
         text = open(os.path.join(ROOT, name)).read()

@@ -67,7 +67,7 @@ def test_cpp_example_pifpaf_sequence(tmp_path):
 def test_reference_stream_scheduler_builds_over_the_dropin_and_runs_with_a_mock_engine():
     """SURVEY 8f-2: `hyperpose::make_stream(engine, parser)` (include/hyperpose/stream/stream.hpp:311-319) with the reference's
     own scheduler sources (src/stream.cpp, src/thread_pool.cpp) compiled unchanged:
-      * instantiates and links over the B200 `tensorrt` / `paf` classes (examples/stream_api_b200);
+      * instantiates and links over the drop-in `tensorrt` / `paf` classes (examples/stream_api_b200);
       * the same program with a stand-in engine / parser (no GPU) runs the scheduler end to end: every frame reaches the sink,
         the poses drawn equal the operator-API count, the stream shuts down."""
     exe = hb.build_stream_example()

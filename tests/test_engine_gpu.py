@@ -1,4 +1,4 @@
-"""GPU tests of the DNN engine (tcgen05 implicit-GEMM convs) against a plain PyTorch fp32 reference.
+"""GPU tests of the DNN engine (wgmma implicit-GEMM convs) against a plain PyTorch fp32 reference.
 
 Tolerances (written here, as the contract asks):
   * vs the torch reference with fp16 rounding emulated at the same points: max |diff| <= 2e-3 * max|ref| + 2e-3
@@ -42,15 +42,15 @@ def test_tiny_net_every_layer(hw, N):
         try:
             got = eng.debug_read_buffer(bi, N).astype(np.float32).transpose(0, 3, 1, 2)
         except capi.HyperposeError as ex:
-            # the un-pooled output of a conv whose 2x2 max-pool runs in its epilogue is never written; the pooled buffer that
-            # follows is compared like every other one, which checks conv + pool together
+            # the output of a conv whose 2x2 max-pool / 1x1 depthwise op runs in its epilogue is never written; the buffer that
+            # follows is compared like every other one, which checks the two together
             assert ex.status == capi.HP_ERR_UNSUPPORTED, ex
             continue
         ref = rbufs[bi].cpu().numpy()
         if bi == 0:   # im2col buffer: compare its centre tap (k = 4*3 + c) with the normalised image
             if not os.environ.get("HPB_NO_STEM3"):
-                # fused 3x3 stem (conv_stem3_kernel): the patches never leave shared memory, this buffer is not written;
-                # buffer 1 (the first conv's output) checks the stem, test_f32_nchw_entry_matches_u8_entry the im2col kernel
+                # fused 3x3 stem: the patches never leave shared memory, this buffer is not written; buffer 1 (the first conv's
+                # output) checks the stem, test_f32_nchw_entry_matches_u8_entry the im2col kernel
                 assert not got.any()
                 continue
             got = got[:, 12:15]
@@ -99,8 +99,8 @@ def test_mobilenet_thin_openpose(hw, N):
         try:
             got = eng.debug_read_buffer(bi, N).astype(np.float32).transpose(0, 3, 1, 2)
         except capi.HyperposeError as ex:
-            # the un-pooled output of a conv whose 2x2 max-pool runs in its epilogue is never written; the pooled buffer that
-            # follows is compared like every other one, which checks conv + pool together
+            # the output of a conv whose 2x2 max-pool / 1x1 depthwise op runs in its epilogue is never written; the buffer that
+            # follows is compared like every other one, which checks the two together
             assert ex.status == capi.HP_ERR_UNSUPPORTED, ex
             continue
         _check(got, rbufs[bi].cpu().numpy(), 4e-3, 4e-3, f"buffer {bi}")
@@ -128,8 +128,8 @@ def test_resnet50_lw_openpose(hw, N):
         try:
             got = eng.debug_read_buffer(bi, N).astype(np.float32).transpose(0, 3, 1, 2)
         except capi.HyperposeError as ex:
-            # the un-pooled output of a conv whose 2x2 max-pool runs in its epilogue is never written; the pooled buffer that
-            # follows is compared like every other one, which checks conv + pool together
+            # the output of a conv whose 2x2 max-pool / 1x1 depthwise op runs in its epilogue is never written; the buffer that
+            # follows is compared like every other one, which checks the two together
             assert ex.status == capi.HP_ERR_UNSUPPORTED, ex
             continue
         _check(got, rbufs[bi].cpu().numpy(), 6e-3, 6e-3, f"buffer {bi}")
@@ -266,8 +266,8 @@ def test_gpu_frame_resize_bit_exact_vs_oracle(src_hw, keep):
 
 def test_full_size_batch_permutation_invariance():
     """size-independent property at the full BASELINE cfg3 size (368x656, batch 16): frames are independent, so permuting
-    the batch permutes the outputs bit-for-bit -- exercises im2col tiles that straddle row and image boundaries, the
-    swapped-operand units and the TMA store clipping at full scale."""
+    the batch permutes the outputs bit-for-bit -- exercises im2col tiles that straddle row and image boundaries and the
+    ragged last pixel tile at full scale."""
     g = models.openpose_vgg19(0, n_stages=2)
     H, W, N = 368, 656, 16
     frames = syn.make_frames_u8(12, N, H, W)
@@ -287,8 +287,8 @@ def test_full_size_batch_permutation_invariance():
 
 
 def test_fused_3x3_stem_kernel_matches_im2col_path():
-    """3x3 stems: conv_stem3_kernel (default; table-driven gather straight from the u8 frames) == the im2col-buffer path
-    (HPB_NO_STEM3) == the first fused version (HPB_STEM3_V1), on an odd-sized input (partial tiles, all four borders)"""
+    """3x3 stems: the fused u8 stem (default; warpgroup 0 of conv_wgmma_kernel gathers the patches straight from the u8 frames)
+    == the im2col-buffer path (HPB_NO_STEM3), on an odd-sized input (partial tiles, all four borders)"""
     import subprocess, sys, textwrap
     code = textwrap.dedent('''
         import numpy as np, sys
@@ -302,18 +302,17 @@ def test_fused_3x3_stem_kernel_matches_im2col_path():
     ''') % os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
     import tempfile
     outs = []
-    for env in ({}, {"HPB_NO_STEM3": "1"}, {"HPB_STEM3_V1": "1"}):
+    for env in ({}, {"HPB_NO_STEM3": "1"}):
         with tempfile.NamedTemporaryFile(suffix=".npy") as f:
             r = subprocess.run([sys.executable, "-c", code, f.name], env={**os.environ, **env}, capture_output=True, text=True, timeout=300)
             assert r.returncode == 0, r.stderr
             outs.append(np.load(f.name))
-    # the three paths feed the same fp16 patch values to the same MMA shape: results agree to fp32 summation order
+    # the two paths feed the same fp16 patch values to the same MMA shape: results agree to fp32 summation order
     assert np.allclose(outs[0], outs[1], rtol=0, atol=1e-4 * np.abs(outs[0]).max())
-    assert np.allclose(outs[0], outs[2], rtol=0, atol=1e-4 * np.abs(outs[0]).max())
 
 
 def test_halo_box_kernel_matches_im2col_kernels():
-    """conv_halo_kernel (one TMA halo box per 16 x 8-pixel tile serves every filter tap through shifted UMMA descriptors)
+    """conv_halo_kernel (one TMA halo box per 16 x 8-pixel tile serves every filter tap through shifted wgmma descriptors)
     == the per-tap im2col-mode kernels, on ragged sizes (partial tiles on the right / bottom, all four zero-padded borders,
     grouped and 7x7 layers with HPB_HALO=all)"""
     import subprocess, sys, tempfile, textwrap
@@ -341,36 +340,9 @@ def test_halo_box_kernel_matches_im2col_kernels():
     m = np.abs(outs[0]).max()
     assert m > 0
     # same fp16 operands, same fp32 accumulator; only the order of the k-steps differs (chunk-major instead of tap-major)
-    # (through ~40 layers with fp16 activations the re-ordered sums differ by a few fp16 roundings: 8e-4 * max measured)
+    # (through ~40 layers with fp16 activations the re-ordered sums differ by a few fp16 roundings)
     assert np.abs(outs[1] - outs[0]).max() <= 2e-3 * m, np.abs(outs[1] - outs[0]).max() / m
     assert np.abs(outs[2] - outs[0]).max() <= 2e-3 * m
-
-
-def test_weight_multicast_swap_kernel_is_bit_identical():
-    """conv_tcgen05_swap_kernel<true> (HPB_SWAP_MC=1: clusters of two CTAs, each loads half of every weight tile and multicasts it
-    to both) feeds the same operands to the same MMAs in the same order as the plain variant: outputs are bit-identical -- small
-    (odd unit counts: a cluster whose second CTA runs past the end) and at the full cfg3 size"""
-    import subprocess, sys, tempfile, textwrap
-    code = textwrap.dedent('''
-        import numpy as np, sys
-        sys.path.insert(0, %r)
-        from hyperpose_b200 import capi, models, synthetic as syn
-        outs = []
-        for (h, w, n, st) in ((72, 104, 2, 2), (56, 88, 3, 3), (368, 656, 3, 6)):
-            e = capi.Engine(models.openpose_vgg19(0, n_stages=st).to_pack(), (w, h), max_batch_size=n)
-            e.infer_u8(syn.make_frames_u8(5, n, h, w)); c, p = e.read_outputs(n)
-            outs += [c.ravel(), p.ravel()]
-            e.close()
-        np.save(sys.argv[1], np.concatenate(outs))
-    ''') % os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    outs = []
-    for env in ({"HPB_SWAP_MC": "0"}, {"HPB_SWAP_MC": "1"}):
-        with tempfile.NamedTemporaryFile(suffix=".npy") as f:
-            r = subprocess.run([sys.executable, "-c", code, f.name], env={**os.environ, **env}, capture_output=True, text=True, timeout=300)
-            assert r.returncode == 0, r.stderr[-2000:]
-            outs.append(np.load(f.name))
-    assert np.isfinite(outs[0]).all() and np.abs(outs[0]).max() > 0
-    assert np.array_equal(outs[0], outs[1])
 
 
 def test_max_pool_fused_into_the_halo_epilogue_is_bit_identical(monkeypatch):
@@ -459,27 +431,3 @@ def test_tma_tiled_depthwise_kernel_is_bit_identical(monkeypatch, hw, N):
     for bi, b in tiled.items():
         assert b == plain[bi], f"buffer {bi} ({g.buffers[bi]}) differs between the TMA-tiled and the per-lane-load depthwise kernels"
     assert tiled_outs[0].tobytes() == plain_outs[0].tobytes() and tiled_outs[1].tobytes() == plain_outs[1].tobytes()
-
-
-@pytest.mark.gpu
-def test_n_half_tiles_of_a_ragged_last_round_are_bit_identical(monkeypatch):
-    """conv_tcgen05_kernel's work list: when the last round of 128-pixel x 256-channel tiles would occupy at most half of the CTAs, those
-    tiles run as N-halves (128 x 128; 128 x 64 for 128-channel tiles) on twice as many CTAs.  Same MMAs per output element, same k order:
-    the bytes must not change (HPB_NO_SPLIT=1 = the plain tile list).  ResNet50 + LW-OpenPose at 368x432 / batch 8 has such layers of
-    every kind (46x54 maps = 156 pixel tiles: 128 channels -> 8 tiles in the ragged round, 512 -> 16, 1024 -> 32, 2048 -> 64;
-    92x108 maps = 621 pixel tiles: 256 channels -> 29)."""
-    g = models.resnet50_lw_openpose(0)
-    H, W, N = 368, 432, 8
-    frames = syn.make_frames_u8(29, N, H, W)
-
-    def run():
-        eng = capi.Engine(g.to_pack(), (W, H), max_batch_size=N)
-        eng.infer_u8(frames)
-        outs = eng.read_outputs(N)
-        eng.close()
-        return outs
-
-    split = run()
-    monkeypatch.setenv("HPB_NO_SPLIT", "1")
-    plain = run()
-    assert split[0].tobytes() == plain[0].tobytes() and split[1].tobytes() == plain[1].tobytes()

@@ -1,5 +1,5 @@
 """The data_type::kFLOAT engine (include/hyperpose/operator/dnn/tensorrt.hpp:14-22,48,61): fp32 activations in HBM,
-tcgen05.mma.kind::tf32 (conv_tf32_kernel), fp32 helper kernels -- hp_engine_create_ex(..., HP_DTYPE_TF32).
+wgmma kind tf32 (conv_wgmma_kernel<float, ...>), fp32 helper kernels -- hp_engine_create_ex(..., HP_DTYPE_TF32).
 
 Checker: oracle/torch_backbone.py in plain fp32 (TF32 off in torch).  Tolerance, stated here as the contract asks: TF32 keeps a
 10-bit mantissa on the conv operands (weights and activations rounded to nearest by their producers), everything else is fp32,

@@ -64,15 +64,19 @@ def test_gpu_decoder_equals_reference_golden(gold, case):
 
 
 @pytest.mark.gpu
-@pytest.mark.skipif(not oracle.pifpaf_ref_available(), reason="oracle/_ref/libref_pifpaf.so not built")
-def test_gpu_decoder_batched_vs_live_reference():
+def test_gpu_decoder_batched_vs_live_reference(golden_dir):
+    """against the reference decoder's records for these fields (tests/golden/ref_pifpaf_live.npz), and against the live reference
+    where oracle/_ref is built (which must then still produce the stored records)"""
+    live = np.load(os.path.join(golden_dir, "ref_pifpaf_live.npz"))
     N, h, w = 8, 49, 49
     fields = [syn.make_pifpaf_fields(100 + i, (1, 9), h, w) for i in range(N)]
     pif = np.stack([f[0] for f in fields]); paf = np.stack([f[1] for f in fields])
     dec = capi.PifPafParser(385, 385, 0.1)
     got = dec.process_batch(pif, paf)
     for i in range(N):
-        want = oracle.ref_pifpaf_process(pif[i], paf[i], 385, 385, 0.1)
+        want = live[f"batched_{i}"]
+        if oracle.pifpaf_ref_available():
+            assert oracle.ref_pifpaf_process(pif[i], paf[i], 385, 385, 0.1).tobytes() == want.tobytes(), f"frame {i}: live reference != golden"
         d = _diff(got[i], want)
         assert d is None, f"frame {i}: {d}"
     dec.close()

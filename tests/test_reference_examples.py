@@ -3,9 +3,9 @@ north star: "drops into the existing C++ examples unchanged") -- build here and 
 
 Build (hyperpose_b200/build.py::build_reference_examples): every source is compiled where it lies in the reference tree --
 the example, examples/utils.cpp, and the reference's own src/{stream,thread_pool,logging,human,data}.cpp (scheduler,
-draw_human, non_scaling_resize) -- over the unchanged public headers, with the B200 classes of csrc/hyperpose_api underneath
+draw_human, non_scaling_resize) -- over the unchanged public headers, with the drop-in classes of csrc/hyperpose_api underneath
 and the OpenCV / gflags stand-ins of csrc/shim (neither library exists in this image).  The binaries land in
-examples/ref_build/ and travel to the GPU box with the snapshot.
+examples/ref_build/; where the reference tree is absent the tests skip.
 
 Inputs: the shim's only image container is binary PPM, so the "images" are P6 files named *.png and the "video" is P6 frames
 back to back; model files are HPB2PACK packs named as the example expects (.onnx where it insists on that suffix)."""
@@ -50,7 +50,7 @@ def _read_p6_stream(path):
 def _exes():
     exes = hb.build_reference_examples()
     if exes is None:
-        pytest.skip("reference examples not built (need /root/reference at build time; the GPU box uses the prebuilt binaries)")
+        pytest.skip("reference examples not built (need /root/reference at build time)")
     return exes
 
 
@@ -61,7 +61,7 @@ def test_reference_examples_build_unmodified_against_the_dropin():
     for name, exe in exes.items():
         assert os.path.exists(exe), name
     syms = subprocess.run(["nm", "-C", "--defined-only", exes["cli"]], capture_output=True, text=True).stdout
-    # the reference's own scheduler / drawing code is in the binary, over the B200 engine and parsers
+    # the reference's own scheduler / drawing code is in the binary, over the drop-in engine and parsers
     for want in ["hyperpose::basic_stream_manager::write_to(cv::VideoWriter&)", "hyperpose::draw_human(cv::Mat&",
                  "hyperpose::non_scaling_resize(", "hyperpose::dnn::tensorrt::inference(std::vector<cv::Mat", "hyperpose::parser::paf::process(",
                  "hyperpose::parser::pifpaf::process(", "hyperpose::parser::pose_proposal::process("]:
@@ -117,7 +117,7 @@ def test_operator_api_batched_images_pifpaf_example_runs(tmp_path):
 @pytest.mark.gpu
 def test_stream_api_video_paf_example_runs(tmp_path):
     """examples/stream_api_video_paf.example.cpp:80-95, unmodified: hp::make_stream(engine, parser); stream.async() << capture;
-    stream.sync() >> writer -- the reference's own scheduler threads over the B200 engine / parser, video in, video out"""
+    stream.sync() >> writer -- the reference's own scheduler threads over the drop-in engine / parser, video in, video out"""
     exes = _exes()
     _, video, frames = _write_inputs(tmp_path, 11, 64, 96)
     pack = tmp_path / "tiny.pack"

@@ -1,5 +1,5 @@
 """Per-op CUDA-event times of the cfg3 graph (engine only, 40 profiled steps after warm-up); one line per op.
-Used to compare kernel variants selected by environment switches (HPB_HALO, HPB_NO_STEM3, HPB_NO_SWAP, ...)."""
+Used to compare kernel variants selected by environment switches (HPB_HALO, HPB_NO_STEM3, HPB_NO_POOL_FUSE, ...)."""
 import json
 import os
 import sys
