@@ -264,83 +264,6 @@ __global__ void __launch_bounds__(256, 3) dwconv3_col_kernel(const __half* __res
 #undef HP_FMA4
 }
 
-// Two depthwise 3x3 / stride-1 convolutions of the SAME input with different filters (the first separable block of the conf and
-// the paf branch of a MobilenetThin-OpenPose stage, mbv2_th_openpose.py:111-128: both read the 1216-channel concat tensor) in one
-// pass: a thread owns one column x, 2 channels and a run of rows, loads each input pixel ONCE (3 x 4-byte loads per row) and feeds
-// both filter sets; outputs go to out0 / out1.  Same column-marching scheme and the same accumulation order per output as
-// dwconv3_col_kernel (bit-identical); the second read of the 48 MB input and six of the twelve launches per network disappear.
-__global__ void __launch_bounds__(256, 3) dwconv3_col_dual_kernel(const __half* __restrict__ in, int in_ld, __half* __restrict__ out0, __half* __restrict__ out1, int out_ld,
-                                                               const float* __restrict__ w0 /*[9][C] | bias[C] | alpha[C]*/, const float* __restrict__ w1,
-                                                               int N, int H, int W, int C, int rows_per_chunk, int chunks)
-{
-    const size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    const int cv = C / 2;
-    const size_t total = (size_t)N * chunks * W * cv;
-    if (idx >= total) return;
-    const int c0 = (int)(idx % cv) * 2;
-    size_t t = idx / cv;
-    const int x = (int)(t % W); t /= W;
-    const int chunk = (int)(t % chunks);
-    const int n = (int)(t / chunks);
-    const int oh0 = chunk * rows_per_chunk, oh1 = min(oh0 + rows_per_chunk, H);
-    if (oh0 >= oh1) return;
-    float2 wa[9], wb[9];
-#pragma unroll
-    for (int k = 0; k < 9; ++k) { wa[k] = __ldg((const float2*)(w0 + (size_t)k * C + c0)); wb[k] = __ldg((const float2*)(w1 + (size_t)k * C + c0)); }
-    const float2 bsa = __ldg((const float2*)(w0 + (size_t)9 * C + c0)), ala = __ldg((const float2*)(w0 + (size_t)10 * C + c0));
-    const float2 bsb = __ldg((const float2*)(w1 + (size_t)9 * C + c0)), alb = __ldg((const float2*)(w1 + (size_t)10 * C + c0));
-    const bool has_l = x > 0, has_r = x + 1 < W;
-    const size_t row_in = (size_t)W * in_ld, row_out = (size_t)W * out_ld;
-    const __half* rp = in + ((size_t)n * H * W + x) * in_ld + c0;
-    __half* opa = out0 + ((size_t)n * H * W + x) * out_ld + c0 + (size_t)oh0 * row_out;
-    __half* opb = out1 + ((size_t)n * H * W + x) * out_ld + c0 + (size_t)oh0 * row_out;
-    float2 a0 = { 0.f, 0.f }, a1 = a0, a2 = a0, b0 = a0, b1 = a0, b2 = a0;   // output rows ih-1, ih, ih+1 of branch a / b
-#define HP_FMA2(acc, wv, xv) { acc.x = fmaf(xv.x, wv.x, acc.x); acc.y = fmaf(xv.y, wv.y, acc.y); }
-#define HP_DWD_EMIT(A, B)                                                                                                          \
-    {                                                                                                                               \
-        float y0 = A.x + bsa.x, y1 = A.y + bsa.y, z0 = B.x + bsb.x, z1 = B.y + bsb.y;                                                 \
-        y0 = y0 > 0.f ? y0 : y0 * ala.x; y1 = y1 > 0.f ? y1 : y1 * ala.y;                                                             \
-        z0 = z0 > 0.f ? z0 : z0 * alb.x; z1 = z1 > 0.f ? z1 : z1 * alb.y;                                                             \
-        *(__half2*)opa = __floats2half2_rn(y0, y1);                                                                                   \
-        *(__half2*)opb = __floats2half2_rn(z0, z1);                                                                                   \
-        opa += row_out; opb += row_out;                                                                                               \
-    }
-#define HP_DWD_STEP(A0, A1, A2, B0, B1, B2, IH)                                                                                    \
-    {                                                                                                                               \
-        uint32_t ul = 0u, ur = 0u;                                                                                                   \
-        const uint32_t uc = *(const uint32_t*)rp;                                                                                    \
-        if (has_l) ul = *(const uint32_t*)(rp - in_ld);                                                                              \
-        if (has_r) ur = *(const uint32_t*)(rp + in_ld);                                                                              \
-        rp += row_in;                                                                                                                \
-        const float2 vl = __half22float2(*(const __half2*)&ul), vm = __half22float2(*(const __half2*)&uc), vr = __half22float2(*(const __half2*)&ur); \
-        HP_FMA2(A0, wa[6], vl); HP_FMA2(A0, wa[7], vm); HP_FMA2(A0, wa[8], vr);                                                      \
-        HP_FMA2(A1, wa[3], vl); HP_FMA2(A1, wa[4], vm); HP_FMA2(A1, wa[5], vr);                                                      \
-        A2 = make_float2(0.f, 0.f);                                                                                                  \
-        HP_FMA2(A2, wa[0], vl); HP_FMA2(A2, wa[1], vm); HP_FMA2(A2, wa[2], vr);                                                      \
-        HP_FMA2(B0, wb[6], vl); HP_FMA2(B0, wb[7], vm); HP_FMA2(B0, wb[8], vr);                                                      \
-        HP_FMA2(B1, wb[3], vl); HP_FMA2(B1, wb[4], vm); HP_FMA2(B1, wb[5], vr);                                                      \
-        B2 = make_float2(0.f, 0.f);                                                                                                  \
-        HP_FMA2(B2, wb[0], vl); HP_FMA2(B2, wb[1], vm); HP_FMA2(B2, wb[2], vr);                                                      \
-        if ((IH) - 1 >= oh0) HP_DWD_EMIT(A0, B0);                                                                                    \
-    }
-    const int ih_first = max(oh0 - 1, 0), ih_last = min(oh1, H - 1);
-    rp += (size_t)ih_first * row_in;
-    int ih = ih_first;
-    for (; ih + 2 <= ih_last; ih += 3) {
-        HP_DWD_STEP(a0, a1, a2, b0, b1, b2, ih);
-        HP_DWD_STEP(a1, a2, a0, b1, b2, b0, ih + 1);
-        HP_DWD_STEP(a2, a0, a1, b2, b0, b1, ih + 2);
-    }
-    for (; ih <= ih_last; ++ih) {
-        HP_DWD_STEP(a0, a1, a2, b0, b1, b2, ih);
-        a0 = a1; a1 = a2; b0 = b1; b1 = b2;
-    }
-    if (oh1 - 1 >= ih_last) HP_DWD_EMIT(a0, b0);
-#undef HP_DWD_STEP
-#undef HP_DWD_EMIT
-#undef HP_FMA2
-}
-
 // Depthwise 3x3 / stride 1 with the input staged by TMA (channel counts that are multiples of 64; NB = 1: one filter set, NB = 2: the two
 // filter sets of a MobilenetThin stage's conf / paf branch on the same input).  The per-lane loads of dwconv3_col_kernel keep too few
 // bytes in flight (the warps mostly wait on L1TEX loads at a small fraction of the DRAM bandwidth), so here a persistent CTA pulls
@@ -352,7 +275,7 @@ __global__ void __launch_bounds__(256, 3) dwconv3_col_dual_kernel(const __half* 
 struct DwTmaParams {
     __half* out0; __half* out1; int out_ld;
     const float* w0; const float* w1;   // [9][C] | bias[C] | alpha[C]
-    int N, H, W, C, ctiles, tiles_x, tiles_y, wbo, hb, n_items, stages, ct_fastest;
+    int H, W, C, ctiles, tiles_x, tiles_y, wbo, hb, n_items, stages;
 };
 constexpr int DWT_THREADS = 384;   // 12 warps
 constexpr int DWT_STAGE_MAX = 73728;   // bytes of one tile buffer at most (3 of them + barriers fit 227 KB)
@@ -373,21 +296,25 @@ __global__ void __launch_bounds__(DWT_THREADS, 1) dwconv3_tma_kernel(const __gri
         ptx::fence_barrier_init();
     }
     __syncthreads();
+    // work item -> tile: item = ((n * tiles_y + ty) * tiles_x + tx) * ctiles + ct, the channel tile fastest so that concurrent CTAs
+    // read whole pixels
+    auto tile_of = [&](int item, int& ct, int& tx, int& ty, int& n) {
+        ct = item % p.ctiles; item /= p.ctiles;
+        tx = item % p.tiles_x; item /= p.tiles_x;
+        ty = item % p.tiles_y;
+        n = item / p.tiles_y;
+    };
     // k-th tile of this CTA -> its buffer (thread 0 only)
     auto issue = [&](int k) {
         const int item = (int)blockIdx.x + k * (int)gridDim.x;
         if (item >= p.n_items) return;
-        int t = item, ct = 0;
-        if (p.ct_fastest) { ct = t % p.ctiles; t /= p.ctiles; }
-        const int tx = t % p.tiles_x; t /= p.tiles_x;
-        const int ty = t % p.tiles_y; t /= p.tiles_y;
-        const int n = t % p.N;
-        if (!p.ct_fastest) ct = t / p.N;
+        int ct, tx, ty, n;
+        tile_of(item, ct, tx, ty, n);
         const int s = k % p.stages;
         ptx::mbar_expect_tx(bars + 8u * s, stage_bytes);
         ptx::tma_load_4d(base + (uint32_t)s * stage_bytes, &tmap_in, bars + 8u * s, ct * 64, tx * p.wbo - 1, ty * p.hb - 1, n);
     };
-    ptx::pdl_wait();   // (HPB_PDL) the prologue above may run under the previous kernel's tail; its results are visible from here on
+    ptx::pdl_wait();   // the prologue above may run under the previous kernel's tail; its results are visible from here on
     if (threadIdx.x == 0)
         for (int k = 0; k < p.stages - 1; ++k) issue(k);
     const size_t row_out = (size_t)p.W * p.out_ld;
@@ -398,12 +325,8 @@ __global__ void __launch_bounds__(DWT_THREADS, 1) dwconv3_tma_kernel(const __gri
         if (item >= p.n_items) break;
         __syncthreads();   // every warp is done with tile k-1: its buffer takes tile k + stages - 1
         if (threadIdx.x == 0) issue(k + p.stages - 1);
-        int t = item, ct = 0;
-        if (p.ct_fastest) { ct = t % p.ctiles; t /= p.ctiles; }
-        const int tx = t % p.tiles_x; t /= p.tiles_x;
-        const int ty = t % p.tiles_y; t /= p.tiles_y;
-        const int n = t % p.N;
-        if (!p.ct_fastest) ct = t / p.N;
+        int ct, tx, ty, n;
+        tile_of(item, ct, tx, ty, n);
         const int c0 = ct * 64 + lane * 2;
         if (ct != ct_loaded) {
             ct_loaded = ct;
@@ -553,38 +476,28 @@ __global__ void __launch_bounds__(256) maxpool2_kernel(const __half* __restrict_
 }
 
 // ---------------------------------------------------------------------------------------------
-// tensor maps (driver entry point fetched at run time: no link-time dependency on libcuda)
+// tensor maps (driver entry points fetched at run time: no link-time dependency on libcuda)
 // ---------------------------------------------------------------------------------------------
+void* driver_entry_point(const char* name)
+{
+    void* p = nullptr;
+    cudaDriverEntryPointQueryResult qres;
+    if (cudaGetDriverEntryPoint(name, &p, cudaEnableDefault, &qres) != cudaSuccess || qres != cudaDriverEntryPointSuccess) return nullptr;
+    return p;
+}
+
 typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
                                     const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
                                     CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-PFN_encodeTiled get_encode_fn()
-{
-    static PFN_encodeTiled fn = nullptr;
-    if (!fn) {
-        void* p = nullptr;
-        cudaDriverEntryPointQueryResult qres;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qres) == cudaSuccess && qres == cudaDriverEntryPointSuccess)
-            fn = (PFN_encodeTiled)p;
-    }
-    return fn;
-}
-
 typedef CUresult (*PFN_encodeIm2col)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*, const int*, const int*,
                                      cuuint32_t, cuuint32_t, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion,
                                      CUtensorMapFloatOOBfill);
-// activations [N,H,W,C] fp16 in im2col mode: 128 consecutive output pixels x 64 channels per load; the bounding box
+// activations [N,H,W,C] fp16 (fp32) in im2col mode: 128 consecutive output pixels x 64 (32) channels per load; the bounding box
 // [-pad, dim - pad) holds one base position per output pixel, filter taps are the im2col offsets of the copy instruction
-int make_tmap_act_im2col(CUtensorMap* m, const void* base, int N, int H, int W, int C, int R, int S, int pixels_per_load = CONV_BLOCK_M, bool f32 = false)
+int make_tmap_act_im2col(CUtensorMap* m, const void* base, int N, int H, int W, int C, int R, int S, bool f32)
 {
     const int es = f32 ? 4 : 2;
-    static PFN_encodeIm2col enc = nullptr;
-    if (!enc) {
-        void* p = nullptr;
-        cudaDriverEntryPointQueryResult qres;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeIm2col", &p, cudaEnableDefault, &qres) == cudaSuccess && qres == cudaDriverEntryPointSuccess)
-            enc = (PFN_encodeIm2col)p;
-    }
+    const auto enc = (PFN_encodeIm2col)driver_entry_point("cuTensorMapEncodeIm2col");
     if (!enc) { set_error("cuTensorMapEncodeIm2col entry point not available"); return HP_ERR_CUDA; }
     cuuint64_t dims[4] = { (cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)N };
     cuuint64_t strides[3] = { (cuuint64_t)C * es, (cuuint64_t)W * C * es, (cuuint64_t)H * W * C * es };
@@ -592,15 +505,15 @@ int make_tmap_act_im2col(CUtensorMap* m, const void* base, int N, int H, int W, 
     int lower[2] = { -pad_w, -pad_h };
     int upper[2] = { pad_w - (S - 1), pad_h - (R - 1) };
     cuuint32_t estr[4] = { 1, 1, 1, 1 };
-    CUresult r = enc(m, f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, (void*)base, dims, strides, lower, upper, f32 ? 32 : 64, (cuuint32_t)pixels_per_load, estr,
+    CUresult r = enc(m, f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, (void*)base, dims, strides, lower, upper, f32 ? 32 : 64, (cuuint32_t)CONV_BLOCK_M, estr,
                      CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeIm2col failed: %d (N=%d H=%d W=%d C=%d R=%d S=%d)", (int)r, N, H, W, C, R, S); return HP_ERR_CUDA; }
     return HP_OK;
 }
-// weights [rows, K] fp16 K-major: dims (K, rows), box (64, BN)
-int make_tmap_wgt(CUtensorMap* m, const void* base, int rows, int K, int BN, bool f32 = false)
+// weights [rows, K] fp16 (fp32) K-major: dims (K, rows), box (64 (32), BN)
+int make_tmap_wgt(CUtensorMap* m, const void* base, int rows, int K, int BN, bool f32)
 {
-    PFN_encodeTiled enc = get_encode_fn();
+    const auto enc = (PFN_encodeTiled)driver_entry_point("cuTensorMapEncodeTiled");
     if (!enc) { set_error("cuTensorMapEncodeTiled entry point not available"); return HP_ERR_CUDA; }
     cuuint64_t dims[2] = { (cuuint64_t)K, (cuuint64_t)rows };
     cuuint64_t strides[1] = { (cuuint64_t)K * (f32 ? 4 : 2) };
@@ -612,35 +525,20 @@ int make_tmap_wgt(CUtensorMap* m, const void* base, int rows, int K, int BN, boo
     return HP_OK;
 }
 
-// activations [N,H,W,C] fp16 as a 4-D tiled tensor (C, W, H, N), box {64 ch, box_w, box_h, 1}, 128B swizzle: the halo-box loads
-// of conv_halo_kernel (out-of-tensor elements: zero-filled on load)
-int make_tmap_act_box(CUtensorMap* m, const __half* base, int N, int H, int W, int C, int box_w, int box_h)
+// a C-channel view (channel stride ld) of activations [N,H,W,ld] fp16 as a 4-D tiled tensor (C, W, H, N), box {64 ch, box_w, box_h, 1},
+// out-of-tensor elements zero-filled on load.  The halo-box loads of conv_halo_kernel take the 128B swizzle, the halo'd tiles of
+// dwconv3_tma_kernel none (a pixel's 64 channels = 128 contiguous bytes of shared memory).
+int make_tmap_act_box(CUtensorMap* m, const __half* base, int N, int H, int W, int C, int ld, int box_w, int box_h, CUtensorMapSwizzle swizzle)
 {
-    PFN_encodeTiled enc = get_encode_fn();
-    if (!enc) { set_error("cuTensorMapEncodeTiled entry point not available"); return HP_ERR_CUDA; }
-    cuuint64_t dims[4] = { (cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)N };
-    cuuint64_t strides[3] = { (cuuint64_t)C * 2, (cuuint64_t)W * C * 2, (cuuint64_t)H * W * C * 2 };
-    cuuint32_t box[4] = { 64, (cuuint32_t)box_w, (cuuint32_t)box_h, 1 };
-    cuuint32_t estr[4] = { 1, 1, 1, 1 };
-    CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, (void*)base, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                     CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled(box) failed: %d (N=%d H=%d W=%d C=%d box %dx%d)", (int)r, N, H, W, C, box_w, box_h); return HP_ERR_CUDA; }
-    return HP_OK;
-}
-
-// a C-channel view (channel stride ld) of activations [N,H,W,ld] fp16 as a 4-D tiled tensor (C, W, H, N), box {64 ch, box_w, box_h, 1}, no
-// swizzle (a pixel's 64 channels = 128 contiguous bytes of shared memory): the halo'd tiles of dwconv3_tma_kernel
-int make_tmap_act_box_plain(CUtensorMap* m, const __half* base, int N, int H, int W, int C, int ld, int box_w, int box_h)
-{
-    PFN_encodeTiled enc = get_encode_fn();
+    const auto enc = (PFN_encodeTiled)driver_entry_point("cuTensorMapEncodeTiled");
     if (!enc) { set_error("cuTensorMapEncodeTiled entry point not available"); return HP_ERR_CUDA; }
     cuuint64_t dims[4] = { (cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)N };
     cuuint64_t strides[3] = { (cuuint64_t)ld * 2, (cuuint64_t)W * ld * 2, (cuuint64_t)H * W * ld * 2 };
     cuuint32_t box[4] = { 64, (cuuint32_t)box_w, (cuuint32_t)box_h, 1 };
     cuuint32_t estr[4] = { 1, 1, 1, 1 };
     CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, (void*)base, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                     CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled(plain box) failed: %d (N=%d H=%d W=%d C=%d ld=%d box %dx%d)", (int)r, N, H, W, C, ld, box_w, box_h); return HP_ERR_CUDA; }
+                     swizzle, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled(box) failed: %d (N=%d H=%d W=%d C=%d ld=%d box %dx%d)", (int)r, N, H, W, C, ld, box_w, box_h); return HP_ERR_CUDA; }
     return HP_OK;
 }
 
@@ -666,34 +564,73 @@ struct ConvPlan {
     ConvParams prm;
     CUtensorMap tmap_a, tmap_b;
     CUtensorMap tmap_x;          // halo plan: the input as a 4-D tensor with a (16+R-1) x (8+S-1)-pixel box
-    __half* d_w = nullptr;
-    float* d_w32 = nullptr;      // tf32 plan: fp32 K-major weights, rounded to TF32
-    bool tf32 = false;
-    // halo-box kernel (conv_halo_kernel): one TMA box per 16 x 8-pixel tile and channel chunk serves every filter tap
-    bool halo = false;
-    bool pool_fused = false;    // the 2x2 max-pool that follows is taken in the halo kernel's epilogue (hp.out is the POOLED buffer)
-    bool monotone_act = false;  // every PReLU slope of the layer is >= 0
-    HaloParams hp;
-    int stem_R = 0;              // 3 | 7: u8 input runs the fused stem (conv_wgmma_kernel<__half, BN, false, R>), the im2col op is skipped
+    void* d_w = nullptr;         // K-major weights: fp16, or fp32 rounded to TF32 (the engine's dtype)
+    bool monotone_act = false;   // every PReLU slope of the layer is >= 0
+    HaloParams hp;               // halo plan: conv_halo_kernel's parameters
     float* d_bias = nullptr;
     float* d_alpha = nullptr;
-    int grid = 0;
     size_t smem = 0;
-    int built_for_N = 0;
     double flops_per_frame = 0;
 };
 
+// What run_graph launches for an op: decided once when the engine is created, by build_conv_plan and the fusion passes
+enum class Launch : uint8_t {
+    None,           // taken by the launch of a neighbouring op (a conv epilogue, or the first op of a TMA depthwise pair)
+    Im2col,         // im2col3_kernel
+    StemOrIm2col,   // u8 frames: nothing, the consumer conv (ConvStem) gathers its patches from the frames; f32 entry: im2col3_kernel
+    Conv,           // conv_wgmma_kernel
+    ConvStem,       // u8 frames: conv_wgmma_kernel with the fused R x R stem (R = po.R); f32 entry: as Conv
+    Halo,           // conv_halo_kernel: one TMA box per 16 x 8-pixel tile and channel chunk serves every filter tap
+    HaloPool,       // conv_halo_kernel with the 2x2 max-pool that follows in its epilogue (hp.out is the POOLED buffer)
+    DwTma,          // dwconv3_tma_kernel<1>
+    DwTmaPair,      // dwconv3_tma_kernel<2>: this op and the next one (same input, other filters)
+    DwCol,          // dwconv3_col_kernel
+    DwStrip,        // dwconv_kernel<K, stride>
+    MaxPool,        // maxpool2_kernel
+    Heads,          // two pifpaf_head_kernel launches
+    // TF32 engine: fp32 activations (conv_tf32.cuh); its convs are Conv
+    Im2colF32, DwF32, MaxPoolF32, HeadsF32,
+};
+
+// kernels an op launches per run: what launch_count counts, and what a graph replay of the step stands for
+int kernels_launched(Launch k, bool u8_input)
+{
+    switch (k) {
+    case Launch::None: return 0;
+    case Launch::StemOrIm2col: return u8_input ? 0 : 1;
+    case Launch::Heads: case Launch::HeadsF32: return 2;
+    default: return 1;
+    }
+}
+
+// does op q read buffer b (its input, a residual, or the second head input)?  The im2col op reads the frames.
+bool reads_buffer(const PackOp& q, uint32_t b)
+{
+    if (q.type == OP_IM2COL3) return false;
+    return q.in_buf == b || (((q.type == OP_CONV && q.res_mode) || q.type == OP_PIFPAF_HEAD) && q.res_buf == b);
+}
+
 struct EngOp {
-    bool fused_into_stem = false; // OP_IM2COL3 whose consumer gathers its patches from the u8 frames itself: skipped for u8 input
-    bool fused_into_prev = false; // OP_MAXPOOL2 / 1x1 OP_DWCONV taken in the epilogue of the conv before it / second OP_DWCONV of a dual launch: never launched
-    bool dual_with_next = false;  // OP_DWCONV: the next op is a depthwise conv of the same input -- one dwconv3_col_dual_kernel serves both
-    bool dw_tma = false;          // OP_DWCONV 3x3 / stride 1, C % 64 == 0: dwconv3_tma_kernel (input tiles staged by TMA)
-    CUtensorMap tmap_dw;
-    int dwt_wbo = 0, dwt_hb = 0, dwt_tiles_x = 0, dwt_tiles_y = 0, dwt_stages = 0;
-    size_t dwt_smem = 0;
+    Launch launch = Launch::None;
     PackOp po;
     ConvPlan plan;              // OP_CONV only
     float* d_dw = nullptr;      // OP_DWCONV: [K*K][C] weights | bias[C] | alpha[C]
+    // DwTma / DwTmaPair: the input's halo'd tiles
+    CUtensorMap tmap_dw;
+    int dwt_wbo = 0, dwt_hb = 0, dwt_tiles_x = 0, dwt_tiles_y = 0, dwt_stages = 0;
+    size_t dwt_smem = 0;
+};
+
+// Environment switches, read once by hp_engine_create_ex.  Each selects the plainer form of a fused or TMA kernel path, the
+// reference the tests compare the default against.
+struct EngOptions {
+    enum { HALO_AUTO, HALO_NONE, HALO_ALL } halo = HALO_AUTO;   // HPB_HALO=all | anything else; unset: 3x3 layers whose tile grid wastes <= 6 %
+    bool stem3 = true;           // fused 3x3 stem; HPB_NO_STEM3 keeps the im2col buffer
+    bool pool_fuse = true;       // HPB_NO_POOL_FUSE
+    bool dw1_fuse = true;        // HPB_NO_DW1_FUSE
+    bool dw_pair = true;         // HPB_NO_DW_DUAL
+    bool dw_tma = true;          // HPB_NO_DW_TMA
+    int pifpaf_reserve_sms = 0;  // HPB_PIFPAF_RESERVE_SMS (default min(max_batch, 16)), bounded by half the SMs
 };
 
 // TF "SAME": out = ceil(in / stride), pad_before = max((out - 1) * stride + k - in, 0) / 2
@@ -719,9 +656,11 @@ struct hp_engine {
     double factor = 1.0 / 255;
     int flip_rgb = 1;
     int num_sms = 132;
+    EngOptions opt;
     PackHeader hdr;
     std::vector<EngBuffer> bufs;
     std::vector<EngOp> ops;
+    int step_kernels = 0;          // kernels of one run of the whole graph on u8 frames
     float* d_conf = nullptr;
     float* d_paf = nullptr;
     int out_h = 0, out_w = 0;
@@ -791,109 +730,32 @@ inline float tf32_round(float x)
     return x;
 }
 
-// data_type::kFLOAT plan: fp32 activations on the TF32 grid, conv_wgmma_kernel<float, ...>
-int build_conv_plan_tf32(hp_engine* e, EngOp& op, const float* blob)
+// The conv's GEMM operands, epilogue and tensor maps.  data_type::kHALF: fp16 activations and weights, 64-channel chunks;
+// data_type::kFLOAT (HP_DTYPE_TF32): fp32 activations on the TF32 grid, 32-channel chunks (conv_wgmma_kernel<float, ...>).
+int build_conv_plan(hp_engine* e, EngOp& op, const float* blob)
 {
     const PackOp& po = op.po;
     ConvPlan& pl = op.plan;
-    pl.tf32 = true;
+    const bool tf32 = e->dtype == HP_DTYPE_TF32;
+    const int chunk = tf32 ? 32 : 64;
+    const size_t es = tf32 ? sizeof(float) : sizeof(__half);
     const EngBuffer& ib = e->bufs[po.in_buf];
     const int G = (int)po.groups, R = (int)po.R, S = (int)po.S, cin_g = (int)po.cin_g, cout_g = (int)po.cout_g;
     const bool im2col = po.im2col_input != 0;
     if (im2col && (G != 1 || R * S * cin_g > ib.channels)) { set_error("engine: bad im2col conv"); return HP_ERR_ARG; }
-    if (!im2col && G > 1 && cin_g % 32 != 0) { set_error("engine(tf32): grouped conv needs cin_g %% 32 == 0 (got %d)", cin_g); return HP_ERR_UNSUPPORTED; }
-    const int eR = im2col ? 1 : R, eS = im2col ? 1 : S;
-    const int ecin = im2col ? round_up(R * S * cin_g, 32) : round_up(cin_g, 32);
-    if ((int)po.in_ch_off + G * ecin > ib.channels && !(G == 1 && (int)po.in_ch_off + ecin <= round_up(ib.channels, 32) && false)) {
-        // a 32-channel chunk may not run past the buffer: the engine pads conv inputs to 64 channels, so this only trips on a bad pack
-        set_error("engine(tf32): conv reads channels [%d,%d) of a %d-channel buffer", po.in_ch_off, po.in_ch_off + G * ecin, ib.channels);
-        return HP_ERR_ARG;
-    }
-    const int BN = pick_bn(cout_g);
-    const int cout_pad = round_up(cout_g, BN);
-    const int K = eR * eS * ecin;
-    std::vector<float> w((size_t)G * cout_pad * K, 0.f), bias((size_t)G * cout_pad, 0.f), alpha((size_t)G * cout_pad, 0.f);
-    const float* Wt = blob + po.w_off;
-    for (int g = 0; g < G; ++g)
-        for (int o = 0; o < cout_g; ++o) {
-            bias[(size_t)g * cout_pad + o] = blob[po.b_off + (size_t)g * cout_g + o];
-            alpha[(size_t)g * cout_pad + o] = blob[po.a_off + (size_t)g * cout_g + o];
-            for (int c = 0; c < cin_g; ++c)
-                for (int r = 0; r < R; ++r)
-                    for (int s2 = 0; s2 < S; ++s2) {
-                        const float v = Wt[((((size_t)g * cout_g + o) * cin_g + c) * R + r) * S + s2];
-                        const size_t k = im2col ? (size_t)((r * S + s2) * cin_g + c) : ((size_t)(r * S + s2) * ecin + c);
-                        w[((size_t)g * cout_pad + o) * K + k] = tf32_round(v);
-                    }
-        }
-    HP_CUDA_TRY(cudaMalloc(&pl.d_w32, w.size() * sizeof(float)));
-    HP_CUDA_TRY(cudaMalloc(&pl.d_bias, bias.size() * sizeof(float)));
-    HP_CUDA_TRY(cudaMalloc(&pl.d_alpha, alpha.size() * sizeof(float)));
-    HP_CUDA_TRY(cudaMemcpy(pl.d_w32, w.data(), w.size() * sizeof(float), cudaMemcpyHostToDevice));
-    HP_CUDA_TRY(cudaMemcpy(pl.d_bias, bias.data(), bias.size() * sizeof(float), cudaMemcpyHostToDevice));
-    HP_CUDA_TRY(cudaMemcpy(pl.d_alpha, alpha.data(), alpha.size() * sizeof(float), cudaMemcpyHostToDevice));
-
-    ConvParams& p = pl.prm;
-    memset(&p, 0, sizeof(p));
-    p.Nb = e->max_batch; p.H = ib.H; p.W = ib.W;
-    p.R = eR; p.S = eS; p.groups = G; p.cin_g = ecin;
-    p.cout_g = cout_g; p.cout_g_pad = cout_pad; p.BN = BN;
-    p.m_tiles = (int)(((size_t)e->max_batch * p.H * p.W + CONV_BLOCK_M - 1) / CONV_BLOCK_M);
-    p.in_ch_off = (int)po.in_ch_off;
-    p.bias = pl.d_bias; p.alpha = pl.d_alpha;
-    p.out_mode = (int)po.out_mode;
-    if (po.out_mode == OUT_F32_NCHW_SPLIT) {
-        p.out = e->d_conf; p.out2 = e->d_paf; p.split = (int)po.split;
-        if ((int)po.split != (int)e->hdr.conf_channels || cout_g - (int)po.split != (int)e->hdr.paf_channels || G != 1) {
-            set_error("engine: output conv must produce conf(%u)+paf(%u) channels", e->hdr.conf_channels, e->hdr.paf_channels);
-            return HP_ERR_ARG;
-        }
-    } else {
-        const EngBuffer& ob = e->bufs[po.out_buf];
-        if (ob.H != ib.H || ob.W != ib.W || (int)po.out_ch_off + G * cout_g > ob.channels) { set_error("engine: conv output buffer mismatch"); return HP_ERR_ARG; }
-        p.out = ob.d; p.out_ld = ob.channels; p.out_ch_off = (int)po.out_ch_off;
-    }
-    if (po.res_mode) {
-        if (po.out_mode != OUT_F16_NHWC || po.res_buf >= e->bufs.size()) { set_error("engine: bad residual"); return HP_ERR_ARG; }
-        const EngBuffer& rb = e->bufs[po.res_buf];
-        if (rb.H != ib.H || rb.W != ib.W || (int)po.res_ch_off + G * cout_g > rb.channels || po.res_ch_off % 8 || cout_g % 16) { set_error("engine: residual buffer mismatch"); return HP_ERR_ARG; }
-        p.res = rb.d; p.res_ld = rb.channels; p.res_ch_off = (int)po.res_ch_off; p.res_mode = (int)po.res_mode;
-    }
-    p.num_stages = conv_pick_stages(BN);
-    int rc = make_tmap_act_im2col(&pl.tmap_a, ib.d, e->max_batch, ib.H, ib.W, ib.channels, eR, eS, CONV_BLOCK_M, true);
-    if (rc) return rc;
-    rc = make_tmap_wgt(&pl.tmap_b, pl.d_w32, G * cout_pad, K, BN, true);
-    if (rc) return rc;
-    pl.smem = conv_smem_bytes(BN, p.num_stages);
-    pl.flops_per_frame = 2.0 * ib.H * ib.W * (double)G * cout_g * cin_g * R * S;
-    return HP_OK;
-}
-
-int build_conv_plan(hp_engine* e, EngOp& op, const float* blob)
-{
-    if (e->dtype == HP_DTYPE_TF32) return build_conv_plan_tf32(e, op, blob);
-    const PackOp& po = op.po;
-    ConvPlan& pl = op.plan;
-    const EngBuffer& ib = e->bufs[po.in_buf];
-    const int G = (int)po.groups;
-    int R = (int)po.R, S = (int)po.S, cin_g = (int)po.cin_g;
-    const int cout_g = (int)po.cout_g;
-    const bool im2col = po.im2col_input != 0;
-    if (im2col && (G != 1 || R * S * cin_g > ib.channels)) { set_error("engine: bad im2col conv"); return HP_ERR_ARG; }
-    if (!im2col && G > 1 && cin_g % 64 != 0) { set_error("engine: grouped conv needs cin_g %% 64 == 0 (got %d)", cin_g); return HP_ERR_UNSUPPORTED; }
+    if (!im2col && G > 1 && cin_g % chunk != 0) { set_error("engine: grouped conv needs cin_g %% %d == 0 (got %d)", chunk, cin_g); return HP_ERR_UNSUPPORTED; }
     // effective GEMM view
     const int eR = im2col ? 1 : R, eS = im2col ? 1 : S;
-    const int ecin = im2col ? round_up(R * S * cin_g, 64) : round_up(cin_g, 64);
-    if ((int)po.in_ch_off + (G - 1) * ecin + ecin > ib.channels) {
+    const int ecin = im2col ? round_up(R * S * cin_g, chunk) : round_up(cin_g, chunk);
+    if ((int)po.in_ch_off + G * ecin > ib.channels) {
         set_error("engine: conv reads channels [%d,%d) of a %d-channel buffer", po.in_ch_off, po.in_ch_off + G * ecin, ib.channels);
         return HP_ERR_ARG;
     }
     const int BN = pick_bn(cout_g);
     const int cout_pad = round_up(cout_g, BN);
     const int K = eR * eS * ecin;
-    // repack fp32 [G][cout][cin][R][S] -> fp16 [G][cout_pad][R][S][cin_pad]
-    std::vector<__half> w((size_t)G * cout_pad * K, __float2half(0.f));
-    std::vector<float> bias((size_t)G * cout_pad, 0.f), alpha((size_t)G * cout_pad, 0.f);
+    // repack fp32 [G][cout][cin][R][S] -> [G][cout_pad][R][S][cin_pad]
+    std::vector<float> w((size_t)G * cout_pad * K, 0.f), bias((size_t)G * cout_pad, 0.f), alpha((size_t)G * cout_pad, 0.f);
     const float* W = blob + po.w_off;
     for (int g = 0; g < G; ++g)
         for (int o = 0; o < cout_g; ++o) {
@@ -904,13 +766,18 @@ int build_conv_plan(hp_engine* e, EngOp& op, const float* blob)
                     for (int s = 0; s < S; ++s) {
                         const float v = W[((((size_t)g * cout_g + o) * cin_g + c) * R + r) * S + s];
                         const size_t k = im2col ? (size_t)((r * S + s) * cin_g + c) : ((size_t)(r * S + s) * ecin + c);
-                        w[((size_t)g * cout_pad + o) * K + k] = __float2half_rn(v);
+                        w[((size_t)g * cout_pad + o) * K + k] = tf32 ? tf32_round(v) : v;
                     }
         }
-    HP_CUDA_TRY(cudaMalloc(&pl.d_w, w.size() * sizeof(__half)));
+    std::vector<__half> wh;
+    if (!tf32) {
+        wh.resize(w.size());
+        for (size_t i = 0; i < w.size(); ++i) wh[i] = __float2half_rn(w[i]);
+    }
+    HP_CUDA_TRY(cudaMalloc(&pl.d_w, w.size() * es));
     HP_CUDA_TRY(cudaMalloc(&pl.d_bias, bias.size() * sizeof(float)));
     HP_CUDA_TRY(cudaMalloc(&pl.d_alpha, alpha.size() * sizeof(float)));
-    HP_CUDA_TRY(cudaMemcpy(pl.d_w, w.data(), w.size() * sizeof(__half), cudaMemcpyHostToDevice));
+    HP_CUDA_TRY(cudaMemcpy(pl.d_w, tf32 ? (const void*)w.data() : (const void*)wh.data(), w.size() * es, cudaMemcpyHostToDevice));
     HP_CUDA_TRY(cudaMemcpy(pl.d_bias, bias.data(), bias.size() * sizeof(float), cudaMemcpyHostToDevice));
     HP_CUDA_TRY(cudaMemcpy(pl.d_alpha, alpha.data(), alpha.size() * sizeof(float), cudaMemcpyHostToDevice));
 
@@ -941,54 +808,37 @@ int build_conv_plan(hp_engine* e, EngOp& op, const float* blob)
         if (rb.H != ib.H || rb.W != ib.W || (int)po.res_ch_off + G * cout_g > rb.channels || po.res_ch_off % 8 || cout_g % 16) { set_error("engine: residual buffer mismatch"); return HP_ERR_ARG; }
         p.res = rb.d; p.res_ld = rb.channels; p.res_ch_off = (int)po.res_ch_off; p.res_mode = (int)po.res_mode;
     }
-    int rc = make_tmap_act_im2col(&pl.tmap_a, ib.d, e->max_batch, ib.H, ib.W, ib.channels, eR, eS);
+    int rc = make_tmap_act_im2col(&pl.tmap_a, ib.d, e->max_batch, ib.H, ib.W, ib.channels, eR, eS, tf32);
     if (rc) return rc;
-    rc = make_tmap_wgt(&pl.tmap_b, pl.d_w, G * cout_pad, K, BN);
+    rc = make_tmap_wgt(&pl.tmap_b, pl.d_w, G * cout_pad, K, BN, tf32);
     if (rc) return rc;
     pl.smem = conv_smem_bytes(BN, p.num_stages);
     pl.flops_per_frame = 2.0 * ib.H * ib.W * (double)G * cout_g * cin_g * R * S;
+    op.launch = Launch::Conv;
+    if (tf32) return HP_OK;
     pl.monotone_act = true;
     for (float a : alpha) if (!(a >= 0.f)) { pl.monotone_act = false; break; }
     // Halo-box kernel for RxS layers whose 16 x 8 tile grid wastes little of the image (the early VGG layers): the A operand comes
-    // from L2 once per chunk instead of once per tap.  HPB_HALO=0 disables it, HPB_HALO=all takes every eligible layer.
-    {
-        const char* hv = getenv("HPB_HALO");
-        const int ty = (ib.H + HALO_TH - 1) / HALO_TH, tx = (ib.W + HALO_TW - 1) / HALO_TW;
-        const double waste = (double)ty * HALO_TH * tx * HALO_TW / ((double)ib.H * ib.W) - 1.0;
-        const bool shape_ok = !im2col && eR == eS && (eR == 3 || eR == 5 || eR == 7) && !po.res_mode && po.out_mode == OUT_F16_NHWC;
-        const bool want = hv ? (strcmp(hv, "all") == 0) : (eR == 3 && waste <= 0.06);
-        if (shape_ok && want) {
-            const EngBuffer& ob = e->bufs[po.out_buf];
-            HaloParams& h = pl.hp;
-            memset(&h, 0, sizeof(h));
-            h.Nb = e->max_batch; h.H = ib.H; h.W = ib.W; h.R = eR; h.S = eS; h.groups = G; h.cin_g = ecin;
-            h.cout_g = cout_g; h.cout_g_pad = cout_pad; h.in_ch_off = (int)po.in_ch_off;
-            h.tiles_x = tx; h.tiles_y = ty;
-            h.box_bytes = halo_box_bytes(eR, eS);
-            h.num_stages = conv_halo_pick_stages(eR, eS, BN);
-            h.bias = pl.d_bias; h.alpha = pl.d_alpha;
-            h.out = ob.d; h.out_ld = ob.channels; h.out_ch_off = (int)po.out_ch_off;
-            rc = make_tmap_act_box(&pl.tmap_x, ib.d, e->max_batch, ib.H, ib.W, ib.channels, HALO_TW + eS - 1, HALO_TH + eR - 1);
-            if (rc) return rc;
-            pl.halo = true;
-            pl.smem = conv_halo_smem_bytes(eR, eS, BN, h.num_stages);
-        }
-    }
-    // Fused stem: the first conv reads the u8 frames itself, the im2col buffer is never written.  HPB_NO_STEM3 keeps the im2col
-    // buffer for 3x3 stems, HPB_NO_STEM for every stem.
-    if (im2col && !po.res_mode && po.out_mode == OUT_F16_NHWC && R == S && (R == 7 || (R == 3 && !getenv("HPB_NO_STEM3"))) && !getenv("HPB_NO_STEM")) {
-        for (auto& o2 : e->ops) {   // the patch-gather op feeding this conv: its stride / tap size define the stem geometry
-            if (o2.po.type != OP_IM2COL3 || o2.po.out_buf != po.in_buf) continue;
-            if ((int)(o2.po.R ? o2.po.R : 3) != R || cin_g != 3) break;
-            const int stride = o2.po.stride ? (int)o2.po.stride : 1;
-            p.in_h = e->in_h; p.in_w = e->in_w; p.stem_stride = stride;
-            p.stem_pad_h = same_pad_before(e->in_h, R, stride); p.stem_pad_w = same_pad_before(e->in_w, R, stride);
-            p.factor = e->factor; p.flip = e->flip_rgb;
-            p.mean[0] = e->hdr.mean[0]; p.mean[1] = e->hdr.mean[1]; p.mean[2] = e->hdr.mean[2];
-            pl.stem_R = R;
-            o2.fused_into_stem = true;
-            break;
-        }
+    // from L2 once per chunk instead of once per tap.
+    const int ty = (ib.H + HALO_TH - 1) / HALO_TH, tx = (ib.W + HALO_TW - 1) / HALO_TW;
+    const double waste = (double)ty * HALO_TH * tx * HALO_TW / ((double)ib.H * ib.W) - 1.0;
+    const bool shape_ok = !im2col && eR == eS && (eR == 3 || eR == 5 || eR == 7) && !po.res_mode && po.out_mode == OUT_F16_NHWC;
+    const bool want = e->opt.halo == EngOptions::HALO_AUTO ? (eR == 3 && waste <= 0.06) : e->opt.halo == EngOptions::HALO_ALL;
+    if (shape_ok && want) {
+        const EngBuffer& ob = e->bufs[po.out_buf];
+        HaloParams& h = pl.hp;
+        memset(&h, 0, sizeof(h));
+        h.Nb = e->max_batch; h.H = ib.H; h.W = ib.W; h.R = eR; h.S = eS; h.groups = G; h.cin_g = ecin;
+        h.cout_g = cout_g; h.cout_g_pad = cout_pad; h.in_ch_off = (int)po.in_ch_off;
+        h.tiles_x = tx; h.tiles_y = ty;
+        h.box_bytes = halo_box_bytes(eR, eS);
+        h.num_stages = conv_halo_pick_stages(eR, eS, BN);
+        h.bias = pl.d_bias; h.alpha = pl.d_alpha;
+        h.out = ob.d; h.out_ld = ob.channels; h.out_ch_off = (int)po.out_ch_off;
+        rc = make_tmap_act_box(&pl.tmap_x, ib.d, e->max_batch, ib.H, ib.W, ib.channels, ib.channels, HALO_TW + eS - 1, HALO_TH + eR - 1, CU_TENSOR_MAP_SWIZZLE_128B);
+        if (rc) return rc;
+        op.launch = Launch::Halo;
+        pl.smem = conv_halo_smem_bytes(eR, eS, BN, h.num_stages);
     }
     return HP_OK;
 }
@@ -997,7 +847,7 @@ int build_conv_plan(hp_engine* e, EngOp& op, const float* blob)
 // the previous kernel of the stream has already left, and orders itself behind that kernel's completion with griddepcontrol.wait
 // before it touches memory.  The persistent conv kernels trigger their dependents at their own start.  It pays where a step is a
 // chain of short kernels and costs where they are long, so the engine turns it on by itself when the mean work per launch is small
-// (hp_engine::use_pdl, decided at creation); HPB_PDL=0|1 overrides.
+// (hp_engine::use_pdl, decided at creation).
 thread_local bool tl_use_pdl = false;   // set by the op loop from hp_engine::use_pdl for the launches it issues on this thread
 static inline cudaLaunchConfig_t pdl_config(int grid, int block, size_t smem, cudaStream_t st, cudaLaunchAttribute* at)
 {
@@ -1063,33 +913,30 @@ void launch_dw_tma(hp_engine* e, const EngOp& op, const EngOp* pair, int N, cuda
     p.out1 = pair ? e->bufs[pair->po.out_buf].d + pair->po.out_ch_off : nullptr;
     p.out_ld = ob.channels;
     p.w0 = op.d_dw; p.w1 = pair ? pair->d_dw : nullptr;
-    p.N = N; p.H = ib.H; p.W = ib.W; p.C = (int)po.cout_g; p.ctiles = p.C / 64;
+    p.H = ib.H; p.W = ib.W; p.C = (int)po.cout_g; p.ctiles = p.C / 64;
     p.tiles_x = op.dwt_tiles_x; p.tiles_y = op.dwt_tiles_y; p.wbo = op.dwt_wbo; p.hb = op.dwt_hb; p.stages = op.dwt_stages;
     p.n_items = N * p.tiles_y * p.tiles_x * p.ctiles;
     const int grid = std::min(p.n_items, std::max(1, e->num_sms - e->reserve_sms));
-    static const int threads = getenv("HPB_DWT_THREADS") ? std::max(32, std::min(DWT_THREADS, atoi(getenv("HPB_DWT_THREADS")) / 32 * 32)) : DWT_THREADS;
-    static const int order = getenv("HPB_DWT_ORDER") ? atoi(getenv("HPB_DWT_ORDER")) : 1;   // channel tile fastest: concurrent CTAs read whole pixels
-    p.ct_fastest = order;
-    if (pair) launch_pdl(dwconv3_tma_kernel<2>, grid, threads, op.dwt_smem, st, op.tmap_dw, p);
-    else      launch_pdl(dwconv3_tma_kernel<1>, grid, threads, op.dwt_smem, st, op.tmap_dw, p);
+    if (pair) launch_pdl(dwconv3_tma_kernel<2>, grid, DWT_THREADS, op.dwt_smem, st, op.tmap_dw, p);
+    else      launch_pdl(dwconv3_tma_kernel<1>, grid, DWT_THREADS, op.dwt_smem, st, op.tmap_dw, p);
 }
 
+// conv_wgmma_kernel, or conv_halo_kernel for Launch::Halo / HaloPool
 int launch_conv(hp_engine* e, EngOp& op, int N, cudaStream_t st, bool u8_input)
 {
     ConvPlan& pl = op.plan;
     ConvParams p = pl.prm;
     p.Nb = N;
-    const int stem_R = u8_input ? pl.stem_R : 0;
+    const int stem_R = op.launch == Launch::ConvStem && u8_input ? (int)op.po.R : 0;
     p.frames = e->cur_frames ? e->cur_frames : e->d_frames;
-    if (pl.halo) {
+    if (op.launch == Launch::Halo || op.launch == Launch::HaloPool) {
         HaloParams h = pl.hp;
         h.Nb = N;
         const long items = (long)N * h.tiles_x * h.tiles_y * h.groups * (h.cout_g_pad / p.BN);
         cudaLaunchAttribute at[1];
         const cudaLaunchConfig_t cfg = pdl_config((int)std::min<long>(e->num_sms - e->reserve_sms, items), CONV_THREADS, pl.smem, st, at);
         void* args[] = { (void*)&pl.tmap_x, (void*)&pl.tmap_b, (void*)&h };
-        HP_CUDA_TRY(cudaLaunchKernelExC(&cfg, halo_kernel(pl.pool_fused, p.BN), args));
-        e->launches++;
+        HP_CUDA_TRY(cudaLaunchKernelExC(&cfg, halo_kernel(op.launch == Launch::HaloPool, p.BN), args));
         return HP_OK;
     }
     p.m_tiles = (int)(((size_t)N * p.H * p.W + CONV_BLOCK_M - 1) / CONV_BLOCK_M);
@@ -1098,8 +945,7 @@ int launch_conv(hp_engine* e, EngOp& op, int N, cudaStream_t st, bool u8_input)
     cudaLaunchAttribute at[1];
     const cudaLaunchConfig_t cfg = pdl_config(grid, CONV_THREADS, pl.smem, st, at);
     void* args[] = { (void*)&pl.tmap_a, (void*)&pl.tmap_b, (void*)&p };
-    HP_CUDA_TRY(cudaLaunchKernelExC(&cfg, conv_kernel(pl.tf32, p.res_mode != 0, p.BN, stem_R), args));
-    e->launches++;
+    HP_CUDA_TRY(cudaLaunchKernelExC(&cfg, conv_kernel(e->dtype == HP_DTYPE_TF32, p.res_mode != 0, p.BN, stem_R), args));
     return HP_OK;
 }
 
@@ -1125,47 +971,16 @@ void collect_profile(hp_engine* e)
     while (collect_one(e, true)) {}
 }
 
-// every non-conv op of the graph on fp32 activation buffers (data_type::kFLOAT engine)
-void run_helper_op_tf32(hp_engine* e, EngOp& op, int N, bool u8_input, cudaStream_t st)
+// the OpenPifPaf head op: pif fields [N,17,5,h,w] from in_buf, paf fields [N,19,9,h,w] from res_buf
+template <typename T>
+void launch_heads(hp_engine* e, const PackOp& po, int N, cudaStream_t st)
 {
-    const PackOp& po = op.po;
-    if (po.type == OP_IM2COL3) {
-        EngBuffer& ob = e->bufs[po.out_buf];
-        const int R = po.R ? (int)po.R : 3, stride = po.stride ? (int)po.stride : 1;
-        const int ph = same_pad_before(e->in_h, R, stride), pw = same_pad_before(e->in_w, R, stride);
-        const size_t total = (size_t)N * ob.H * ob.W * (ob.channels / 4);
-        const unsigned blocks = (unsigned)((total + 255) / 256);
-        const uint8_t* fr = e->cur_frames ? e->cur_frames : e->d_frames;
-        if (u8_input) im2col_f32_kernel<true><<<blocks, 256, 0, st>>>(fr, (float*)ob.d, N, e->in_h, e->in_w, e->factor, e->flip_rgb, e->hdr.mean[0], e->hdr.mean[1], e->hdr.mean[2],
-                                                                     R, stride, ob.H, ob.W, ph, pw, ob.channels);
-        else im2col_f32_kernel<false><<<blocks, 256, 0, st>>>(e->d_input_f32, (float*)ob.d, N, e->in_h, e->in_w, 1.0, 0, e->hdr.mean[0], e->hdr.mean[1], e->hdr.mean[2],
-                                                              R, stride, ob.H, ob.W, ph, pw, ob.channels);
-        e->launches++;
-    } else if (po.type == OP_PIFPAF_HEAD) {
-        EngBuffer& a = e->bufs[po.in_buf];
-        EngBuffer& b = e->bufs[po.res_buf];
-        const size_t t1 = (size_t)N * 17 * 5 * e->out_h * e->out_w, t2 = (size_t)N * 19 * 9 * e->out_h * e->out_w;
-        pifpaf_head_kernel<float><<<(int)((t1 + 255) / 256), 256, 0, st>>>((const float*)a.d, a.channels, e->d_conf, N, a.H, a.W, 17, 5, e->out_h, e->out_w, 0);
-        pifpaf_head_kernel<float><<<(int)((t2 + 255) / 256), 256, 0, st>>>((const float*)b.d, b.channels, e->d_paf, N, b.H, b.W, 19, 9, e->out_h, e->out_w, 1);
-        e->launches += 2;
-    } else if (po.type == OP_DWCONV) {
-        EngBuffer& ib = e->bufs[po.in_buf];
-        EngBuffer& ob = e->bufs[po.out_buf];
-        const int C = (int)po.cout_g, K = (int)po.R, stride = po.stride ? (int)po.stride : 1;
-        const size_t total = (size_t)N * ob.H * ob.W * (C / 4);
-        const float* dw = op.d_dw;
-        dwconv_f32_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>((const float*)ib.d + po.in_ch_off, ib.channels, (float*)ob.d + po.out_ch_off, ob.channels, dw,
-            dw + (size_t)K * K * C, dw + (size_t)K * K * C + C, N, ib.H, ib.W, C, ob.H, ob.W, K, stride, same_pad_before(ib.H, K, stride), same_pad_before(ib.W, K, stride));
-        e->launches++;
-    } else if (po.type == OP_MAXPOOL2) {
-        EngBuffer& ib = e->bufs[po.in_buf];
-        EngBuffer& ob = e->bufs[po.out_buf];
-        const int C = (int)po.cout_g, K = po.R ? (int)po.R : 2;
-        const size_t total = (size_t)N * ob.H * ob.W * (C / 4);
-        maxpool_f32_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>((const float*)ib.d + po.in_ch_off, (float*)ob.d + po.out_ch_off, N, ib.H, ib.W, ib.channels, C, ob.channels,
-                                                                           ob.H, ob.W, K, same_pad_before(ib.H, K, 2), same_pad_before(ib.W, K, 2));
-        e->launches++;
-    }
+    if (e->heads_wait) cudaStreamWaitEvent(st, e->heads_wait, 0);   // the previous batch's decoder has read the field tensors
+    const EngBuffer& a = e->bufs[po.in_buf];
+    const EngBuffer& b = e->bufs[po.res_buf];
+    const size_t t1 = (size_t)N * 17 * 5 * e->out_h * e->out_w, t2 = (size_t)N * 19 * 9 * e->out_h * e->out_w;
+    pifpaf_head_kernel<T><<<(int)((t1 + 255) / 256), 256, 0, st>>>((const T*)a.d, a.channels, e->d_conf, N, a.H, a.W, 17, 5, e->out_h, e->out_w, 0);
+    pifpaf_head_kernel<T><<<(int)((t2 + 255) / 256), 256, 0, st>>>((const T*)b.d, b.channels, e->d_paf, N, b.H, b.W, 19, 9, e->out_h, e->out_w, 1);
 }
 
 int run_graph(hp_engine* e, int N, bool u8_input, cudaStream_t st, int first = 0, int last = -1)
@@ -1180,99 +995,119 @@ int run_graph(hp_engine* e, int N, bool u8_input, cudaStream_t st, int first = 0
         cudaEventRecord(evset[0], st);
     }
     tl_use_pdl = e->use_pdl;
+    const uint8_t* frames = e->cur_frames ? e->cur_frames : e->d_frames;
     for (int oi = first; oi <= last; ++oi) {
         EngOp& op = e->ops[oi];
         const PackOp& po = op.po;
-        if (e->dtype == HP_DTYPE_TF32 && po.type != OP_CONV) {
-            run_helper_op_tf32(e, op, N, u8_input, st);
-        } else if (po.type == OP_IM2COL3 && op.fused_into_stem && u8_input) {
-            // the consumer gathers its patches from the frames itself: nothing to do here
-        } else if (po.type == OP_IM2COL3) {
-            EngBuffer& ob = e->bufs[po.out_buf];
-            const int R = po.R ? (int)po.R : 3;
-            const int chunks = ob.channels / 64;
-            const size_t total = (size_t)N * ob.H * ob.W;
-            const dim3 blocks((unsigned)((total + 255) / 256), (unsigned)chunks);
-            const int stride = po.stride ? (int)po.stride : 1;
+        const int K = (int)po.R, stride = po.stride ? (int)po.stride : 1;
+        switch (op.launch) {
+        case Launch::None:
+            break;
+        case Launch::StemOrIm2col:
+            if (u8_input) break;   // the consumer conv gathers its patches from the frames itself
+            [[fallthrough]];
+        case Launch::Im2col: {
+            const EngBuffer& ob = e->bufs[po.out_buf];
+            const int R = K ? K : 3, chunks = ob.channels / 64;
+            const dim3 blocks((unsigned)(((size_t)N * ob.H * ob.W + 255) / 256), (unsigned)chunks);
             const int ph = same_pad_before(e->in_h, R, stride), pw = same_pad_before(e->in_w, R, stride);
 #define HP_IM2COL(U8, RR, SRC, FAC, FLIP) im2col3_kernel<U8, RR><<<blocks, 256, 0, st>>>(SRC, ob.d, N, e->in_h, e->in_w, FAC, FLIP, \
                 e->hdr.mean[0], e->hdr.mean[1], e->hdr.mean[2], stride, ob.H, ob.W, ph, pw, chunks)
-            const uint8_t* fr = e->cur_frames ? e->cur_frames : e->d_frames;
-            if (u8_input) { if (R == 3) HP_IM2COL(true, 3, fr, e->factor, e->flip_rgb); else HP_IM2COL(true, 7, fr, e->factor, e->flip_rgb); }
+            if (u8_input) { if (R == 3) HP_IM2COL(true, 3, frames, e->factor, e->flip_rgb); else HP_IM2COL(true, 7, frames, e->factor, e->flip_rgb); }
             else          { if (R == 3) HP_IM2COL(false, 3, e->d_input_f32, 1.0, 0); else HP_IM2COL(false, 7, e->d_input_f32, 1.0, 0); }
 #undef HP_IM2COL
-            e->launches++;
-        } else if (po.type == OP_PIFPAF_HEAD) {
-            if (e->heads_wait) cudaStreamWaitEvent(st, e->heads_wait, 0);   // the previous batch's decoder has read the field tensors
-            EngBuffer& a = e->bufs[po.in_buf];
-            EngBuffer& b = e->bufs[po.res_buf];
-            const size_t t1 = (size_t)N * 17 * 5 * e->out_h * e->out_w, t2 = (size_t)N * 19 * 9 * e->out_h * e->out_w;
-            pifpaf_head_kernel<__half><<<(int)((t1 + 255) / 256), 256, 0, st>>>(a.d, a.channels, e->d_conf, N, a.H, a.W, 17, 5, e->out_h, e->out_w, 0);
-            pifpaf_head_kernel<__half><<<(int)((t2 + 255) / 256), 256, 0, st>>>(b.d, b.channels, e->d_paf, N, b.H, b.W, 19, 9, e->out_h, e->out_w, 1);
-            e->launches += 2;
-        } else if (po.type == OP_DWCONV && op.fused_into_prev) {
-            // served by the dual launch of the depthwise op before it
-        } else if (po.type == OP_DWCONV && op.dual_with_next) {
-            EngBuffer& ib = e->bufs[po.in_buf];
-            EngBuffer& ob = e->bufs[po.out_buf];
-            const EngOp& nx = e->ops[oi + 1];
+            break;
+        }
+        case Launch::Conv: case Launch::ConvStem: case Launch::Halo: case Launch::HaloPool:
+            launch_conv(e, op, N, st, u8_input);
+            break;
+        case Launch::DwTma:
+            launch_dw_tma(e, op, nullptr, N, st);
+            break;
+        case Launch::DwTmaPair:
+            launch_dw_tma(e, op, &e->ops[oi + 1], N, st);
+            break;
+        case Launch::DwCol: {
+            // column-marching kernel: enough row chunks to give every SM a few blocks
+            const EngBuffer& ib = e->bufs[po.in_buf];
+            const EngBuffer& ob = e->bufs[po.out_buf];
             const int C = (int)po.cout_g;
-            if (op.dw_tma) {
-                launch_dw_tma(e, op, &nx, N, st);
-            } else {
-                const size_t base = ((size_t)N * ib.W * (C / 2) + 255) / 256;
-                int chunks = (int)((4 * (size_t)e->num_sms + base - 1) / base);
-                chunks = std::max(1, std::min(chunks, std::max(1, ib.H / 4)));
-                const int rows = (ib.H + chunks - 1) / chunks;
-                chunks = (ib.H + rows - 1) / rows;
-                const size_t tot = (size_t)N * chunks * ib.W * (C / 2);
-                dwconv3_col_dual_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, st>>>(ib.d + po.in_ch_off, ib.channels, ob.d + po.out_ch_off, ob.d + nx.po.out_ch_off, ob.channels,
-                    op.d_dw, nx.d_dw, N, ib.H, ib.W, C, rows, chunks);
-            }
-            e->launches++;
-        } else if (po.type == OP_DWCONV) {
-            EngBuffer& ib = e->bufs[po.in_buf];
-            EngBuffer& ob = e->bufs[po.out_buf];
-            const int C = (int)po.cout_g, K = (int)po.R, stride = po.stride ? (int)po.stride : 1;
+            const size_t base = ((size_t)N * ib.W * (C / 4) + 255) / 256;
+            int chunks = (int)((4 * (size_t)e->num_sms + base - 1) / base);
+            chunks = std::max(1, std::min(chunks, std::max(1, ib.H / 4)));
+            const int rows = (ib.H + chunks - 1) / chunks;
+            chunks = (ib.H + rows - 1) / rows;
+            const size_t tot = (size_t)N * chunks * ib.W * (C / 4);
+            dwconv3_col_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, st>>>(ib.d + po.in_ch_off, ib.channels, ob.d + po.out_ch_off, ob.channels, op.d_dw,
+                op.d_dw + (size_t)9 * C, op.d_dw + (size_t)9 * C + C, N, ib.H, ib.W, C, rows, chunks);
+            break;
+        }
+        case Launch::DwStrip: {   // 3x3 / stride 2 and 1x1
+            const EngBuffer& ib = e->bufs[po.in_buf];
+            const EngBuffer& ob = e->bufs[po.out_buf];
+            const int C = (int)po.cout_g;
             const size_t total = (size_t)N * ob.H * ((ob.W + DW_STRIP - 1) / DW_STRIP) * (C / 8);
             const int blocks = (int)((total + 255) / 256);
             const float* dw = op.d_dw;
 #define HP_DW(KK, SS) dwconv_kernel<KK, SS><<<blocks, 256, 0, st>>>(ib.d + po.in_ch_off, ib.channels, ob.d + po.out_ch_off, ob.channels, dw, \
                 dw + (size_t)KK * KK * C, dw + (size_t)KK * KK * C + C, N, ib.H, ib.W, C, ob.H, ob.W, same_pad_before(ib.H, KK, SS), same_pad_before(ib.W, KK, SS))
-            if (op.dw_tma) {
-                launch_dw_tma(e, op, nullptr, N, st);
-            } else if (K == 3 && stride == 1 && !getenv("HPB_DW_STRIP")) {
-                // column-marching kernel: enough row chunks to give every SM a few blocks
-                const size_t base = ((size_t)N * ib.W * (C / 4) + 255) / 256;
-                int chunks = (int)((4 * (size_t)e->num_sms + base - 1) / base);
-                chunks = std::max(1, std::min(chunks, std::max(1, ib.H / 4)));
-                const int rows = (ib.H + chunks - 1) / chunks;
-                chunks = (ib.H + rows - 1) / rows;
-                const size_t tot = (size_t)N * chunks * ib.W * (C / 4);
-                dwconv3_col_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, st>>>(ib.d + po.in_ch_off, ib.channels, ob.d + po.out_ch_off, ob.channels, dw,
-                    dw + (size_t)9 * C, dw + (size_t)9 * C + C, N, ib.H, ib.W, C, rows, chunks);
-            } else if (K == 3) { if (stride == 2) HP_DW(3, 2); else HP_DW(3, 1); }
-            else        { if (stride == 2) HP_DW(1, 2); else HP_DW(1, 1); }
+            if (K == 3) HP_DW(3, 2);
+            else if (stride == 2) HP_DW(1, 2);
+            else HP_DW(1, 1);
 #undef HP_DW
-            e->launches++;
-        } else if (po.type == OP_MAXPOOL2 && op.fused_into_prev) {
-            // taken in the epilogue of the conv before it
-        } else if (po.type == OP_MAXPOOL2) {
-            EngBuffer& ib = e->bufs[po.in_buf];
-            EngBuffer& ob = e->bufs[po.out_buf];
-            const int C = (int)po.cout_g;
-            const size_t total = (size_t)N * ob.H * ob.W * (C / 8);
-            const int K = po.R ? (int)po.R : 2;
-            if (K == 3)
-                maxpool2_kernel<3><<<(int)((total + 255) / 256), 256, 0, st>>>(ib.d + po.in_ch_off, ob.d + po.out_ch_off, N, ib.H, ib.W, ib.channels, C, ob.channels, ob.H, ob.W,
-                                                                            same_pad_before(ib.H, 3, 2), same_pad_before(ib.W, 3, 2));
-            else
-                maxpool2_kernel<2><<<(int)((total + 255) / 256), 256, 0, st>>>(ib.d + po.in_ch_off, ob.d + po.out_ch_off, N, ib.H, ib.W, ib.channels, C, ob.channels, ob.H, ob.W,
-                                                                            same_pad_before(ib.H, 2, 2), same_pad_before(ib.W, 2, 2));
-            e->launches++;
-        } else if (po.type == OP_CONV) {
-            launch_conv(e, op, N, st, u8_input);
+            break;
         }
+        case Launch::MaxPool: {
+            const EngBuffer& ib = e->bufs[po.in_buf];
+            const EngBuffer& ob = e->bufs[po.out_buf];
+            const int C = (int)po.cout_g;
+            const int blocks = (int)(((size_t)N * ob.H * ob.W * (C / 8) + 255) / 256);
+            if (K == 3)
+                maxpool2_kernel<3><<<blocks, 256, 0, st>>>(ib.d + po.in_ch_off, ob.d + po.out_ch_off, N, ib.H, ib.W, ib.channels, C, ob.channels, ob.H, ob.W,
+                                                           same_pad_before(ib.H, 3, 2), same_pad_before(ib.W, 3, 2));
+            else
+                maxpool2_kernel<2><<<blocks, 256, 0, st>>>(ib.d + po.in_ch_off, ob.d + po.out_ch_off, N, ib.H, ib.W, ib.channels, C, ob.channels, ob.H, ob.W,
+                                                           same_pad_before(ib.H, 2, 2), same_pad_before(ib.W, 2, 2));
+            break;
+        }
+        case Launch::Heads:
+            launch_heads<__half>(e, po, N, st);
+            break;
+        case Launch::Im2colF32: {
+            const EngBuffer& ob = e->bufs[po.out_buf];
+            const int R = K ? K : 3;
+            const int ph = same_pad_before(e->in_h, R, stride), pw = same_pad_before(e->in_w, R, stride);
+            const unsigned blocks = (unsigned)(((size_t)N * ob.H * ob.W * (ob.channels / 4) + 255) / 256);
+            if (u8_input) im2col_f32_kernel<true><<<blocks, 256, 0, st>>>(frames, (float*)ob.d, N, e->in_h, e->in_w, e->factor, e->flip_rgb, e->hdr.mean[0], e->hdr.mean[1], e->hdr.mean[2],
+                                                                         R, stride, ob.H, ob.W, ph, pw, ob.channels);
+            else im2col_f32_kernel<false><<<blocks, 256, 0, st>>>(e->d_input_f32, (float*)ob.d, N, e->in_h, e->in_w, 1.0, 0, e->hdr.mean[0], e->hdr.mean[1], e->hdr.mean[2],
+                                                                  R, stride, ob.H, ob.W, ph, pw, ob.channels);
+            break;
+        }
+        case Launch::DwF32: {
+            const EngBuffer& ib = e->bufs[po.in_buf];
+            const EngBuffer& ob = e->bufs[po.out_buf];
+            const int C = (int)po.cout_g;
+            const size_t total = (size_t)N * ob.H * ob.W * (C / 4);
+            const float* dw = op.d_dw;
+            dwconv_f32_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>((const float*)ib.d + po.in_ch_off, ib.channels, (float*)ob.d + po.out_ch_off, ob.channels, dw,
+                dw + (size_t)K * K * C, dw + (size_t)K * K * C + C, N, ib.H, ib.W, C, ob.H, ob.W, K, stride, same_pad_before(ib.H, K, stride), same_pad_before(ib.W, K, stride));
+            break;
+        }
+        case Launch::MaxPoolF32: {
+            const EngBuffer& ib = e->bufs[po.in_buf];
+            const EngBuffer& ob = e->bufs[po.out_buf];
+            const int C = (int)po.cout_g, KP = K ? K : 2;
+            const size_t total = (size_t)N * ob.H * ob.W * (C / 4);
+            maxpool_f32_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>((const float*)ib.d + po.in_ch_off, (float*)ob.d + po.out_ch_off, N, ib.H, ib.W, ib.channels, C, ob.channels,
+                                                                               ob.H, ob.W, KP, same_pad_before(ib.H, KP, 2), same_pad_before(ib.W, KP, 2));
+            break;
+        }
+        case Launch::HeadsF32:
+            launch_heads<float>(e, po, N, st);
+            break;
+        }
+        e->launches += kernels_launched(op.launch, u8_input);
         if (prof) cudaEventRecord(evset[oi + 1], st);
     }
     if (prof) e->ev_head++;
@@ -1296,7 +1131,6 @@ void free_engine(hp_engine* e)
     for (auto& b : e->bufs) if (b.d) cudaFree(b.d);
     for (auto& o : e->ops) {
         if (o.plan.d_w) cudaFree(o.plan.d_w);
-        if (o.plan.d_w32) cudaFree(o.plan.d_w32);
         if (o.plan.d_bias) cudaFree(o.plan.d_bias);
         if (o.plan.d_alpha) cudaFree(o.plan.d_alpha);
         if (o.d_dw) cudaFree(o.d_dw);
@@ -1391,6 +1225,15 @@ int hp_engine_create_ex(hp_engine** out, const void* pack, size_t pack_bytes, in
     hp_engine* e = new hp_engine();
     e->device = device; e->dtype = dtype; e->in_h = in_h; e->in_w = in_w; e->max_batch = max_batch;
     e->factor = factor; e->flip_rgb = flip_rgb; e->hdr = hdr; e->num_sms = prop.multiProcessorCount;
+    EngOptions& opt = e->opt;
+    if (const char* v = getenv("HPB_HALO")) opt.halo = strcmp(v, "all") == 0 ? EngOptions::HALO_ALL : EngOptions::HALO_NONE;
+    opt.stem3 = !getenv("HPB_NO_STEM3");
+    opt.pool_fuse = !getenv("HPB_NO_POOL_FUSE");
+    opt.dw1_fuse = !getenv("HPB_NO_DW1_FUSE");
+    opt.dw_pair = !getenv("HPB_NO_DW_DUAL");
+    opt.dw_tma = !getenv("HPB_NO_DW_TMA");
+    const char* rs = getenv("HPB_PIFPAF_RESERVE_SMS");
+    opt.pifpaf_reserve_sms = std::max(0, std::min(rs ? atoi(rs) : std::min(max_batch, 16), e->num_sms / 2));
     const uint8_t* ptr = (const uint8_t*)pack + sizeof(PackHeader);
     const PackBuffer* pb = (const PackBuffer*)ptr;
     const PackOp* pops = (const PackOp*)(ptr + hdr.n_buffers * sizeof(PackBuffer));
@@ -1423,18 +1266,20 @@ int hp_engine_create_ex(hp_engine** out, const void* pack, size_t pack_bytes, in
     }
     e->ops.resize(hdr.n_ops);
     size_t max_smem = 0;
-    for (uint32_t i = 0; i < hdr.n_ops; ++i) e->ops[i].po = pops[i];   // (plan building looks at neighbouring ops)
+    const bool tf32 = dtype == HP_DTYPE_TF32;
     for (uint32_t i = 0; i < hdr.n_ops; ++i) {
-        const PackOp& po = pops[i];
+        EngOp& op = e->ops[i];
+        op.po = pops[i];
+        const PackOp& po = op.po;
         if ((po.type != OP_IM2COL3 && po.in_buf >= hdr.n_buffers) || (po.out_mode != OUT_F32_NCHW_SPLIT && po.type != OP_PIFPAF_HEAD && po.out_buf >= hdr.n_buffers)) {
             set_error("engine: op %u references a missing buffer", i);
             return fail(HP_ERR_ARG);
         }
         if (po.type == OP_CONV) {
-            rc = build_conv_plan(e, e->ops[i], blob.data());
+            rc = build_conv_plan(e, op, blob.data());
             if (rc) return fail(rc);
-            max_smem = std::max(max_smem, e->ops[i].plan.smem);
-            e->flops_per_frame += e->ops[i].plan.flops_per_frame;
+            max_smem = std::max(max_smem, op.plan.smem);
+            e->flops_per_frame += op.plan.flops_per_frame;
         } else if (po.type == OP_IM2COL3) {
             const int stride = po.stride ? (int)po.stride : 1;
             const int R = po.R ? (int)po.R : 3;
@@ -1442,6 +1287,7 @@ int hp_engine_create_ex(hp_engine** out, const void* pack, size_t pack_bytes, in
                 set_error("engine: im2col buffer must hold roundup(R*R*3,64) channels at the stem resolution");
                 return fail(HP_ERR_ARG);
             }
+            op.launch = tf32 ? Launch::Im2colF32 : Launch::Im2col;
         } else if (po.type == OP_DWCONV) {
             const int C = (int)po.cout_g, K = (int)po.R, stride = po.stride ? (int)po.stride : 1;
             const EngBuffer& ib = e->bufs[po.in_buf];
@@ -1458,152 +1304,156 @@ int hp_engine_create_ex(hp_engine** out, const void* pack, size_t pack_bytes, in
                 w[(size_t)K * K * C + c] = blob[po.b_off + c];
                 w[(size_t)K * K * C + C + c] = blob[po.a_off + c];
             }
-            if (cudaMalloc(&e->ops[i].d_dw, w.size() * sizeof(float)) != cudaSuccess ||
-                cudaMemcpy(e->ops[i].d_dw, w.data(), w.size() * sizeof(float), cudaMemcpyHostToDevice) != cudaSuccess) {
+            if (cudaMalloc(&op.d_dw, w.size() * sizeof(float)) != cudaSuccess ||
+                cudaMemcpy(op.d_dw, w.data(), w.size() * sizeof(float), cudaMemcpyHostToDevice) != cudaSuccess) {
                 set_error("engine: depthwise weight upload failed");
                 return fail(HP_ERR_CUDA);
             }
             e->flops_per_frame += 2.0 * ob.H * ob.W * C * K * K;
+            op.launch = tf32 ? Launch::DwF32 : K == 3 && stride == 1 ? Launch::DwCol : Launch::DwStrip;
         } else if (po.type == OP_MAXPOOL2) {
             if (po.cout_g % 8 || e->bufs[po.out_buf].down != e->bufs[po.in_buf].down + 1 || (po.R != 0 && po.R != 2 && po.R != 3)) { set_error("engine: bad maxpool op %u", i); return fail(HP_ERR_ARG); }
+            op.launch = tf32 ? Launch::MaxPoolF32 : Launch::MaxPool;
         } else if (po.type == OP_PIFPAF_HEAD) {
             if (hdr.head_type != 1 || po.res_buf >= hdr.n_buffers || hdr.conf_channels != 85 || hdr.paf_channels != 171 ||
                 e->bufs[po.in_buf].channels < 340 || e->bufs[po.res_buf].channels < 684) { set_error("engine: bad pifpaf head op"); return fail(HP_ERR_ARG); }
+            op.launch = tf32 ? Launch::HeadsF32 : Launch::Heads;
         } else {
             set_error("engine: unknown op type %u", po.type);
             return fail(HP_ERR_UNSUPPORTED);
         }
     }
-    // conv (halo kernel) -> 2x2 max-pool: the pool moves into the conv's epilogue when nobody else reads the un-pooled tensor.
-    // HPB_NO_POOL_FUSE=1 keeps the two launches.
-    if (dtype == HP_DTYPE_F16 && !getenv("HPB_NO_POOL_FUSE")) {
-        for (size_t i = 0; i + 1 < e->ops.size(); ++i) {
-            EngOp& c = e->ops[i]; EngOp& m = e->ops[i + 1];
-            if (c.po.type != OP_CONV || !c.plan.halo || !c.plan.monotone_act || m.po.type != OP_MAXPOOL2 || (m.po.R != 0 && m.po.R != 2)) continue;
-            const EngBuffer& cb = e->bufs[c.po.out_buf];
-            const EngBuffer& pb = e->bufs[m.po.out_buf];
-            const int C = (int)c.po.groups * (int)c.po.cout_g;
-            if (m.po.in_buf != c.po.out_buf || m.po.in_ch_off != c.po.out_ch_off || (int)m.po.cout_g != C || c.plan.hp.cout_g_pad != c.plan.hp.cout_g ||
-                (cb.H & 1) || (cb.W & 1) || pb.H != cb.H / 2 || pb.W != cb.W / 2 || (int)m.po.out_ch_off + C > pb.channels) continue;
-            bool other_reader = false;
-            for (size_t k = 0; k < e->ops.size(); ++k) {
-                if (k == i + 1) continue;
-                const PackOp& q = e->ops[k].po;
-                if (q.type == OP_IM2COL3) continue;
-                if (q.in_buf == c.po.out_buf || ((q.type == OP_CONV && q.res_mode) || q.type == OP_PIFPAF_HEAD) && q.res_buf == c.po.out_buf) other_reader = true;
-            }
-            if (other_reader) continue;
-            c.plan.hp.out = pb.d; c.plan.hp.out_ld = pb.channels; c.plan.hp.out_ch_off = (int)m.po.out_ch_off;
-            c.plan.pool_fused = true;
-            m.fused_into_prev = true;
-            e->bufs[c.po.out_buf].fused_away = true;
+    // The fusion passes below (fp16 engines) settle how each op launches.
+    // Fused stem: the first conv gathers its patches from the u8 frames itself, the im2col buffer is never written.
+    for (EngOp& c : e->ops) {
+        const PackOp& po = c.po;
+        const int R = (int)po.R;
+        if (tf32 || c.launch != Launch::Conv || !po.im2col_input || po.res_mode || po.out_mode != OUT_F16_NHWC || po.S != po.R || !(R == 7 || (R == 3 && opt.stem3))) continue;
+        for (EngOp& m : e->ops) {   // the patch-gather op feeding this conv: its stride / tap size define the stem geometry
+            if (m.po.type != OP_IM2COL3 || m.po.out_buf != po.in_buf) continue;
+            if ((int)(m.po.R ? m.po.R : 3) != R || po.cin_g != 3) break;
+            ConvParams& p = c.plan.prm;
+            const int stride = m.po.stride ? (int)m.po.stride : 1;
+            p.in_h = in_h; p.in_w = in_w; p.stem_stride = stride;
+            p.stem_pad_h = same_pad_before(in_h, R, stride); p.stem_pad_w = same_pad_before(in_w, R, stride);
+            p.factor = factor; p.flip = flip_rgb;
+            p.mean[0] = hdr.mean[0]; p.mean[1] = hdr.mean[1]; p.mean[2] = hdr.mean[2];
+            c.launch = Launch::ConvStem;
+            m.launch = Launch::StemOrIm2col;
+            break;
         }
+    }
+    // conv (halo kernel) -> 2x2 max-pool: the pool moves into the conv's epilogue when nobody else reads the un-pooled tensor
+    for (size_t i = 0; opt.pool_fuse && i + 1 < e->ops.size(); ++i) {
+        EngOp& c = e->ops[i]; EngOp& m = e->ops[i + 1];
+        if (c.launch != Launch::Halo || !c.plan.monotone_act || m.po.type != OP_MAXPOOL2 || (m.po.R != 0 && m.po.R != 2)) continue;
+        const EngBuffer& cb = e->bufs[c.po.out_buf];
+        const EngBuffer& pb = e->bufs[m.po.out_buf];
+        const int C = (int)c.po.groups * (int)c.po.cout_g;
+        if (m.po.in_buf != c.po.out_buf || m.po.in_ch_off != c.po.out_ch_off || (int)m.po.cout_g != C || c.plan.hp.cout_g_pad != c.plan.hp.cout_g ||
+            (cb.H & 1) || (cb.W & 1) || pb.H != cb.H / 2 || pb.W != cb.W / 2 || (int)m.po.out_ch_off + C > pb.channels) continue;
+        bool other_reader = false;
+        for (size_t k = 0; k < e->ops.size(); ++k)
+            if (k != i + 1 && reads_buffer(e->ops[k].po, c.po.out_buf)) other_reader = true;
+        if (other_reader) continue;
+        c.plan.hp.out = pb.d; c.plan.hp.out_ld = pb.channels; c.plan.hp.out_ch_off = (int)m.po.out_ch_off;
+        c.launch = Launch::HaloPool;
+        m.launch = Launch::None;
+        e->bufs[c.po.out_buf].fused_away = true;
     }
     // conv -> 1x1 "depthwise" (per-channel affine + PReLU; the filter_size (1,1) separable blocks, mbv2_th_openpose.py:121,127,144,151):
-    // applied in the conv's epilogue when the tensor in between has no other reader before it is overwritten.  HPB_NO_DW1_FUSE=1 keeps both launches.
-    if (dtype == HP_DTYPE_F16 && !getenv("HPB_NO_DW1_FUSE")) {
-        for (size_t i = 0; i + 1 < e->ops.size(); ++i) {
-            EngOp& c = e->ops[i]; EngOp& d = e->ops[i + 1];
-            if (c.po.type != OP_CONV || d.po.type != OP_DWCONV || d.po.R != 1 || (d.po.stride ? d.po.stride : 1) != 1) continue;
-            const ConvParams& cp = c.plan.prm;
-            const int Ctot = (int)c.po.groups * (int)c.po.cout_g;
-            if (c.plan.halo || c.po.out_mode != OUT_F16_NHWC || cp.cout_g_pad != cp.cout_g || cp.cout_g % 16 ||
-                d.po.in_buf != c.po.out_buf || d.po.in_ch_off != c.po.out_ch_off || (int)d.po.cout_g != Ctot || d.po.out_buf == c.po.out_buf) continue;
-            if (d.po.out_buf == c.po.in_buf) {
-                // the fused conv would write the tensor it reads.  That is safe only when every tile reads exactly the (pixels, channels) it
-                // writes and has consumed them before its epilogue: a 1x1 conv whose group g maps channels [off + g*c, off + (g+1)*c) onto
-                // themselves with ONE n-tile per group (MobilenetThin's grouped 128 -> 128 pointwise convs on the ping-pong buffers)
-                if (cp.R != 1 || cp.S != 1 || cp.cin_g != cp.cout_g || cp.BN != cp.cout_g || (int)d.po.out_ch_off != cp.in_ch_off) continue;
-            }
-            if (c.po.res_mode && d.po.out_buf == c.po.res_buf) continue;
-            // the tensor between the two must be dead afterwards: no reader before the next writer of the same channels
-            bool safe = true, rewritten = false;
-            for (size_t k = i + 2; k < e->ops.size() && safe && !rewritten; ++k) {
-                const PackOp& q = e->ops[k].po;
-                if (q.type == OP_IM2COL3) continue;
-                if (q.in_buf == c.po.out_buf || (((q.type == OP_CONV && q.res_mode) || q.type == OP_PIFPAF_HEAD) && q.res_buf == c.po.out_buf)) safe = false;
-                else if (q.type != OP_PIFPAF_HEAD && q.out_mode != OUT_F32_NCHW_SPLIT && q.out_buf == c.po.out_buf) {
-                    const int qc = q.type == OP_CONV ? (int)q.groups * (int)q.cout_g : (int)q.cout_g;
-                    if (q.out_ch_off <= c.po.out_ch_off && (int)q.out_ch_off + qc >= (int)c.po.out_ch_off + Ctot) rewritten = true; else safe = false;
-                }
-            }
-            if (!safe) continue;
-            const EngBuffer& ob = e->bufs[d.po.out_buf];
-            if ((int)d.po.out_ch_off + Ctot > ob.channels) continue;
-            c.plan.prm.out = ob.d; c.plan.prm.out_ld = ob.channels; c.plan.prm.out_ch_off = (int)d.po.out_ch_off;
-            c.plan.prm.post_w = d.d_dw; c.plan.prm.post_b = d.d_dw + Ctot; c.plan.prm.post_a = d.d_dw + 2 * (size_t)Ctot;
-            d.fused_into_prev = true;
-            if (!rewritten) e->bufs[c.po.out_buf].fused_away = true;   // its final content would have been this conv's output
+    // applied in the epilogue of conv_wgmma_kernel when the tensor in between has no other reader before it is overwritten
+    for (size_t i = 0; opt.dw1_fuse && i + 1 < e->ops.size(); ++i) {
+        EngOp& c = e->ops[i]; EngOp& d = e->ops[i + 1];
+        if ((c.launch != Launch::Conv && c.launch != Launch::ConvStem) || d.launch != Launch::DwStrip || d.po.R != 1 || (d.po.stride ? d.po.stride : 1) != 1) continue;
+        const ConvParams& cp = c.plan.prm;
+        const int Ctot = (int)c.po.groups * (int)c.po.cout_g;
+        if (c.po.out_mode != OUT_F16_NHWC || cp.cout_g_pad != cp.cout_g || cp.cout_g % 16 ||
+            d.po.in_buf != c.po.out_buf || d.po.in_ch_off != c.po.out_ch_off || (int)d.po.cout_g != Ctot || d.po.out_buf == c.po.out_buf) continue;
+        if (d.po.out_buf == c.po.in_buf) {
+            // the fused conv would write the tensor it reads.  That is safe only when every tile reads exactly the (pixels, channels) it
+            // writes and has consumed them before its epilogue: a 1x1 conv whose group g maps channels [off + g*c, off + (g+1)*c) onto
+            // themselves with ONE n-tile per group (MobilenetThin's grouped 128 -> 128 pointwise convs on the ping-pong buffers)
+            if (cp.R != 1 || cp.S != 1 || cp.cin_g != cp.cout_g || cp.BN != cp.cout_g || (int)d.po.out_ch_off != cp.in_ch_off) continue;
         }
-    }
-    // two depthwise 3x3 / stride-1 convs of the same input (conf / paf branch of a MobilenetThin stage): one dual launch
-    if (dtype == HP_DTYPE_F16 && !getenv("HPB_NO_DW_DUAL") && !getenv("HPB_DW_STRIP")) {
-        for (size_t i = 0; i + 1 < e->ops.size(); ++i) {
-            EngOp& a = e->ops[i]; EngOp& b = e->ops[i + 1];
-            if (a.po.type != OP_DWCONV || b.po.type != OP_DWCONV || a.fused_into_prev) continue;
-            const int st_a = a.po.stride ? (int)a.po.stride : 1, st_b = b.po.stride ? (int)b.po.stride : 1;
-            if (a.po.R != 3 || b.po.R != 3 || st_a != 1 || st_b != 1 || a.po.in_buf != b.po.in_buf || a.po.in_ch_off != b.po.in_ch_off ||
-                a.po.cout_g != b.po.cout_g || a.po.out_buf != b.po.out_buf || a.po.out_buf == a.po.in_buf) continue;
-            a.dual_with_next = true;
-            b.fused_into_prev = true;
+        if (c.po.res_mode && d.po.out_buf == c.po.res_buf) continue;
+        // the tensor between the two must be dead afterwards: no reader before the next writer of the same channels
+        bool safe = true, rewritten = false;
+        for (size_t k = i + 2; k < e->ops.size() && safe && !rewritten; ++k) {
+            const PackOp& q = e->ops[k].po;
+            if (reads_buffer(q, c.po.out_buf)) safe = false;
+            else if (q.type != OP_IM2COL3 && q.type != OP_PIFPAF_HEAD && q.out_mode != OUT_F32_NCHW_SPLIT && q.out_buf == c.po.out_buf) {
+                const int qc = q.type == OP_CONV ? (int)q.groups * (int)q.cout_g : (int)q.cout_g;
+                if (q.out_ch_off <= c.po.out_ch_off && (int)q.out_ch_off + qc >= (int)c.po.out_ch_off + Ctot) rewritten = true; else safe = false;
+            }
         }
+        if (!safe) continue;
+        const EngBuffer& ob = e->bufs[d.po.out_buf];
+        if ((int)d.po.out_ch_off + Ctot > ob.channels) continue;
+        c.plan.prm.out = ob.d; c.plan.prm.out_ld = ob.channels; c.plan.prm.out_ch_off = (int)d.po.out_ch_off;
+        c.plan.prm.post_w = d.d_dw; c.plan.prm.post_b = d.d_dw + Ctot; c.plan.prm.post_a = d.d_dw + 2 * (size_t)Ctot;
+        d.launch = Launch::None;
+        if (!rewritten) e->bufs[c.po.out_buf].fused_away = true;   // its final content would have been this conv's output
     }
     // depthwise 3x3 / stride 1 on a multiple of 64 channels: input tiles through TMA (dwconv3_tma_kernel)
-    if (dtype == HP_DTYPE_F16 && !getenv("HPB_NO_DW_TMA") && !getenv("HPB_DW_STRIP")) {
-        size_t dwt_max = 0;
-        for (size_t i = 0; i < e->ops.size(); ++i) {
-            EngOp& a = e->ops[i];
-            const PackOp& po = a.po;
-            if (po.type != OP_DWCONV || a.fused_into_prev || po.R != 3 || (po.stride ? (int)po.stride : 1) != 1 || po.cout_g % 64 || po.in_buf == po.out_buf) continue;
-            const EngBuffer& ib = e->bufs[po.in_buf];
-            if (ib.channels % 8 || po.in_ch_off % 8) continue;
-            const int C = (int)po.cout_g;
-            const int nx = (ib.W + 61) / 62, wbo = (ib.W + nx - 1) / nx, bw = wbo + 2;
-            // tile height: the tallest of 8 / 6 / 4 / 3 / 2 rows that fits a buffer and still gives every SM two tiles at the full batch
-            int hb = 2;
-            const int hb_max = getenv("HPB_DWT_HB") ? atoi(getenv("HPB_DWT_HB")) : 8;
-            for (int cand : { 8, 6, 4, 3, 2 }) {
-                if (cand > hb_max) continue;
-                if (cand > std::max(2, ib.H) || (size_t)(cand + 2) * bw * 128 > (size_t)DWT_STAGE_MAX) continue;
-                const size_t items = (size_t)e->max_batch * ((ib.H + cand - 1) / cand) * nx * (C / 64);
-                hb = cand;
-                if (items >= 2 * (size_t)e->num_sms) break;
-            }
-            const size_t stage = (size_t)(hb + 2) * bw * 128;
-            if (stage > (size_t)DWT_STAGE_MAX) continue;
-            a.dwt_stages = (int)std::min<size_t>(4, (200 * 1024) / stage);
-            if (a.dwt_stages < 2) continue;
-            a.dwt_wbo = wbo; a.dwt_hb = hb; a.dwt_tiles_x = nx; a.dwt_tiles_y = (ib.H + hb - 1) / hb;
-            a.dwt_smem = a.dwt_stages * stage + 128 + 64;
-            if (make_tmap_act_box_plain(&a.tmap_dw, ib.d + po.in_ch_off, e->max_batch, ib.H, ib.W, C, ib.channels, bw, hb + 2) != HP_OK) return fail(HP_ERR_CUDA);
-            a.dw_tma = true;
-            dwt_max = std::max(dwt_max, a.dwt_smem);
+    size_t dwt_max = 0;
+    for (EngOp& a : e->ops) {
+        const PackOp& po = a.po;
+        if (!opt.dw_tma || a.launch != Launch::DwCol || po.cout_g % 64 || po.in_buf == po.out_buf) continue;
+        const EngBuffer& ib = e->bufs[po.in_buf];
+        const int C = (int)po.cout_g;
+        const int nx = (ib.W + 61) / 62, wbo = (ib.W + nx - 1) / nx, bw = wbo + 2;
+        // tile height: the tallest of 8 / 6 / 4 / 3 / 2 rows that fits a buffer and still gives every SM two tiles at the full batch
+        int hb = 2;
+        for (int cand : { 8, 6, 4, 3, 2 }) {
+            if (cand > std::max(2, ib.H) || (size_t)(cand + 2) * bw * 128 > (size_t)DWT_STAGE_MAX) continue;
+            const size_t items = (size_t)e->max_batch * ((ib.H + cand - 1) / cand) * nx * (C / 64);
+            hb = cand;
+            if (items >= 2 * (size_t)e->num_sms) break;
         }
-        if (dwt_max > 0 && (cudaFuncSetAttribute(dwconv3_tma_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dwt_max) != cudaSuccess ||
-                            cudaFuncSetAttribute(dwconv3_tma_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dwt_max) != cudaSuccess)) {
-            set_error("engine: cannot opt in to %zu bytes of dynamic shared memory (depthwise)", dwt_max);
-            return fail(HP_ERR_CUDA);
-        }
+        const size_t stage = (size_t)(hb + 2) * bw * 128;
+        if (stage > (size_t)DWT_STAGE_MAX) continue;
+        a.dwt_stages = (int)std::min<size_t>(4, (200 * 1024) / stage);
+        if (a.dwt_stages < 2) continue;
+        a.dwt_wbo = wbo; a.dwt_hb = hb; a.dwt_tiles_x = nx; a.dwt_tiles_y = (ib.H + hb - 1) / hb;
+        a.dwt_smem = a.dwt_stages * stage + 128 + 64;
+        if (make_tmap_act_box(&a.tmap_dw, ib.d + po.in_ch_off, e->max_batch, ib.H, ib.W, C, ib.channels, bw, hb + 2, CU_TENSOR_MAP_SWIZZLE_NONE) != HP_OK) return fail(HP_ERR_CUDA);
+        a.launch = Launch::DwTma;
+        dwt_max = std::max(dwt_max, a.dwt_smem);
+    }
+    if (dwt_max > 0 && (cudaFuncSetAttribute(dwconv3_tma_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dwt_max) != cudaSuccess ||
+                        cudaFuncSetAttribute(dwconv3_tma_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dwt_max) != cudaSuccess)) {
+        set_error("engine: cannot opt in to %zu bytes of dynamic shared memory (depthwise)", dwt_max);
+        return fail(HP_ERR_CUDA);
+    }
+    // two TMA depthwise convs of the same input (the conf / paf branch of a MobilenetThin stage): one launch with both filter sets
+    for (size_t i = 0; opt.dw_pair && i + 1 < e->ops.size(); ++i) {
+        EngOp& a = e->ops[i]; EngOp& b = e->ops[i + 1];
+        if (a.launch != Launch::DwTma || b.launch != Launch::DwTma || a.po.in_buf != b.po.in_buf || a.po.in_ch_off != b.po.in_ch_off ||
+            a.po.cout_g != b.po.cout_g || a.po.out_buf != b.po.out_buf) continue;
+        a.launch = Launch::DwTmaPair;
+        b.launch = Launch::None;
     }
     // programmatic dependent launch pays where the step is a chain of short kernels (MobilenetThin: 73 launches of ~2 GFLOP at batch 8)
     // and costs where they are long (VGG19: 140 GFLOP per launch); see launch_pdl
-    {
-        int launches = 0;
-        for (const EngOp& o : e->ops)
-            if ((o.po.type == OP_CONV || o.po.type == OP_DWCONV || o.po.type == OP_MAXPOOL2) && !o.fused_into_prev) ++launches;
-        const double per_launch = launches ? e->flops_per_frame * e->max_batch / launches : 0.0;
-        e->use_pdl = dtype == HP_DTYPE_F16 && launches > 0 && per_launch < 10e9;
-        if (const char* v = getenv("HPB_PDL")) e->use_pdl = atoi(v) != 0;
+    int launches = 0;
+    for (const EngOp& o : e->ops) {
+        if ((o.po.type == OP_CONV || o.po.type == OP_DWCONV || o.po.type == OP_MAXPOOL2) && o.launch != Launch::None) ++launches;
+        e->step_kernels += kernels_launched(o.launch, true);
     }
+    const double per_launch = launches ? e->flops_per_frame * e->max_batch / launches : 0.0;
+    e->use_pdl = !tf32 && launches > 0 && per_launch < 10e9;
     for (const EngOp& o : e->ops) {
         if (o.po.type != OP_CONV) continue;
-        if (o.plan.halo && cudaFuncSetAttribute(halo_kernel(o.plan.pool_fused, o.plan.prm.BN), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)max_smem) != cudaSuccess) {
+        if ((o.launch == Launch::Halo || o.launch == Launch::HaloPool) &&
+            cudaFuncSetAttribute(halo_kernel(o.launch == Launch::HaloPool, o.plan.prm.BN), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)max_smem) != cudaSuccess) {
             set_error("engine: cannot opt in to %zu bytes of dynamic shared memory (halo)", max_smem);
             return fail(HP_ERR_CUDA);
         }
+        const int stem_R = o.launch == Launch::ConvStem ? (int)o.po.R : 0;
         for (int v = 0; v < 3; ++v)   // plain, residual, and (for a stem) the fused u8 form
-            if ((v < 2 || o.plan.stem_R) &&
-                cudaFuncSetAttribute(conv_kernel(o.plan.tf32, v == 1, o.plan.prm.BN, v == 2 ? o.plan.stem_R : 0), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)max_smem) != cudaSuccess) {
+            if ((v < 2 || stem_R) &&
+                cudaFuncSetAttribute(conv_kernel(tf32, v == 1, o.plan.prm.BN, v == 2 ? stem_R : 0), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)max_smem) != cudaSuccess) {
                 set_error("engine: cannot opt in to %zu bytes of dynamic shared memory", max_smem);
                 return fail(HP_ERR_CUDA);
             }
@@ -1950,7 +1800,7 @@ int hp_engine_get_profile(hp_engine* e, double* ms_per_op, int* op_type, double*
 //
 // The per-batch launch sequence (every conv + the two parser kernels + the result D2H, ~60 nodes at cfg3) is captured
 // once per slot into a CUDA graph and replayed with one cudaGraphLaunch; it is re-captured when anything baked into it
-// changes (batch size, parser thresholds / capacities, benchmark override).  HPB_NO_GRAPH=1 launches directly.
+// changes (batch size, parser thresholds / capacities, benchmark override).
 // ---------------------------------------------------------------------------------------------------------------------
 int hp_paf_prepare(hp_paf* p, int N, int c_conf, int c_paf, int H, int W);
 int hp_paf_state(const hp_paf* p, float* thresholds2, int* ints6);
@@ -1976,48 +1826,79 @@ int pose_enqueue_compute(hp_engine* e, hp_engine::PoseSlot& sl, cudaStream_t st)
     return hp_paf_copy_results_host_async(sl.parser, sl.pin_humans, sl.pin_counts, sl.N, (void*)st);
 }
 
-int pose_slot_prepare(hp_engine* e, hp_engine::PoseSlot& sl, int idx, hp_paf* parser, int N)
+// what both pipelined calls need in a slot: its own frame buffer (the plain entry points keep hp_engine::d_frames), the upload and
+// completion events, and pinned record buffers for hcap humans per frame.  A captured graph holds their addresses: it goes when they move.
+int slot_alloc(hp_engine* e, hp_engine::PoseSlot& sl, int hcap)
 {
-    const size_t fbytes = (size_t)e->max_batch * e->in_h * e->in_w * 3;
     if (!e->copy_stream) HP_CUDA_TRY(cudaStreamCreateWithFlags(&e->copy_stream, cudaStreamNonBlocking));
-    (void)idx;
-    if (!sl.d_frames) HP_CUDA_TRY(cudaMalloc(&sl.d_frames, fbytes + 16));   // own buffers: the plain entry points keep hp_engine::d_frames
+    if (!sl.d_frames) HP_CUDA_TRY(cudaMalloc(&sl.d_frames, (size_t)e->max_batch * e->in_h * e->in_w * 3 + 16));
     if (!sl.h2d_done) HP_CUDA_TRY(cudaEventCreateWithFlags(&sl.h2d_done, cudaEventDisableTiming));
     if (!sl.done) HP_CUDA_TRY(cudaEventCreateWithFlags(&sl.done, cudaEventDisableTiming));
-    int rc = hp_paf_prepare(parser, N, (int)e->hdr.conf_channels, (int)e->hdr.paf_channels, e->out_h, e->out_w);
-    if (rc) return rc;
-    float kf[2]; int ki[6];
-    hp_paf_state(parser, kf, ki);
-    const size_t need_h = (size_t)e->max_batch * ki[4];
+    const size_t need_h = (size_t)e->max_batch * hcap, need_c = (size_t)2 * e->max_batch;
+    if ((sl.pin_humans_n < need_h || sl.pin_counts_n < need_c) && sl.graph) { cudaGraphExecDestroy(sl.graph); sl.graph = nullptr; }
     if (sl.pin_humans_n < need_h) {
         if (sl.pin_humans) cudaFreeHost(sl.pin_humans);
         sl.pin_humans = nullptr; sl.pin_humans_n = 0;
         HP_CUDA_TRY(cudaMallocHost(&sl.pin_humans, need_h * sizeof(hp_human)));
         sl.pin_humans_n = need_h;
-        if (sl.graph) { cudaGraphExecDestroy(sl.graph); sl.graph = nullptr; }   // the captured D2H targets moved
     }
-    if (sl.pin_counts_n < (size_t)2 * e->max_batch) {
+    if (sl.pin_counts_n < need_c) {
         if (sl.pin_counts) cudaFreeHost(sl.pin_counts);
         sl.pin_counts = nullptr; sl.pin_counts_n = 0;
-        HP_CUDA_TRY(cudaMallocHost(&sl.pin_counts, (size_t)2 * e->max_batch * sizeof(int)));
-        sl.pin_counts_n = (size_t)2 * e->max_batch;
-        if (sl.graph) { cudaGraphExecDestroy(sl.graph); sl.graph = nullptr; }
+        HP_CUDA_TRY(cudaMallocHost(&sl.pin_counts, need_c * sizeof(int)));
+        sl.pin_counts_n = need_c;
     }
+    sl.hcap = hcap;
+    return HP_OK;
+}
+
+// the N frames of a submitted batch into the slot's device buffer, ordered before the engine stream's next work: frames already in
+// HBM by a D2D copy on the engine stream, host frames by an H2D on the copy stream (pageable ones through the slot's pinned staging,
+// free since the slot was collected)
+int slot_upload(hp_engine* e, hp_engine::PoseSlot& sl, const uint8_t* frames, int N, bool device_src)
+{
+    const size_t bytes = (size_t)N * e->in_h * e->in_w * 3;
+    if (device_src) {
+        HP_CUDA_TRY(cudaMemcpyAsync(sl.d_frames, frames, bytes, cudaMemcpyDeviceToDevice, e->stream));
+        return HP_OK;
+    }
+    cudaPointerAttributes attr;
+    const bool pinned = (cudaPointerGetAttributes(&attr, frames) == cudaSuccess && attr.type == cudaMemoryTypeHost);
+    if (!pinned) cudaGetLastError();
+    const uint8_t* src = frames;
+    if (!pinned) {
+        if (!sl.pin_frames) HP_CUDA_TRY(cudaMallocHost(&sl.pin_frames, (size_t)e->max_batch * e->in_h * e->in_w * 3));
+        memcpy(sl.pin_frames, frames, bytes);
+        src = sl.pin_frames;
+    }
+    HP_CUDA_TRY(cudaMemcpyAsync(sl.d_frames, src, bytes, cudaMemcpyHostToDevice, e->copy_stream));
+    HP_CUDA_TRY(cudaEventRecord(sl.h2d_done, e->copy_stream));
+    HP_CUDA_TRY(cudaStreamWaitEvent(e->stream, sl.h2d_done, 0));
+    return HP_OK;
+}
+
+int pose_slot_prepare(hp_engine* e, hp_engine::PoseSlot& sl, hp_paf* parser, int N)
+{
+    int rc = hp_paf_prepare(parser, N, (int)e->hdr.conf_channels, (int)e->hdr.paf_channels, e->out_h, e->out_w);
+    if (rc) return rc;
+    float kf[2]; int ki[6];
+    hp_paf_state(parser, kf, ki);
+    rc = slot_alloc(e, sl, ki[4]);
+    if (rc) return rc;
     // anything the captured sequence bakes in
     const bool same = sl.graph && sl.key_N == N && sl.key_parser == (const void*)parser && memcmp(sl.key_f, kf, sizeof(kf)) == 0 && memcmp(sl.key_i, ki, sizeof(ki)) == 0 &&
                       sl.key_ovr[0] == (const void*)e->override_conf && sl.key_ovr[1] == (const void*)e->override_paf;
     if (!same && sl.graph) { cudaGraphExecDestroy(sl.graph); sl.graph = nullptr; }
     sl.key_N = N; sl.key_parser = parser; memcpy(sl.key_f, kf, sizeof(kf)); memcpy(sl.key_i, ki, sizeof(ki));
     sl.key_ovr[0] = e->override_conf; sl.key_ovr[1] = e->override_paf;
-    sl.N = N; sl.hcap = ki[4]; sl.parser = parser; sl.decoder = nullptr;
+    sl.N = N; sl.parser = parser; sl.decoder = nullptr;
     return HP_OK;
 }
 
 // enqueue this slot's compute on the engine stream: graph replay when possible, direct launches otherwise
 int pose_launch(hp_engine* e, hp_engine::PoseSlot& sl)
 {
-    static const bool no_graph = getenv("HPB_NO_GRAPH") != nullptr;
-    if (!no_graph && e->graphs_ok && !e->profiling) {
+    if (e->graphs_ok && !e->profiling) {
         if (!sl.graph) {
             cudaGraph_t g = nullptr;
             if (cudaStreamBeginCapture(e->stream, cudaStreamCaptureModeThreadLocal) == cudaSuccess) {
@@ -2033,15 +1914,7 @@ int pose_launch(hp_engine* e, hp_engine::PoseSlot& sl)
         if (sl.graph) {
             HP_CUDA_TRY(cudaGraphLaunch(sl.graph, e->stream));
             e->graph_launches++;
-            // the replay runs the same kernels the direct path counts: every engine op + the parser's two
-            int n_k = 2;
-            for (auto& op : e->ops) {
-                const uint32_t t = op.po.type;
-                if (t == OP_IM2COL3 && op.fused_into_stem) continue;
-                if ((t == OP_MAXPOOL2 || t == OP_DWCONV) && op.fused_into_prev) continue;
-                n_k += (t == OP_PIFPAF_HEAD) ? 2 : 1;
-            }
-            e->launches += n_k;
+            e->launches += e->step_kernels + 2;   // the replay runs what the direct path counts: the engine's step + the parser's two kernels
             return HP_OK;
         }
     }
@@ -2055,29 +1928,13 @@ extern "C" {
 // ---- OpenPifPaf packs: engine on its stream, decoder on the decoder's stream, two batches in flight ----
 static int pifpaf_slot_prepare(hp_engine* e, hp_engine::PoseSlot& sl, hp_pifpaf* dec, int N)
 {
-    const size_t fbytes = (size_t)e->max_batch * e->in_h * e->in_w * 3;
-    if (!e->copy_stream) HP_CUDA_TRY(cudaStreamCreateWithFlags(&e->copy_stream, cudaStreamNonBlocking));
-    if (!sl.d_frames) HP_CUDA_TRY(cudaMalloc(&sl.d_frames, fbytes + 16));
-    if (!sl.h2d_done) HP_CUDA_TRY(cudaEventCreateWithFlags(&sl.h2d_done, cudaEventDisableTiming));
-    if (!sl.done) HP_CUDA_TRY(cudaEventCreateWithFlags(&sl.done, cudaEventDisableTiming));
-    if (!sl.conv_done) HP_CUDA_TRY(cudaEventCreateWithFlags(&sl.conv_done, cudaEventDisableTiming));
     if (sl.graph) { cudaGraphExecDestroy(sl.graph); sl.graph = nullptr; }   // (a PAF-parser graph of an earlier use of this slot)
     int hcap = 0;
     hp_pifpaf_pipeline_info(dec, nullptr, nullptr, &hcap);
-    const size_t need_h = (size_t)e->max_batch * hcap;
-    if (sl.pin_humans_n < need_h) {
-        if (sl.pin_humans) cudaFreeHost(sl.pin_humans);
-        sl.pin_humans = nullptr; sl.pin_humans_n = 0;
-        HP_CUDA_TRY(cudaMallocHost(&sl.pin_humans, need_h * sizeof(hp_human)));
-        sl.pin_humans_n = need_h;
-    }
-    if (sl.pin_counts_n < (size_t)2 * e->max_batch) {
-        if (sl.pin_counts) cudaFreeHost(sl.pin_counts);
-        sl.pin_counts = nullptr; sl.pin_counts_n = 0;
-        HP_CUDA_TRY(cudaMallocHost(&sl.pin_counts, (size_t)2 * e->max_batch * sizeof(int)));
-        sl.pin_counts_n = (size_t)2 * e->max_batch;
-    }
-    sl.N = N; sl.hcap = hcap; sl.parser = nullptr; sl.decoder = dec;
+    const int rc = slot_alloc(e, sl, hcap);
+    if (rc) return rc;
+    if (!sl.conv_done) HP_CUDA_TRY(cudaEventCreateWithFlags(&sl.conv_done, cudaEventDisableTiming));
+    sl.N = N; sl.parser = nullptr; sl.decoder = dec;
     return HP_OK;
 }
 
@@ -2114,29 +1971,9 @@ static int pose_submit_pifpaf(hp_engine* e, hp_pifpaf* dec, const uint8_t* frame
     if (sl.busy) { set_error("hp_pose_submit_pifpaf: two batches are already in flight -- collect ticket %d first", idx); return HP_ERR_ARG; }
     int rc = pifpaf_slot_prepare(e, sl, dec, N);
     if (rc) return rc;
-    // the decoder's growth kernel (one warp per frame) runs underneath the next batch's convolutions: leave it some SMs
-    {
-        static const char* rs = getenv("HPB_PIFPAF_RESERVE_SMS");
-        const int want = rs ? atoi(rs) : std::min(e->max_batch, 16);
-        e->reserve_sms = std::max(0, std::min(want, e->num_sms / 2));
-    }
-    const size_t bytes = (size_t)N * e->in_h * e->in_w * 3;
-    if (device_src) {
-        HP_CUDA_TRY(cudaMemcpyAsync(sl.d_frames, frames, bytes, cudaMemcpyDeviceToDevice, e->stream));
-    } else {
-        cudaPointerAttributes attr;
-        const bool pinned = (cudaPointerGetAttributes(&attr, frames) == cudaSuccess && attr.type == cudaMemoryTypeHost);
-        if (!pinned) cudaGetLastError();
-        const uint8_t* src = frames;
-        if (!pinned) {
-            if (!sl.pin_frames) HP_CUDA_TRY(cudaMallocHost(&sl.pin_frames, (size_t)e->max_batch * e->in_h * e->in_w * 3));
-            memcpy(sl.pin_frames, frames, bytes);
-            src = sl.pin_frames;
-        }
-        HP_CUDA_TRY(cudaMemcpyAsync(sl.d_frames, src, bytes, cudaMemcpyHostToDevice, e->copy_stream));
-        HP_CUDA_TRY(cudaEventRecord(sl.h2d_done, e->copy_stream));
-        HP_CUDA_TRY(cudaStreamWaitEvent(e->stream, sl.h2d_done, 0));
-    }
+    e->reserve_sms = e->opt.pifpaf_reserve_sms;   // the decoder's growth kernel (one warp per frame) runs underneath the next batch's convolutions
+    rc = slot_upload(e, sl, frames, N, device_src);
+    if (rc) return rc;
     rc = pifpaf_enqueue(e, sl);
     if (rc) return rc;
     sl.busy = true;
@@ -2154,25 +1991,10 @@ static int pose_submit(hp_engine* e, hp_paf* parser, const uint8_t* frames, int 
     const int idx = e->next_slot;
     hp_engine::PoseSlot& sl = e->slots[idx];
     if (sl.busy) { set_error("hp_pose_submit: two batches are already in flight -- collect ticket %d first", idx); return HP_ERR_ARG; }
-    int rc = pose_slot_prepare(e, sl, idx, parser, N);
+    int rc = pose_slot_prepare(e, sl, parser, N);
     if (rc) return rc;
-    const size_t bytes = (size_t)N * e->in_h * e->in_w * 3;
-    if (device_src) {   // frames already in HBM: a D2D copy into the slot (the captured graph reads the slot's buffer), on the compute stream
-        HP_CUDA_TRY(cudaMemcpyAsync(sl.d_frames, frames, bytes, cudaMemcpyDeviceToDevice, e->stream));
-    } else {
-        cudaPointerAttributes attr;
-        const bool pinned = (cudaPointerGetAttributes(&attr, frames) == cudaSuccess && attr.type == cudaMemoryTypeHost);
-        if (!pinned) cudaGetLastError();
-        const uint8_t* src = frames;
-        if (!pinned) {   // pageable caller memory: through this slot's pinned staging (free: the slot was collected)
-            if (!sl.pin_frames) HP_CUDA_TRY(cudaMallocHost(&sl.pin_frames, (size_t)e->max_batch * e->in_h * e->in_w * 3));
-            memcpy(sl.pin_frames, frames, bytes);
-            src = sl.pin_frames;
-        }
-        HP_CUDA_TRY(cudaMemcpyAsync(sl.d_frames, src, bytes, cudaMemcpyHostToDevice, e->copy_stream));
-        HP_CUDA_TRY(cudaEventRecord(sl.h2d_done, e->copy_stream));
-        HP_CUDA_TRY(cudaStreamWaitEvent(e->stream, sl.h2d_done, 0));
-    }
+    rc = slot_upload(e, sl, frames, N, device_src);   // (the captured graph reads the slot's buffer)
+    if (rc) return rc;
     rc = pose_launch(e, sl);
     if (rc) return rc;
     HP_CUDA_TRY(cudaEventRecord(sl.done, e->stream));
@@ -2236,7 +2058,7 @@ int hp_pose_collect(hp_engine* e, int ticket, hp_human* out, int cap, int* n_out
         // the reference is unbounded: grow the parser capacity that overflowed and run this slot's frames again (they are still
         // in its device buffer), synchronously and outside the graph
         if (hp_paf_grow_capacity(sl.parser, flags) != HP_OK) { set_error("hp_pose_collect: parser capacity limit reached (flags=%d)", flags); return HP_ERR_CAPACITY; }
-        int rc = pose_slot_prepare(e, sl, ticket, sl.parser, N);
+        int rc = pose_slot_prepare(e, sl, sl.parser, N);
         if (rc) return rc;
         rc = pose_enqueue_compute(e, sl, e->stream);
         if (rc) return rc;
