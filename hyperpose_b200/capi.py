@@ -196,7 +196,7 @@ EXPORTS += [
     "hp_pose_submit_u8_host", "hp_pose_collect", "hp_pose_stats", "hp_paf_prepare", "hp_paf_state", "hp_paf_copy_results_host_async",
     "hp_paf_grow_capacity", "hp_pool_create", "hp_pool_destroy", "hp_pool_size", "hp_pool_set_capacity", "hp_pool_run_u8_host",
     "hp_pool_set_output_override", "hp_pool_launch_count", "hp_default_device", "hp_handoff_device_of",
-    "hp_engine_create_ex", "hp_engine_dtype", "hp_pose_submit_u8_device",
+    "hp_engine_create_ex", "hp_engine_dtype", "hp_pose_submit_u8_device", "hp_engine_debug_op_kernel",
 ]
 
 
@@ -220,6 +220,7 @@ def _bind_engine(L):
     L.hp_engine_debug_read_buffer.argtypes = [vp, C.c_int, vp, C.c_int, ip, ip, ip]
     L.hp_engine_debug_write_buffer.argtypes = [vp, C.c_int, vp, C.c_int]
     L.hp_engine_debug_run_ops.argtypes = [vp, C.c_int, C.c_int, C.c_int]
+    L.hp_engine_debug_op_kernel.argtypes = [vp, C.c_int, C.c_char_p, C.c_int]
     L.hp_pose_run_u8_host.argtypes = [vp, vp, vp, C.c_int, vp, C.c_int, ip]
     L.hp_engine_stage_frame_u8.argtypes = [vp, C.c_int, vp, C.c_int, C.c_int, C.c_int]
     L.hp_engine_infer_staged.argtypes = [vp, C.c_int]
@@ -378,6 +379,12 @@ class Engine:
 
     def debug_run_ops(self, first: int, last: int, n: int):
         check(lib().hp_engine_debug_run_ops(self._h, first, last, n))
+
+    def debug_op_kernel(self, op: int) -> str:
+        """the kernel op `op` launches on the next run over u8 frames, e.g. "conv<f16,48,res>", "halo<64,pool>", "none" """
+        buf = C.create_string_buffer(64)
+        check(lib().hp_engine_debug_op_kernel(self._h, op, buf, len(buf)))
+        return buf.value.decode()
 
     def set_output_override(self, d_conf_ptr: int, d_paf_ptr: int):
         check(lib().hp_engine_set_output_override(self._h, d_conf_ptr, d_paf_ptr))

@@ -797,6 +797,12 @@ int build_conv_plan(hp_engine* e, EngOp& op, const float* blob)
             set_error("engine: output conv must produce conf(%u)+paf(%u) channels", e->hdr.conf_channels, e->hdr.paf_channels);
             return HP_ERR_ARG;
         }
+        // the conf / paf outputs hold out_h x out_w planes: the conv writes one per input pixel
+        if (e->hdr.head_type != 0 || ib.H != e->out_h || ib.W != e->out_w) {
+            set_error("engine: output conv op %d reads a %dx%d buffer but the outputs are %dx%d conf/paf planes (head_type %u)",
+                      (int)(&op - e->ops.data()), ib.H, ib.W, e->out_h, e->out_w, e->hdr.head_type);
+            return HP_ERR_ARG;
+        }
     } else {
         const EngBuffer& ob = e->bufs[po.out_buf];
         if (ob.H != ib.H || ob.W != ib.W || (int)po.out_ch_off + G * cout_g > ob.channels) { set_error("engine: conv output buffer mismatch"); return HP_ERR_ARG; }
@@ -1312,11 +1318,23 @@ int hp_engine_create_ex(hp_engine** out, const void* pack, size_t pack_bytes, in
             e->flops_per_frame += 2.0 * ob.H * ob.W * C * K * K;
             op.launch = tf32 ? Launch::DwF32 : K == 3 && stride == 1 ? Launch::DwCol : Launch::DwStrip;
         } else if (po.type == OP_MAXPOOL2) {
-            if (po.cout_g % 8 || e->bufs[po.out_buf].down != e->bufs[po.in_buf].down + 1 || (po.R != 0 && po.R != 2 && po.R != 3)) { set_error("engine: bad maxpool op %u", i); return fail(HP_ERR_ARG); }
+            // 8 channels per 16-byte load (fp16) / two float4 loads (fp32): both offsets aligned, both channel ranges inside their buffers
+            const EngBuffer& ib = e->bufs[po.in_buf];
+            const EngBuffer& ob = e->bufs[po.out_buf];
+            if (po.cout_g % 8 || ob.down != ib.down + 1 || (po.R != 0 && po.R != 2 && po.R != 3) || po.in_ch_off % 8 || po.out_ch_off % 8 ||
+                (uint64_t)po.in_ch_off + po.cout_g > (uint64_t)ib.channels || (uint64_t)po.out_ch_off + po.cout_g > (uint64_t)ob.channels) {
+                set_error("engine: bad maxpool op %u", i);
+                return fail(HP_ERR_ARG);
+            }
             op.launch = tf32 ? Launch::MaxPoolF32 : Launch::MaxPool;
         } else if (po.type == OP_PIFPAF_HEAD) {
+            // the head kernels read input row y >> 1 for every output row y < out_h: both inputs must be at the output resolution
             if (hdr.head_type != 1 || po.res_buf >= hdr.n_buffers || hdr.conf_channels != 85 || hdr.paf_channels != 171 ||
-                e->bufs[po.in_buf].channels < 340 || e->bufs[po.res_buf].channels < 684) { set_error("engine: bad pifpaf head op"); return fail(HP_ERR_ARG); }
+                e->bufs[po.in_buf].channels < 340 || e->bufs[po.res_buf].channels < 684 ||
+                e->bufs[po.in_buf].down != (int)hdr.out_down_shift || e->bufs[po.res_buf].down != (int)hdr.out_down_shift) {
+                set_error("engine: bad pifpaf head op %u", i);
+                return fail(HP_ERR_ARG);
+            }
             op.launch = tf32 ? Launch::HeadsF32 : Launch::Heads;
         } else {
             set_error("engine: unknown op type %u", po.type);
@@ -1741,6 +1759,40 @@ int hp_engine_debug_run_ops(hp_engine* e, int first_op, int last_op, int N)
     int rc = run_graph(e, N, true, e->stream, first_op, last_op);
     if (rc) return rc;
     HP_CUDA_TRY(cudaStreamSynchronize(e->stream));
+    return HP_OK;
+}
+
+// test hook: the kernel op `op` launches on the next run over u8 frames, as decided when the engine was created (EngOp::launch and
+// the conv plan's tile width): conv<f16|tf32,BN[,res][,stem3|stem7]>, halo<BN[,pool]>, dw_strip<K,S>, dw_col, dw_tma<1|2>, dw_f32,
+// maxpool<K>, maxpool_f32, im2col, heads, or none when a neighbouring op's launch covers it
+int hp_engine_debug_op_kernel(const hp_engine* e, int op, char* name, int cap)
+{
+    if (!e || op < 0 || op >= (int)e->ops.size() || !name || cap <= 0) { set_error("hp_engine_debug_op_kernel: bad argument"); return HP_ERR_ARG; }
+    const EngOp& o = e->ops[op];
+    const PackOp& po = o.po;
+    const int BN = o.plan.prm.BN;
+    const bool tf32 = e->dtype == HP_DTYPE_TF32;
+    std::string s;
+    switch (o.launch) {
+    case Launch::None: case Launch::StemOrIm2col: s = "none"; break;
+    case Launch::Im2col: case Launch::Im2colF32: s = "im2col"; break;
+    case Launch::Conv:
+        s = std::string("conv<") + (tf32 ? "tf32," : "f16,") + std::to_string(BN) + (o.plan.prm.res_mode ? ",res>" : ">");
+        break;
+    case Launch::ConvStem: s = "conv<f16," + std::to_string(BN) + ",stem" + std::to_string(po.R) + ">"; break;
+    case Launch::Halo: s = "halo<" + std::to_string(BN) + ">"; break;
+    case Launch::HaloPool: s = "halo<" + std::to_string(BN) + ",pool>"; break;
+    case Launch::DwTma: s = "dw_tma<1>"; break;
+    case Launch::DwTmaPair: s = "dw_tma<2>"; break;
+    case Launch::DwCol: s = "dw_col"; break;
+    case Launch::DwStrip: s = "dw_strip<" + std::to_string(po.R) + "," + std::to_string(po.stride ? po.stride : 1) + ">"; break;
+    case Launch::MaxPool: s = "maxpool<" + std::to_string(po.R ? po.R : 2) + ">"; break;
+    case Launch::Heads: case Launch::HeadsF32: s = "heads"; break;
+    case Launch::DwF32: s = "dw_f32"; break;
+    case Launch::MaxPoolF32: s = "maxpool_f32"; break;
+    }
+    if ((int)s.size() >= cap) { set_error("hp_engine_debug_op_kernel: %zu-character name, capacity %d", s.size(), cap); return HP_ERR_CAPACITY; }
+    memcpy(name, s.c_str(), s.size() + 1);
     return HP_OK;
 }
 

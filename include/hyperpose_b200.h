@@ -218,6 +218,10 @@ long long hp_engine_launch_count(const hp_engine* e);
 int hp_engine_debug_read_buffer(hp_engine* e, int buf, void* out_f16, int N, int* H, int* W, int* C);
 int hp_engine_debug_write_buffer(hp_engine* e, int buf, const void* in_f16, int N);
 int hp_engine_debug_run_ops(hp_engine* e, int first_op, int last_op, int N);
+/* test hook: the kernel op `op` launches on the next run over u8 frames, fixed at creation, as a NUL-terminated name in
+ * name[cap]: "conv<f16|tf32,BN[,res][,stem3|stem7]>", "halo<BN[,pool]>", "dw_strip<K,S>", "dw_col", "dw_tma<1|2>", "dw_f32",
+ * "maxpool<K>", "maxpool_f32", "im2col", "heads", or "none" for an op that a neighbouring op's launch covers */
+int hp_engine_debug_op_kernel(const hp_engine* e, int op, char* name, int cap);
 
 /* benchmark hook (SURVEY 8d): after the last conv of every run, copy these DEVICE tensors over the engine's
  * conf/paf outputs, so that random-init weights still give the parser a realistic load.  NULL disables it. */
