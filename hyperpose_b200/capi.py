@@ -155,7 +155,7 @@ class PafParser:
 
     def debug_timing(self, N: int):
         """HPB_PAF_TIMING=1: (cta[N,19,4] ns stamps: start, ordered, candidates, matched; asm[N,6]: assembly start, end | path in the low
-        two bits, then -- component-parallel path only -- staged, labelled, grouped, lanes done)"""
+        two bits (2 component-parallel, 1 sequential), then -- component-parallel path only -- staged, labelled, grouped, lanes done)"""
         out = np.zeros(N * (N_PAIRS * 4 + 6), np.uint64)
         lib().hp_paf_debug_timing.argtypes = [C.c_void_p, C.c_void_p, C.c_int]
         check(lib().hp_paf_debug_timing(self._h, out.ctypes.data, N))

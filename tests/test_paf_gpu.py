@@ -98,14 +98,14 @@ def test_noise_field_many_peaks_capacity_growth():
 
 
 def _assembly_paths(parser, N):
-    """which get_humans path assembled each frame of the last batch (needs HPB_PAF_TIMING=1): 2 component-parallel, 0 register, 1 shared memory"""
+    """which get_humans path assembled each frame of the last batch (needs HPB_PAF_TIMING=1): 2 component-parallel, 1 sequential"""
     _, asm = parser.debug_timing(N)
     return [int(v) & 3 for v in asm[:, 1]]
 
 
 def test_component_parallel_assembly_is_the_path_taken_and_the_sequential_paths_agree(monkeypatch):
     """crowd frames: the component-parallel get_humans (one lane per connected component of the peak / connection graph) is what runs,
-    and it equals the oracle; with HPB_PAF_SEQ_ASSEMBLY=1 the same frames go through the sequential register path -- same bytes"""
+    and it equals the oracle; with HPB_PAF_SEQ_ASSEMBLY=1 the same frames go through the sequential path -- same bytes"""
     monkeypatch.setenv("HPB_PAF_TIMING", "1")
     N, hf, wf = 6, 46, 82
     conf, paf = syn.make_batch_tensors(1000, N, (10, 20), hf, wf)
@@ -118,9 +118,23 @@ def test_component_parallel_assembly_is_the_path_taken_and_the_sequential_paths_
         _cmp_frame(got[i], want[i], f"fast frame{i}")
     monkeypatch.setenv("HPB_PAF_SEQ_ASSEMBLY", "1")
     got2 = parser.process_batch(conf, paf)
-    assert all(v in (0, 1) for v in _assembly_paths(parser, N))
+    assert _assembly_paths(parser, N) == [1] * N
     for i in range(N):
         assert got2[i].tobytes() == got[i].tobytes()
+    parser.close()
+
+
+def test_mixed_path_crowd_batch_vs_oracle(monkeypatch):
+    """cfg4-sized crowd batch in which one frame (15) has a merge that invents a peak id: that frame alone is handed back to the
+    sequential path, the other 31 stay on the component-parallel path, and every frame equals the oracle"""
+    monkeypatch.setenv("HPB_PAF_TIMING", "1")
+    N = 32
+    conf, paf = syn.make_batch_tensors(1001, N, (10, 20), 46, 54)
+    parser = capi.PafParser()
+    got = parser.process_batch(conf, paf)
+    assert _assembly_paths(parser, N) == [1 if i == 15 else 2 for i in range(N)]
+    for i in range(N):
+        _cmp_frame(got[i], oracle.oracle_process(conf[i], paf[i]), f"frame{i}")
     parser.close()
 
 

@@ -21,7 +21,7 @@ print("candidates  (us) mean dur", (rel[:, :, 2] - rel[:, :, 1]).mean(), "max", 
 print("matched     (us) mean dur", (rel[:, :, 3] - rel[:, :, 2]).mean(), "max", (rel[:, :, 3] - rel[:, :, 2]).max())
 print("limb phase end (us) per frame max", rel[:, :, 3].max(axis=1).round(1))
 print("assembly start", a[:, 0].round(1))
-print("assembly dur  ", (a[:, 1] - a[:, 0]).round(1), "path (2 component-parallel, 0 register, 1 shared memory):", (asm[:, 1] & 3).tolist())
+print("assembly dur  ", (a[:, 1] - a[:, 0]).round(1), "path (2 component-parallel, 1 sequential):", (asm[:, 1] & 3).tolist())
 print("  of which staged / labelled / grouped / lanes / output (us, mean over the frames on the component-parallel path):",
       [round(float(x), 2) for x in ((a[:, 2] - a[:, 0]).mean(), (a[:, 3] - a[:, 2]).mean(), (a[:, 4] - a[:, 3]).mean(), (a[:, 5] - a[:, 4]).mean(), (a[:, 1] - a[:, 5]).mean())])
 print("kernel span (us)", a[:, 1].max())
