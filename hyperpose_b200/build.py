@@ -85,6 +85,24 @@ def build_cpp_example(ref_root: str = "/root/reference") -> str | None:
     return exe
 
 
+def build_dtype_probe(ref_root: str = "/root/reference") -> str | None:
+    """examples/dtype_probe_b200.cpp: one f32 frame through the drop-in `tensorrt` built with a given `data_type` (or from a serialized
+    pack, HPB_DTYPE), outputs to a file -- which arithmetic the drop-in selected.  Built like build_cpp_example; returns the binary path,
+    or the prebuilt one / None when the reference headers are absent."""
+    exe = os.path.join(ROOT, "examples", "dtype_probe_b200")
+    if not os.path.isdir(os.path.join(ref_root, "include", "hyperpose")):
+        return exe if os.path.exists(exe) else None
+    srcs = [os.path.join(CSRC, "hyperpose_api", "tensorrt.cpp"), os.path.join(ROOT, "examples", "dtype_probe_b200.cpp")]
+    if _newer(srcs + [LIB, os.path.join(ROOT, "include", "hyperpose_b200.h")], exe):
+        cmd = ["g++", "-std=c++17", "-O2", "-DHP_B200_STANDALONE", "-I" + os.path.join(CSRC, "shim"), "-I" + os.path.join(ref_root, "include"),
+               "-I" + os.path.join(ROOT, "include")] + srcs + ["-L" + PKG, "-lhyperpose_b200", "-Wl,-rpath,$ORIGIN/../hyperpose_b200", "-o", exe]
+        r = subprocess.run(cmd, capture_output=True, text=True)
+        if r.returncode:
+            sys.stderr.write(r.stdout + r.stderr)
+            raise RuntimeError("dtype probe failed to compile against the reference headers")
+    return exe
+
+
 def build_stream_example(ref_root: str = "/root/reference", mock: bool = False) -> str | None:
     """examples/stream_api_b200.cpp: the reference's STREAM API on the drop-in.  The scheduler is the reference's own --
     include/hyperpose/stream/stream.hpp instantiated as it is, src/stream.cpp + src/thread_pool.cpp + src/logging.cpp compiled from

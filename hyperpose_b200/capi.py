@@ -9,6 +9,7 @@ from __future__ import annotations
 
 import ctypes as C
 import os
+import struct
 
 import numpy as np
 
@@ -197,6 +198,7 @@ EXPORTS += [
     "hp_paf_grow_capacity", "hp_pool_create", "hp_pool_destroy", "hp_pool_size", "hp_pool_set_capacity", "hp_pool_run_u8_host",
     "hp_pool_set_output_override", "hp_pool_launch_count", "hp_default_device", "hp_handoff_device_of",
     "hp_engine_create_ex", "hp_engine_dtype", "hp_pose_submit_u8_device", "hp_engine_debug_op_kernel",
+    "hp_engine_calibrate_u8", "hp_pack_int8_calibrated",
 ]
 
 
@@ -221,6 +223,8 @@ def _bind_engine(L):
     L.hp_engine_debug_write_buffer.argtypes = [vp, C.c_int, vp, C.c_int]
     L.hp_engine_debug_run_ops.argtypes = [vp, C.c_int, C.c_int, C.c_int]
     L.hp_engine_debug_op_kernel.argtypes = [vp, C.c_int, C.c_char_p, C.c_int]
+    L.hp_engine_calibrate_u8.argtypes = [vp, vp, C.c_int, vp, C.c_int]
+    L.hp_pack_int8_calibrated.argtypes = [vp, C.c_size_t]
     L.hp_pose_run_u8_host.argtypes = [vp, vp, vp, C.c_int, vp, C.c_int, ip]
     L.hp_engine_stage_frame_u8.argtypes = [vp, C.c_int, vp, C.c_int, C.c_int, C.c_int]
     L.hp_engine_infer_staged.argtypes = [vp, C.c_int]
@@ -255,7 +259,8 @@ class Engine:
 
     def __init__(self, pack: bytes, input_size, max_batch_size: int = 8, factor: float = 1.0 / 255, flip_rgb: bool = True,
                  device: int = 0, dtype: str = "f16"):
-        """dtype: "f16" (= data_type::kHALF) or "tf32" (= data_type::kFLOAT of the reference ctor, tensorrt.hpp:14-22)"""
+        """dtype: "f16" (= data_type::kHALF), "tf32" (= data_type::kFLOAT of the reference ctor, tensorrt.hpp:14-22) or "int8"
+        (= data_type::kINT8: needs a pack with a scale table, Graph.set_int8_scales)"""
         L = lib()
         if not getattr(L, "_engine_bound", False):
             _bind_engine(L)
@@ -264,7 +269,7 @@ class Engine:
         self._pack = pack
         self.dtype = dtype
         check(L.hp_engine_create_ex(C.byref(self._h), pack, len(pack), int(input_size[0]), int(input_size[1]), max_batch_size,
-                                    factor, 1 if flip_rgb else 0, device, {"f16": 0, "tf32": 1}[dtype]))
+                                    factor, 1 if flip_rgb else 0, device, {"f16": 0, "tf32": 1, "int8": 2}[dtype]))
         v = [C.c_int() for _ in range(7)]
         fl = C.c_double()
         check(L.hp_engine_info(self._h, *[C.byref(x) for x in v], C.byref(fl)))
@@ -369,13 +374,28 @@ class Engine:
     def debug_read_buffer(self, buf: int, n: int) -> np.ndarray:
         H, W, Cc = C.c_int(), C.c_int(), C.c_int()
         check(lib().hp_engine_debug_read_buffer(self._h, buf, None, n, C.byref(H), C.byref(W), C.byref(Cc)))
-        out = np.empty((n, H.value, W.value, Cc.value), np.float32 if self.dtype == "tf32" else np.float16)
+        out = np.empty((n, H.value, W.value, Cc.value), self._elem)
         check(lib().hp_engine_debug_read_buffer(self._h, buf, out.ctypes.data, n, C.byref(H), C.byref(W), C.byref(Cc)))
         return out
 
     def debug_write_buffer(self, buf: int, arr: np.ndarray):
-        arr = np.ascontiguousarray(arr, np.float32 if self.dtype == "tf32" else np.float16)
+        arr = np.ascontiguousarray(arr, self._elem)
         check(lib().hp_engine_debug_write_buffer(self._h, buf, arr.ctypes.data, arr.shape[0]))
+
+    @property
+    def _elem(self):
+        """element type of the activation buffers"""
+        return {"f16": np.float16, "tf32": np.float32, "int8": np.int8}[self.dtype]
+
+    def calibrate(self, frames: np.ndarray, absmax=None) -> np.ndarray:
+        """INT8 calibration (TensorRT's min-max calibrator) on a "tf32" engine: u8 frames [N,in_h,in_w,3] (N may exceed max_batch)
+        -> per-buffer max |x|, folded into `absmax` when given (a running maximum).  Graph.set_int8_scales turns it into scales."""
+        frames = np.ascontiguousarray(frames, np.uint8)
+        assert frames.ndim == 4 and frames.shape[1:] == (self.in_h, self.in_w, 3), frames.shape
+        n_buf = struct.unpack_from("<I", self._pack, 12)[0]
+        out = np.zeros(n_buf, np.float32) if absmax is None else np.array(absmax, np.float32).reshape(-1).copy()
+        check(lib().hp_engine_calibrate_u8(self._h, frames.ctypes.data, frames.shape[0], out.ctypes.data, out.size))
+        return out
 
     def debug_run_ops(self, first: int, last: int, n: int):
         check(lib().hp_engine_debug_run_ops(self._h, first, last, n))

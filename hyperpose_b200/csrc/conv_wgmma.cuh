@@ -66,7 +66,17 @@ struct ConvParams {
     int in_h, in_w, stem_stride, stem_pad_h, stem_pad_w, flip;
     double factor;
     float mean[3];
+    // INT8 engine (conv_wgmma_kernel<int8_t, ...>): v = (float)acc * mul[c] + bias[c], mul = s_in * s_w[c]; a residual reads
+    // q_r * res_scale; NHWC stores clamp(rint(y * out_inv_scale), -127, 127)
+    const float* mul;          // [groups * cout_g_pad]
+    float out_inv_scale, res_scale;
+    int in_g_stride;           // input channels between groups (the real cin_g: a group's padded last k-step reads on into the next
+                               // group's channels, or past the buffer's end as zeros, against zero weights)
 };
+
+// accumulator element of conv_wgmma_kernel<T, ...>: fp32 for the fp16 / TF32 engines, s32 for the INT8 engine
+template <typename T> struct ConvAcc { using type = float; };
+template <> struct ConvAcc<int8_t> { using type = int; };
 
 namespace ptx {
 
@@ -178,11 +188,16 @@ template <int R> __device__ __forceinline__ void fence_acc(float (&d)[R])
 #pragma unroll
     for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
+template <int R> __device__ __forceinline__ void fence_acc(int (&d)[R])
+{
+#pragma unroll
+    for (int i = 0; i < R; ++i) asm volatile("" : "+r"(d[i])::"memory");
+}
 
 // D[64 x N] (+)= A[64 x K] * B[N x K]^T, both operands K-major in 128B-swizzled shared memory; K = 32 bytes of the element type
 // (16 fp16 / 8 tf32); scale_d = 0 overwrites D.  One specialisation per (element type, N) because the register list is part of the
 // instruction.
-template <typename T, int N> __device__ __forceinline__ void wgmma(float (&d)[N / 2], uint64_t da, uint64_t db, uint32_t scale_d);
+template <typename T, int N> __device__ __forceinline__ void wgmma(typename ConvAcc<T>::type (&d)[N / 2], uint64_t da, uint64_t db, uint32_t scale_d);
 template <> __device__ __forceinline__ void wgmma<__half, 16>(float (&d)[8], uint64_t da, uint64_t db, uint32_t scale_d)
 {
     asm volatile(
@@ -304,6 +319,66 @@ template <> __device__ __forceinline__ void wgmma<float, 128>(float (&d)[64], ui
         : "l"(da), "l"(db), "r"(scale_d));
 }
 
+template <> __device__ __forceinline__ void wgmma<int8_t, 16>(int (&d)[8], uint64_t da, uint64_t db, uint32_t scale_d)
+{
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n16k32.s32.s8.s8 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7}, "
+        "%8, %9, p;\n\t}"
+        : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7])
+        : "l"(da), "l"(db), "r"(scale_d));
+}
+template <> __device__ __forceinline__ void wgmma<int8_t, 32>(int (&d)[16], uint64_t da, uint64_t db, uint32_t scale_d)
+{
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k32.s32.s8.s8 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
+        "%16, %17, p;\n\t}"
+        : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15])
+        : "l"(da), "l"(db), "r"(scale_d));
+}
+template <> __device__ __forceinline__ void wgmma<int8_t, 48>(int (&d)[24], uint64_t da, uint64_t db, uint32_t scale_d)
+{
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %26, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n48k32.s32.s8.s8 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23}, "
+        "%24, %25, p;\n\t}"
+        : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23])
+        : "l"(da), "l"(db), "r"(scale_d));
+}
+template <> __device__ __forceinline__ void wgmma<int8_t, 64>(int (&d)[32], uint64_t da, uint64_t db, uint32_t scale_d)
+{
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k32.s32.s8.s8 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+        "%32, %33, p;\n\t}"
+        : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31])
+        : "l"(da), "l"(db), "r"(scale_d));
+}
+template <> __device__ __forceinline__ void wgmma<int8_t, 96>(int (&d)[48], uint64_t da, uint64_t db, uint32_t scale_d)
+{
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %50, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n96k32.s32.s8.s8 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47}, "
+        "%48, %49, p;\n\t}"
+        : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]), "+r"(d[32]), "+r"(d[33]), "+r"(d[34]), "+r"(d[35]), "+r"(d[36]), "+r"(d[37]), "+r"(d[38]), "+r"(d[39]), "+r"(d[40]), "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]), "+r"(d[46]), "+r"(d[47])
+        : "l"(da), "l"(db), "r"(scale_d));
+}
+template <> __device__ __forceinline__ void wgmma<int8_t, 128>(int (&d)[64], uint64_t da, uint64_t db, uint32_t scale_d)
+{
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k32.s32.s8.s8 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+        "%64, %65, p;\n\t}"
+        : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]), "+r"(d[32]), "+r"(d[33]), "+r"(d[34]), "+r"(d[35]), "+r"(d[36]), "+r"(d[37]), "+r"(d[38]), "+r"(d[39]), "+r"(d[40]), "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]), "+r"(d[46]), "+r"(d[47]), "+r"(d[48]), "+r"(d[49]), "+r"(d[50]), "+r"(d[51]), "+r"(d[52]), "+r"(d[53]), "+r"(d[54]), "+r"(d[55]), "+r"(d[56]), "+r"(d[57]), "+r"(d[58]), "+r"(d[59]), "+r"(d[60]), "+r"(d[61]), "+r"(d[62]), "+r"(d[63])
+        : "l"(da), "l"(db), "r"(scale_d));
+}
 } // namespace ptx
 
 struct ConvTile {
@@ -374,15 +449,25 @@ __device__ __forceinline__ void im2col_chunk(const void* __restrict__ in, uint4*
 
 // T = __half: fp16 activations, kind f16; T = float: fp32 activations on the TF32 grid, kind tf32 (the data_type::kFLOAT engine:
 // every producer of a conv operand rounds to TF32 with round-to-nearest, so the tensor core's truncation on read is exact).
+// T = int8_t: the INT8 engine -- symmetric int8 activations and per-output-channel int8 weights, kind s8 (k32) with exact s32
+// accumulation; the epilogue (conv_epilogue_i8) rescales, adds bias / residual, applies PReLU and requantizes in fp32 with
+// separately rounded operations, so that a CPU model reproduces every output byte.
 // kRes: residual epilogue compiled in (ResNet / LW-OpenPose blocks).
 // kStemR = 3 | 7: fused u8 stem -- the conv's input is the RxRx3 patch of each output pixel gathered from the u8 frames by the 128
 // threads of warpgroup 0 straight into the swizzled A tile (im2col_chunk, the same values im2col3_kernel writes), so the im2col
 // buffer is never written; the B tile still comes by TMA.
+// y -> int8 of the output buffer: clamp(rint(y * inv_s), -127, 127), the product rounded on its own
+__device__ __forceinline__ int8_t quantize_i8(float y, float inv_s)
+{
+    return (int8_t)min(max(__float2int_rn(__fmul_rn(y, inv_s)), -127), 127);
+}
+
 template <typename T, int BN, bool kRes, int kStemR = 0>
 __global__ void __launch_bounds__(CONV_THREADS, 1)
 conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b, const ConvParams p)
 {
     constexpr bool kF16 = std::is_same<T, __half>::value;
+    constexpr bool kI8 = std::is_same<T, int8_t>::value;
     constexpr int BK = 128 / (int)sizeof(T);                 // channels per k-step
     constexpr int STAGE_BYTES = CONV_A_BYTES + BN * 128;      // a multiple of 1024: every tile stays aligned to the swizzle atom
     extern __shared__ uint8_t smem_raw[];
@@ -457,7 +542,7 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
             for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
                 const ConvTile t = decode_tile(p, tile, n_tiles_g);
                 const PixelPos q0 = unflatten(p, t.p0);
-                const int a_ch0 = p.in_ch_off + t.g * p.cin_g;
+                const int a_ch0 = p.in_ch_off + t.g * (kI8 ? p.in_g_stride : p.cin_g);
                 const int b_row = t.g * p.cout_g_pad + t.n0;
                 int kcol = 0;
                 for (int r = 0; r < p.R; ++r)
@@ -482,7 +567,7 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
     const int col0 = 2 * (lane & 3);                           // columns col0 + 8 j + {0, 1}
     const int total_px = p.Nb * p.H * p.W;
     const uint32_t smem0 = ptx::smem_u32(smem);
-    float acc[BN / 2];
+    typename ConvAcc<T>::type acc[BN / 2];
     int stage = 0;
     uint32_t phase = 0;
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
@@ -526,6 +611,43 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
             for (int j = 0; j < BN / 8; ++j) {
                 const int c = 8 * j + col0;
                 if (c >= n_valid) break;
+                if constexpr (kI8) {   // no FMA contraction anywhere: every product and sum is rounded on its own
+                    const float* mul = p.mul + t.g * p.cout_g_pad + t.n0;
+                    const bool two = c + 1 < n_valid;
+                    float y[2], r[2] = { 0.f, 0.f };
+                    if (kRes && p.res_mode) {
+                        const size_t ri = pix * p.res_ld + p.res_ch_off + t.g * p.cout_g + t.n0 + c;
+                        const char2 rq = *(const char2*)((const int8_t*)p.res + ri);
+                        r[0] = __fmul_rn((float)rq.x, p.res_scale); r[1] = __fmul_rn((float)rq.y, p.res_scale);
+                    }
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) {
+                        float v = __fadd_rn(__fmul_rn((float)acc[4 * j + 2 * h + e], __ldg(mul + c + e)), __ldg(bias + c + e));
+                        if (kRes && p.res_mode == 1) v = __fadd_rn(v, r[e]);
+                        v = v > 0.f ? v : __fmul_rn(v, __ldg(alpha + c + e));
+                        if (kRes && p.res_mode == 2) v = __fadd_rn(v, r[e]);
+                        y[e] = v;
+                    }
+                    if (p.out_mode == OUT_F16_NHWC) {
+                        int8_t* o = (int8_t*)p.out + pix * p.out_ld + och + c;
+                        const int8_t q0 = quantize_i8(y[0], p.out_inv_scale), q1 = quantize_i8(y[1], p.out_inv_scale);
+                        if (two && pair_ok) *(char2*)o = make_char2(q0, q1);
+                        else { o[0] = q0; if (two) o[1] = q1; }
+                    } else {
+#pragma unroll
+                        for (int e = 0; e < 2; ++e) {
+                            if (e == 1 && !two) break;
+                            const int ch = t.n0 + c + e;
+                            if (ch < p.split) {
+                                ((float*)p.out)[(((size_t)q.n * p.split + ch) * p.H + q.h) * p.W + q.w] = y[e];
+                            } else {
+                                const int c2 = ch - p.split, n2 = p.cout_g - p.split;
+                                ((float*)p.out2)[(((size_t)q.n * n2 + c2) * p.H + q.h) * p.W + q.w] = y[e];
+                            }
+                        }
+                    }
+                    continue;
+                }
                 float a0 = acc[4 * j + 2 * h] + __ldg(bias + c), a1 = acc[4 * j + 2 * h + 1] + __ldg(bias + c + 1);
                 float r0 = 0.f, r1 = 0.f;
                 if (kRes && p.res_mode) {   // (residual layers: cout_g % 16 == 0, so both channels exist and the pair is aligned)

@@ -26,6 +26,7 @@
 #include "common.h"
 #include "conv_wgmma.cuh"
 #include "conv_tf32.cuh"
+#include "conv_int8.cuh"
 #include "handoff.h"
 #include "pair_math.cuh"
 #include "pack_format.h"
@@ -492,11 +493,19 @@ typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_
 typedef CUresult (*PFN_encodeIm2col)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*, const int*, const int*,
                                      cuuint32_t, cuuint32_t, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion,
                                      CUtensorMapFloatOOBfill);
-// activations [N,H,W,C] fp16 (fp32) in im2col mode: 128 consecutive output pixels x 64 (32) channels per load; the bounding box
-// [-pad, dim - pad) holds one base position per output pixel, filter taps are the im2col offsets of the copy instruction
-int make_tmap_act_im2col(CUtensorMap* m, const void* base, int N, int H, int W, int C, int R, int S, bool f32)
+// TMA element type and size of an engine's activations / weights (the copy ignores signedness: int8 travels as UINT8)
+CUtensorMapDataType tmap_type(int dtype)
 {
-    const int es = f32 ? 4 : 2;
+    return dtype == HP_DTYPE_TF32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : dtype == HP_DTYPE_INT8 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+}
+int elem_bytes(int dtype) { return dtype == HP_DTYPE_TF32 ? 4 : dtype == HP_DTYPE_INT8 ? 1 : 2; }
+
+// activations [N,H,W,C] fp16 (fp32, int8) in im2col mode: 128 consecutive output pixels x 128 bytes of channels per load; the bounding
+// box [-pad, dim - pad) holds one base position per output pixel, filter taps are the im2col offsets of the copy instruction.
+// Channels past C read as zeros.
+int make_tmap_act_im2col(CUtensorMap* m, const void* base, int N, int H, int W, int C, int R, int S, int dtype)
+{
+    const int es = elem_bytes(dtype);
     const auto enc = (PFN_encodeIm2col)driver_entry_point("cuTensorMapEncodeIm2col");
     if (!enc) { set_error("cuTensorMapEncodeIm2col entry point not available"); return HP_ERR_CUDA; }
     cuuint64_t dims[4] = { (cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)N };
@@ -505,21 +514,22 @@ int make_tmap_act_im2col(CUtensorMap* m, const void* base, int N, int H, int W, 
     int lower[2] = { -pad_w, -pad_h };
     int upper[2] = { pad_w - (S - 1), pad_h - (R - 1) };
     cuuint32_t estr[4] = { 1, 1, 1, 1 };
-    CUresult r = enc(m, f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, (void*)base, dims, strides, lower, upper, f32 ? 32 : 64, (cuuint32_t)CONV_BLOCK_M, estr,
+    CUresult r = enc(m, tmap_type(dtype), 4, (void*)base, dims, strides, lower, upper, 128 / es, (cuuint32_t)CONV_BLOCK_M, estr,
                      CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeIm2col failed: %d (N=%d H=%d W=%d C=%d R=%d S=%d)", (int)r, N, H, W, C, R, S); return HP_ERR_CUDA; }
     return HP_OK;
 }
-// weights [rows, K] fp16 (fp32) K-major: dims (K, rows), box (64 (32), BN)
-int make_tmap_wgt(CUtensorMap* m, const void* base, int rows, int K, int BN, bool f32)
+// weights [rows, K] fp16 (fp32, int8) K-major: dims (K, rows), box (128 bytes, BN)
+int make_tmap_wgt(CUtensorMap* m, const void* base, int rows, int K, int BN, int dtype)
 {
+    const int es = elem_bytes(dtype);
     const auto enc = (PFN_encodeTiled)driver_entry_point("cuTensorMapEncodeTiled");
     if (!enc) { set_error("cuTensorMapEncodeTiled entry point not available"); return HP_ERR_CUDA; }
     cuuint64_t dims[2] = { (cuuint64_t)K, (cuuint64_t)rows };
-    cuuint64_t strides[1] = { (cuuint64_t)K * (f32 ? 4 : 2) };
-    cuuint32_t box[2] = { f32 ? 32u : 64u, (cuuint32_t)BN };
+    cuuint64_t strides[1] = { (cuuint64_t)K * es };
+    cuuint32_t box[2] = { (cuuint32_t)(128 / es), (cuuint32_t)BN };
     cuuint32_t estr[2] = { 1, 1 };
-    CUresult r = enc(m, f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, (void*)base, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+    CUresult r = enc(m, tmap_type(dtype), 2, (void*)base, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                      CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled(weights) failed: %d (rows=%d K=%d BN=%d)", (int)r, rows, K, BN); return HP_ERR_CUDA; }
     return HP_OK;
@@ -569,6 +579,7 @@ struct ConvPlan {
     HaloParams hp;               // halo plan: conv_halo_kernel's parameters
     float* d_bias = nullptr;
     float* d_alpha = nullptr;
+    float* d_mul = nullptr;      // INT8 engine: s_in * s_w[o] per (padded) output channel
     size_t smem = 0;
     double flops_per_frame = 0;
 };
@@ -590,6 +601,8 @@ enum class Launch : uint8_t {
     Heads,          // two pifpaf_head_kernel launches
     // TF32 engine: fp32 activations (conv_tf32.cuh); its convs are Conv
     Im2colF32, DwF32, MaxPoolF32, HeadsF32,
+    // INT8 engine: int8 activations (conv_int8.cuh); its convs are Conv
+    Im2colI8, DwI8, MaxPoolI8,
 };
 
 // kernels an op launches per run: what launch_count counts, and what a graph replay of the step stands for
@@ -651,7 +664,8 @@ struct EngBuffer {
 
 struct hp_engine {
     int device = 0;
-    int dtype = 0;   // HP_DTYPE_F16 | HP_DTYPE_TF32
+    int dtype = 0;   // HP_DTYPE_F16 | HP_DTYPE_TF32 | HP_DTYPE_INT8
+    std::vector<float> act_scale;   // INT8 engine: the pack's scale of every activation buffer
     int in_h = 0, in_w = 0, max_batch = 0;
     double factor = 1.0 / 255;
     int flip_rgb = 1;
@@ -731,24 +745,36 @@ inline float tf32_round(float x)
 }
 
 // The conv's GEMM operands, epilogue and tensor maps.  data_type::kHALF: fp16 activations and weights, 64-channel chunks;
-// data_type::kFLOAT (HP_DTYPE_TF32): fp32 activations on the TF32 grid, 32-channel chunks (conv_wgmma_kernel<float, ...>).
+// data_type::kFLOAT (HP_DTYPE_TF32): fp32 activations on the TF32 grid, 32-channel chunks (conv_wgmma_kernel<float, ...>);
+// data_type::kINT8 (HP_DTYPE_INT8): int8 activations and per-output-channel int8 weights, 128-channel chunks
+// (conv_wgmma_kernel<int8_t, ...>).  An INT8 k-step may run past the input buffer's last channel: the TMA reads those as zeros.
 int build_conv_plan(hp_engine* e, EngOp& op, const float* blob)
 {
     const PackOp& po = op.po;
     ConvPlan& pl = op.plan;
-    const bool tf32 = e->dtype == HP_DTYPE_TF32;
-    const int chunk = tf32 ? 32 : 64;
-    const size_t es = tf32 ? sizeof(float) : sizeof(__half);
+    const bool tf32 = e->dtype == HP_DTYPE_TF32, i8 = e->dtype == HP_DTYPE_INT8;
+    const int chunk = tf32 ? 32 : i8 ? 128 : 64;
+    const size_t es = (size_t)elem_bytes(e->dtype);
     const EngBuffer& ib = e->bufs[po.in_buf];
     const int G = (int)po.groups, R = (int)po.R, S = (int)po.S, cin_g = (int)po.cin_g, cout_g = (int)po.cout_g;
     const bool im2col = po.im2col_input != 0;
     if (im2col && (G != 1 || R * S * cin_g > ib.channels)) { set_error("engine: bad im2col conv"); return HP_ERR_ARG; }
-    if (!im2col && G > 1 && cin_g % chunk != 0) { set_error("engine: grouped conv needs cin_g %% %d == 0 (got %d)", chunk, cin_g); return HP_ERR_UNSUPPORTED; }
+    if (!im2col && G > 1 && cin_g % (i8 ? 16 : chunk) != 0) { set_error("engine: grouped conv needs cin_g %% %d == 0 (got %d)", i8 ? 16 : chunk, cin_g); return HP_ERR_UNSUPPORTED; }
     // effective GEMM view
     const int eR = im2col ? 1 : R, eS = im2col ? 1 : S;
     const int ecin = im2col ? round_up(R * S * cin_g, chunk) : round_up(cin_g, chunk);
-    if ((int)po.in_ch_off + G * ecin > ib.channels) {
-        set_error("engine: conv reads channels [%d,%d) of a %d-channel buffer", po.in_ch_off, po.in_ch_off + G * ecin, ib.channels);
+    const int reads = i8 ? (im2col ? R * S * cin_g : G * cin_g) : G * ecin;   // channels that must lie inside the buffer
+    if ((int)po.in_ch_off + reads > ib.channels) {
+        set_error("engine: conv reads channels [%d,%d) of a %d-channel buffer", po.in_ch_off, po.in_ch_off + reads, ib.channels);
+        return HP_ERR_ARG;
+    }
+    if (i8 && (long long)R * S * cin_g * 127 * 127 > 0x7fffffffLL) {   // the s32 accumulator must stay exact
+        set_error("engine: INT8 conv op %d sums %d products per output (%dx%dx%d); the s32 accumulator is exact up to %d", (int)(&op - e->ops.data()), R * S * cin_g,
+                  R, S, cin_g, 0x7fffffff / (127 * 127));
+        return HP_ERR_UNSUPPORTED;
+    }
+    if (i8 && ib.channels % 16) {   // a TMA row stride is a multiple of 16 bytes
+        set_error("engine: INT8 conv op %d reads buffer %u of %d channels (needs a multiple of 16)", (int)(&op - e->ops.data()), po.in_buf, ib.channels);
         return HP_ERR_ARG;
     }
     const int BN = pick_bn(cout_g);
@@ -770,14 +796,33 @@ int build_conv_plan(hp_engine* e, EngOp& op, const float* blob)
                     }
         }
     std::vector<__half> wh;
-    if (!tf32) {
+    if (!tf32 && !i8) {
         wh.resize(w.size());
         for (size_t i = 0; i < w.size(); ++i) wh[i] = __float2half_rn(w[i]);
+    }
+    // INT8: s_w[o] = max |W[o]| / 127 (1 for an all-zero row), q = clamp(nearbyint(W / s_w), -127, 127), mul[o] = s_in * s_w[o]
+    std::vector<int8_t> wq;
+    std::vector<float> mul;
+    if (i8) {
+        wq.assign(w.size(), 0);
+        mul.assign(bias.size(), 0.f);
+        const float s_in = e->act_scale[po.in_buf];
+        for (size_t row = 0; row < (size_t)G * cout_pad; ++row) {
+            if ((int)(row % cout_pad) >= cout_g) continue;
+            const float* wr = w.data() + row * K;
+            float amax = 0.f;
+            for (int k = 0; k < K; ++k) amax = std::max(amax, fabsf(wr[k]));
+            const float sw = amax > 0.f ? amax / 127.0f : 1.0f;
+            for (int k = 0; k < K; ++k) wq[row * K + k] = (int8_t)std::min(127.0f, std::max(-127.0f, nearbyintf(wr[k] / sw)));
+            mul[row] = s_in * sw;
+        }
+        HP_CUDA_TRY(cudaMalloc(&pl.d_mul, mul.size() * sizeof(float)));
+        HP_CUDA_TRY(cudaMemcpy(pl.d_mul, mul.data(), mul.size() * sizeof(float), cudaMemcpyHostToDevice));
     }
     HP_CUDA_TRY(cudaMalloc(&pl.d_w, w.size() * es));
     HP_CUDA_TRY(cudaMalloc(&pl.d_bias, bias.size() * sizeof(float)));
     HP_CUDA_TRY(cudaMalloc(&pl.d_alpha, alpha.size() * sizeof(float)));
-    HP_CUDA_TRY(cudaMemcpy(pl.d_w, tf32 ? (const void*)w.data() : (const void*)wh.data(), w.size() * es, cudaMemcpyHostToDevice));
+    HP_CUDA_TRY(cudaMemcpy(pl.d_w, tf32 ? (const void*)w.data() : i8 ? (const void*)wq.data() : (const void*)wh.data(), w.size() * es, cudaMemcpyHostToDevice));
     HP_CUDA_TRY(cudaMemcpy(pl.d_bias, bias.data(), bias.size() * sizeof(float), cudaMemcpyHostToDevice));
     HP_CUDA_TRY(cudaMemcpy(pl.d_alpha, alpha.data(), alpha.size() * sizeof(float), cudaMemcpyHostToDevice));
 
@@ -807,21 +852,24 @@ int build_conv_plan(hp_engine* e, EngOp& op, const float* blob)
         const EngBuffer& ob = e->bufs[po.out_buf];
         if (ob.H != ib.H || ob.W != ib.W || (int)po.out_ch_off + G * cout_g > ob.channels) { set_error("engine: conv output buffer mismatch"); return HP_ERR_ARG; }
         p.out = ob.d; p.out_ld = ob.channels; p.out_ch_off = (int)po.out_ch_off;
+        if (i8) p.out_inv_scale = 1.0f / e->act_scale[po.out_buf];
     }
+    if (i8) { p.mul = pl.d_mul; p.in_g_stride = cin_g; }
     if (po.res_mode) {
         if (po.out_mode != OUT_F16_NHWC || po.res_buf >= e->bufs.size()) { set_error("engine: bad residual"); return HP_ERR_ARG; }
         const EngBuffer& rb = e->bufs[po.res_buf];
         if (rb.H != ib.H || rb.W != ib.W || (int)po.res_ch_off + G * cout_g > rb.channels || po.res_ch_off % 8 || cout_g % 16) { set_error("engine: residual buffer mismatch"); return HP_ERR_ARG; }
         p.res = rb.d; p.res_ld = rb.channels; p.res_ch_off = (int)po.res_ch_off; p.res_mode = (int)po.res_mode;
+        if (i8) p.res_scale = e->act_scale[po.res_buf];
     }
-    int rc = make_tmap_act_im2col(&pl.tmap_a, ib.d, e->max_batch, ib.H, ib.W, ib.channels, eR, eS, tf32);
+    int rc = make_tmap_act_im2col(&pl.tmap_a, ib.d, e->max_batch, ib.H, ib.W, ib.channels, eR, eS, e->dtype);
     if (rc) return rc;
-    rc = make_tmap_wgt(&pl.tmap_b, pl.d_w, G * cout_pad, K, BN, tf32);
+    rc = make_tmap_wgt(&pl.tmap_b, pl.d_w, G * cout_pad, K, BN, e->dtype);
     if (rc) return rc;
     pl.smem = conv_smem_bytes(BN, p.num_stages);
     pl.flops_per_frame = 2.0 * ib.H * ib.W * (double)G * cout_g * cin_g * R * S;
     op.launch = Launch::Conv;
-    if (tf32) return HP_OK;
+    if (e->dtype != HP_DTYPE_F16) return HP_OK;   // the TF32 and INT8 engines have no halo kernel
     pl.monotone_act = true;
     for (float a : alpha) if (!(a >= 0.f)) { pl.monotone_act = false; break; }
     // Halo-box kernel for RxS layers whose 16 x 8 tile grid wastes little of the image (the early VGG layers): the A operand comes
@@ -900,11 +948,12 @@ const void* halo_kernel_bn(int BN)
     return nullptr;
 }
 const void* halo_kernel(bool pool, int BN) { return pool ? halo_kernel_bn<true>(BN) : halo_kernel_bn<false>(BN); }
-const void* conv_kernel(bool tf32, bool res, int BN, int stem_R = 0)
+const void* conv_kernel(int dtype, bool res, int BN, int stem_R = 0)
 {
     if (stem_R == 3) return conv_kernel_bn<__half, false, 3>(BN);
     if (stem_R == 7) return conv_kernel_bn<__half, false, 7>(BN);
-    if (tf32) return res ? conv_kernel_bn<float, true>(BN) : conv_kernel_bn<float, false>(BN);
+    if (dtype == HP_DTYPE_TF32) return res ? conv_kernel_bn<float, true>(BN) : conv_kernel_bn<float, false>(BN);
+    if (dtype == HP_DTYPE_INT8) return res ? conv_kernel_bn<int8_t, true>(BN) : conv_kernel_bn<int8_t, false>(BN);
     return res ? conv_kernel_bn<__half, true>(BN) : conv_kernel_bn<__half, false>(BN);
 }
 
@@ -951,7 +1000,7 @@ int launch_conv(hp_engine* e, EngOp& op, int N, cudaStream_t st, bool u8_input)
     cudaLaunchAttribute at[1];
     const cudaLaunchConfig_t cfg = pdl_config(grid, CONV_THREADS, pl.smem, st, at);
     void* args[] = { (void*)&pl.tmap_a, (void*)&pl.tmap_b, (void*)&p };
-    HP_CUDA_TRY(cudaLaunchKernelExC(&cfg, conv_kernel(e->dtype == HP_DTYPE_TF32, p.res_mode != 0, p.BN, stem_R), args));
+    HP_CUDA_TRY(cudaLaunchKernelExC(&cfg, conv_kernel(e->dtype, p.res_mode != 0, p.BN, stem_R), args));
     return HP_OK;
 }
 
@@ -1112,6 +1161,38 @@ int run_graph(hp_engine* e, int N, bool u8_input, cudaStream_t st, int first = 0
         case Launch::HeadsF32:
             launch_heads<float>(e, po, N, st);
             break;
+        case Launch::Im2colI8: {
+            const EngBuffer& ob = e->bufs[po.out_buf];
+            const int R = K ? K : 3;
+            const int ph = same_pad_before(e->in_h, R, stride), pw = same_pad_before(e->in_w, R, stride);
+            const unsigned blocks = (unsigned)(((size_t)N * ob.H * ob.W * (ob.channels / 4) + 255) / 256);
+            const float inv_s = 1.0f / e->act_scale[po.out_buf];
+            if (u8_input) im2col_i8_kernel<true><<<blocks, 256, 0, st>>>(frames, (int8_t*)ob.d, N, e->in_h, e->in_w, e->factor, e->flip_rgb, e->hdr.mean[0], e->hdr.mean[1],
+                                                                        e->hdr.mean[2], R, stride, ob.H, ob.W, ph, pw, ob.channels, inv_s);
+            else im2col_i8_kernel<false><<<blocks, 256, 0, st>>>(e->d_input_f32, (int8_t*)ob.d, N, e->in_h, e->in_w, 1.0, 0, e->hdr.mean[0], e->hdr.mean[1], e->hdr.mean[2],
+                                                                 R, stride, ob.H, ob.W, ph, pw, ob.channels, inv_s);
+            break;
+        }
+        case Launch::DwI8: {
+            const EngBuffer& ib = e->bufs[po.in_buf];
+            const EngBuffer& ob = e->bufs[po.out_buf];
+            const int C = (int)po.cout_g;
+            const size_t total = (size_t)N * ob.H * ob.W * (C / 4);
+            const float* dw = op.d_dw;
+            dwconv_i8_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>((const int8_t*)ib.d + po.in_ch_off, ib.channels, (int8_t*)ob.d + po.out_ch_off, ob.channels, dw,
+                dw + (size_t)K * K * C, dw + (size_t)K * K * C + C, N, ib.H, ib.W, C, ob.H, ob.W, K, stride, same_pad_before(ib.H, K, stride), same_pad_before(ib.W, K, stride),
+                e->act_scale[po.in_buf], 1.0f / e->act_scale[po.out_buf]);
+            break;
+        }
+        case Launch::MaxPoolI8: {
+            const EngBuffer& ib = e->bufs[po.in_buf];
+            const EngBuffer& ob = e->bufs[po.out_buf];
+            const int C = (int)po.cout_g, KP = K ? K : 2;
+            const size_t total = (size_t)N * ob.H * ob.W * (C / 4);
+            maxpool_i8_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>((const int8_t*)ib.d + po.in_ch_off, (int8_t*)ob.d + po.out_ch_off, N, ib.H, ib.W, ib.channels, C, ob.channels,
+                                                                              ob.H, ob.W, KP, same_pad_before(ib.H, KP, 2), same_pad_before(ib.W, KP, 2));
+            break;
+        }
         }
         e->launches += kernels_launched(op.launch, u8_input);
         if (prof) cudaEventRecord(evset[oi + 1], st);
@@ -1139,6 +1220,7 @@ void free_engine(hp_engine* e)
         if (o.plan.d_w) cudaFree(o.plan.d_w);
         if (o.plan.d_bias) cudaFree(o.plan.d_bias);
         if (o.plan.d_alpha) cudaFree(o.plan.d_alpha);
+        if (o.plan.d_mul) cudaFree(o.plan.d_mul);
         if (o.d_dw) cudaFree(o.d_dw);
     }
     if (e->d_conf) cudaFree(e->d_conf);
@@ -1184,7 +1266,7 @@ int hp_engine_dtype(const hp_engine* e) { return e ? e->dtype : HP_ERR_ARG; }
 int hp_engine_create_ex(hp_engine** out, const void* pack, size_t pack_bytes, int in_w, int in_h, int max_batch,
                         double factor, int flip_rgb, int device, int dtype)
 {
-    if (dtype != HP_DTYPE_F16 && dtype != HP_DTYPE_TF32) { set_error("hp_engine_create_ex: unknown dtype %d", dtype); return HP_ERR_ARG; }
+    if (dtype != HP_DTYPE_F16 && dtype != HP_DTYPE_TF32 && dtype != HP_DTYPE_INT8) { set_error("hp_engine_create_ex: unknown dtype %d", dtype); return HP_ERR_ARG; }
 
     if (!out || !pack) { set_error("hp_engine_create: null argument"); return HP_ERR_ARG; }
     *out = nullptr;
@@ -1204,8 +1286,30 @@ int hp_engine_create_ex(hp_engine** out, const void* pack, size_t pack_bytes, in
         set_error("hp_engine_create: implausible pack header (%u buffers, %u ops, %llu blob floats)", hdr.n_buffers, hdr.n_ops, (unsigned long long)hdr.blob_floats);
         return HP_ERR_ARG;
     }
-    const size_t need = sizeof(PackHeader) + (size_t)hdr.n_buffers * sizeof(PackBuffer) + (size_t)hdr.n_ops * sizeof(PackOp) + (size_t)hdr.blob_floats * sizeof(float);
+    const uint32_t n_scales = hdr.reserved[0];   // INT8 calibration table: 0 or n_buffers scales after the blob
+    if (n_scales != 0 && n_scales != hdr.n_buffers) { set_error("hp_engine_create: the pack's scale table has %u entries for %u buffers", n_scales, hdr.n_buffers); return HP_ERR_ARG; }
+    const size_t need = sizeof(PackHeader) + (size_t)hdr.n_buffers * sizeof(PackBuffer) + (size_t)hdr.n_ops * sizeof(PackOp) + (size_t)hdr.blob_floats * sizeof(float) +
+                        (size_t)n_scales * sizeof(float);
     if (pack_bytes < need) { set_error("hp_engine_create: truncated pack (%zu < %zu bytes)", pack_bytes, need); return HP_ERR_ARG; }
+    std::vector<float> act_scale;
+    if (dtype == HP_DTYPE_INT8) {
+        if (hdr.head_type != 0) { set_error("hp_engine_create: the INT8 engine has no OpenPifPaf heads (pack head_type %u)", hdr.head_type); return HP_ERR_ARG; }
+        if (n_scales == 0) { set_error("hp_engine_create: the pack has no INT8 scale table (export it with an INT8 calibration)"); return HP_ERR_ARG; }
+        act_scale.resize(n_scales);
+        memcpy(act_scale.data(), (const uint8_t*)pack + need - (size_t)n_scales * sizeof(float), (size_t)n_scales * sizeof(float));
+        for (uint32_t b = 0; b < n_scales; ++b)
+            if (!(std::isfinite(act_scale[b]) && act_scale[b] > 0.f)) { set_error("hp_engine_create: INT8 scale of buffer %u is %g (needs a finite value > 0)", b, (double)act_scale[b]); return HP_ERR_ARG; }
+        const PackOp* vops = (const PackOp*)((const uint8_t*)pack + sizeof(PackHeader) + (size_t)hdr.n_buffers * sizeof(PackBuffer));
+        for (uint32_t i = 0; i < hdr.n_ops; ++i) {
+            PackOp po;
+            memcpy(&po, vops + i, sizeof(po));
+            if (po.type == OP_MAXPOOL2 && po.in_buf < n_scales && po.out_buf < n_scales && act_scale[po.in_buf] != act_scale[po.out_buf]) {
+                set_error("hp_engine_create: INT8 max-pool op %u reads buffer %u (scale %g) but writes buffer %u (scale %g); they must be equal", i, po.in_buf,
+                          (double)act_scale[po.in_buf], po.out_buf, (double)act_scale[po.out_buf]);
+                return HP_ERR_ARG;
+            }
+        }
+    }
     {
         const PackOp* vops = (const PackOp*)((const uint8_t*)pack + sizeof(PackHeader) + (size_t)hdr.n_buffers * sizeof(PackBuffer));
         auto in_blob = [&](uint64_t off, uint64_t count) { return off <= hdr.blob_floats && count <= hdr.blob_floats - off; };
@@ -1231,6 +1335,7 @@ int hp_engine_create_ex(hp_engine** out, const void* pack, size_t pack_bytes, in
     hp_engine* e = new hp_engine();
     e->device = device; e->dtype = dtype; e->in_h = in_h; e->in_w = in_w; e->max_batch = max_batch;
     e->factor = factor; e->flip_rgb = flip_rgb; e->hdr = hdr; e->num_sms = prop.multiProcessorCount;
+    e->act_scale = std::move(act_scale);
     EngOptions& opt = e->opt;
     if (const char* v = getenv("HPB_HALO")) opt.halo = strcmp(v, "all") == 0 ? EngOptions::HALO_ALL : EngOptions::HALO_NONE;
     opt.stem3 = !getenv("HPB_NO_STEM3");
@@ -1256,7 +1361,7 @@ int hp_engine_create_ex(hp_engine** out, const void* pack, size_t pack_bytes, in
         b.H = in_h; b.W = in_w;
         for (int d = 0; d < b.down; ++d) { b.H = (b.H + 1) / 2; b.W = (b.W + 1) / 2; }
         if (b.channels % 8) { set_error("engine: buffer %u has %d channels (need a multiple of 8)", i, b.channels); return fail(HP_ERR_ARG); }
-        const size_t bytes = (size_t)max_batch * b.H * b.W * b.channels * (dtype == HP_DTYPE_TF32 ? sizeof(float) : sizeof(__half));
+        const size_t bytes = (size_t)max_batch * b.H * b.W * b.channels * (size_t)elem_bytes(dtype);
         if (cudaMalloc(&b.d, bytes) != cudaSuccess) { set_error("engine: cudaMalloc(%zu) failed", bytes); return fail(HP_ERR_CUDA); }
         cudaMemset(b.d, 0, bytes); // padding channels must read as zero
     }
@@ -1272,7 +1377,7 @@ int hp_engine_create_ex(hp_engine** out, const void* pack, size_t pack_bytes, in
     }
     e->ops.resize(hdr.n_ops);
     size_t max_smem = 0;
-    const bool tf32 = dtype == HP_DTYPE_TF32;
+    const bool tf32 = dtype == HP_DTYPE_TF32, i8 = dtype == HP_DTYPE_INT8;
     for (uint32_t i = 0; i < hdr.n_ops; ++i) {
         EngOp& op = e->ops[i];
         op.po = pops[i];
@@ -1293,7 +1398,7 @@ int hp_engine_create_ex(hp_engine** out, const void* pack, size_t pack_bytes, in
                 set_error("engine: im2col buffer must hold roundup(R*R*3,64) channels at the stem resolution");
                 return fail(HP_ERR_ARG);
             }
-            op.launch = tf32 ? Launch::Im2colF32 : Launch::Im2col;
+            op.launch = tf32 ? Launch::Im2colF32 : i8 ? Launch::Im2colI8 : Launch::Im2col;
         } else if (po.type == OP_DWCONV) {
             const int C = (int)po.cout_g, K = (int)po.R, stride = po.stride ? (int)po.stride : 1;
             const EngBuffer& ib = e->bufs[po.in_buf];
@@ -1316,7 +1421,7 @@ int hp_engine_create_ex(hp_engine** out, const void* pack, size_t pack_bytes, in
                 return fail(HP_ERR_CUDA);
             }
             e->flops_per_frame += 2.0 * ob.H * ob.W * C * K * K;
-            op.launch = tf32 ? Launch::DwF32 : K == 3 && stride == 1 ? Launch::DwCol : Launch::DwStrip;
+            op.launch = tf32 ? Launch::DwF32 : i8 ? Launch::DwI8 : K == 3 && stride == 1 ? Launch::DwCol : Launch::DwStrip;
         } else if (po.type == OP_MAXPOOL2) {
             // 8 channels per 16-byte load (fp16) / two float4 loads (fp32): both offsets aligned, both channel ranges inside their buffers
             const EngBuffer& ib = e->bufs[po.in_buf];
@@ -1326,7 +1431,7 @@ int hp_engine_create_ex(hp_engine** out, const void* pack, size_t pack_bytes, in
                 set_error("engine: bad maxpool op %u", i);
                 return fail(HP_ERR_ARG);
             }
-            op.launch = tf32 ? Launch::MaxPoolF32 : Launch::MaxPool;
+            op.launch = tf32 ? Launch::MaxPoolF32 : i8 ? Launch::MaxPoolI8 : Launch::MaxPool;
         } else if (po.type == OP_PIFPAF_HEAD) {
             // the head kernels read input row y >> 1 for every output row y < out_h: both inputs must be at the output resolution
             if (hdr.head_type != 1 || po.res_buf >= hdr.n_buffers || hdr.conf_channels != 85 || hdr.paf_channels != 171 ||
@@ -1341,12 +1446,12 @@ int hp_engine_create_ex(hp_engine** out, const void* pack, size_t pack_bytes, in
             return fail(HP_ERR_UNSUPPORTED);
         }
     }
-    // The fusion passes below (fp16 engines) settle how each op launches.
+    // The fusion passes below (fp16 engines; the TF32 and INT8 engines launch every op on its own) settle how each op launches.
     // Fused stem: the first conv gathers its patches from the u8 frames itself, the im2col buffer is never written.
     for (EngOp& c : e->ops) {
         const PackOp& po = c.po;
         const int R = (int)po.R;
-        if (tf32 || c.launch != Launch::Conv || !po.im2col_input || po.res_mode || po.out_mode != OUT_F16_NHWC || po.S != po.R || !(R == 7 || (R == 3 && opt.stem3))) continue;
+        if (dtype != HP_DTYPE_F16 || c.launch != Launch::Conv || !po.im2col_input || po.res_mode || po.out_mode != OUT_F16_NHWC || po.S != po.R || !(R == 7 || (R == 3 && opt.stem3))) continue;
         for (EngOp& m : e->ops) {   // the patch-gather op feeding this conv: its stride / tap size define the stem geometry
             if (m.po.type != OP_IM2COL3 || m.po.out_buf != po.in_buf) continue;
             if ((int)(m.po.R ? m.po.R : 3) != R || po.cin_g != 3) break;
@@ -1460,7 +1565,7 @@ int hp_engine_create_ex(hp_engine** out, const void* pack, size_t pack_bytes, in
         e->step_kernels += kernels_launched(o.launch, true);
     }
     const double per_launch = launches ? e->flops_per_frame * e->max_batch / launches : 0.0;
-    e->use_pdl = !tf32 && launches > 0 && per_launch < 10e9;
+    e->use_pdl = dtype == HP_DTYPE_F16 && launches > 0 && per_launch < 10e9;
     for (const EngOp& o : e->ops) {
         if (o.po.type != OP_CONV) continue;
         if ((o.launch == Launch::Halo || o.launch == Launch::HaloPool) &&
@@ -1471,7 +1576,7 @@ int hp_engine_create_ex(hp_engine** out, const void* pack, size_t pack_bytes, in
         const int stem_R = o.launch == Launch::ConvStem ? (int)o.po.R : 0;
         for (int v = 0; v < 3; ++v)   // plain, residual, and (for a stem) the fused u8 form
             if ((v < 2 || stem_R) &&
-                cudaFuncSetAttribute(conv_kernel(tf32, v == 1, o.plan.prm.BN, v == 2 ? stem_R : 0), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)max_smem) != cudaSuccess) {
+                cudaFuncSetAttribute(conv_kernel(dtype, v == 1, o.plan.prm.BN, v == 2 ? stem_R : 0), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)max_smem) != cudaSuccess) {
                 set_error("engine: cannot opt in to %zu bytes of dynamic shared memory", max_smem);
                 return fail(HP_ERR_CUDA);
             }
@@ -1736,7 +1841,7 @@ int hp_engine_debug_read_buffer(hp_engine* e, int buf, void* out_f16, int N, int
     if (C) *C = b.channels;
     if (b.fused_away && out_f16) { set_error("hp_engine_debug_read_buffer: buffer %d is not materialised (the max-pool / 1x1 depthwise op that reads it runs in the producing conv's epilogue; HPB_NO_POOL_FUSE=1 / HPB_NO_DW1_FUSE=1 keep it)", buf); return HP_ERR_UNSUPPORTED; }
     HP_CUDA_TRY(cudaStreamSynchronize(e->stream));
-    const size_t es = e->dtype == HP_DTYPE_TF32 ? sizeof(float) : sizeof(__half);   // element type follows the engine's dtype
+    const size_t es = (size_t)elem_bytes(e->dtype);   // element type follows the engine's dtype
     if (out_f16) HP_CUDA_TRY(cudaMemcpy(out_f16, b.d, (size_t)N * b.H * b.W * b.channels * es, cudaMemcpyDeviceToHost));
     return HP_OK;
 }
@@ -1747,7 +1852,7 @@ int hp_engine_debug_write_buffer(hp_engine* e, int buf, const void* in_f16, int 
     HP_CUDA_TRY(cudaSetDevice(e->device));
     const EngBuffer& b = e->bufs[buf];
     HP_CUDA_TRY(cudaStreamSynchronize(e->stream));
-    const size_t es = e->dtype == HP_DTYPE_TF32 ? sizeof(float) : sizeof(__half);
+    const size_t es = (size_t)elem_bytes(e->dtype);
     HP_CUDA_TRY(cudaMemcpy(b.d, in_f16, (size_t)N * b.H * b.W * b.channels * es, cudaMemcpyHostToDevice));
     return HP_OK;
 }
@@ -1762,22 +1867,71 @@ int hp_engine_debug_run_ops(hp_engine* e, int first_op, int last_op, int N)
     return HP_OK;
 }
 
+// INT8 calibration (TensorRT's IInt8MinMaxCalibrator): runs the graph op by op on a TF32 engine and folds max |x| of every op's
+// output buffer into absmax[out_buf] -- a running maximum over calls and over the max_batch-frame chunks of the N frames
+int hp_engine_calibrate_u8(hp_engine* e, const uint8_t* frames, int N, float* absmax, int n_buffers)
+{
+    if (!e || !frames || !absmax || N <= 0) { set_error("hp_engine_calibrate_u8: bad argument"); return HP_ERR_ARG; }
+    if (e->dtype != HP_DTYPE_TF32) { set_error("hp_engine_calibrate_u8: calibration runs on a TF32 engine (this one has dtype %d)", e->dtype); return HP_ERR_ARG; }
+    if (n_buffers != (int)e->bufs.size()) { set_error("hp_engine_calibrate_u8: %d absmax entries for %zu buffers", n_buffers, e->bufs.size()); return HP_ERR_ARG; }
+    for (int b = 0; b < n_buffers; ++b)
+        if (!(absmax[b] >= 0.f)) { set_error("hp_engine_calibrate_u8: absmax[%d] = %g (the running maximum starts at values >= 0)", b, (double)absmax[b]); return HP_ERR_ARG; }
+    HP_CUDA_TRY(cudaSetDevice(e->device));
+    HP_CUDA_TRY(cudaStreamSynchronize(e->stream));
+    unsigned* d_amax = nullptr;
+    HP_CUDA_TRY(cudaMalloc(&d_amax, (size_t)n_buffers * sizeof(unsigned)));
+    auto done = [&](int rc) { cudaFree(d_amax); return rc; };
+    if (cudaMemcpy(d_amax, absmax, (size_t)n_buffers * sizeof(float), cudaMemcpyHostToDevice) != cudaSuccess) { set_error("hp_engine_calibrate_u8: upload failed"); return done(HP_ERR_CUDA); }
+    const size_t frame_bytes = (size_t)e->in_h * e->in_w * 3;
+    for (int f0 = 0; f0 < N; f0 += e->max_batch) {
+        const int n = std::min(e->max_batch, N - f0);
+        memcpy(e->pin_frames, frames + (size_t)f0 * frame_bytes, (size_t)n * frame_bytes);
+        if (cudaMemcpyAsync(e->d_frames, e->pin_frames, (size_t)n * frame_bytes, cudaMemcpyHostToDevice, e->stream) != cudaSuccess) { set_error("hp_engine_calibrate_u8: H2D failed"); return done(HP_ERR_CUDA); }
+        for (int oi = 0; oi < (int)e->ops.size(); ++oi) {
+            const int rc = run_graph(e, n, true, e->stream, oi, oi);
+            if (rc) return done(rc);
+            const PackOp& po = e->ops[oi].po;
+            if (po.type == OP_PIFPAF_HEAD || (po.type == OP_CONV && po.out_mode == OUT_F32_NCHW_SPLIT)) continue;
+            const EngBuffer& b = e->bufs[po.out_buf];
+            const size_t cnt = (size_t)n * b.H * b.W * b.channels;
+            absmax_f32_kernel<<<(unsigned)std::min<size_t>(1024, (cnt + 255) / 256), 256, 0, e->stream>>>((const float*)b.d, cnt, d_amax + po.out_buf);
+        }
+        if (cudaStreamSynchronize(e->stream) != cudaSuccess) { set_error("hp_engine_calibrate_u8: %s", cudaGetErrorString(cudaGetLastError())); return done(HP_ERR_CUDA); }
+    }
+    if (cudaMemcpy(absmax, d_amax, (size_t)n_buffers * sizeof(float), cudaMemcpyDeviceToHost) != cudaSuccess) { set_error("hp_engine_calibrate_u8: read-back failed"); return done(HP_ERR_CUDA); }
+    return done(HP_OK);
+}
+
+// 1 when `pack` is a model pack that carries an INT8 scale table (what data_type::kINT8 needs), else 0; host only
+int hp_pack_int8_calibrated(const void* pack, size_t pack_bytes)
+{
+    if (!pack || pack_bytes < sizeof(PackHeader)) return 0;
+    PackHeader hdr;
+    memcpy(&hdr, pack, sizeof(hdr));
+    if (memcmp(hdr.magic, PACK_MAGIC, 8) != 0 || hdr.version != PACK_VERSION || hdr.n_buffers == 0 || hdr.reserved[0] != hdr.n_buffers ||
+        hdr.n_buffers > 65536 || hdr.n_ops > 65536 || hdr.blob_floats > ((uint64_t)1 << 34))
+        return 0;
+    const size_t need = sizeof(PackHeader) + (size_t)hdr.n_buffers * sizeof(PackBuffer) + (size_t)hdr.n_ops * sizeof(PackOp) +
+                        ((size_t)hdr.blob_floats + hdr.n_buffers) * sizeof(float);
+    return pack_bytes >= need ? 1 : 0;
+}
+
 // test hook: the kernel op `op` launches on the next run over u8 frames, as decided when the engine was created (EngOp::launch and
-// the conv plan's tile width): conv<f16|tf32,BN[,res][,stem3|stem7]>, halo<BN[,pool]>, dw_strip<K,S>, dw_col, dw_tma<1|2>, dw_f32,
-// maxpool<K>, maxpool_f32, im2col, heads, or none when a neighbouring op's launch covers it
+// the conv plan's tile width): conv<f16|tf32|i8,BN[,res][,stem3|stem7]>, halo<BN[,pool]>, dw_strip<K,S>, dw_col, dw_tma<1|2>, dw_f32,
+// dw_i8, maxpool<K>, maxpool_f32, maxpool_i8, im2col, im2col_i8, heads, or none when a neighbouring op's launch covers it
 int hp_engine_debug_op_kernel(const hp_engine* e, int op, char* name, int cap)
 {
     if (!e || op < 0 || op >= (int)e->ops.size() || !name || cap <= 0) { set_error("hp_engine_debug_op_kernel: bad argument"); return HP_ERR_ARG; }
     const EngOp& o = e->ops[op];
     const PackOp& po = o.po;
     const int BN = o.plan.prm.BN;
-    const bool tf32 = e->dtype == HP_DTYPE_TF32;
+    const char* dt = e->dtype == HP_DTYPE_TF32 ? "tf32," : e->dtype == HP_DTYPE_INT8 ? "i8," : "f16,";
     std::string s;
     switch (o.launch) {
     case Launch::None: case Launch::StemOrIm2col: s = "none"; break;
     case Launch::Im2col: case Launch::Im2colF32: s = "im2col"; break;
     case Launch::Conv:
-        s = std::string("conv<") + (tf32 ? "tf32," : "f16,") + std::to_string(BN) + (o.plan.prm.res_mode ? ",res>" : ">");
+        s = std::string("conv<") + dt + std::to_string(BN) + (o.plan.prm.res_mode ? ",res>" : ">");
         break;
     case Launch::ConvStem: s = "conv<f16," + std::to_string(BN) + ",stem" + std::to_string(po.R) + ">"; break;
     case Launch::Halo: s = "halo<" + std::to_string(BN) + ">"; break;
@@ -1790,6 +1944,9 @@ int hp_engine_debug_op_kernel(const hp_engine* e, int op, char* name, int cap)
     case Launch::Heads: case Launch::HeadsF32: s = "heads"; break;
     case Launch::DwF32: s = "dw_f32"; break;
     case Launch::MaxPoolF32: s = "maxpool_f32"; break;
+    case Launch::Im2colI8: s = "im2col_i8"; break;
+    case Launch::DwI8: s = "dw_i8"; break;
+    case Launch::MaxPoolI8: s = "maxpool_i8"; break;
     }
     if ((int)s.size() >= cap) { set_error("hp_engine_debug_op_kernel: %zu-character name, capacity %d", s.size(), cap); return HP_ERR_CAPACITY; }
     memcpy(name, s.c_str(), s.size() + 1);

@@ -30,13 +30,20 @@ namespace dnn {
         }
         // data_type of the reference ctor (tensorrt.hpp:14-22,48,61): kFLOAT (the default every example uses) selects the wgmma
         // kind tf32 engine (fp32 tensors, TF32 multiplies -- TensorRT's own FP32 convolution math on tensor-core GPUs), kHALF the
-        // f16 engine.  A serialized engine carries no precision argument in the reference API (its plan was built with one): the pack
-        // runs as kHALF unless HPB_DTYPE=tf32 says otherwise.
-        int dtype_of(const data_type& t) { return t.val == data_type::kHALF ? HP_DTYPE_F16 : HP_DTYPE_TF32; }
+        // f16 engine, kINT8 the int8 engine when the pack carries a calibration table (hyperpose_b200.export --int8-calibration) and
+        // the tf32 engine otherwise.  A serialized engine carries no precision argument in the reference API (its plan was built with
+        // one): the pack runs as kHALF unless HPB_DTYPE=tf32 | int8 says otherwise.
+        constexpr int INT8_IF_CALIBRATED = -1;
+        int dtype_of(const data_type& t)
+        {
+            return t.val == data_type::kHALF ? HP_DTYPE_F16 : t.val == data_type::kINT8 ? INT8_IF_CALIBRATED : HP_DTYPE_TF32;
+        }
         int serialized_dtype()
         {
             const char* v = std::getenv("HPB_DTYPE");
-            return (v && std::string(v) == "tf32") ? HP_DTYPE_TF32 : HP_DTYPE_F16;
+            if (v && std::string(v) == "tf32") return HP_DTYPE_TF32;
+            if (v && std::string(v) == "int8") return HP_DTYPE_INT8;
+            return HP_DTYPE_F16;
         }
         hp_engine* load_engine(const std::string& path, cv::Size input_size, int max_batch, double factor, bool flip_rgb, int dtype)
         {
@@ -46,6 +53,7 @@ namespace dnn {
             f.seekg(0);
             std::vector<char> blob((size_t)n);
             if (!f.read(blob.data(), n)) die("cannot read model pack " + path);
+            if (dtype == INT8_IF_CALIBRATED) dtype = hp_pack_int8_calibrated(blob.data(), blob.size()) ? HP_DTYPE_INT8 : HP_DTYPE_TF32;
             hp_engine* e = nullptr;
             // the reference API has no device argument: HPB_DEVICE=<ordinal> | rr (round-robin per engine instance), default 0
             if (hp_engine_create_ex(&e, blob.data(), blob.size(), input_size.width, input_size.height, max_batch, factor, flip_rgb ? 1 : 0, hp_default_device(), dtype) != HP_OK)

@@ -1,7 +1,7 @@
 // pack_format.h -- the flat model pack consumed by hp_engine_create (replaces the reference's
 // .onnx/.uff/.trt model files, include/hyperpose/utility/model.hpp:13-32; SURVEY 8f rank 1).
 // Little-endian; written by hyperpose_b200/models.py.
-//   PackHeader | PackBuffer[n_buffers] | PackOp[n_ops] | float blob[]
+//   PackHeader | PackBuffer[n_buffers] | PackOp[n_ops] | float blob[] | float act_scale[n_act_scales]
 // The graph is a straight list of ops over numbered activation buffers (fp16 NHWC on the device).
 #pragma once
 #include <stdint.h>
@@ -29,7 +29,8 @@ struct PackHeader {
     uint32_t out_down_shift;              // outputs are at (H >> shift, W >> shift)
     float mean[3];                        // subtracted after scaling, per model-input channel (backbones.py:455)
     uint32_t head_type;                   // 0: conf/paf at (H >> shift); 1: OpenPifPaf fields at 2*(H >> shift) - 1 (pixel-shuffled, cropped)
-    uint32_t reserved[4];                 // keeps blob_floats 8-byte aligned at offset 64
+    uint32_t reserved[4];                 // keeps blob_floats 8-byte aligned at offset 64.  reserved[0] = n_act_scales: 0, or n_buffers
+                                          // when the INT8 calibration table (one fp32 scale per activation buffer) follows the blob
     uint64_t blob_floats;
 };
 

@@ -60,6 +60,7 @@ class Graph:
     head_type: int = 0                 # 1: OpenPifPaf fields (pif[17,5,ho,wo] / paf[19,9,ho,wo] in the conf / paf output slots)
     buffers: list = field(default_factory=list)   # (channels, down_shift)
     ops: list = field(default_factory=list)
+    act_scales: np.ndarray | None = None          # INT8 calibration table: one fp32 scale per buffer (set_int8_scales), or None
 
     def add_buffer(self, channels: int, down_shift: int) -> int:
         assert channels % 8 == 0
@@ -88,8 +89,31 @@ class Graph:
                            alpha=np.ascontiguousarray(alpha, np.float32).reshape(-1), name=name,
                            res_buf=res_buf, res_ch_off=res_ch_off, res_mode=res_mode))
 
+    def set_int8_scales(self, absmax) -> None:
+        """INT8 scale table from per-buffer max |x| (Engine.calibrate): s = absmax / 127, an all-zero buffer gets 1.  A max-pool works
+        on the int8 values, so its input and output buffers need one scale: buffers joined by max-pools share the largest absmax among
+        them (a pool's output buffer may also hold other ops' results, e.g. MobilenetThin's concat: none of them is clipped)."""
+        a = np.asarray(absmax, np.float32).reshape(-1).copy()
+        assert a.size == len(self.buffers), (a.size, len(self.buffers))
+        root = list(range(a.size))
+
+        def find(b):
+            while root[b] != b:
+                root[b] = root[root[b]]
+                b = root[b]
+            return b
+        for op in self.ops:
+            if op.type == OP_MAXPOOL2:
+                root[find(op.out_buf)] = find(op.in_buf)
+        top = {}
+        for b in range(a.size):
+            top[find(b)] = max(top.get(find(b), np.float32(0)), a[b])
+        a = np.array([top[find(b)] for b in range(a.size)], np.float32)
+        self.act_scales = np.where(a > 0, a / np.float32(127.0), np.float32(1.0)).astype(np.float32)
+
     # ---- serialisation (layout of pack_format.h) ----
     def to_pack(self) -> bytes:
+        """the pack; with act_scales set, the INT8 scale table follows the blob and the header's reserved[0] counts it"""
         blob = []
         off = 0
         op_recs = []
@@ -103,10 +127,15 @@ class Graph:
                                        op.cin_g, op.cout_g, op.out_mode, op.split, op.im2col_input, op.stride,
                                        op.res_buf, op.res_ch_off, op.res_mode, 0, w_off, b_off, a_off))
         blob_arr = np.concatenate(blob).astype("<f4") if blob else np.zeros(0, "<f4")
+        table = b""
+        if self.act_scales is not None:
+            assert len(self.act_scales) == len(self.buffers), (len(self.act_scales), len(self.buffers))
+            table = np.asarray(self.act_scales, "<f4").tobytes()
         hdr = struct.pack("<8s6I3f5IQ", PACK_MAGIC, PACK_VERSION, len(self.buffers), len(self.ops), self.conf_channels,
-                          self.paf_channels, self.out_down_shift, *[float(m) for m in self.mean], self.head_type, 0, 0, 0, 0, blob_arr.size)
+                          self.paf_channels, self.out_down_shift, *[float(m) for m in self.mean], self.head_type,
+                          len(self.buffers) if table else 0, 0, 0, 0, blob_arr.size)
         bufs = b"".join(struct.pack("<2I", c, d) for c, d in self.buffers)
-        return hdr + bufs + b"".join(op_recs) + blob_arr.tobytes()
+        return hdr + bufs + b"".join(op_recs) + blob_arr.tobytes() + table
 
     def flops_per_frame(self, in_h: int, in_w: int) -> float:
         total = 0.0

@@ -164,12 +164,22 @@ int hp_engine_create(hp_engine** out, const void* pack, size_t pack_bytes, int i
 /* The same with the arithmetic the reference's `data_type` ctor argument selects (tensorrt.hpp:14-22,48,61):
  *   HP_DTYPE_F16  (= data_type::kHALF):  fp16 operands and activations, fp32 accumulation -- what hp_engine_create builds;
  *   HP_DTYPE_TF32 (= data_type::kFLOAT, the reference default): fp32 activations in HBM, wgmma kind tf32 (fp32 operands
- *                 read with a 10-bit mantissa by the tensor core, fp32 accumulation) -- TensorRT's own FP32 mode on tensor-core GPUs. */
+ *                 read with a 10-bit mantissa by the tensor core, fp32 accumulation) -- TensorRT's own FP32 mode on tensor-core GPUs;
+ *   HP_DTYPE_INT8 (= data_type::kINT8): symmetric int8 activations (one fp32 scale per buffer, from the pack's calibration table)
+ *                 and per-output-channel int8 weights, wgmma kind s8 with s32 accumulation.  Needs a pack with a scale table
+ *                 (hp_pack_int8_calibrated); no OpenPifPaf heads.  HP_ERR_ARG names the op or buffer a pack is refused for. */
 #define HP_DTYPE_F16 0
 #define HP_DTYPE_TF32 1
+#define HP_DTYPE_INT8 2
 int hp_engine_create_ex(hp_engine** out, const void* pack, size_t pack_bytes, int in_w, int in_h, int max_batch,
                         double factor, int flip_rgb, int device, int dtype);
 int hp_engine_dtype(const hp_engine* e);
+/* 1 when the model pack carries an INT8 scale table (one scale per activation buffer), else 0.  Host only. */
+int hp_pack_int8_calibrated(const void* pack, size_t pack_bytes);
+/* INT8 calibration as TensorRT's IInt8MinMaxCalibrator: on an HP_DTYPE_TF32 engine (HP_ERR_ARG on any other), runs the graph op by
+ * op on HOST u8 frames [N,in_h,in_w,3] (N may exceed max_batch) and folds max |x| of every op's output buffer into
+ * absmax[n_buffers] -- a running maximum, so start from zeros and call again for more frames.  Scale = absmax / 127. */
+int hp_engine_calibrate_u8(hp_engine* e, const uint8_t* frames, int N, float* absmax, int n_buffers);
 void hp_engine_destroy(hp_engine* e);
 /* max_batch_size() / input_size() (tensorrt.hpp:81-85) + output geometry; any pointer may be NULL */
 int hp_engine_info(const hp_engine* e, int* in_w, int* in_h, int* max_batch, int* c_conf, int* c_paf, int* out_h, int* out_w,
@@ -213,14 +223,14 @@ int hp_handoff_stats(long long* published, long long* hits, long long* batch_par
 int hp_engine_copy_outputs_device(hp_engine* e, float* d_conf, float* d_paf, int N, void* stream);
 int hp_engine_sync(hp_engine* e);
 long long hp_engine_launch_count(const hp_engine* e);
-/* test hooks: read / write an activation buffer (NHWC; fp16 elements on an HP_DTYPE_F16 engine, fp32 on HP_DTYPE_TF32),
+/* test hooks: read / write an activation buffer (NHWC; fp16 elements on an HP_DTYPE_F16 engine, fp32 on HP_DTYPE_TF32, int8 on HP_DTYPE_INT8),
  * run a sub-range [first,last] of the op list */
 int hp_engine_debug_read_buffer(hp_engine* e, int buf, void* out_f16, int N, int* H, int* W, int* C);
 int hp_engine_debug_write_buffer(hp_engine* e, int buf, const void* in_f16, int N);
 int hp_engine_debug_run_ops(hp_engine* e, int first_op, int last_op, int N);
 /* test hook: the kernel op `op` launches on the next run over u8 frames, fixed at creation, as a NUL-terminated name in
- * name[cap]: "conv<f16|tf32,BN[,res][,stem3|stem7]>", "halo<BN[,pool]>", "dw_strip<K,S>", "dw_col", "dw_tma<1|2>", "dw_f32",
- * "maxpool<K>", "maxpool_f32", "im2col", "heads", or "none" for an op that a neighbouring op's launch covers */
+ * name[cap]: "conv<f16|tf32|i8,BN[,res][,stem3|stem7]>", "halo<BN[,pool]>", "dw_strip<K,S>", "dw_col", "dw_tma<1|2>", "dw_f32", "dw_i8",
+ * "maxpool<K>", "maxpool_f32", "maxpool_i8", "im2col", "im2col_i8", "heads", or "none" for an op that a neighbouring op's launch covers */
 int hp_engine_debug_op_kernel(const hp_engine* e, int op, char* name, int cap);
 
 /* benchmark hook (SURVEY 8d): after the last conv of every run, copy these DEVICE tensors over the engine's
