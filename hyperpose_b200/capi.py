@@ -597,7 +597,7 @@ class PifPafParser:
 
 
 EXPORTS += ["hp_ppn_create", "hp_ppn_destroy", "hp_ppn_set_point_thresh", "hp_ppn_set_limb_thresh", "hp_ppn_set_nms_thresh",
-            "hp_ppn_process_host", "hp_ppn_process_device", "hp_ppn_fetch", "hp_ppn_launch_count"]
+            "hp_ppn_process_host", "hp_ppn_process_device", "hp_ppn_process_device_strided", "hp_ppn_fetch", "hp_ppn_launch_count"]
 
 
 class PoseProposalParser:
@@ -614,6 +614,7 @@ class PoseProposalParser:
             f.argtypes = [vp, cf]
         L.hp_ppn_process_host.argtypes = [vp] + [vp] * 6 + [ci] * 7 + [vp, ci, ip]
         L.hp_ppn_process_device.argtypes = [vp] + [vp] * 6 + [ci] * 7 + [vp]
+        L.hp_ppn_process_device_strided.argtypes = [vp] + [vp] * 6 + [ci] * 7 + [C.c_size_t] * 2 + [vp]
         L.hp_ppn_fetch.argtypes = [vp, vp, ci, ip, ci]
         L.hp_ppn_launch_count.argtypes = [vp]
         L.hp_ppn_launch_count.restype = C.c_longlong
@@ -656,6 +657,31 @@ class PoseProposalParser:
         K = np.asarray(conf_iou).shape[0]
         return self.process_batch(*[np.asarray(t)[None, :K] for t in (conf_point, x, y, w, h)], np.asarray(edge)[None], cap=cap)[0]
 
+    def process_device(self, d_conf_point: int, d_x: int, d_y: int, d_w: int, d_h: int, d_edge: int, N: int, K: int, gh: int, gw: int,
+                       E: int, nh: int, nw: int, stream: int = 0, box_frame_stride: int | None = None, edge_frame_stride: int | None = None):
+        """device tensors (pointers), asynchronous; results by fetch(N).  The frame strides are in floats (default: dense,
+        K*gh*gw and E*nh*nw*gh*gw).  A PPN engine's outputs parse in place: see ppn_engine_pointers."""
+        check(lib().hp_ppn_process_device_strided(
+            self._h, d_conf_point, d_x, d_y, d_w, d_h, d_edge, N, K, gh, gw, E, nh, nw,
+            K * gh * gw if box_frame_stride is None else box_frame_stride,
+            E * nh * nw * gh * gw if edge_frame_stride is None else edge_frame_stride, stream))
+
+    def fetch(self, N: int, cap: int = 256):
+        out = np.zeros((N, cap), HUMAN_DT)
+        n = (C.c_int * N)()
+        check(lib().hp_ppn_fetch(self._h, out.ctypes.data, cap, n, N))
+        return [out[i, :n[i]].copy() for i in range(N)]
+
     @property
     def launch_count(self) -> int:
         return int(lib().hp_ppn_launch_count(self._h))
+
+
+def ppn_engine_pointers(engine: "Engine") -> dict:
+    """PoseProposalParser.process_device arguments for a PPN engine's (head_type 2) device outputs, parsed in place: conf slot
+    [N,6,K,gh,gw] -> conf_point + 0, x + 2KG, y + 3KG, w + 4KG, h + 5KG floats (G = gh*gw), box_frame_stride 6KG; the paf slot
+    [N,E,nh,nw,gh,gw] is the edge tensor, edge_frame_stride E*nh*nw*G"""
+    d_conf, d_paf, _ = engine.device_outputs()
+    K, G = engine.c_conf // 6, engine.out_h * engine.out_w
+    ptrs = [d_conf + t * K * G * 4 for t in (0, 2, 3, 4, 5)] + [d_paf]
+    return dict(ptrs=ptrs, K=K, gh=engine.out_h, gw=engine.out_w, box_frame_stride=6 * K * G, edge_frame_stride=engine.c_paf * G)

@@ -425,6 +425,35 @@ __global__ void __launch_bounds__(256) pifpaf_head_kernel(const T* __restrict__ 
     out[idx] = v;
 }
 
+// Pose Proposal Network head (hyperpose/Model/pose_proposal/model.py:84-93 + restore_coor :111-119, inference branch): the raw
+// 1x1-conv output [N,gh,gw,raw_ld] -> sigmoid -> conf slot [N,6,K,gh,gw] (conf_point, conf_iou, x, y, w, h; the cell's offset and the
+// size scaled to the network input) and edge slot [N,L*nh*nw,gh,gw] (the tf.reshape of :93 moves no data).  One thread per output
+// element, in output order; every operation rounded on its own.
+template <typename T>
+__global__ void __launch_bounds__(256) ppn_head_kernel(const T* __restrict__ raw, int raw_ld, float* __restrict__ conf, float* __restrict__ edge,
+                                                       int N, int gh, int gw, int K, int n_edge, float cw, float ch, float in_w, float in_h)
+{
+    const size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const int G = gh * gw, nb = 6 * K, C = nb + n_edge;
+    if (idx >= (size_t)N * C * G) return;
+    const int pix = (int)(idx % G);
+    const size_t t = idx / G;
+    const int c = (int)(t % C), n = (int)(t / C);
+    const int x = pix % gw, y = pix / gw;
+    const float v = (float)raw[((size_t)n * G + pix) * raw_ld + c];
+    const float s = 1.f / (1.f + expf(-v));
+    if (c >= nb) { edge[((size_t)n * n_edge + (c - nb)) * G + pix] = s; return; }
+    float o = s;
+    switch (c / K) {
+    case 2: o = __fmul_rn(__fadd_rn(s, (float)x), cw); break;
+    case 3: o = __fmul_rn(__fadd_rn(s, (float)y), ch); break;
+    case 4: o = __fmul_rn(s, in_w); break;
+    case 5: o = __fmul_rn(s, in_h); break;
+    default: break;   // conf_point, conf_iou
+    }
+    conf[((size_t)n * nb + c) * G + pix] = o;
+}
+
 // KxK (K = 2 or 3) stride-2 max pool, NHWC fp16, 8 channels per thread; TF "SAME" semantics (window clipped at the border).
 template <int K>
 __global__ void __launch_bounds__(256) maxpool2_kernel(const __half* __restrict__ in, __half* __restrict__ out,
@@ -599,8 +628,9 @@ enum class Launch : uint8_t {
     DwStrip,        // dwconv_kernel<K, stride>
     MaxPool,        // maxpool2_kernel
     Heads,          // two pifpaf_head_kernel launches
+    PpnHead,        // ppn_head_kernel
     // TF32 engine: fp32 activations (conv_tf32.cuh); its convs are Conv
-    Im2colF32, DwF32, MaxPoolF32, HeadsF32,
+    Im2colF32, DwF32, MaxPoolF32, HeadsF32, PpnHeadF32,
     // INT8 engine: int8 activations (conv_int8.cuh); its convs are Conv
     Im2colI8, DwI8, MaxPoolI8,
 };
@@ -1038,6 +1068,19 @@ void launch_heads(hp_engine* e, const PackOp& po, int N, cudaStream_t st)
     pifpaf_head_kernel<T><<<(int)((t2 + 255) / 256), 256, 0, st>>>((const T*)b.d, b.channels, e->d_paf, N, b.H, b.W, 19, 9, e->out_h, e->out_w, 1);
 }
 
+// the PPN head op: boxes [N,6,K,gh,gw] into the conf slot, edges [N,L,nh,nw,gh,gw] into the paf slot, from in_buf.  restore_coor's grid
+// size is the engine's input size over the output grid, rounded once to fp32.
+template <typename T>
+void launch_ppn_head(hp_engine* e, const PackOp& po, int N, cudaStream_t st)
+{
+    const EngBuffer& a = e->bufs[po.in_buf];
+    const int K = (int)po.cout_g, n_edge = (int)(po.groups * po.R * po.S);
+    const size_t total = (size_t)N * (6 * K + n_edge) * e->out_h * e->out_w;
+    ppn_head_kernel<T><<<(unsigned)((total + 255) / 256), 256, 0, st>>>((const T*)a.d, a.channels, e->d_conf, e->d_paf, N, e->out_h, e->out_w, K, n_edge,
+                                                                        (float)((double)e->in_w / e->out_w), (float)((double)e->in_h / e->out_h),
+                                                                        (float)e->in_w, (float)e->in_h);
+}
+
 int run_graph(hp_engine* e, int N, bool u8_input, cudaStream_t st, int first = 0, int last = -1)
 {
     if (last < 0) last = (int)e->ops.size() - 1;
@@ -1160,6 +1203,12 @@ int run_graph(hp_engine* e, int N, bool u8_input, cudaStream_t st, int first = 0
         }
         case Launch::HeadsF32:
             launch_heads<float>(e, po, N, st);
+            break;
+        case Launch::PpnHead:
+            launch_ppn_head<__half>(e, po, N, st);
+            break;
+        case Launch::PpnHeadF32:
+            launch_ppn_head<float>(e, po, N, st);
             break;
         case Launch::Im2colI8: {
             const EngBuffer& ob = e->bufs[po.out_buf];
@@ -1293,7 +1342,7 @@ int hp_engine_create_ex(hp_engine** out, const void* pack, size_t pack_bytes, in
     if (pack_bytes < need) { set_error("hp_engine_create: truncated pack (%zu < %zu bytes)", pack_bytes, need); return HP_ERR_ARG; }
     std::vector<float> act_scale;
     if (dtype == HP_DTYPE_INT8) {
-        if (hdr.head_type != 0) { set_error("hp_engine_create: the INT8 engine has no OpenPifPaf heads (pack head_type %u)", hdr.head_type); return HP_ERR_ARG; }
+        if (hdr.head_type != 0) { set_error("hp_engine_create: the INT8 engine has no OpenPifPaf or PPN heads (pack head_type %u)", hdr.head_type); return HP_ERR_ARG; }
         if (n_scales == 0) { set_error("hp_engine_create: the pack has no INT8 scale table (export it with an INT8 calibration)"); return HP_ERR_ARG; }
         act_scale.resize(n_scales);
         memcpy(act_scale.data(), (const uint8_t*)pack + need - (size_t)n_scales * sizeof(float), (size_t)n_scales * sizeof(float));
@@ -1382,7 +1431,8 @@ int hp_engine_create_ex(hp_engine** out, const void* pack, size_t pack_bytes, in
         EngOp& op = e->ops[i];
         op.po = pops[i];
         const PackOp& po = op.po;
-        if ((po.type != OP_IM2COL3 && po.in_buf >= hdr.n_buffers) || (po.out_mode != OUT_F32_NCHW_SPLIT && po.type != OP_PIFPAF_HEAD && po.out_buf >= hdr.n_buffers)) {
+        if ((po.type != OP_IM2COL3 && po.in_buf >= hdr.n_buffers) ||
+            (po.out_mode != OUT_F32_NCHW_SPLIT && po.type != OP_PIFPAF_HEAD && po.type != OP_PPN_HEAD && po.out_buf >= hdr.n_buffers)) {
             set_error("engine: op %u references a missing buffer", i);
             return fail(HP_ERR_ARG);
         }
@@ -1441,6 +1491,31 @@ int hp_engine_create_ex(hp_engine** out, const void* pack, size_t pack_bytes, in
                 return fail(HP_ERR_ARG);
             }
             op.launch = tf32 ? Launch::HeadsF32 : Launch::Heads;
+        } else if (po.type == OP_PPN_HEAD) {
+            // one thread per output element reads raw channel c < 6K + L*nh*nw of the pixel it writes: the input must hold them all at
+            // the output resolution; the parser indexes key points 0..17 (COCO limb table)
+            const uint64_t K = po.cout_g, n_edge = (uint64_t)po.groups * po.R * po.S;
+            const EngBuffer& ib = e->bufs[po.in_buf];
+            if (hdr.head_type != 2) { set_error("engine: PPN head op %u in a pack with head_type %u (needs 2)", i, hdr.head_type); return fail(HP_ERR_ARG); }
+            if (ib.down != (int)hdr.out_down_shift) {
+                set_error("engine: PPN head op %u reads buffer %u at down-shift %d but the outputs are at %u", i, po.in_buf, ib.down, hdr.out_down_shift);
+                return fail(HP_ERR_ARG);
+            }
+            if (K < 18 || K > 4096 || n_edge == 0 || n_edge > (1u << 20)) {
+                set_error("engine: PPN head op %u has K=%llu key points and %llu edge channels (needs K >= 18 for the COCO limb table)", i,
+                          (unsigned long long)K, (unsigned long long)n_edge);
+                return fail(HP_ERR_ARG);
+            }
+            if ((uint64_t)ib.channels < 6 * K + n_edge) {
+                set_error("engine: PPN head op %u reads %llu channels of a %d-channel buffer", i, (unsigned long long)(6 * K + n_edge), ib.channels);
+                return fail(HP_ERR_ARG);
+            }
+            if (hdr.conf_channels != 6 * K || hdr.paf_channels != n_edge) {
+                set_error("engine: PPN head op %u writes %llu box and %llu edge channels but the pack header says conf %u / paf %u", i,
+                          (unsigned long long)(6 * K), (unsigned long long)n_edge, hdr.conf_channels, hdr.paf_channels);
+                return fail(HP_ERR_ARG);
+            }
+            op.launch = tf32 ? Launch::PpnHeadF32 : Launch::PpnHead;
         } else {
             set_error("engine: unknown op type %u", po.type);
             return fail(HP_ERR_UNSUPPORTED);
@@ -1505,7 +1580,7 @@ int hp_engine_create_ex(hp_engine** out, const void* pack, size_t pack_bytes, in
         for (size_t k = i + 2; k < e->ops.size() && safe && !rewritten; ++k) {
             const PackOp& q = e->ops[k].po;
             if (reads_buffer(q, c.po.out_buf)) safe = false;
-            else if (q.type != OP_IM2COL3 && q.type != OP_PIFPAF_HEAD && q.out_mode != OUT_F32_NCHW_SPLIT && q.out_buf == c.po.out_buf) {
+            else if (q.type != OP_IM2COL3 && q.type != OP_PIFPAF_HEAD && q.type != OP_PPN_HEAD && q.out_mode != OUT_F32_NCHW_SPLIT && q.out_buf == c.po.out_buf) {
                 const int qc = q.type == OP_CONV ? (int)q.groups * (int)q.cout_g : (int)q.cout_g;
                 if (q.out_ch_off <= c.po.out_ch_off && (int)q.out_ch_off + qc >= (int)c.po.out_ch_off + Ctot) rewritten = true; else safe = false;
             }
@@ -1603,6 +1678,7 @@ int hp_engine_info(const hp_engine* e, int* in_w, int* in_h, int* max_batch, int
 }
 
 // 0: conf[c_conf,h,w] / paf[c_paf,h,w] for hyperpose::parser::paf; 1: OpenPifPaf fields pif[17,5,h,w] / paf[19,9,h,w]
+// 2: Pose Proposal Network boxes [6,K,h,w] / edges [L,nh,nw,h,w] for hyperpose::parser::pose_proposal
 int hp_engine_head_type(const hp_engine* e) { return e ? (int)e->hdr.head_type : HP_ERR_ARG; }
 
 // frames: HOST u8 [N, in_h, in_w, 3] (already network-sized, BGR like cv::Mat).  Asynchronous on the engine stream.
@@ -1891,7 +1967,7 @@ int hp_engine_calibrate_u8(hp_engine* e, const uint8_t* frames, int N, float* ab
             const int rc = run_graph(e, n, true, e->stream, oi, oi);
             if (rc) return done(rc);
             const PackOp& po = e->ops[oi].po;
-            if (po.type == OP_PIFPAF_HEAD || (po.type == OP_CONV && po.out_mode == OUT_F32_NCHW_SPLIT)) continue;
+            if (po.type == OP_PIFPAF_HEAD || po.type == OP_PPN_HEAD || (po.type == OP_CONV && po.out_mode == OUT_F32_NCHW_SPLIT)) continue;
             const EngBuffer& b = e->bufs[po.out_buf];
             const size_t cnt = (size_t)n * b.H * b.W * b.channels;
             absmax_f32_kernel<<<(unsigned)std::min<size_t>(1024, (cnt + 255) / 256), 256, 0, e->stream>>>((const float*)b.d, cnt, d_amax + po.out_buf);
@@ -1918,7 +1994,7 @@ int hp_pack_int8_calibrated(const void* pack, size_t pack_bytes)
 
 // test hook: the kernel op `op` launches on the next run over u8 frames, as decided when the engine was created (EngOp::launch and
 // the conv plan's tile width): conv<f16|tf32|i8,BN[,res][,stem3|stem7]>, halo<BN[,pool]>, dw_strip<K,S>, dw_col, dw_tma<1|2>, dw_f32,
-// dw_i8, maxpool<K>, maxpool_f32, maxpool_i8, im2col, im2col_i8, heads, or none when a neighbouring op's launch covers it
+// dw_i8, maxpool<K>, maxpool_f32, maxpool_i8, im2col, im2col_i8, heads, ppn_head, or none when a neighbouring op's launch covers it
 int hp_engine_debug_op_kernel(const hp_engine* e, int op, char* name, int cap)
 {
     if (!e || op < 0 || op >= (int)e->ops.size() || !name || cap <= 0) { set_error("hp_engine_debug_op_kernel: bad argument"); return HP_ERR_ARG; }
@@ -1942,6 +2018,7 @@ int hp_engine_debug_op_kernel(const hp_engine* e, int op, char* name, int cap)
     case Launch::DwStrip: s = "dw_strip<" + std::to_string(po.R) + "," + std::to_string(po.stride ? po.stride : 1) + ">"; break;
     case Launch::MaxPool: s = "maxpool<" + std::to_string(po.R ? po.R : 2) + ">"; break;
     case Launch::Heads: case Launch::HeadsF32: s = "heads"; break;
+    case Launch::PpnHead: case Launch::PpnHeadF32: s = "ppn_head"; break;
     case Launch::DwF32: s = "dw_f32"; break;
     case Launch::MaxPoolF32: s = "maxpool_f32"; break;
     case Launch::Im2colI8: s = "im2col_i8"; break;
@@ -2173,7 +2250,7 @@ static int pose_submit_pifpaf(hp_engine* e, hp_pifpaf* dec, const uint8_t* frame
 {
     if (!e || !dec || !frames || !ticket) { set_error("hp_pose_submit_pifpaf: null argument"); return HP_ERR_ARG; }
     if (N <= 0 || N > e->max_batch) { set_error("Input batch size overflow: Yours@%d Max@%d", N, e->max_batch); return HP_ERR_BATCH; }
-    if (e->hdr.head_type != 1) { set_error("hp_pose_submit_pifpaf: the model pack has conf / PAF outputs (use hp_pose_submit_u8_host)"); return HP_ERR_UNSUPPORTED; }
+    if (e->hdr.head_type != 1) { set_error("hp_pose_submit_pifpaf: the model pack has no OpenPifPaf heads (head_type %u)", e->hdr.head_type); return HP_ERR_UNSUPPORTED; }
     HP_CUDA_TRY(cudaSetDevice(e->device));
     const int idx = e->next_slot;
     hp_engine::PoseSlot& sl = e->slots[idx];
@@ -2195,7 +2272,11 @@ static int pose_submit(hp_engine* e, hp_paf* parser, const uint8_t* frames, int 
 {
     if (!e || !parser || !frames || !ticket) { set_error("hp_pose_submit: null argument"); return HP_ERR_ARG; }
     if (N <= 0 || N > e->max_batch) { set_error("Input batch size overflow: Yours@%d Max@%d", N, e->max_batch); return HP_ERR_BATCH; }
-    if (e->hdr.head_type != 0) { set_error("hp_pose_submit: the model pack has OpenPifPaf heads (use hp_engine_infer_u8_host + hp_pifpaf_process_device)"); return HP_ERR_UNSUPPORTED; }
+    if (e->hdr.head_type == 1) { set_error("hp_pose_submit: the model pack has OpenPifPaf heads (use hp_engine_infer_u8_host + hp_pifpaf_process_device)"); return HP_ERR_UNSUPPORTED; }
+    if (e->hdr.head_type != 0) {
+        set_error("hp_pose_submit: the model pack has Pose Proposal Network heads (use hp_engine_infer_u8_device + hp_ppn_process_device_strided on the engine's outputs)");
+        return HP_ERR_UNSUPPORTED;
+    }
     HP_CUDA_TRY(cudaSetDevice(e->device));
     const int idx = e->next_slot;
     hp_engine::PoseSlot& sl = e->slots[idx];

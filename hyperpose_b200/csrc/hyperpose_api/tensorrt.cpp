@@ -5,7 +5,8 @@
 // accept the path of an HPB2PACK model pack (hyperpose_b200/models.py) in place of the .uff/.onnx/.trt file;
 // a file that is not a pack is a fatal error, like an unparsable model in the reference (tensorrt.cpp:141-158).
 // inference() returns, per image, the outputs ordered by name (conf < paf, tensorrt.cpp:405; paf < pif for OpenPifPaf
-// packs) as host feature_map_t objects with shape [C,H,W] ([19,9,h,w] / [17,5,h,w]), exactly as the reference does;
+// packs; the seven Pose Proposal Network maps for PPN packs) as host feature_map_t objects with shape [C,H,W] ([19,9,h,w] /
+// [17,5,h,w]; [K,gh,gw] x6 and [17,9,9,gh,gw]), exactly as the reference does;
 // the same buffers are published for the device-resident hand-off to the parsers (csrc/handoff.h).
 #include <cstdio>
 #include <cstdlib>
@@ -107,10 +108,42 @@ namespace dnn {
         // [17,5,h,w] -- the order pifpaf::process(packet[0], packet[1]) relies on (src/pifpaf.cpp:6-7).
         // The buffers are filled by ONE call that also publishes them for the device-resident hand-off (handoff.h): the
         // parser.process() calls that follow find the batch on the device and parse it once.
+        // Pose Proposal Network packs (head_type 2): seven maps per image, conf_point, conf_iou, x, y, w, h [K,gh,gw] and edge
+        // [L,nh,nw,gh,gw] -- the order pose_proposal::process(const std::vector<feature_map_t>&) reads them in
+        // (proposal_network.hpp:51-62), under names that sort in that order.  A plain read-back: no parser looks PPN tensors up.
+        std::vector<internal_t> collect_ppn(hp_engine* e, size_t batch, int cc, int cp, int oh, int ow)
+        {
+            static const char* const names[6] = { "0_conf_point", "1_conf_iou", "2_x", "3_y", "4_w", "5_h" };
+            const size_t plane = (size_t)oh * ow, K = (size_t)cc / 6, n_edge = 17 * 9 * 9;
+            if (cc % 6 || (size_t)cp != n_edge) die("PPN pack with " + std::to_string(cc) + " box / " + std::to_string(cp) + " edge channels (needs 6K / 17*9*9)");
+            std::vector<std::unique_ptr<float[]>> boxes(batch);
+            std::vector<std::unique_ptr<char[]>> edges(batch);
+            std::vector<float*> pa(batch), pb(batch);
+            for (size_t j = 0; j < batch; ++j) {
+                boxes[j].reset(new float[cc * plane]);
+                edges[j].reset(new char[cp * plane * sizeof(float)]);
+                pa[j] = boxes[j].get();
+                pb[j] = reinterpret_cast<float*>(edges[j].get());
+            }
+            if (hp_engine_read_outputs_frames(e, pa.data(), pb.data(), (int)batch, 0) != HP_OK) die("hp_engine_read_outputs_frames");
+            std::vector<internal_t> ret(batch);
+            for (size_t j = 0; j < batch; ++j) {
+                for (int t = 0; t < 6; ++t) {
+                    std::unique_ptr<char[]> m(new char[K * plane * sizeof(float)]);
+                    std::memcpy(m.get(), pa[j] + t * K * plane, K * plane * sizeof(float));
+                    ret[j].emplace_back(names[t], std::move(m), std::vector<int>{ (int)K, oh, ow });
+                }
+                ret[j].emplace_back("6_edge", std::move(edges[j]), std::vector<int>{ 17, 9, 9, oh, ow });
+            }
+            return ret;
+        }
+
         std::vector<internal_t> collect(hp_engine* e, size_t batch, int cc, int cp, int oh, int ow)
         {
             const size_t plane = (size_t)oh * ow;
-            const bool pifpaf = hp_engine_head_type(e) == 1;
+            const int head = hp_engine_head_type(e);
+            if (head == 2) return collect_ppn(e, batch, cc, cp, oh, ow);
+            const bool pifpaf = head == 1;
             std::vector<std::unique_ptr<char[]>> a(batch), b(batch);
             std::vector<float*> pa(batch), pb(batch);
             for (size_t j = 0; j < batch; ++j) {

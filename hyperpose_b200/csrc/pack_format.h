@@ -18,7 +18,10 @@ enum PackOpType : uint32_t {
     OP_MAXPOOL2 = 3, // RxR (R = 2 or 3) stride-2 max-pool, TF "SAME" semantics (out = ceil(in/2), window clipped at the border)
     OP_PIFPAF_HEAD = 5, // OpenPifPaf heads: pixel-shuffle(2) + crop + sigmoid/softplus + index grid of the two raw 1x1-conv outputs
                         // (in_buf = pif raw [.,.,340+], res_buf = paf raw [.,.,684+]) -> engine outputs pif[N,17,5,ho,wo], paf[N,19,9,ho,wo]
-    OP_DWCONV = 4    // depthwise KxK (K = 1 or 3) conv, stride 1/2, TF "SAME" padding, + bias + PReLU; HBM-bound CUDA-core kernel
+    OP_DWCONV = 4,   // depthwise KxK (K = 1 or 3) conv, stride 1/2, TF "SAME" padding, + bias + PReLU; HBM-bound CUDA-core kernel
+    OP_PPN_HEAD = 6  // Pose Proposal Network head: sigmoid + restore_coor of one raw 1x1-conv output (in_buf [.,.,6K + L*nh*nw+]) ->
+                     // engine outputs conf[N,6,K,gh,gw] (conf_point, conf_iou, x, y, w, h) and paf[N,L,nh,nw,gh,gw];
+                     // cout_g = K, groups = L, R x S = nh x nw
 };
 
 struct PackHeader {
@@ -28,7 +31,8 @@ struct PackHeader {
     uint32_t conf_channels, paf_channels; // channels of the two fp32 NCHW outputs handed to the parser
     uint32_t out_down_shift;              // outputs are at (H >> shift, W >> shift)
     float mean[3];                        // subtracted after scaling, per model-input channel (backbones.py:455)
-    uint32_t head_type;                   // 0: conf/paf at (H >> shift); 1: OpenPifPaf fields at 2*(H >> shift) - 1 (pixel-shuffled, cropped)
+    uint32_t head_type;                   // 0: conf/paf at (H >> shift); 1: OpenPifPaf fields at 2*(H >> shift) - 1 (pixel-shuffled, cropped);
+                                          // 2: Pose Proposal Network boxes / edges at (H >> shift) (OP_PPN_HEAD)
     uint32_t reserved[4];                 // keeps blob_floats 8-byte aligned at offset 64.  reserved[0] = n_act_scales: 0, or n_buffers
                                           // when the INT8 calibration table (one fp32 scale per activation buffer) follows the blob
     uint64_t blob_floats;

@@ -16,6 +16,7 @@
 #include <stdint.h>
 #include <string.h>
 
+#include <mutex>
 #include <type_traits>
 #include <vector>
 
@@ -50,6 +51,7 @@ struct __align__(16) Box {
 struct PpnParams {
     const float *conf, *x, *y, *w, *h, *edge;
     int K, gh, gw, E, nh, nw, net_w, net_h;
+    size_t box_stride, edge_stride;   // floats from one frame's box / edge maps to the next (the engine's conf slot holds 6 maps per frame)
     float pt, lt, nt;
     int cap_c;              // candidate keys (power of two)
     hp_human* humans; int hcap;
@@ -116,12 +118,12 @@ __global__ void __launch_bounds__(THREADS, 1) ppn_parse_kernel(PpnParams P)
     __shared__ int s_nthr[NPARTS], s_nret[NPARTS];
     __shared__ int s_cnt, s_nh, s_flags, s_nkeep;
 
-    const float* conf = P.conf + (size_t)f * P.K * G;
-    const float* bx = P.x + (size_t)f * P.K * G;
-    const float* by = P.y + (size_t)f * P.K * G;
-    const float* bw = P.w + (size_t)f * P.K * G;
-    const float* bh = P.h + (size_t)f * P.K * G;
-    const float* edge = P.edge + (size_t)f * P.E * nn * G;
+    const float* conf = P.conf + (size_t)f * P.box_stride;
+    const float* bx = P.x + (size_t)f * P.box_stride;
+    const float* by = P.y + (size_t)f * P.box_stride;
+    const float* bw = P.w + (size_t)f * P.box_stride;
+    const float* bh = P.h + (size_t)f * P.box_stride;
+    const float* edge = P.edge + (size_t)f * P.edge_stride;
     if (tid == 0) { s_nh = 0; s_flags = 0; }
 
     // ---- A + B: threshold, decode, sort ascending by (conf, grid), NMS -- one warp per key-point type ----
@@ -404,6 +406,23 @@ int hp_ppn_create(hp_ppn** out, int net_w, int net_h, float point_thresh, float 
     hp_ppn* p = new hp_ppn();
     p->device = device; p->net_w = net_w; p->net_h = net_h; p->pt = point_thresh; p->lt = limb_thresh; p->nt = nms_thresh;
     if (cudaDeviceGetAttribute(&p->smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, device) != cudaSuccess) { delete p; hpb::set_error("cudaDeviceGetAttribute failed"); return HP_ERR_CUDA; }
+    {
+        // The dynamic shared-memory cap of the parse kernels is process-wide state.  It is raised once per device, to everything a
+        // launch may ask for, before any parser of that device launches: parsers used from several threads at once (the reference's
+        // stream scheduler parses on a thread pool, one parser per thread) never set it while another thread launches.
+        static std::mutex mu;
+        static std::vector<char> raised;
+        std::lock_guard<std::mutex> lk(mu);
+        if (raised.size() <= (size_t)device) raised.resize(device + 1, 0);
+        if (!raised[device]) {
+            const int cap = p->smem_optin - 1024;
+            if (cudaFuncSetAttribute(ppn_parse_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, cap) != cudaSuccess ||
+                cudaFuncSetAttribute(ppn_parse_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, cap) != cudaSuccess) {
+                delete p; hpb::set_error("hp_ppn_create: cudaFuncSetAttribute failed: %s", cudaGetErrorString(cudaGetLastError())); return HP_ERR_CUDA;
+            }
+            raised[device] = 1;
+        }
+    }
     if (cudaStreamCreateWithFlags(&p->stream, cudaStreamNonBlocking) != cudaSuccess) { delete p; hpb::set_error("cudaStreamCreate failed"); return HP_ERR_CUDA; }
     *out = p;
     return HP_OK;
@@ -425,11 +444,26 @@ int hp_ppn_set_nms_thresh(hp_ppn* p, float t) { if (!p) return HP_ERR_ARG; p->nt
 int hp_ppn_process_device(hp_ppn* p, const float* d_conf, const float* d_x, const float* d_y, const float* d_w, const float* d_h,
                           const float* d_edge, int N, int K, int gh, int gw, int E, int nh, int nw, void* stream)
 {
+    const size_t G = (size_t)(gh > 0 ? gh : 0) * (gw > 0 ? gw : 0);
+    return hp_ppn_process_device_strided(p, d_conf, d_x, d_y, d_w, d_h, d_edge, N, K, gh, gw, E, nh, nw, (size_t)(K > 0 ? K : 0) * G,
+                                         (size_t)(E > 0 ? E : 0) * (nh > 0 ? nh : 0) * (nw > 0 ? nw : 0) * G, stream);
+}
+
+int hp_ppn_process_device_strided(hp_ppn* p, const float* d_conf, const float* d_x, const float* d_y, const float* d_w, const float* d_h,
+                                  const float* d_edge, int N, int K, int gh, int gw, int E, int nh, int nw, size_t box_frame_stride,
+                                  size_t edge_frame_stride, void* stream)
+{
     if (!p || !d_conf || !d_x || !d_y || !d_w || !d_h || !d_edge || N <= 0 || gh <= 0 || gw <= 0 || E < 0 || nh <= 0 || nw <= 0) {
         hpb::set_error("hp_ppn_process_device: bad argument"); return HP_ERR_ARG;
     }
     // COCOPAIR_STD indexes key-point lists 0..17: with fewer the reference's key_points.at() throws (:187-188)
     if (K < NPARTS) { hpb::set_error("hp_ppn: K=%d key-point maps, the COCO limb table needs 18", K); return HP_ERR_ARG; }
+    // a frame's maps must not overlap the next frame's: K maps of gh*gw, E*nh*nw edge planes
+    if (box_frame_stride < (size_t)K * gh * gw || edge_frame_stride < (size_t)E * nh * nw * gh * gw) {
+        hpb::set_error("hp_ppn_process_device: frame strides %zu / %zu floats are shorter than one frame's %d box / %d edge maps of %dx%d",
+                       box_frame_stride, edge_frame_stride, K, E * nh * nw, gh, gw);
+        return HP_ERR_ARG;
+    }
     const int G = gh * gw;
     if (G > 16384) { hpb::set_error("hp_ppn: %dx%d grid not supported", gh, gw); return HP_ERR_UNSUPPORTED; }
     HP_CUDA_TRY(cudaSetDevice(p->device));
@@ -446,14 +480,13 @@ int hp_ppn_process_device(hp_ppn* p, const float* d_conf, const float* d_x, cons
     size_t dyn = want * 8;
     if (dyn < tables) dyn = tables;
     const size_t smem = fixed + dyn;
-    HP_CUDA_TRY(cudaFuncSetAttribute(ppn_parse_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    HP_CUDA_TRY(cudaFuncSetAttribute(ppn_parse_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     if (p->use_spill) HP_CUDA_TRY(p->spill.ensure((size_t)N * spill_bytes()));
     HP_CUDA_TRY(p->humans.ensure((size_t)N * p->hcap));
     HP_CUDA_TRY(p->counters.ensure((size_t)N * 2));
     PpnParams P;
     P.conf = d_conf; P.x = d_x; P.y = d_y; P.w = d_w; P.h = d_h; P.edge = d_edge;
     P.K = K; P.gh = gh; P.gw = gw; P.E = E; P.nh = nh; P.nw = nw; P.net_w = p->net_w; P.net_h = p->net_h;
+    P.box_stride = box_frame_stride; P.edge_stride = edge_frame_stride;
     P.pt = p->pt; P.lt = p->lt; P.nt = p->nt; P.cap_c = (int)want;
     P.humans = p->humans.p; P.hcap = p->hcap; P.human_cnt = p->counters.p; P.flags = p->counters.p + N;
     P.spill = p->spill.p;

@@ -4,7 +4,8 @@
                                     [--int8-calibration frames.npy [--factor F] [--no-flip-rgb]]
 
 `--weights` is a TensorLayer `save_weights(format="npz")` file of the reference's model of that architecture -- OpenPose-VGG19 (also
-the name-keyed `npz_dict` form), MobilenetThin-OpenPose, LightWeightOpenPose on ResNet-50, PifPaf on ResNet-50; hyperpose_b200/weights.py
+the name-keyed `npz_dict` form), MobilenetThin-OpenPose, LightWeightOpenPose on ResNet-50, PifPaf on ResNet-50, Pose Proposal Networks
+on ResNet-18 / ResNet-50; hyperpose_b200/weights.py
 spells out the all_weights order of each, BatchNorm statistics are folded.  Without it the pack holds seeded random weights, which is
 what the benchmarks and tests use (no trained model can be downloaded offline).  Replaces the .onnx / .uff / .trt files of
 include/hyperpose/utility/model.hpp:13-32 (SURVEY.md 8f rank 1).
@@ -26,7 +27,8 @@ from . import models, weights
 def main(argv=None) -> int:
     ap = argparse.ArgumentParser(description=__doc__.split("\n")[0])
     ap.add_argument("--model", default="openpose_vgg19",
-                    choices=["openpose_vgg19", "mobilenet_thin_openpose", "resnet50_lw_openpose", "resnet50_pifpaf", "tiny_test_net"])
+                    choices=["openpose_vgg19", "mobilenet_thin_openpose", "resnet50_lw_openpose", "resnet50_pifpaf", "ppn_resnet18", "ppn_resnet50",
+                             "tiny_test_net"])
     ap.add_argument("--out", required=True)
     ap.add_argument("--weights", default=None, help="TensorLayer save_weights(format='npz') file of the same architecture")
     ap.add_argument("--seed", type=int, default=0)
@@ -38,7 +40,8 @@ def main(argv=None) -> int:
     a = ap.parse_args(argv)
     if a.weights:
         loaders = {"openpose_vgg19": weights.ListWeights, "mobilenet_thin_openpose": weights.MobilenetThinWeights,
-                   "resnet50_lw_openpose": weights.Resnet50LwWeights, "resnet50_pifpaf": weights.Resnet50PifPafWeights}
+                   "resnet50_lw_openpose": weights.Resnet50LwWeights, "resnet50_pifpaf": weights.Resnet50PifPafWeights,
+                   "ppn_resnet18": weights.Ppn18Weights, "ppn_resnet50": weights.Ppn50Weights}
         if a.model not in loaders:
             ap.error(f"--weights: no trained-weight layout for {a.model}")
         g = getattr(models, a.model)(weights=loaders[a.model].from_npz(a.weights))

@@ -19,7 +19,7 @@ from dataclasses import dataclass, field
 
 import numpy as np
 
-OP_IM2COL3, OP_CONV, OP_MAXPOOL2, OP_DWCONV, OP_PIFPAF_HEAD = 1, 2, 3, 4, 5
+OP_IM2COL3, OP_CONV, OP_MAXPOOL2, OP_DWCONV, OP_PIFPAF_HEAD, OP_PPN_HEAD = 1, 2, 3, 4, 5, 6
 OUT_F16_NHWC, OUT_F32_NCHW_SPLIT = 0, 1
 PACK_MAGIC = b"HPB2PACK"
 PACK_VERSION = 2
@@ -58,6 +58,7 @@ class Graph:
     out_down_shift: int = 3
     mean: tuple = (0.0, 0.0, 0.0)
     head_type: int = 0                 # 1: OpenPifPaf fields (pif[17,5,ho,wo] / paf[19,9,ho,wo] in the conf / paf output slots)
+                                       # 2: Pose Proposal Network (boxes [6,K,gh,gw] / edges [L,nh,nw,gh,gw] in the conf / paf output slots)
     buffers: list = field(default_factory=list)   # (channels, down_shift)
     ops: list = field(default_factory=list)
     act_scales: np.ndarray | None = None          # INT8 calibration table: one fp32 scale per buffer (set_int8_scales), or None
@@ -558,6 +559,111 @@ def resnet50_pifpaf(seed: int = 0, weights=None) -> Graph:
         wpaf, bpaf = _he(rng, 1, 684, 2048, 1, 1, 0.5), (rng.standard_normal(684) * 0.1).astype(np.float32)
     g.add_conv(cur, paf_raw, wpaf, bpaf, lin(684), name="paf_head")
     g.ops.append(Op(OP_PIFPAF_HEAD, in_buf=pif_raw, res_buf=paf_raw, name="pifpaf_heads"))
+    return g
+
+
+PPN_K, PPN_L, PPN_NH, PPN_NW = 18, 17, 9, 9     # pose_proposal/model.py:14-15 defaults: key points, limbs, 9 x 9 neighbourhood
+
+
+def _ppn_stem(g, rng, ws):
+    """7x7/2 conv (no bias) + BN + ReLU, then the 3x3/2 max-pool: (buffer, channels, down_shift) at stride 4"""
+    col = g.add_buffer(192, 1); g.add_im2col(col, stride=2, ksize=7)
+    c1 = g.add_buffer(64, 1)
+    if ws:
+        w = ws.conv("conv1", 64, 3, 7)[0][None]; sc, sh = ws.bn("bn1", 64)
+    else:
+        w = _he(rng, 1, 64, 3, 7, 7); sc, sh = _bn_fold(rng, 64)
+    g.add_conv(col, c1, w * sc.reshape(1, 64, 1, 1, 1), sh, np.zeros(64, np.float32), im2col_input=1, name="conv1+bn1")
+    x = g.add_buffer(64, 2); g.add_maxpool(c1, x, 64, "maxpool_1", ksize=3)
+    return x, 64, 2
+
+
+def _ppn_head(g, rng, ws, cur, cur_c, cur_d):
+    """pose_proposal/model.py:43-79: add_block_1 / add_block_2 (3x3 conv + bias, BN, leaky ReLU 0.1 = PReLU with every slope 0.1),
+    add_block_3 (1x1 conv + bias to 6K + L*nh*nw channels), then OP_PPN_HEAD (sigmoid + restore_coor, :84-93,:111-119)"""
+    n_out = 6 * PPN_K + PPN_L * PPN_NH * PPN_NW
+    leaky = lambda n: np.full(n, 0.1, np.float32)
+    for i, ci in ((1, cur_c), (2, 512)):
+        if ws:
+            w, b = ws.conv(f"add{i}", 512, ci, 3); w = w[None]; sc, sh = ws.bn(f"add{i}.bn", 512)
+        else:
+            w = _he(rng, 1, 512, ci, 3, 3); b = (rng.standard_normal(512) * 0.05).astype(np.float32); sc, sh = _bn_fold(rng, 512)
+        nxt = g.add_buffer(512, cur_d)
+        g.add_conv(cur, nxt, w * sc.reshape(1, 512, 1, 1, 1), sh + b * sc, leaky(512), name=f"add_block_{i}")
+        cur = nxt
+    raw = g.add_buffer((n_out + 7) // 8 * 8, cur_d)      # 1485 -> 1488 channels
+    if ws:
+        w, b = ws.conv("add3", n_out, 512, 1); w = w[None]
+    else:
+        w = _he(rng, 1, n_out, 512, 1, 1, 1.0); b = (rng.standard_normal(n_out) * 0.1).astype(np.float32)
+    g.add_conv(cur, raw, w, b, np.ones(n_out, np.float32), name="add_block_3")
+    g.ops.append(Op(OP_PPN_HEAD, in_buf=raw, R=PPN_NH, S=PPN_NW, groups=PPN_L, cout_g=PPN_K, name="ppn_head"))
+
+
+def ppn_resnet18(seed: int = 0, weights=None) -> Graph:
+    """Pose Proposal Network on ResNet-18 (the default backbone of hyperpose/Model/pose_proposal/model.py:39-42):
+    Resnet18_backbone(scale_size=32) (backbones.py:512-585: 7x7/2 stem, 3x3/2 max-pool, blocks 2_1 .. 5_1; block_5_2 exists only
+    with `pretraining`, :535-536,:552, so it is not built), stride 32, 512 channels, then the PPN head (_ppn_head).
+    A block is relu(bn(conv3x3(relu(bn(conv3x3/s(x))))) + res) with res = bn(conv1x1/s(x)) when it down-samples.  A stride-2 conv
+    runs at stride 1 and a one-hot depthwise op sub-samples it (exact, see _resnet50_body).  BatchNorm folded.
+    `weights`: a hyperpose_b200.weights.Ppn18Weights; default = seeded random values."""
+    rng = np.random.default_rng(seed)
+    ws = weights
+    g = Graph("ppn_resnet18", 6 * PPN_K, PPN_L * PPN_NH * PPN_NW, 5, mean=(0.0, 0.0, 0.0), head_type=2)
+    relu = lambda n: np.zeros(n, np.float32)
+    lin = lambda n: np.ones(n, np.float32)
+
+    def conv_bn(in_buf, out_buf, ci, co, k, act, name, gain, **kw):
+        if ws:
+            w = ws.conv(f"{name}.conv", co, ci, k)[0][None]; sc, sh = ws.bn(f"{name}.bn", co)
+        else:
+            w = _he(rng, 1, co, ci, k, k, gain); sc, sh = _bn_fold(rng, co)
+        g.add_conv(in_buf, out_buf, w * sc.reshape(1, co, 1, 1, 1), sh, relu(co) if act else lin(co), name=name, **kw)
+
+    def subsample(in_buf, out_buf, C, centre3, name):
+        w = np.zeros((C, 3, 3), np.float32) if centre3 else np.ones((C, 1, 1), np.float32)
+        if centre3:
+            w[:, 1, 1] = 1.0
+        g.add_dwconv(in_buf, out_buf, w, np.zeros(C, np.float32), lin(C), stride=2, name=name)
+
+    cur, cur_c, cur_d = _ppn_stem(g, rng, ws)
+    for name, nf, st, ds in RESNET18_BLOCKS:
+        d_out = cur_d + (1 if st == 2 else 0)
+        a = g.add_buffer(nf, cur_d)
+        conv_bn(cur, a, cur_c, nf, 3, True, f"{name}_1", 2.0)
+        if st == 2:
+            a2 = g.add_buffer(nf, d_out); subsample(a, a2, nf, True, f"{name}_1_sub"); a = a2
+        if ds:
+            src = cur
+            if st == 2:
+                src = g.add_buffer(cur_c, d_out); subsample(cur, src, cur_c, False, f"{name}_ds_sub")
+            res = g.add_buffer(nf, d_out)
+            conv_bn(src, res, cur_c, nf, 1, False, f"{name}_ds", 1.0)
+        else:
+            res = cur
+        out = g.add_buffer(nf, d_out)
+        conv_bn(a, out, nf, nf, 3, True, f"{name}_2", 0.5, res_buf=res, res_mode=1)    # relu(x + res)
+        cur, cur_c, cur_d = out, nf, d_out
+    _ppn_head(g, rng, ws, cur, cur_c, cur_d)
+    return g
+
+
+# (block name, n_filter, stride, is_down_sample) of Resnet18_backbone(scale_size=32) (backbones.py:529-535)
+RESNET18_BLOCKS = [("block_2_1", 64, 1, False), ("block_2_2", 64, 1, False), ("block_3_1", 128, 2, True), ("block_3_2", 128, 1, False),
+                   ("block_4_1", 256, 2, True), ("block_4_2", 256, 1, False), ("block_5_1", 512, 2, True)]
+
+
+def ppn_resnet50(seed: int = 0, weights=None) -> Graph:
+    """Pose Proposal Network on ResNet-50 (the model zoo's ppn-resnet50-V2-HW=384x384, scripts/downloader.py:15):
+    Resnet50_backbone(scale_size=32, use_pool=True) (backbones.py:587-698: 7x7/2 stem, 3x3/2 max-pool, 16 bottleneck blocks with
+    stride-2 first blocks in stages 3-5), stride 32, 2048 channels, then the PPN head (_ppn_head).  BatchNorm folded.
+    `weights`: a hyperpose_b200.weights.Ppn50Weights; default = seeded random values."""
+    rng = np.random.default_rng(seed)
+    ws = weights
+    g = Graph("ppn_resnet50", 6 * PPN_K, PPN_L * PPN_NH * PPN_NW, 5, mean=(0.0, 0.0, 0.0), head_type=2)
+    x, c, d = _ppn_stem(g, rng, ws)
+    cur, cur_c, cur_d = _resnet50_body(g, rng, ws, x, c, d, [(64, 3, 1), (128, 4, 2), (256, 6, 2), (512, 3, 2)])
+    _ppn_head(g, rng, ws, cur, cur_c, cur_d)
     return g
 
 

@@ -4,6 +4,7 @@
   * MobilenetThin-OpenPose    openpose/model/mbv2_th_openpose.py + backbones.py:233-297              -> MobilenetThinWeights
   * LW-OpenPose on ResNet-50  openpose/model/lw_openpose.py + backbones.py:587-698                   -> Resnet50LwWeights
   * PifPaf on ResNet-50       pifpaf/model.py:41-281 + backbones.py:587-698                          -> Resnet50PifPafWeights
+  * PPN on ResNet-18 / -50    pose_proposal/model.py:14-119 + backbones.py:512-698                   -> Ppn18Weights / Ppn50Weights
 
 The reference saves a trained model with TensorLayer's `Model.save_weights(path, format="npz")`: an ORDERED list of
 arrays = `model.all_weights`, i.e. layer-creation order; most layers carry auto-generated names
@@ -318,6 +319,55 @@ def resnet50_pifpaf_layer_order(n_pos: int = 17, n_limbs: int = 19):
     _resnet50_order(order, [(64, 3, 1), (128, 4, 2), (256, 6, 2), (512, 3, 2)])
     order += [("conv", "pif_head", n_pos * 5 * 4, 2048, 1), ("conv", "paf_head", n_limbs * 9 * 4, 2048, 1)]
     return order
+
+
+def _ppn_head_order(order, cin, K: int = 18, L: int = 17, nh: int = 9, nw: int = 9):
+    """PoseProposal's add_layer_1 / add_layer_2 (Conv2d 3x3 with bias, BatchNorm) and add_layer_3 (Conv2d 1x1 with bias),
+    pose_proposal/model.py:43-79, created after the backbone"""
+    order += [("conv", "add1", 512, cin, 3), ("bn", "add1.bn", 512, 0, 0), ("conv", "add2", 512, 512, 3), ("bn", "add2.bn", 512, 0, 0),
+              ("conv", "add3", 6 * K + L * nh * nw, 512, 1)]
+
+
+def ppn_resnet18_layer_order():
+    """all_weights order of PoseProposal on Resnet18_backbone(scale_size=32) (backbones.py:512-585): conv_1_1 (no bias), bn_1_1, then
+    the blocks; inside a Res_block `main_block` is created before `down_sample` (:564-576), so the shortcut's conv / bn come last"""
+    from .models import RESNET18_BLOCKS
+    order = [("conv_nobias", "conv1", 64, 3, 7), ("bn", "bn1", 64, 0, 0)]
+    cin = 64
+    for name, nf, _, ds in RESNET18_BLOCKS:
+        order += [("conv_nobias", f"{name}_1.conv", nf, cin, 3), ("bn", f"{name}_1.bn", nf, 0, 0),
+                  ("conv_nobias", f"{name}_2.conv", nf, nf, 3), ("bn", f"{name}_2.bn", nf, 0, 0)]
+        if ds:
+            order += [("conv_nobias", f"{name}_ds.conv", nf, cin, 1), ("bn", f"{name}_ds.bn", nf, 0, 0)]
+        cin = nf
+    _ppn_head_order(order, 512)
+    return order
+
+
+def ppn_resnet50_layer_order():
+    """all_weights order of PoseProposal on Resnet50_backbone(scale_size=32, use_pool=True) (backbones.py:587-698)"""
+    order = []
+    _resnet50_order(order, [(64, 3, 1), (128, 4, 2), (256, 6, 2), (512, 3, 2)])
+    _ppn_head_order(order, 2048)
+    return order
+
+
+class Ppn18Weights(BnNetWeights):
+    def __init__(self, arrays):
+        super().__init__(arrays, ppn_resnet18_layer_order())
+
+    @classmethod
+    def from_npz(cls, path: str):
+        return cls(load_params_npz(path))
+
+
+class Ppn50Weights(BnNetWeights):
+    def __init__(self, arrays):
+        super().__init__(arrays, ppn_resnet50_layer_order())
+
+    @classmethod
+    def from_npz(cls, path: str):
+        return cls(load_params_npz(path))
 
 
 class Resnet50LwWeights(BnNetWeights):

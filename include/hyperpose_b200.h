@@ -147,6 +147,13 @@ int hp_ppn_process_host(hp_ppn* p, const float* conf_point, const float* x, cons
 /* same with DEVICE tensors, asynchronous on `stream` (NULL = the parser's own); results by hp_ppn_fetch */
 int hp_ppn_process_device(hp_ppn* p, const float* d_conf_point, const float* d_x, const float* d_y, const float* d_w, const float* d_h,
                           const float* d_edge, int N, int K, int gh, int gw, int E, int nh, int nw, void* stream);
+/* the same with the distance from one frame's maps to the next given in floats: box_frame_stride for conf_point / x / y / w / h
+ * (hp_ppn_process_device: K*gh*gw), edge_frame_stride for edge (E*nh*nw*gh*gw).  A PPN engine's outputs (head_type 2) are parsed
+ * in place with d_conf_point = conf slot + 0, d_x = + 2*K*gh*gw, d_y = + 3*K*gh*gw, d_w = + 4*K*gh*gw, d_h = + 5*K*gh*gw,
+ * box_frame_stride = 6*K*gh*gw, d_edge = the paf slot, edge_frame_stride = E*nh*nw*gh*gw. */
+int hp_ppn_process_device_strided(hp_ppn* p, const float* d_conf_point, const float* d_x, const float* d_y, const float* d_w, const float* d_h,
+                                  const float* d_edge, int N, int K, int gh, int gw, int E, int nh, int nw, size_t box_frame_stride,
+                                  size_t edge_frame_stride, void* stream);
 int hp_ppn_fetch(hp_ppn* p, hp_human* out, int cap, int* n_out, int N);
 long long hp_ppn_launch_count(const hp_ppn* p);
 
@@ -213,7 +220,10 @@ int hp_engine_read_outputs_host(hp_engine* e, float* conf, float* paf, int N);
  * (other address, other shape, any changed byte, publication older than 4 batches) takes the ordinary host path; the
  * results are identical.  Publishing is opt-in (publish = 0 is a plain read-back). */
 int hp_engine_read_outputs_frames(hp_engine* e, float* const* conf_frames, float* const* paf_frames, int N, int publish);
-/* 0: conf/paf maps for hyperpose::parser::paf; 1: OpenPifPaf fields (pif, paf) for hyperpose::parser::pifpaf */
+/* 0: conf/paf maps for hyperpose::parser::paf; 1: OpenPifPaf fields (pif, paf) for hyperpose::parser::pifpaf;
+ * 2: Pose Proposal Network outputs for hyperpose::parser::pose_proposal -- conf slot [6,K,gh,gw] (conf_point, conf_iou, x, y, w, h;
+ * boxes in network-input pixels), paf slot [L,nh,nw,gh,gw] (edges), c_conf = 6K, c_paf = L*nh*nw.  The hp_pose_* calls refuse it:
+ * parse with hp_ppn_process_device_strided on the engine's device outputs. */
 int hp_engine_head_type(const hp_engine* e);
 /* the publication mechanism above: global switch (default on; env HPB_NO_HANDOFF disables) and counters
  * (batches published, process() calls served from a device snapshot, batched parses run, look-ups that fell back) */
