@@ -667,7 +667,7 @@ struct EngOp {
 // Environment switches, read once by hp_engine_create_ex.  Each selects the plainer form of a fused or TMA kernel path, the
 // reference the tests compare the default against.
 struct EngOptions {
-    enum { HALO_AUTO, HALO_NONE, HALO_ALL } halo = HALO_AUTO;   // HPB_HALO=all | anything else; unset: 3x3 layers whose tile grid wastes <= 6 %
+    enum { HALO_AUTO, HALO_NONE, HALO_ALL } halo = HALO_AUTO;   // HPB_HALO=all | anything else; unset: build_conv_plan's rule
     bool stem3 = true;           // fused 3x3 stem; HPB_NO_STEM3 keeps the im2col buffer
     bool pool_fuse = true;       // HPB_NO_POOL_FUSE
     bool dw1_fuse = true;        // HPB_NO_DW1_FUSE
@@ -902,12 +902,20 @@ int build_conv_plan(hp_engine* e, EngOp& op, const float* blob)
     if (e->dtype != HP_DTYPE_F16) return HP_OK;   // the TF32 and INT8 engines have no halo kernel
     pl.monotone_act = true;
     for (float a : alpha) if (!(a >= 0.f)) { pl.monotone_act = false; break; }
-    // Halo-box kernel for RxS layers whose 16 x 8 tile grid wastes little of the image (the early VGG layers): the A operand comes
-    // from L2 once per chunk instead of once per tap.
+    // Halo-box kernel: the A operand comes from L2 once per chunk instead of once per tap, in exchange for the pixels its 16 x 8 tile
+    // grid computes outside the image (waste).  Per-layer times of the cfg3 / cfg4 / cfg5 graphs at their benchmark batch sizes on
+    // both kernels (tools/layer_times.py, DESIGN.md §4) give the rule:
+    //  * 3x3 layers whose grid wastes at most 6 % of the image: always (VGG conv1_2 -- conv2_2, 1.4-1.6x faster);
+    //  * layers of two or more 64-channel chunks whose grid wastes at most 25 %, when the im2col grid needs more than one round of
+    //    CTAs: the 3x3 layers of 128-512 channels at 46x54 to 193x193 (5-32 % faster) and OpenPose's 7x7 refinement convs (within 3 % either way).
+    // It loses on one-chunk layers (ResNet-50's 64-channel 3x3 at 92x108 and 193x193: 7-17 % slower) and where the grid wastes half the
+    // image (49x49 and 25x25: 6-10 % slower).  Launches of at most one round were not measured; they keep the first rule only.
     const int ty = (ib.H + HALO_TH - 1) / HALO_TH, tx = (ib.W + HALO_TW - 1) / HALO_TW;
     const double waste = (double)ty * HALO_TH * tx * HALO_TW / ((double)ib.H * ib.W) - 1.0;
     const bool shape_ok = !im2col && eR == eS && (eR == 3 || eR == 5 || eR == 7) && !po.res_mode && po.out_mode == OUT_F16_NHWC;
-    const bool want = e->opt.halo == EngOptions::HALO_AUTO ? (eR == 3 && waste <= 0.06) : e->opt.halo == EngOptions::HALO_ALL;
+    const bool rounds = (long)p.m_tiles * G * (cout_pad / BN) > e->num_sms - e->reserve_sms;
+    const bool faster = (eR == 3 && waste <= 0.06) || (rounds && ecin >= 2 * CONV_BLOCK_K && waste <= 0.25);
+    const bool want = e->opt.halo == EngOptions::HALO_AUTO ? faster : e->opt.halo == EngOptions::HALO_ALL;
     if (shape_ok && want) {
         const EngBuffer& ob = e->bufs[po.out_buf];
         HaloParams& h = pl.hp;
