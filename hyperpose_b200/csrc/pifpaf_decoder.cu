@@ -89,9 +89,13 @@ __device__ __forceinline__ float approx_exp(float x) // :224-232
     return x;
 }
 
+// Qualifying cells are compacted into shared memory in chunks of at most HR_CHUNK, and each chunk is applied before the
+// next is compacted: the cells still reach the map in ascending order, and the field size is not limited by shared memory.
+constexpr int HR_CHUNK = 2048;
+
 __global__ void __launch_bounds__(256) pif_hr_kernel(const float* __restrict__ pif, float* __restrict__ hr, Geo g, float v_th)
 {
-    extern __shared__ int sCells[]; // qualifying cells of this field, ascending (the reference's scan order)
+    __shared__ int sCells[HR_CHUNK]; // qualifying cells of this chunk, ascending (the reference's scan order)
     __shared__ int sCount, sWarpCnt[8];
     const int field = blockIdx.x, frame = blockIdx.y;
     const int hw = g.H * g.W;
@@ -99,58 +103,61 @@ __global__ void __launch_bounds__(256) pif_hr_kernel(const float* __restrict__ p
     float* map = hr + ((size_t)frame * NKP + field) * g.HR * g.WR;
     const int tid = threadIdx.x;
     for (int i = tid; i < g.HR * g.WR; i += 256) map[i] = 0.f; // vfill (:296)
-    if (tid == 0) sCount = 0;
-    __syncthreads();
-    // ordered compaction of the cells with conf > v_th (:322-330)
-    for (int base = 0; base < hw; base += 256) {
-        const int j = base + tid;
-        const bool q = j < hw && p[j] > v_th;
-        const unsigned b = __ballot_sync(0xffffffffu, q);
-        if ((tid & 31) == 0) sWarpCnt[tid >> 5] = __popc(b);
-        __syncthreads();
-        int off = sCount;
-        for (int w = 0; w < (tid >> 5); ++w) off += sWarpCnt[w];
-        if (q) sCells[off + __popc(b & ((1u << (tid & 31)) - 1u))] = j;
-        __syncthreads();
-        if (tid == 0) {
-            int t = 0;
-            for (int w = 0; w < 8; ++w) t += sWarpCnt[w];
-            sCount += t;
-        }
-        __syncthreads();
-    }
-    const int n = sCount;
     const int ty = tid >> 4, tx = tid & 15; // this thread owns the pixels with (yy % 16, xx % 16) == (ty, tx)
-    for (int c = 0; c < n; ++c) {
-        const int j = sCells[c];
-        const float conf = p[j];
-        const float cx = __fmul_rn(p[hw + j], PP_STRIDE);
-        const float cy = __fmul_rn(p[2 * hw + j], PP_STRIDE);
-        const float cs = (float)fmax(1.0, 0.5 * (double)p[4 * hw + j] * (double)PP_STRIDE); // :329 (double promotion)
-        const float cv = __fmul_rn(conf, 0.0625f);                                          // v / PIF_NN (:349)
-        const float tc = __fmul_rn(cs, 1.0f);                                               // truncate = 1 (:352)
-        // scalarSquareAddGaussWitMax bounds (:210-213): clip in float, then truncate to integer
-        const long long minx = (long long)clipf(__fsub_rn(cx, tc), 0.f, (float)(g.WR - 1));
-        const long long maxx = (long long)clipf(__fadd_rn(__fadd_rn(cx, tc), 1.f), (float)(minx + 1), (float)g.WR);
-        const long long miny = (long long)clipf(__fsub_rn(cy, tc), 0.f, (float)(g.HR - 1));
-        const long long maxy = (long long)clipf(__fadd_rn(__fadd_rn(cy, tc), 1.f), (float)(miny + 1), (float)g.HR);
-        const float tc2 = __fmul_rn(tc, tc);
-        const float cs2 = __fmul_rn(cs, cs);
-        long long x0 = minx + ((tx - (int)(minx & 15)) & 15);
-        long long y0 = miny + ((ty - (int)(miny & 15)) & 15);
-        for (long long xx = x0; xx < maxx; xx += 16) {
-            const float dx = __fsub_rn((float)xx, cx), dx2 = __fmul_rn(dx, dx);
-            for (long long yy = y0; yy < maxy; yy += 16) {
-                const float dy = __fsub_rn((float)yy, cy), dy2 = __fmul_rn(dy, dy);
-                const float d2 = __fadd_rn(dx2, dy2);
-                if (d2 > tc2) continue;
-                float vv;
-                if (dx2 < 0.25f && dy2 < 0.25f) vv = cv;
-                else vv = __fmul_rn(cv, approx_exp((float)(-0.5 * (double)d2 / (double)cs2))); // :233
-                float* px = map + yy * g.WR + xx;
-                *px = fminf(1.0f, __fadd_rn(*px, vv)); // += then clamp (:234-235)
+    for (int base = 0; base < hw;) {
+        if (tid == 0) sCount = 0;
+        __syncthreads(); // also orders the zero fill before the first chunk is applied (pixels are filled by other threads)
+        // ordered compaction of the cells with conf > v_th (:322-330); one step adds at most 256 cells
+        for (; base < hw && sCount <= HR_CHUNK - 256; base += 256) {
+            const int j = base + tid;
+            const bool q = j < hw && p[j] > v_th;
+            const unsigned b = __ballot_sync(0xffffffffu, q);
+            if ((tid & 31) == 0) sWarpCnt[tid >> 5] = __popc(b);
+            __syncthreads();
+            int off = sCount;
+            for (int w = 0; w < (tid >> 5); ++w) off += sWarpCnt[w];
+            if (q) sCells[off + __popc(b & ((1u << (tid & 31)) - 1u))] = j;
+            __syncthreads();
+            if (tid == 0) {
+                int t = 0;
+                for (int w = 0; w < 8; ++w) t += sWarpCnt[w];
+                sCount += t;
+            }
+            __syncthreads();
+        }
+        const int n = sCount;
+        for (int c = 0; c < n; ++c) {
+            const int j = sCells[c];
+            const float conf = p[j];
+            const float cx = __fmul_rn(p[hw + j], PP_STRIDE);
+            const float cy = __fmul_rn(p[2 * hw + j], PP_STRIDE);
+            const float cs = (float)fmax(1.0, 0.5 * (double)p[4 * hw + j] * (double)PP_STRIDE); // :329 (double promotion)
+            const float cv = __fmul_rn(conf, 0.0625f);                                          // v / PIF_NN (:349)
+            const float tc = __fmul_rn(cs, 1.0f);                                               // truncate = 1 (:352)
+            // scalarSquareAddGaussWitMax bounds (:210-213): clip in float, then truncate to integer
+            const long long minx = (long long)clipf(__fsub_rn(cx, tc), 0.f, (float)(g.WR - 1));
+            const long long maxx = (long long)clipf(__fadd_rn(__fadd_rn(cx, tc), 1.f), (float)(minx + 1), (float)g.WR);
+            const long long miny = (long long)clipf(__fsub_rn(cy, tc), 0.f, (float)(g.HR - 1));
+            const long long maxy = (long long)clipf(__fadd_rn(__fadd_rn(cy, tc), 1.f), (float)(miny + 1), (float)g.HR);
+            const float tc2 = __fmul_rn(tc, tc);
+            const float cs2 = __fmul_rn(cs, cs);
+            long long x0 = minx + ((tx - (int)(minx & 15)) & 15);
+            long long y0 = miny + ((ty - (int)(miny & 15)) & 15);
+            for (long long xx = x0; xx < maxx; xx += 16) {
+                const float dx = __fsub_rn((float)xx, cx), dx2 = __fmul_rn(dx, dx);
+                for (long long yy = y0; yy < maxy; yy += 16) {
+                    const float dy = __fsub_rn((float)yy, cy), dy2 = __fmul_rn(dy, dy);
+                    const float d2 = __fadd_rn(dx2, dy2);
+                    if (d2 > tc2) continue;
+                    float vv;
+                    if (dx2 < 0.25f && dy2 < 0.25f) vv = cv;
+                    else vv = __fmul_rn(cv, approx_exp((float)(-0.5 * (double)d2 / (double)cs2))); // :233
+                    float* px = map + yy * g.WR + xx;
+                    *px = fminf(1.0f, __fadd_rn(*px, vv)); // += then clamp (:234-235)
+                }
             }
         }
+        __syncthreads(); // every thread has read sCount and sCells before the next chunk is compacted
     }
 }
 
@@ -734,7 +741,7 @@ int hp_pifpaf_process_device(hp_pifpaf* p, const float* d_pif, const float* d_pa
     HP_CUDA_TRY(cudaMemsetAsync(p->counters.p, 0, (size_t)N * (1 + NBONE * 2 + 2 + 4) * sizeof(int), st));
     HP_CUDA_TRY(cudaMemsetAsync(p->occ_grow.p, 0, (size_t)N * NKP * hr_px, st));
     HP_CUDA_TRY(cudaMemsetAsync(p->occ_nms.p, 0, (size_t)N * NKP * nms_h * nms_w, st));
-    pif_hr_kernel<<<dim3(NKP, N), 256, hw * sizeof(int), st>>>(d_pif, p->hr.p, g, 0.1f);
+    pif_hr_kernel<<<dim3(NKP, N), 256, 0, st>>>(d_pif, p->hr.p, g, 0.1f);
     pif_seeds_kernel<<<N, 256, 0, st>>>(d_pif, p->hr.p, g, p->seeds_raw.p, seed_cnt, p->seed_cap, flags);
     pif_seed_sort_kernel<<<dim3((p->seed_cap + 255) / 256, N), 256, 0, st>>>(p->seeds_raw.p, p->seeds.p, seed_cnt, p->seed_cap);
     caf_filter_kernel<<<dim3(NBONE, N), 256, 0, st>>>(d_paf, p->hr.p, g, p->lists.p, list_cnt);

@@ -11,6 +11,8 @@
 2. ref_humans.npz  -- human_t lists produced by the reference's OWN src/paf.cpp (compiled
                       verbatim into oracle/_ref by oracle/Makefile) on the seeded synthetic
                       frames of hyperpose_b200/synthetic.py (SURVEY 8d configs).
+3. ref_pifpaf_large.npz (`python tests/golden/make_golden.py pifpaf_large`) -- the reference's own
+                      PifPaf decoder on fields of real frame sizes (PIFPAF_LARGE_CASES).
 """
 import hashlib
 import os
@@ -45,6 +47,15 @@ RESIZE_CASES = [(360, 640, 368, 656), (480, 640, 368, 656), (720, 1280, 368, 656
 # (name, seed, persons, h, w, keypoint_thresh) of the PifPaf decode pin (BASELINE config 5: 385x385 -> 49x49 fields)
 PIFPAF_CASES = [("pp_p2", 4, 2, 49, 49, 0.1), ("pp_p5", 5, 5, 49, 49, 0.1), ("pp_crowd", 6, (6, 12), 49, 49, 0.1), ("pp_empty", 7, 0, 49, 49, 0.1),
                 ("pp_rect", 8, 3, 47, 55, 0.1), ("pp_thr", 9, 4, 49, 49, 0.3), ("pp_small", 10, 2, 25, 33, 0.1)]
+
+
+# (name, seed, persons, h, w, scale range in cells) of the PifPaf decode pin at real frame sizes (keypoint threshold 0.1):
+# 99 x 124 = 12,276 cells and 99 x 125 bracket the field size a whole field's cells once fitted in 48 KiB of shared memory;
+# 89 x 159 is a 1280 x 720 input, 91 x 161 a 1281 x 721 one.  Scales of 4-8 cells give 33-65 px footprints on the
+# high-resolution map; "pl_dense" has more than 8192 seeds, the decoder's initial seed capacity.
+PIFPAF_LARGE_CASES = [("pl_99x124", 30, (6, 10), 99, 124, (4.0, 8.0)), ("pl_99x125", 31, (6, 10), 99, 125, (4.0, 8.0)),
+                      ("pl_89x159", 32, (6, 12), 89, 159, (1.0, 8.0)), ("pl_91x161", 33, (6, 12), 91, 161, (4.0, 8.0)),
+                      ("pl_161x161", 34, (8, 12), 161, 161, (4.0, 8.0)), ("pl_dense", 35, 40, 161, 161, (1.0, 1.5))]
 
 
 # (name, seed, persons, net_w, net_h, gh, gw, nh, nw, point_thresh, limb_thresh, nms_thresh, distractors) of the Pose Proposal pin
@@ -168,6 +179,19 @@ def make_pifpaf_live():
     np.savez_compressed(os.path.join(HERE, "ref_pifpaf_live.npz"), **out)
 
 
+def make_pifpaf_large():
+    """the reference decoder on PIFPAF_LARGE_CASES (tests/test_pifpaf_stages.py)"""
+    from hyperpose_b200 import synthetic as syn
+    import oracle
+    out = {}
+    for (name, seed, P, h, w, scale) in PIFPAF_LARGE_CASES:
+        pif, paf = syn.make_pifpaf_fields(seed, P, h, w, scale=scale)
+        out[name + "_humans"] = oracle.ref_pifpaf_process(pif, paf, (h - 1) * 8 + 1, (w - 1) * 8 + 1, 0.1)
+        out[name + "_in_sha"] = np.array(sha(pif) + sha(paf))
+    np.savez_compressed(os.path.join(HERE, "ref_pifpaf_large.npz"), **out)
+    print({k: len(v) for k, v in out.items() if k.endswith("_humans")})
+
+
 def make_ppn():
     """goldens of the reference's own src/pose_proposal.cpp (oracle/_ref/libref_ppn.so) on seeded synthetic tensors"""
     from hyperpose_b200 import synthetic as syn
@@ -188,5 +212,7 @@ if __name__ == "__main__" and "area" in sys.argv[1:]:
 if __name__ == "__main__":
     if "ppn" in sys.argv[1:]:
         make_ppn()
+    elif "pifpaf_large" in sys.argv[1:]:
+        make_pifpaf_large()
     else:
         main()
