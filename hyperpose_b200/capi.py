@@ -31,6 +31,7 @@ EXPORTS = [
     "hp_paf_create", "hp_paf_destroy", "hp_paf_set_conf_thresh", "hp_paf_set_paf_thresh", "hp_paf_set_capacity",
     "hp_paf_process_host", "hp_paf_process_host_batched", "hp_paf_process_device", "hp_paf_fetch",
     "hp_paf_debug_peaks", "hp_paf_debug_connections", "hp_paf_launch_count", "hp_paf_copy_results_device", "hp_paf_debug_timing",
+    "hp_paf_debug_plan",
 ]
 
 
@@ -161,6 +162,18 @@ class PafParser:
         lib().hp_paf_debug_timing.argtypes = [C.c_void_p, C.c_void_p, C.c_int]
         check(lib().hp_paf_debug_timing(self._h, out.ctypes.data, N))
         return out[:N * N_PAIRS * 4].reshape(N, N_PAIRS, 4), out[N * N_PAIRS * 4:].reshape(N, 6)
+
+    PLAN_FIELDS = ("generic", "rz_mode", "tab_staged", "stage_bytes", "limb_dyn_bytes", "fast_asm", "wide_tile_rows", "wide_tile_cols")
+
+    def debug_plan(self) -> dict:
+        """the code paths the last launch took (hp_paf_debug_plan): up-maps materialised (generic) and their resize regime, up-sampling
+        tables (tab_staged) and PAF planes (stage_bytes > 0) in the limb kernel's shared memory, the limb kernel's dynamic shared
+        memory, component-parallel assembly (fast_asm), the peak kernel's tile rows on the direct up-sampling path (wide_tile_rows)
+        and tile columns on the generic staging loop (wide_tile_cols)"""
+        out = np.zeros(len(self.PLAN_FIELDS), np.int32)
+        lib().hp_paf_debug_plan.argtypes = [C.c_void_p, C.c_void_p, C.c_int]
+        check(lib().hp_paf_debug_plan(self._h, out.ctypes.data, len(out)))
+        return dict(zip(self.PLAN_FIELDS, (int(v) for v in out)))
 
     def copy_results_device(self, d_humans_ptr: int, d_counts_ptr: int, N: int, cap: int, stream: int = 0):
         check(lib().hp_paf_copy_results_device(self._h, d_humans_ptr, d_counts_ptr, N, cap, stream))

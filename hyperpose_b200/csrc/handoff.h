@@ -47,7 +47,7 @@ struct Batch {
     // cache of the batched parse: key = parser kind + its parameters
     int cache_kind = 0;              // 0 empty | 1 PAF | 2 PifPaf
     float key_f[2] = { 0, 0 };
-    int key_i[2] = { 0, 0 };
+    int key_i[3] = { 0, 0, 0 };
     int hcap = 0;
     std::vector<hp_human> humans;    // [N][hcap]
     std::vector<int> counts;         // [N]

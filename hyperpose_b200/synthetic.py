@@ -33,11 +33,13 @@ _TEMPLATE = np.array([
     dtype=np.float64)
 
 
-def random_skeletons(rng: np.random.Generator, n_persons: int, height: int, width: int) -> np.ndarray:
-    """[P,18,2] joint (x, y) positions in network-input pixels."""
+def random_skeletons(rng: np.random.Generator, n_persons: int, height: int, width: int,
+                     person_height=(0.55, 0.9)) -> np.ndarray:
+    """[P,18,2] joint (x, y) positions in network-input pixels; each person's height is drawn uniformly from
+    `person_height` (fractions of the frame height)."""
     out = np.zeros((n_persons, N_PARTS, 2))
     for p in range(n_persons):
-        ph = rng.uniform(0.55, 0.9) * height            # person height in pixels
+        ph = rng.uniform(person_height[0], person_height[1]) * height            # person height in pixels
         pw = ph * rng.uniform(0.75, 0.95)
         x0 = rng.uniform(-0.1 * pw, max(-0.1 * pw + 1.0, width - 0.9 * pw))
         y0 = rng.uniform(0.0, max(1.0, height - ph))
@@ -95,20 +97,21 @@ def conf_paf_from_skeletons(skel: np.ndarray, hf: int, wf: int, rng: np.random.G
     return conf.astype(np.float32), vec.astype(np.float32)
 
 
-def make_frame_tensors(seed: int, n_persons, hf: int = 46, wf: int = 54, noise: float = 0.02):
-    """One frame: (conf[19,hf,wf], paf[38,hf,wf]).  n_persons: int or (lo, hi) inclusive."""
+def make_frame_tensors(seed: int, n_persons, hf: int = 46, wf: int = 54, noise: float = 0.02, person_height=(0.55, 0.9)):
+    """One frame: (conf[19,hf,wf], paf[38,hf,wf]).  n_persons: int or (lo, hi) inclusive; person_height: see random_skeletons."""
     rng = np.random.default_rng(seed)
     if isinstance(n_persons, tuple):
         n_persons = int(rng.integers(n_persons[0], n_persons[1] + 1))
-    skel = random_skeletons(rng, n_persons, hf * STRIDE, wf * STRIDE)
+    skel = random_skeletons(rng, n_persons, hf * STRIDE, wf * STRIDE, person_height)
     return conf_paf_from_skeletons(skel, hf, wf, rng, noise)
 
 
-def make_batch_tensors(seed: int, n_frames: int, n_persons, hf: int = 46, wf: int = 54, noise: float = 0.02):
+def make_batch_tensors(seed: int, n_frames: int, n_persons, hf: int = 46, wf: int = 54, noise: float = 0.02,
+                       person_height=(0.55, 0.9)):
     """(conf[N,19,hf,wf], paf[N,38,hf,wf]); frame i uses seed ``seed*100003 + i``."""
     cs, ps = [], []
     for i in range(n_frames):
-        c, p = make_frame_tensors(seed * 100003 + i, n_persons, hf, wf, noise)
+        c, p = make_frame_tensors(seed * 100003 + i, n_persons, hf, wf, noise, person_height)
         cs.append(c)
         ps.append(p)
     return np.stack(cs), np.stack(ps)

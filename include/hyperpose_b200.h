@@ -102,6 +102,13 @@ int hp_paf_debug_connections(hp_paf* p, int frame, int pair_id, hp_connection* o
 long long hp_paf_launch_count(const hp_paf* p);
 /* diagnostics: with HPB_PAF_TIMING=1 in the environment the limb kernel stamps its phases (%globaltimer, ns); N * (19 * 4 + 6) values */
 int hp_paf_debug_timing(hp_paf* p, unsigned long long* out, int N);
+/* diagnostics: the code paths the last launch took, n >= HP_PAF_PLAN_FIELDS ints: generic (1: the resolution shrinks an axis and the
+ * up-maps are materialised), rz_mode (resize regime of that path, -1 otherwise), tab_staged (limb kernel: up-sampling tables in shared
+ * memory), stage_bytes (limb kernel: shared memory for the two PAF planes of a limb, 0 = read from global memory), limb_dyn_bytes
+ * (dynamic shared memory the limb kernel may use), fast_asm (component-parallel assembly enabled), then the peak kernel's tile rows
+ * with more than 16 source rows (direct up-sampling) and tile columns with more than 64 source columns (generic staging loop). */
+#define HP_PAF_PLAN_FIELDS 8
+int hp_paf_debug_plan(hp_paf* p, int* out, int n);
 /* multi-GPU gather leg: copies the last batch's records (padded to `cap` >= the parser's human capacity per
  * frame) and counts into caller-owned DEVICE buffers, asynchronously on `stream` (NULL = the batch's stream),
  * so they can be handed to NCCL without a host round trip. */

@@ -60,7 +60,7 @@ def load_oracle():
         lib = C.CDLL(os.path.join(HERE, "liborc_paf.so"))
         fp = C.POINTER(C.c_float)
         lib.orc_paf_process.restype = C.c_int
-        lib.orc_paf_process.argtypes = [fp, fp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float,
+        lib.orc_paf_process.argtypes = [fp, fp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float,
                                         C.c_void_p, C.c_int, C.POINTER(C.c_int),
                                         C.c_void_p, C.c_int, C.POINTER(C.c_int),
                                         C.c_void_p, C.c_int, C.POINTER(C.c_int)]
@@ -136,8 +136,10 @@ def gauss_kernel() -> np.ndarray:
 
 
 def oracle_process(conf: np.ndarray, paf: np.ndarray, conf_thresh: float = 0.05, paf_thresh: float = 0.05,
-                   res_w: int = -1, res_h: int = -1, human_cap: int = 512, peak_cap: int = 65536, conn_cap: int = 4096):
-    """Run the restatement on one frame.  Returns dict(humans, peaks, conns[19 lists])."""
+                   res_w: int = -1, res_h: int = -1, human_cap: int = 512, peak_cap: int = 65536, conn_cap: int = 4096,
+                   feat_height: int = -1):
+    """Run the restatement on one frame.  Returns dict(humans, peaks, conns[19 lists]).  res_w / res_h / feat_height: what a
+    paf handle fixed at its first call (the resolution, and the W of that call's maps for the length penalty); -1 = this frame's."""
     conf = np.ascontiguousarray(conf, np.float32)
     paf = np.ascontiguousarray(paf, np.float32)
     assert conf.ndim == 3 and paf.ndim == 3 and conf.shape[1:] == paf.shape[1:]
@@ -147,7 +149,7 @@ def oracle_process(conf: np.ndarray, paf: np.ndarray, conf_thresh: float = 0.05,
     nh, npk = C.c_int(0), C.c_int(0)
     ncn = (C.c_int * N_PAIRS)()
     rc = load_oracle().orc_paf_process(_fp(conf), _fp(paf), conf.shape[0], paf.shape[0], conf.shape[1], conf.shape[2],
-                                       res_w, res_h, conf_thresh, paf_thresh,
+                                       res_w, res_h, feat_height, conf_thresh, paf_thresh,
                                        humans.ctypes.data, human_cap, C.byref(nh),
                                        peaks.ctypes.data, peak_cap, C.byref(npk),
                                        conns.ctypes.data, conn_cap, ncn)

@@ -47,11 +47,13 @@ const float* orc_gauss17_kernel(void);
  * conf [c_conf,H,W], paf [c_paf,H,W] row-major float32.
  * res_w/res_h: paf ctor resolution_size; pass -1,-1 for the default
  *   (width = 4*H, height = 4*W -- the reference's transposed default, paf.cpp:311-315).
+ * feat_height: the length penalty's feature height (paf.cpp:129,354), which a paf handle takes from the W of its FIRST
+ *   call (m_feature_size, paf.cpp:321-332); -1 = this frame's W (a handle's first call).
  * Optional debug outputs may be NULL.
  * returns 0, or <0 on error (-1 bad args, -2 capacity overflow, -3 unsupported resolution).
  */
 int orc_paf_process(const float* conf, const float* paf, int c_conf, int c_paf, int H, int W,
-                    int res_w, int res_h, float conf_thresh, float paf_thresh,
+                    int res_w, int res_h, int feat_height, float conf_thresh, float paf_thresh,
                     orc_human* humans, int human_cap, int* n_humans,
                     orc_peak* peaks, int peak_cap, int* n_peaks,
                     orc_conn* conns /* [19][conn_cap] */, int conn_cap, int* n_conns /* [19] */);

@@ -13,6 +13,9 @@
                       frames of hyperpose_b200/synthetic.py (SURVEY 8d configs).
 3. ref_pifpaf_large.npz (`python tests/golden/make_golden.py pifpaf_large`) -- the reference's own
                       PifPaf decoder on fields of real frame sizes (PIFPAF_LARGE_CASES).
+4. ref_humans_large.npz + cv_pin_large.npz (`python tests/golden/make_golden.py paf_large`) -- the reference's
+                      own src/paf.cpp on PAF_LARGE_CASES, and sha256 of real cv2 INTER_AREA / GaussianBlur at each of
+                      their geometries (PAF_LARGE_PINS).
 """
 import hashlib
 import os
@@ -82,6 +85,103 @@ AREA_FRAME_CASES = [
     ("user_frac", 15, 3, 46, 54, 41, 33, 0.05, 0.05),        # fractional reduction on both axes
     ("user_keep_x", 16, 3, 46, 54, 54, 30, 0.05, 0.05),      # one axis kept (scale 1), the other shrinks: area regime
 ]
+
+
+# parser cases at real frame sizes: (name, seed, persons, hf, wf, res_w, res_h, conf_thresh, paf_thresh, person_height).  The map
+# sizes straddle the size-dependent paths of paf_parser.cu (tests/test_paf_large.py asserts which ones each case takes, with the
+# H100's 200 KiB of dynamic shared memory for the limb kernel): up-sampling tables in shared memory while UW + UH <= 1024
+# (92 x 164 is the last, 92 x 165 / 93 x 164 the first beyond), both PAF planes of a limb while 8 H W + 12288 <= 200 KiB
+# (128 x 188 is the last, 128 x 189 the first beyond), TMA or scalar plane copies (H W divisible by 4 or odd), the peak kernel's
+# direct up-sampling (portrait maps: fewer than ~3.4 up-map rows per source row) and its generic source staging (a resolution
+# within ~1.27x of the map width).  "noise" is a structureless field (uniform PAF noise, uniform conf noise on the parts of
+# NOISY_PARTS, halved elsewhere so that those stay below the threshold): > 1000 peaks per noisy part, > 500 connections per
+# limb between them, the unstaged assembly and capacity growth, while the partial humans of the assembly stay in shared memory.
+PAF_LARGE_CASES = [
+    ("l_90x160", 60, (6, 10), 90, 160, -1, -1, 0.05, 0.05, (0.25, 0.7)),        # 1280 x 720 input
+    ("l_91x161", 61, (6, 10), 91, 161, -1, -1, 0.05, 0.05, (0.25, 0.7)),        # odd H W; UW = 364 = 4 mod 8
+    ("l_92x164", 62, (6, 10), 92, 164, -1, -1, 0.05, 0.05, (0.25, 0.7)),        # 1312 x 736 input; UW + UH = 1024
+    ("l_92x165", 63, (6, 10), 92, 165, -1, -1, 0.05, 0.05, (0.25, 0.7)),
+    ("l_93x164", 64, (6, 10), 93, 164, -1, -1, 0.05, 0.05, (0.25, 0.7)),
+    ("l_128x188", 65, (6, 10), 128, 188, -1, -1, 0.05, 0.05, (0.25, 0.7)),      # H W = 24064
+    ("l_128x189", 66, (6, 10), 128, 189, -1, -1, 0.05, 0.05, (0.25, 0.7)),      # H W = 24192
+    ("l_135x240", 67, (6, 10), 135, 240, -1, -1, 0.05, 0.05, (0.25, 0.7)),      # 1920 x 1080 input; UW = 540
+    ("l_240x135", 68, (4, 8), 240, 135, -1, -1, 0.05, 0.05, (0.25, 0.7)),       # portrait 1080p
+    ("l_160x90", 69, (4, 8), 160, 90, -1, -1, 0.05, 0.05, (0.25, 0.7)),         # portrait 720p
+    ("l_100x110_res", 70, (4, 8), 100, 110, 110, 400, 0.05, 0.05, (0.3, 0.8)),  # up-map width = map width
+    ("l_120x300_res", 71, (4, 8), 120, 300, 330, 1200, 0.05, 0.05, (0.3, 0.8)),  # UW = 330 = 2 mod 8
+    ("l_crowd", 72, (30, 40), 135, 240, -1, -1, 0.05, 0.05, (0.1, 0.3)),
+    ("l_noise", 73, "noise", 135, 240, -1, -1, 0.6, 0.05, None),
+]
+NOISY_PARTS = (1, 2, 3, 5)
+
+# one parser handle fed several map sizes in turn: the resolution and the length penalty's feature height are fixed at its
+# first call (paf.cpp:314-315, 321-332).  The second handle's small map is stretched 8x: much more (46 x 54 at 540 x 960 stretches
+# rows 21x) gives plateaus with exactly equal limb scores, where the reference's unstable std::sort decides (see AREA_FRAME_CASES).
+PAF_HANDLE_SEQUENCES = [((46, 82), (135, 240), (90, 160), (135, 240)), ((135, 240), (68, 120))]
+
+
+def paf_handle_tensors(k, h, w):
+    """(conf, paf) of call k of a PAF_HANDLE_SEQUENCES entry, on h x w maps"""
+    from hyperpose_b200 import synthetic as syn
+    return syn.make_frame_tensors(500 + k, (4, 8), h, w, person_height=(0.3, 0.8))
+
+
+def paf_large_tensors(case):
+    """(conf[19,hf,wf], paf[38,hf,wf]) of a PAF_LARGE_CASES entry"""
+    name, seed, P, hf, wf = case[:5]
+    if P == "noise":
+        rng = np.random.default_rng(seed)
+        conf, paf = rng.random((19, hf, wf), dtype=np.float32), rng.random((38, hf, wf), dtype=np.float32) - 0.5
+        conf[[k for k in range(19) if k not in NOISY_PARTS]] *= np.float32(0.5)
+        return conf, paf
+    from hyperpose_b200 import synthetic as syn
+    return syn.make_frame_tensors(seed, P, hf, wf, person_height=case[9])
+
+
+def _handle_geometries():
+    """(H, W, UH, UW) of every call of PAF_HANDLE_SEQUENCES"""
+    out = []
+    for seq in PAF_HANDLE_SEQUENCES:
+        uw, uh = 4 * seq[0][0], 4 * seq[0][1]
+        out += [(h, w, uh, uw) for (h, w) in seq]
+    return out
+
+
+# (H, W, UH, UW) of the INTER_AREA / GaussianBlur pin at the large geometries
+PAF_LARGE_PINS = sorted({(c[3], c[4], c[6] if c[6] > 0 else 4 * c[4], c[5] if c[5] > 0 else 4 * c[3]) for c in PAF_LARGE_CASES}
+                        | set(_handle_geometries()))
+
+
+def make_paf_large():
+    """tests/golden/ref_humans_large.npz (the reference's own paf.cpp) + cv_pin_large.npz (real cv2)"""
+    import cv2
+    import oracle
+    oracle.build()
+    pin = {"cv2_version": np.array(cv2.__version__)}
+    for i, (h, w, uh, uw) in enumerate(PAF_LARGE_PINS):
+        img = np.random.default_rng(400 + i).random((h, w), dtype=np.float32)
+        up = cv2.resize(img, (uw, uh), interpolation=cv2.INTER_AREA)
+        pin[f"pin{i}_dims"] = np.array([h, w, uh, uw])
+        pin[f"pin{i}_up_sha"] = np.array(sha(up))
+        pin[f"pin{i}_blur_sha"] = np.array(sha(cv2.GaussianBlur(up, (17, 17), 3.0)))
+    np.savez_compressed(os.path.join(HERE, "cv_pin_large.npz"), **pin)
+    ref = {}
+    for case in PAF_LARGE_CASES:
+        name, rw, rh, ct, pt = case[0], case[5], case[6], case[7], case[8]
+        conf, paf = paf_large_tensors(case)
+        rp = oracle.RefParser(ct, pt, rw, rh)
+        ref[name + "_humans"] = rp.process(conf, paf, cap=4096)
+        ref[name + "_in_sha"] = np.array(sha(conf) + sha(paf))
+        rp.close()
+    for s, seq in enumerate(PAF_HANDLE_SEQUENCES):   # one reference handle per sequence, every call through it
+        rp = oracle.RefParser()
+        for k, (h, w) in enumerate(seq):
+            conf, paf = paf_handle_tensors(k, h, w)
+            ref[f"handle{s}_{k}_humans"] = rp.process(conf, paf, cap=4096)
+            ref[f"handle{s}_{k}_in_sha"] = np.array(sha(conf) + sha(paf))
+        rp.close()
+    np.savez_compressed(os.path.join(HERE, "ref_humans_large.npz"), **ref)
+    print({k: len(v) for k, v in ref.items() if k.endswith("_humans")})
 
 
 def make_area():
@@ -214,5 +314,7 @@ if __name__ == "__main__":
         make_ppn()
     elif "pifpaf_large" in sys.argv[1:]:
         make_pifpaf_large()
+    elif "paf_large" in sys.argv[1:]:
+        make_paf_large()
     else:
         main()
