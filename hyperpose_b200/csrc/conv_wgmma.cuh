@@ -728,13 +728,23 @@ inline int conv_pick_stages(int BN)
 constexpr int HALO_TH = 16, HALO_TW = 8;
 constexpr int HALO_BOXES = 2;
 
+// kWide: a work item is TWO consecutive 16 x 8 tiles of the same grid (tiles 2i and 2i + 1 in (image, ty, tx) order, each with its
+// own halo box, so a pair may straddle two rows or two frames) x one n-tile.  Warpgroup 1 computes all 128 pixels of the first tile,
+// warpgroup 2 those of the second (two m64 accumulator blocks each: tile rows 0-7 and 8-15), and both read the same weight stage: one
+// 16 KiB weight tile, one full-barrier wait and one release serve 256 x 128 x 64 MACs instead of 128 x 128 x 64.  Every accumulator
+// row sees the same wgmma sequence (chunk, tap, k16) as in the 128-pixel item, so the outputs are identical.  128 fp32 accumulators
+// per consumer thread need more than the 168 registers of an even 384-thread split: setmaxnreg moves registers from the producer
+// warpgroup (40) to the consumers (232).  With an odd tile count the last item's second tile lies past the batch: its box is loaded
+// (out-of-tensor rows are zero-filled, or a frame beyond N of the max-batch buffer) and computed, and its epilogue is skipped.
+constexpr int HALO_WIDE_PRODUCER_REGS = 40, HALO_WIDE_CONSUMER_REGS = 232;
+
 struct HaloParams {
     int Nb, H, W;
     int R, S, groups, cin_g;
     int cout_g, cout_g_pad;
     int in_ch_off;
     int tiles_x, tiles_y;
-    int box_bytes;              // (16+R-1) * (8+S-1) * 128 rounded up to a multiple of 1024
+    int box_bytes;              // one tile's box: (16+R-1) * (8+S-1) * 128 rounded up to a multiple of 1024
     int num_stages;             // weight ring depth
     const float* bias; const float* alpha;
     __half* out; int out_ld, out_ch_off;   // NHWC output (kPool: the pooled tensor, [Nb, H/2, W/2, out_ld])
@@ -753,18 +763,22 @@ __device__ __forceinline__ uint64_t make_sw128_kmajor_desc_at(uint32_t smem_addr
     d |= (uint64_t)1 << 62;
     return d;
 }
+template <uint32_t N> __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <uint32_t N> __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
 } // namespace ptx
 
-template <int BN, bool kPool>
+template <int BN, bool kPool, bool kWide = false>
 __global__ void __launch_bounds__(CONV_THREADS, 1)
 conv_halo_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_b, const HaloParams p)
 {
+    static_assert(!(kWide && kPool), "the pooled epilogue pairs pixel rows of one m64 block; it has no wide form");
     constexpr int B_BYTES = BN * 128;
+    constexpr int kTiles = kWide ? 2 : 1;   // spatial tiles per item = boxes per box slot = m64 accumulator blocks per warpgroup
     extern __shared__ uint8_t smem_raw[];
     ptx::pdl_launch_dependents();
     uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-    uint8_t* s_box = smem;                                                   // [HALO_BOXES][box_bytes]
-    uint8_t* s_b = s_box + (size_t)HALO_BOXES * p.box_bytes;                 // [num_stages][BN x 128 B]
+    uint8_t* s_box = smem;                                                   // [HALO_BOXES][kTiles][box_bytes]
+    uint8_t* s_b = s_box + (size_t)HALO_BOXES * kTiles * p.box_bytes;        // [num_stages][BN x 128 B]
     uint64_t* a_full = (uint64_t*)(s_b + (size_t)p.num_stages * B_BYTES);    // [HALO_BOXES]
     uint64_t* a_empty = a_full + HALO_BOXES;
     uint64_t* b_full = a_empty + HALO_BOXES;                                 // [CONV_MAX_STAGES]
@@ -774,7 +788,7 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_consta
     const int n_tiles_g = p.cout_g_pad / BN;
     const int nt_total = p.groups * n_tiles_g;
     const int sp_per_img = p.tiles_x * p.tiles_y;
-    const int total_items = p.Nb * sp_per_img * nt_total;
+    const int total_items = (p.Nb * sp_per_img + kTiles - 1) / kTiles * nt_total;
     const int chunks = p.cin_g / CONV_BLOCK_K;
     const int taps = p.R * p.S;
     const int BW = HALO_TW + p.S - 1, BH = HALO_TH + p.R - 1;
@@ -795,11 +809,15 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_consta
     __syncthreads();
     ptx::pdl_wait();
 
-    // item -> (image, spatial tile, group, n-tile); n-tiles vary fastest so that neighbouring CTAs share a halo box in L2
-    auto decode = [&](int item, int& n, int& y0, int& x0, int& g, int& n0) {
-        const int nt = item % nt_total, sp = item / nt_total;
+    // item -> (first spatial tile, group, n-tile); n-tiles vary fastest so that neighbouring CTAs share a halo box in L2
+    auto decode = [&](int item, int& sp, int& g, int& n0) {
+        const int nt = item % nt_total;
+        sp = item / nt_total * kTiles;
         g = nt / n_tiles_g;
         n0 = (nt - g * n_tiles_g) * BN;
+    };
+    // spatial tile -> (image, first output row, first output column)
+    auto tile_pos = [&](int sp, int& n, int& y0, int& x0) {
         n = sp / sp_per_img;
         const int t = sp - n * sp_per_img;
         const int ty = t / p.tiles_x;
@@ -808,20 +826,26 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_consta
     };
 
     if (wg == 0) {
-        // ===================== TMA producer: one halo box per (item, chunk), one weight tile per (item, chunk, tap) =====================
+        if constexpr (kWide) ptx::setmaxnreg_dec<HALO_WIDE_PRODUCER_REGS>();
+        // ===================== TMA producer: kTiles halo boxes per (item, chunk), one weight tile per (item, chunk, tap) =====================
         if (warp == 0 && ptx::elect_one()) {
             int bs = 0, st = 0;
             uint32_t bph = 0, sph = 0;
             const int pad_h = p.R / 2, pad_w = p.S / 2;
             for (int item = blockIdx.x; item < total_items; item += gridDim.x) {
-                int n, y0, x0, g, n0;
-                decode(item, n, y0, x0, g, n0);
+                int sp, g, n0;
+                decode(item, sp, g, n0);
                 for (int c = 0; c < chunks; ++c) {
                     ptx::mbar_wait(ptx::smem_u32(a_empty + bs), bph ^ 1);
                     const uint32_t fa = ptx::smem_u32(a_full + bs);
-                    ptx::mbar_expect_tx(fa, (uint32_t)(BH * BW * 128));
-                    ptx::tma_load_4d(ptx::smem_u32(s_box + (size_t)bs * p.box_bytes), &tmap_x, fa, p.in_ch_off + g * p.cin_g + c * CONV_BLOCK_K,
-                                     x0 - pad_w, y0 - pad_h, n);
+                    ptx::mbar_expect_tx(fa, (uint32_t)(kTiles * BH * BW * 128));
+#pragma unroll
+                    for (int t = 0; t < kTiles; ++t) {
+                        int n, y0, x0;
+                        tile_pos(sp + t, n, y0, x0);
+                        ptx::tma_load_4d(ptx::smem_u32(s_box + (size_t)(bs * kTiles + t) * p.box_bytes), &tmap_x, fa,
+                                         p.in_ch_off + g * p.cin_g + c * CONV_BLOCK_K, x0 - pad_w, y0 - pad_h, n);
+                    }
                     if (++bs == HALO_BOXES) { bs = 0; bph ^= 1; }
                     for (int tap = 0; tap < taps; ++tap) {
                         ptx::mbar_wait(ptx::smem_u32(b_empty + st), sph ^ 1);
@@ -836,34 +860,44 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_consta
         return;
     }
 
-    // ===================== wgmma + epilogue (warpgroups 1, 2: tile rows 8 half .. 8 half + 7) =====================
+    // ===================== wgmma + epilogue =====================
+    // 128-pixel item: warpgroups 1, 2 take tile rows 8 half .. 8 half + 7 of the item's tile (one m64 block each).
+    // wide item: warpgroup 1 + half takes tile `half` of the pair, m64 block m = its tile rows 8 m .. 8 m + 7.
+    if constexpr (kWide) ptx::setmaxnreg_inc<HALO_WIDE_CONSUMER_REGS>();
     const int half = wg - 1;
     const int col0 = 2 * (lane & 3);
-    const int ty0 = half * 8 + (warp & 3) * 2;   // tile row of accumulator row 0 of this thread (row 8: ty0 + 1)
     const int tx = lane >> 2;                    // tile column of this thread's pixels
     const uint32_t sbo = (uint32_t)BW * 128u;
-    float acc[BN / 2];
+    const int box = kWide ? half : 0;            // this warpgroup's box inside a box slot
+    const int row_base = kWide ? 0 : half * 8;   // tile row of block 0's first accumulator row
+    float acc[kTiles][BN / 2];
     int bs = 0, st = 0;
     uint32_t bph = 0, sph = 0;
     for (int item = blockIdx.x; item < total_items; item += gridDim.x) {
-        int n, y0, x0, g, n0;
-        decode(item, n, y0, x0, g, n0);
+        int sp, g, n0;
+        decode(item, sp, g, n0);
         for (int c = 0; c < chunks; ++c) {
             ptx::mbar_wait(ptx::smem_u32(a_full + bs), bph);
-            const uint32_t abase = ptx::smem_u32(s_box + (size_t)bs * p.box_bytes) + (uint32_t)(half * 8 * BW * 128);
+            const uint32_t abase = ptx::smem_u32(s_box + (size_t)(bs * kTiles + box) * p.box_bytes) + (uint32_t)(row_base * BW * 128);
             int prev = 0;
             for (int tap = 0; tap < taps; ++tap) {
                 const int r = tap / p.S, s = tap - r * p.S;
-                const uint64_t da = ptx::make_sw128_kmajor_desc_at(abase + (uint32_t)((r * BW + s) * 128), sbo);
+                uint64_t da[kTiles];
+#pragma unroll
+                for (int m = 0; m < kTiles; ++m) da[m] = ptx::make_sw128_kmajor_desc_at(abase + (uint32_t)(((m * 8 + r) * BW + s) * 128), sbo);
                 const uint64_t db = ptx::make_sw128_kmajor_desc(ptx::smem_u32(s_b + (size_t)st * B_BYTES));
                 ptx::mbar_wait(ptx::smem_u32(b_full + st), sph);
-                ptx::fence_acc(acc);
+#pragma unroll
+                for (int m = 0; m < kTiles; ++m) ptx::fence_acc(acc[m]);
                 ptx::wgmma_fence();
 #pragma unroll
                 for (int k = 0; k < 4; ++k)
-                    ptx::wgmma<__half, BN>(acc, da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), (c | tap | k) != 0 ? 1u : 0u);
+#pragma unroll
+                    for (int m = 0; m < kTiles; ++m)
+                        ptx::wgmma<__half, BN>(acc[m], da[m] + (uint64_t)(k * 2), db + (uint64_t)(k * 2), (c | tap | k) != 0 ? 1u : 0u);
                 ptx::wgmma_commit();
-                ptx::fence_acc(acc);
+#pragma unroll
+                for (int m = 0; m < kTiles; ++m) ptx::fence_acc(acc[m]);
                 if (tap > 0) {
                     ptx::wgmma_wait<1>();
                     if (lane == 0) ptx::mbar_arrive(ptx::smem_u32(b_empty + prev));
@@ -872,7 +906,8 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_consta
                 if (++st == p.num_stages) { st = 0; sph ^= 1; }
             }
             ptx::wgmma_wait<0>();   // every tap of this chunk has read the box
-            ptx::fence_acc(acc);
+#pragma unroll
+            for (int m = 0; m < kTiles; ++m) ptx::fence_acc(acc[m]);
             if (lane == 0) {
                 ptx::mbar_arrive(ptx::smem_u32(b_empty + prev));
                 ptx::mbar_arrive(ptx::smem_u32(a_empty + bs));
@@ -880,18 +915,23 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_consta
             if (++bs == HALO_BOXES) { bs = 0; bph ^= 1; }
         }
 
+        int n, y0, x0;
+        tile_pos(sp + box, n, y0, x0);
+        if (kWide && n >= p.Nb) continue;   // the second tile of an odd tile count's last item
         const float* bias = p.bias + g * p.cout_g_pad + n0;
         const float* alpha = p.alpha + g * p.cout_g_pad + n0;
         const int och = p.out_ch_off + g * p.cout_g + n0;
         const bool pair_ok = ((och | p.out_ld) & 1) == 0;
         if constexpr (kPool) {
+            const int ty0 = row_base + (warp & 3) * 2;   // tile row of accumulator row 0 of this thread (row 8: ty0 + 1)
+            const float (&acc0)[BN / 2] = acc[0];
             // rows ty0 / ty0 + 1 of this thread, then the column partner lane ^ 4; lanes with an even tile column store the pooled pixel
             const int py = (y0 + ty0) >> 1, px = (x0 + tx) >> 1;
             const bool store = (tx & 1) == 0 && py < (p.H >> 1) && px < (p.W >> 1);
             __half* o = p.out + (((size_t)n * (p.H >> 1) + py) * (p.W >> 1) + px) * p.out_ld + och;
 #pragma unroll
             for (int j = 0; j < BN / 8; ++j) {
-                float v0 = fmaxf(acc[4 * j], acc[4 * j + 2]), v1 = fmaxf(acc[4 * j + 1], acc[4 * j + 3]);
+                float v0 = fmaxf(acc0[4 * j], acc0[4 * j + 2]), v1 = fmaxf(acc0[4 * j + 1], acc0[4 * j + 3]);
                 v0 = fmaxf(v0, __shfl_xor_sync(0xffffffffu, v0, 4));
                 v1 = fmaxf(v1, __shfl_xor_sync(0xffffffffu, v1, 4));
                 const int c = 8 * j + col0;
@@ -906,21 +946,25 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_consta
         } else {
             const int n_valid = min(BN, p.cout_g - n0);
 #pragma unroll
-            for (int h = 0; h < 2; ++h) {
-                const int oy = y0 + ty0 + h, ox = x0 + tx;
-                if (oy >= p.H || ox >= p.W) continue;
-                __half* o = p.out + (((size_t)n * p.H + oy) * p.W + ox) * p.out_ld + och;
+            for (int m = 0; m < kTiles; ++m) {
+                const int ty0 = row_base + m * 8 + (warp & 3) * 2;   // tile row of accumulator row 0 of this thread (row 8: ty0 + 1)
 #pragma unroll
-                for (int j = 0; j < BN / 8; ++j) {
-                    const int c = 8 * j + col0;
-                    if (c >= n_valid) break;
-                    float a0 = acc[4 * j + 2 * h] + __ldg(bias + c), a1 = acc[4 * j + 2 * h + 1] + __ldg(bias + c + 1);
-                    a0 = a0 > 0.f ? a0 : a0 * __ldg(alpha + c);
-                    a1 = a1 > 0.f ? a1 : a1 * __ldg(alpha + c + 1);
-                    const __half2 h2 = __floats2half2_rn(a0, a1);
-                    const bool two = c + 1 < n_valid;
-                    if (two && pair_ok) *(__half2*)(o + c) = h2;
-                    else { o[c] = __low2half(h2); if (two) o[c + 1] = __high2half(h2); }
+                for (int h = 0; h < 2; ++h) {
+                    const int oy = y0 + ty0 + h, ox = x0 + tx;
+                    if (oy >= p.H || ox >= p.W) continue;
+                    __half* o = p.out + (((size_t)n * p.H + oy) * p.W + ox) * p.out_ld + och;
+#pragma unroll
+                    for (int j = 0; j < BN / 8; ++j) {
+                        const int c = 8 * j + col0;
+                        if (c >= n_valid) break;
+                        float a0 = acc[m][4 * j + 2 * h] + __ldg(bias + c), a1 = acc[m][4 * j + 2 * h + 1] + __ldg(bias + c + 1);
+                        a0 = a0 > 0.f ? a0 : a0 * __ldg(alpha + c);
+                        a1 = a1 > 0.f ? a1 : a1 * __ldg(alpha + c + 1);
+                        const __half2 h2 = __floats2half2_rn(a0, a1);
+                        const bool two = c + 1 < n_valid;
+                        if (two && pair_ok) *(__half2*)(o + c) = h2;
+                        else { o[c] = __low2half(h2); if (two) o[c + 1] = __high2half(h2); }
+                    }
                 }
             }
         }
@@ -928,14 +972,16 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_consta
 }
 
 inline int halo_box_bytes(int R, int S) { return ((HALO_TH + R - 1) * (HALO_TW + S - 1) * 128 + 1023) & ~1023; }
-inline size_t conv_halo_smem_bytes(int R, int S, int BN, int stages)
+// tiles: spatial tiles per work item (1, or 2 for the wide item: two boxes per box slot)
+inline size_t conv_halo_smem_bytes(int R, int S, int BN, int stages, int tiles = 1)
 {
-    return 1024 + (size_t)HALO_BOXES * halo_box_bytes(R, S) + (size_t)stages * BN * 128 + (2 * HALO_BOXES + 2 * CONV_MAX_STAGES) * 8;
+    return 1024 + (size_t)HALO_BOXES * tiles * halo_box_bytes(R, S) + (size_t)stages * BN * 128 + (2 * HALO_BOXES + 2 * CONV_MAX_STAGES) * 8;
 }
-inline int conv_halo_pick_stages(int R, int S, int BN)
+// as many weight stages as fit, up to CONV_MAX_STAGES (at least 2: a caller that needs more checks the result)
+inline int conv_halo_pick_stages(int R, int S, int BN, int tiles = 1)
 {
     int s = CONV_MAX_STAGES;
-    while (s > 2 && conv_halo_smem_bytes(R, S, BN, s) > CONV_SMEM_LIMIT) --s;
+    while (s > 2 && conv_halo_smem_bytes(R, S, BN, s, tiles) > CONV_SMEM_LIMIT) --s;
     return s;
 }
 

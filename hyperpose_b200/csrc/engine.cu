@@ -622,6 +622,7 @@ enum class Launch : uint8_t {
     ConvStem,       // u8 frames: conv_wgmma_kernel with the fused R x R stem (R = po.R); f32 entry: as Conv
     Halo,           // conv_halo_kernel: one TMA box per 16 x 8-pixel tile and channel chunk serves every filter tap
     HaloPool,       // conv_halo_kernel with the 2x2 max-pool that follows in its epilogue (hp.out is the POOLED buffer)
+    HaloWide,       // conv_halo_kernel with 256-pixel work items: two 16 x 8 tiles share every weight tile
     DwTma,          // dwconv3_tma_kernel<1>
     DwTmaPair,      // dwconv3_tma_kernel<2>: this op and the next one (same input, other filters)
     DwCol,          // dwconv3_col_kernel
@@ -668,6 +669,7 @@ struct EngOp {
 // reference the tests compare the default against.
 struct EngOptions {
     enum { HALO_AUTO, HALO_NONE, HALO_ALL } halo = HALO_AUTO;   // HPB_HALO=all | anything else; unset: build_conv_plan's rule
+    bool halo_wide = true;       // HPB_HALO_NARROW: every halo layer takes the 128-pixel work item
     bool stem3 = true;           // fused 3x3 stem; HPB_NO_STEM3 keeps the im2col buffer
     bool pool_fuse = true;       // HPB_NO_POOL_FUSE
     bool dw1_fuse = true;        // HPB_NO_DW1_FUSE
@@ -772,6 +774,26 @@ inline float tf32_round(float x)
     if ((u & 0x7f800000u) != 0x7f800000u) u = (u + 0x1000u) & 0xffffe000u;
     memcpy(&x, &u, 4);
     return x;
+}
+
+// The halo plan's work item: one 16 x 8 tile (128 pixels), or two tiles sharing every weight tile (conv_halo_kernel<128, false, true>)
+void set_halo_item(EngOp& op, bool wide)
+{
+    HaloParams& h = op.plan.hp;
+    const int tiles = wide ? 2 : 1;
+    h.num_stages = conv_halo_pick_stages(h.R, h.S, op.plan.prm.BN, tiles);
+    op.plan.smem = conv_halo_smem_bytes(h.R, h.S, op.plan.prm.BN, h.num_stages, tiles);
+    op.launch = wide ? Launch::HaloWide : Launch::Halo;
+}
+
+// Which halo layers take the wide item, from per-layer times of both items at the cfg3 / cfg4 / cfg5 benchmark batch sizes
+// (tools/layer_times.py with and without HPB_HALO_NARROW, DESIGN.md §4): OpenPose's 7x7 refinement convs, 49 weight tiles per box,
+// run 13-15 % faster.  The 3x3 layers gain at most 5 % (cin 512 at 46x82 and 46x54) and lose up to 46 % where a launch is a few
+// rounds of short items (cfg4 / cfg5's 128- and 256-channel layers), so they keep the 128-pixel item.  Launches of fewer wide items
+// than SMs were not measured; they leave SMs idle that the 128-pixel launch would use, and keep it.
+bool halo_wide_faster(int R, long wide_items, int sms)
+{
+    return R == 7 && wide_items >= sms;
 }
 
 // The conv's GEMM operands, epilogue and tensor maps.  data_type::kHALF: fp16 activations and weights, 64-channel chunks;
@@ -924,13 +946,16 @@ int build_conv_plan(hp_engine* e, EngOp& op, const float* blob)
         h.cout_g = cout_g; h.cout_g_pad = cout_pad; h.in_ch_off = (int)po.in_ch_off;
         h.tiles_x = tx; h.tiles_y = ty;
         h.box_bytes = halo_box_bytes(eR, eS);
-        h.num_stages = conv_halo_pick_stages(eR, eS, BN);
         h.bias = pl.d_bias; h.alpha = pl.d_alpha;
         h.out = ob.d; h.out_ld = ob.channels; h.out_ch_off = (int)po.out_ch_off;
         rc = make_tmap_act_box(&pl.tmap_x, ib.d, e->max_batch, ib.H, ib.W, ib.channels, ib.channels, HALO_TW + eS - 1, HALO_TH + eR - 1, CU_TENSOR_MAP_SWIZZLE_128B);
         if (rc) return rc;
-        op.launch = Launch::Halo;
-        pl.smem = conv_halo_smem_bytes(eR, eS, BN, h.num_stages);
+        // the wide item: BN = 128 only, and at least 3 weight stages next to its four boxes; HPB_HALO=all takes it wherever it exists
+        const bool wide_ok = e->opt.halo_wide && BN == 128 && conv_halo_pick_stages(eR, eS, BN, 2) >= 3;
+        const long wide_items = ((long)e->max_batch * tx * ty + 1) / 2 * G * (cout_pad / BN);
+        const bool wide_want = e->opt.halo == EngOptions::HALO_AUTO ? halo_wide_faster(eR, wide_items, e->num_sms - e->reserve_sms)
+                                                                    : e->opt.halo == EngOptions::HALO_ALL;
+        set_halo_item(op, wide_ok && wide_want);
     }
     return HP_OK;
 }
@@ -985,7 +1010,12 @@ const void* halo_kernel_bn(int BN)
     }
     return nullptr;
 }
-const void* halo_kernel(bool pool, int BN) { return pool ? halo_kernel_bn<true>(BN) : halo_kernel_bn<false>(BN); }
+// Launch::Halo / HaloPool / HaloWide (the wide item exists for BN = 128 only, see set_halo_item)
+const void* halo_kernel(Launch k, int BN)
+{
+    if (k == Launch::HaloWide) return BN == 128 ? (const void*)conv_halo_kernel<128, false, true> : nullptr;
+    return k == Launch::HaloPool ? halo_kernel_bn<true>(BN) : halo_kernel_bn<false>(BN);
+}
 const void* conv_kernel(int dtype, bool res, int BN, int stem_R = 0)
 {
     if (stem_R == 3) return conv_kernel_bn<__half, false, 3>(BN);
@@ -1014,7 +1044,7 @@ void launch_dw_tma(hp_engine* e, const EngOp& op, const EngOp* pair, int N, cuda
     else      launch_pdl(dwconv3_tma_kernel<1>, grid, DWT_THREADS, op.dwt_smem, st, op.tmap_dw, p);
 }
 
-// conv_wgmma_kernel, or conv_halo_kernel for Launch::Halo / HaloPool
+// conv_wgmma_kernel, or conv_halo_kernel for Launch::Halo / HaloPool / HaloWide
 int launch_conv(hp_engine* e, EngOp& op, int N, cudaStream_t st, bool u8_input)
 {
     ConvPlan& pl = op.plan;
@@ -1022,14 +1052,15 @@ int launch_conv(hp_engine* e, EngOp& op, int N, cudaStream_t st, bool u8_input)
     p.Nb = N;
     const int stem_R = op.launch == Launch::ConvStem && u8_input ? (int)op.po.R : 0;
     p.frames = e->cur_frames ? e->cur_frames : e->d_frames;
-    if (op.launch == Launch::Halo || op.launch == Launch::HaloPool) {
+    if (op.launch == Launch::Halo || op.launch == Launch::HaloPool || op.launch == Launch::HaloWide) {
         HaloParams h = pl.hp;
         h.Nb = N;
-        const long items = (long)N * h.tiles_x * h.tiles_y * h.groups * (h.cout_g_pad / p.BN);
+        const int tiles = op.launch == Launch::HaloWide ? 2 : 1;
+        const long items = ((long)N * h.tiles_x * h.tiles_y + tiles - 1) / tiles * h.groups * (h.cout_g_pad / p.BN);
         cudaLaunchAttribute at[1];
         const cudaLaunchConfig_t cfg = pdl_config((int)std::min<long>(e->num_sms - e->reserve_sms, items), CONV_THREADS, pl.smem, st, at);
         void* args[] = { (void*)&pl.tmap_x, (void*)&pl.tmap_b, (void*)&h };
-        HP_CUDA_TRY(cudaLaunchKernelExC(&cfg, halo_kernel(op.launch == Launch::HaloPool, p.BN), args));
+        HP_CUDA_TRY(cudaLaunchKernelExC(&cfg, halo_kernel(op.launch, p.BN), args));
         return HP_OK;
     }
     p.m_tiles = (int)(((size_t)N * p.H * p.W + CONV_BLOCK_M - 1) / CONV_BLOCK_M);
@@ -1124,7 +1155,7 @@ int run_graph(hp_engine* e, int N, bool u8_input, cudaStream_t st, int first = 0
 #undef HP_IM2COL
             break;
         }
-        case Launch::Conv: case Launch::ConvStem: case Launch::Halo: case Launch::HaloPool:
+        case Launch::Conv: case Launch::ConvStem: case Launch::Halo: case Launch::HaloPool: case Launch::HaloWide:
             launch_conv(e, op, N, st, u8_input);
             break;
         case Launch::DwTma:
@@ -1395,6 +1426,7 @@ int hp_engine_create_ex(hp_engine** out, const void* pack, size_t pack_bytes, in
     e->act_scale = std::move(act_scale);
     EngOptions& opt = e->opt;
     if (const char* v = getenv("HPB_HALO")) opt.halo = strcmp(v, "all") == 0 ? EngOptions::HALO_ALL : EngOptions::HALO_NONE;
+    opt.halo_wide = !getenv("HPB_HALO_NARROW");
     opt.stem3 = !getenv("HPB_NO_STEM3");
     opt.pool_fuse = !getenv("HPB_NO_POOL_FUSE");
     opt.dw1_fuse = !getenv("HPB_NO_DW1_FUSE");
@@ -1552,7 +1584,7 @@ int hp_engine_create_ex(hp_engine** out, const void* pack, size_t pack_bytes, in
     // conv (halo kernel) -> 2x2 max-pool: the pool moves into the conv's epilogue when nobody else reads the un-pooled tensor
     for (size_t i = 0; opt.pool_fuse && i + 1 < e->ops.size(); ++i) {
         EngOp& c = e->ops[i]; EngOp& m = e->ops[i + 1];
-        if (c.launch != Launch::Halo || !c.plan.monotone_act || m.po.type != OP_MAXPOOL2 || (m.po.R != 0 && m.po.R != 2)) continue;
+        if ((c.launch != Launch::Halo && c.launch != Launch::HaloWide) || !c.plan.monotone_act || m.po.type != OP_MAXPOOL2 || (m.po.R != 0 && m.po.R != 2)) continue;
         const EngBuffer& cb = e->bufs[c.po.out_buf];
         const EngBuffer& pb = e->bufs[m.po.out_buf];
         const int C = (int)c.po.groups * (int)c.po.cout_g;
@@ -1563,6 +1595,7 @@ int hp_engine_create_ex(hp_engine** out, const void* pack, size_t pack_bytes, in
             if (k != i + 1 && reads_buffer(e->ops[k].po, c.po.out_buf)) other_reader = true;
         if (other_reader) continue;
         c.plan.hp.out = pb.d; c.plan.hp.out_ld = pb.channels; c.plan.hp.out_ch_off = (int)m.po.out_ch_off;
+        set_halo_item(c, false);   // the pooled epilogue has the 128-pixel item only; its smem is at most the wide one's
         c.launch = Launch::HaloPool;
         m.launch = Launch::None;
         e->bufs[c.po.out_buf].fused_away = true;
@@ -1651,8 +1684,8 @@ int hp_engine_create_ex(hp_engine** out, const void* pack, size_t pack_bytes, in
     e->use_pdl = dtype == HP_DTYPE_F16 && launches > 0 && per_launch < 10e9;
     for (const EngOp& o : e->ops) {
         if (o.po.type != OP_CONV) continue;
-        if ((o.launch == Launch::Halo || o.launch == Launch::HaloPool) &&
-            cudaFuncSetAttribute(halo_kernel(o.launch == Launch::HaloPool, o.plan.prm.BN), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)max_smem) != cudaSuccess) {
+        if ((o.launch == Launch::Halo || o.launch == Launch::HaloPool || o.launch == Launch::HaloWide) &&
+            cudaFuncSetAttribute(halo_kernel(o.launch, o.plan.prm.BN), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)max_smem) != cudaSuccess) {
             set_error("engine: cannot opt in to %zu bytes of dynamic shared memory (halo)", max_smem);
             return fail(HP_ERR_CUDA);
         }
@@ -2020,6 +2053,7 @@ int hp_engine_debug_op_kernel(const hp_engine* e, int op, char* name, int cap)
     case Launch::ConvStem: s = "conv<f16," + std::to_string(BN) + ",stem" + std::to_string(po.R) + ">"; break;
     case Launch::Halo: s = "halo<" + std::to_string(BN) + ">"; break;
     case Launch::HaloPool: s = "halo<" + std::to_string(BN) + ",pool>"; break;
+    case Launch::HaloWide: s = "halo<" + std::to_string(BN) + ",wide>"; break;
     case Launch::DwTma: s = "dw_tma<1>"; break;
     case Launch::DwTmaPair: s = "dw_tma<2>"; break;
     case Launch::DwCol: s = "dw_col"; break;
