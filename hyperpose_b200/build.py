@@ -34,9 +34,12 @@ def _newer(src_files, target):
     return any(os.path.getmtime(s) > t for s in src_files)
 
 
-def build(force: bool = False, verbose: bool = False) -> str:
+def build(force: bool = False, verbose: bool = False, out_dir: str | None = None, defines: tuple = ()) -> str:
+    """-> the library's path: hyperpose_b200/libhyperpose_b200.so, or, for an instrumented variant (`defines`, e.g. HPB_HALO_PHASES
+    for tools/halo_phases.py), out_dir/libhyperpose_b200.so with its objects under out_dir/build"""
     nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-    objdir = os.path.join(PKG, "build")
+    lib = os.path.join(out_dir, "libhyperpose_b200.so") if out_dir else LIB
+    objdir = os.path.join(out_dir or PKG, "build")
     os.makedirs(objdir, exist_ok=True)
     headers = [os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith((".h", ".cuh"))]
     headers.append(os.path.join(ROOT, "include", "hyperpose_b200.h"))
@@ -47,7 +50,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
         o = os.path.join(objdir, os.path.splitext(src)[0] + ".o")
         objs.append(o)
         if force or _newer([s] + headers, o):
-            cmd = [nvcc] + NVCC_FLAGS + extra + ["-c", s, "-o", o]
+            cmd = [nvcc] + NVCC_FLAGS + extra + ["-D" + d for d in defines] + ["-c", s, "-o", o]
             r = subprocess.run(cmd, capture_output=True, text=True)
             if verbose or r.returncode:
                 sys.stderr.write(" ".join(cmd) + "\n" + r.stdout + r.stderr)
@@ -56,13 +59,13 @@ def build(force: bool = False, verbose: bool = False) -> str:
             with open(o + ".ptxas.txt", "w") as f:
                 f.write(r.stderr)
             rebuilt = True
-    if rebuilt or not os.path.exists(LIB):
-        cmd = [nvcc, "-shared", "-o", LIB] + objs  # static cudart (nvcc default); the driver API is reached via cudaGetDriverEntryPoint
+    if rebuilt or not os.path.exists(lib):
+        cmd = [nvcc, "-shared", "-o", lib] + objs  # static cudart (nvcc default); the driver API is reached via cudaGetDriverEntryPoint
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode:
             sys.stderr.write(r.stdout + r.stderr)
             raise RuntimeError("link failed")
-    return LIB
+    return lib
 
 
 def build_cpp_example(ref_root: str = "/root/reference") -> str | None:

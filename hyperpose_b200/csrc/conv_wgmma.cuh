@@ -738,6 +738,29 @@ constexpr int HALO_BOXES = 2;
 // (out-of-tensor rows are zero-filled, or a frame beyond N of the max-batch buffer) and computed, and its epilogue is skipped.
 constexpr int HALO_WIDE_PRODUCER_REGS = 40, HALO_WIDE_CONSUMER_REGS = 232;
 
+// kPP ("ping-pong", 3x3 layers): a work item is one 16 x 8 tile x one n-tile, as in the 128-pixel item, but ONE warpgroup computes
+// all of it (two m64 blocks, tile rows 0-7 and 8-15, the same accumulators and register split as the wide item).  A CTA's items
+// alternate between warpgroups 1 and 2, and both consume the producer's box and weight rings in the CTA's item order.  Two turn
+// barriers pass the tensor pipe back and forth: a warpgroup starts an item's MMAs once the other has ISSUED (not finished) its
+// previous item's, so the pipe does not drain at the hand-off, and each warpgroup's final wait and epilogue run under the other's
+// main loop.  Within an item nothing drains at a chunk boundary: box c is released after the first wait<1> of chunk c + 1, which
+// has seen every MMA of chunk c complete; the box ring (HALO_PP_BOXES) keeps the producer a chunk ahead.  Every accumulator row sees
+// the same (chunk, tap, k16) wgmma sequence as in the 128-pixel item, so the outputs are identical.
+constexpr int HALO_PP_BOXES = 4;
+
+#ifdef HPB_HALO_PHASES
+// instrumented build (tools/halo_phases.py): clock64 cycles of every consumer warpgroup, summed over the CTAs of all halo launches
+enum { HALO_PH_TOTAL, HALO_PH_A_WAIT, HALO_PH_B_WAIT, HALO_PH_MMA_WAIT, HALO_PH_EPILOGUE, HALO_PH_TURN_WAIT, HALO_PH_COUNT };
+__device__ unsigned long long g_halo_phases[HALO_PH_COUNT];
+#define HALO_PH_MARK(t) const long long t = clock64()
+#define HALO_TIMED(i, ...) do { const long long t0_ = clock64(); __VA_ARGS__; ph[i] += clock64() - t0_; } while (0)
+#define HALO_PH_ADD(i, t) (ph[i] += clock64() - (t))
+#else
+#define HALO_PH_MARK(t) do {} while (0)
+#define HALO_TIMED(i, ...) do { __VA_ARGS__; } while (0)
+#define HALO_PH_ADD(i, t) do {} while (0)
+#endif
+
 struct HaloParams {
     int Nb, H, W;
     int R, S, groups, cin_g;
@@ -767,22 +790,91 @@ template <uint32_t N> __device__ __forceinline__ void setmaxnreg_dec() { asm vol
 template <uint32_t N> __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
 } // namespace ptx
 
-template <int BN, bool kPool, bool kWide = false>
+// Stores m64 blocks 0 .. kBlocks - 1 of one warpgroup's accumulators: block m holds tile rows row_base + 8 m .. row_base + 8 m + 7 of
+// the tile at (n, y0, x0).  kPool: the 2x2 max-pool of each block (its rows pair up as (y, y + 1) with y even, see above).
+template <int BN, bool kPool, int kBlocks>
+__device__ __forceinline__ void halo_epilogue(const float (&acc)[kBlocks][BN / 2], const HaloParams& p, int n, int y0, int x0, int g, int n0,
+                                              int row_base, int warp, int lane)
+{
+    const int col0 = 2 * (lane & 3);
+    const int tx = lane >> 2;                    // tile column of this thread's pixels
+    const float* bias = p.bias + g * p.cout_g_pad + n0;
+    const float* alpha = p.alpha + g * p.cout_g_pad + n0;
+    const int och = p.out_ch_off + g * p.cout_g + n0;
+    const bool pair_ok = ((och | p.out_ld) & 1) == 0;
+    if constexpr (kPool) {
+#pragma unroll
+        for (int m = 0; m < kBlocks; ++m) {
+            const int ty0 = row_base + m * 8 + (warp & 3) * 2;   // tile row of accumulator row 0 of this thread (row 8: ty0 + 1)
+            const float (&acc0)[BN / 2] = acc[m];
+            // rows ty0 / ty0 + 1 of this thread, then the column partner lane ^ 4; lanes with an even tile column store the pooled pixel
+            const int py = (y0 + ty0) >> 1, px = (x0 + tx) >> 1;
+            const bool store = (tx & 1) == 0 && py < (p.H >> 1) && px < (p.W >> 1);
+            __half* o = p.out + (((size_t)n * (p.H >> 1) + py) * (p.W >> 1) + px) * p.out_ld + och;
+#pragma unroll
+            for (int j = 0; j < BN / 8; ++j) {
+                float v0 = fmaxf(acc0[4 * j], acc0[4 * j + 2]), v1 = fmaxf(acc0[4 * j + 1], acc0[4 * j + 3]);
+                v0 = fmaxf(v0, __shfl_xor_sync(0xffffffffu, v0, 4));
+                v1 = fmaxf(v1, __shfl_xor_sync(0xffffffffu, v1, 4));
+                const int c = 8 * j + col0;
+                if (!store) continue;
+                float a0 = v0 + __ldg(bias + c), a1 = v1 + __ldg(bias + c + 1);
+                a0 = a0 > 0.f ? a0 : a0 * __ldg(alpha + c);
+                a1 = a1 > 0.f ? a1 : a1 * __ldg(alpha + c + 1);
+                const __half2 h2 = __floats2half2_rn(a0, a1);
+                if (pair_ok) *(__half2*)(o + c) = h2;
+                else { o[c] = __low2half(h2); o[c + 1] = __high2half(h2); }
+            }
+        }
+    } else {
+        const int n_valid = min(BN, p.cout_g - n0);
+#pragma unroll
+        for (int m = 0; m < kBlocks; ++m) {
+            const int ty0 = row_base + m * 8 + (warp & 3) * 2;   // tile row of accumulator row 0 of this thread (row 8: ty0 + 1)
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int oy = y0 + ty0 + h, ox = x0 + tx;
+                if (oy >= p.H || ox >= p.W) continue;
+                __half* o = p.out + (((size_t)n * p.H + oy) * p.W + ox) * p.out_ld + och;
+#pragma unroll
+                for (int j = 0; j < BN / 8; ++j) {
+                    const int c = 8 * j + col0;
+                    if (c >= n_valid) break;
+                    float a0 = acc[m][4 * j + 2 * h] + __ldg(bias + c), a1 = acc[m][4 * j + 2 * h + 1] + __ldg(bias + c + 1);
+                    a0 = a0 > 0.f ? a0 : a0 * __ldg(alpha + c);
+                    a1 = a1 > 0.f ? a1 : a1 * __ldg(alpha + c + 1);
+                    const __half2 h2 = __floats2half2_rn(a0, a1);
+                    const bool two = c + 1 < n_valid;
+                    if (two && pair_ok) *(__half2*)(o + c) = h2;
+                    else { o[c] = __low2half(h2); if (two) o[c + 1] = __high2half(h2); }
+                }
+            }
+        }
+    }
+}
+
+template <int BN, bool kPool, bool kWide = false, bool kPP = false>
 __global__ void __launch_bounds__(CONV_THREADS, 1)
 conv_halo_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_b, const HaloParams p)
 {
     static_assert(!(kWide && kPool), "the pooled epilogue pairs pixel rows of one m64 block; it has no wide form");
+    static_assert(!(kWide && kPP), "an item is either two tiles on two warpgroups or one tile on one warpgroup");
+    static_assert(!kPP || BN == 64 || BN == 128, "the ping-pong item is built for the VGG trunk's widths, BN = 64 and 128");
     constexpr int B_BYTES = BN * 128;
-    constexpr int kTiles = kWide ? 2 : 1;   // spatial tiles per item = boxes per box slot = m64 accumulator blocks per warpgroup
+    constexpr int kTiles = kWide ? 2 : 1;   // spatial tiles per item = boxes per box slot
+    constexpr int kBlocks = kWide || kPP ? 2 : 1;   // m64 accumulator blocks per warpgroup
+    constexpr int kBoxSlots = kPP ? HALO_PP_BOXES : HALO_BOXES;
+    constexpr int kWarpsPerSlot = kPP ? 4 : 8;   // consumer warps that read (and release) one box slot / weight stage
     extern __shared__ uint8_t smem_raw[];
     ptx::pdl_launch_dependents();
     uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-    uint8_t* s_box = smem;                                                   // [HALO_BOXES][kTiles][box_bytes]
-    uint8_t* s_b = s_box + (size_t)HALO_BOXES * kTiles * p.box_bytes;        // [num_stages][BN x 128 B]
-    uint64_t* a_full = (uint64_t*)(s_b + (size_t)p.num_stages * B_BYTES);    // [HALO_BOXES]
-    uint64_t* a_empty = a_full + HALO_BOXES;
-    uint64_t* b_full = a_empty + HALO_BOXES;                                 // [CONV_MAX_STAGES]
+    uint8_t* s_box = smem;                                                   // [kBoxSlots][kTiles][box_bytes]
+    uint8_t* s_b = s_box + (size_t)kBoxSlots * kTiles * p.box_bytes;         // [num_stages][BN x 128 B]
+    uint64_t* a_full = (uint64_t*)(s_b + (size_t)p.num_stages * B_BYTES);    // [kBoxSlots]
+    uint64_t* a_empty = a_full + kBoxSlots;
+    uint64_t* b_full = a_empty + kBoxSlots;                                  // [CONV_MAX_STAGES]
     uint64_t* b_empty = b_full + CONV_MAX_STAGES;
+    uint64_t* turn = b_empty + CONV_MAX_STAGES;                              // kPP: [2], warpgroup 1 + i may start its next item
 
     const int wg = threadIdx.x >> 7, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int n_tiles_g = p.cout_g_pad / BN;
@@ -796,13 +888,17 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_consta
     if (threadIdx.x == 0) {
         ptx::prefetch_tmap(&tmap_x);
         ptx::prefetch_tmap(&tmap_b);
-        for (int i = 0; i < HALO_BOXES; ++i) {
+        for (int i = 0; i < kBoxSlots; ++i) {
             ptx::mbar_init(ptx::smem_u32(a_full + i), 1);
-            ptx::mbar_init(ptx::smem_u32(a_empty + i), 8);   // one arrive per consumer warp
+            ptx::mbar_init(ptx::smem_u32(a_empty + i), kWarpsPerSlot);   // one arrive per consumer warp that reads it
         }
         for (int i = 0; i < p.num_stages; ++i) {
             ptx::mbar_init(ptx::smem_u32(b_full + i), 1);
-            ptx::mbar_init(ptx::smem_u32(b_empty + i), 8);
+            ptx::mbar_init(ptx::smem_u32(b_empty + i), kWarpsPerSlot);
+        }
+        if constexpr (kPP) {
+            ptx::mbar_init(ptx::smem_u32(turn), 4);       // one arrive per warp of the warpgroup that hands over
+            ptx::mbar_init(ptx::smem_u32(turn + 1), 4);
         }
         ptx::fence_barrier_init();
     }
@@ -825,8 +921,12 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_consta
         x0 = (t - ty * p.tiles_x) * HALO_TW;
     };
 
+#ifdef HPB_HALO_PHASES
+    long long ph[HALO_PH_COUNT] = {};
+    HALO_PH_MARK(t_start);
+#endif
     if (wg == 0) {
-        if constexpr (kWide) ptx::setmaxnreg_dec<HALO_WIDE_PRODUCER_REGS>();
+        if constexpr (kWide || kPP) ptx::setmaxnreg_dec<HALO_WIDE_PRODUCER_REGS>();
         // ===================== TMA producer: kTiles halo boxes per (item, chunk), one weight tile per (item, chunk, tap) =====================
         if (warp == 0 && ptx::elect_one()) {
             int bs = 0, st = 0;
@@ -846,7 +946,7 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_consta
                         ptx::tma_load_4d(ptx::smem_u32(s_box + (size_t)(bs * kTiles + t) * p.box_bytes), &tmap_x, fa,
                                          p.in_ch_off + g * p.cin_g + c * CONV_BLOCK_K, x0 - pad_w, y0 - pad_h, n);
                     }
-                    if (++bs == HALO_BOXES) { bs = 0; bph ^= 1; }
+                    if (++bs == kBoxSlots) { bs = 0; bph ^= 1; }
                     for (int tap = 0; tap < taps; ++tap) {
                         ptx::mbar_wait(ptx::smem_u32(b_empty + st), sph ^ 1);
                         const uint32_t fb = ptx::smem_u32(b_full + st);
@@ -863,125 +963,157 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_consta
     // ===================== wgmma + epilogue =====================
     // 128-pixel item: warpgroups 1, 2 take tile rows 8 half .. 8 half + 7 of the item's tile (one m64 block each).
     // wide item: warpgroup 1 + half takes tile `half` of the pair, m64 block m = its tile rows 8 m .. 8 m + 7.
-    if constexpr (kWide) ptx::setmaxnreg_inc<HALO_WIDE_CONSUMER_REGS>();
+    // ping-pong item: warpgroup 1 + half takes the CTA's items half, half + 2, ..., m64 block m = tile rows 8 m .. 8 m + 7.
+    if constexpr (kWide || kPP) ptx::setmaxnreg_inc<HALO_WIDE_CONSUMER_REGS>();
     const int half = wg - 1;
-    const int col0 = 2 * (lane & 3);
-    const int tx = lane >> 2;                    // tile column of this thread's pixels
     const uint32_t sbo = (uint32_t)BW * 128u;
-    const int box = kWide ? half : 0;            // this warpgroup's box inside a box slot
-    const int row_base = kWide ? 0 : half * 8;   // tile row of block 0's first accumulator row
-    float acc[kTiles][BN / 2];
+    float acc[kBlocks][BN / 2];
     int bs = 0, st = 0;
     uint32_t bph = 0, sph = 0;
-    for (int item = blockIdx.x; item < total_items; item += gridDim.x) {
-        int sp, g, n0;
-        decode(item, sp, g, n0);
-        for (int c = 0; c < chunks; ++c) {
-            ptx::mbar_wait(ptx::smem_u32(a_full + bs), bph);
-            const uint32_t abase = ptx::smem_u32(s_box + (size_t)(bs * kTiles + box) * p.box_bytes) + (uint32_t)(row_base * BW * 128);
-            int prev = 0;
-            for (int tap = 0; tap < taps; ++tap) {
-                const int r = tap / p.S, s = tap - r * p.S;
-                uint64_t da[kTiles];
-#pragma unroll
-                for (int m = 0; m < kTiles; ++m) da[m] = ptx::make_sw128_kmajor_desc_at(abase + (uint32_t)(((m * 8 + r) * BW + s) * 128), sbo);
-                const uint64_t db = ptx::make_sw128_kmajor_desc(ptx::smem_u32(s_b + (size_t)st * B_BYTES));
-                ptx::mbar_wait(ptx::smem_u32(b_full + st), sph);
-#pragma unroll
-                for (int m = 0; m < kTiles; ++m) ptx::fence_acc(acc[m]);
-                ptx::wgmma_fence();
-#pragma unroll
-                for (int k = 0; k < 4; ++k)
-#pragma unroll
-                    for (int m = 0; m < kTiles; ++m)
-                        ptx::wgmma<__half, BN>(acc[m], da[m] + (uint64_t)(k * 2), db + (uint64_t)(k * 2), (c | tap | k) != 0 ? 1u : 0u);
-                ptx::wgmma_commit();
-#pragma unroll
-                for (int m = 0; m < kTiles; ++m) ptx::fence_acc(acc[m]);
-                if (tap > 0) {
-                    ptx::wgmma_wait<1>();
-                    if (lane == 0) ptx::mbar_arrive(ptx::smem_u32(b_empty + prev));
-                }
-                prev = st;
-                if (++st == p.num_stages) { st = 0; sph ^= 1; }
-            }
-            ptx::wgmma_wait<0>();   // every tap of this chunk has read the box
-#pragma unroll
-            for (int m = 0; m < kTiles; ++m) ptx::fence_acc(acc[m]);
-            if (lane == 0) {
-                ptx::mbar_arrive(ptx::smem_u32(b_empty + prev));
-                ptx::mbar_arrive(ptx::smem_u32(a_empty + bs));
-            }
-            if (++bs == HALO_BOXES) { bs = 0; bph ^= 1; }
+    if constexpr (kPP) {
+        // ring position after n more entries
+        auto advance = [](int& slot, uint32_t& phase, int n, int depth) {
+            slot += n;
+            phase ^= (uint32_t)(slot / depth) & 1u;
+            slot %= depth;
+        };
+        const int item_stages = chunks * taps;
+        if (half) {   // warpgroup 2 starts behind the CTA's first item
+            advance(bs, bph, chunks, kBoxSlots);
+            advance(st, sph, item_stages, p.num_stages);
         }
-
-        int n, y0, x0;
-        tile_pos(sp + box, n, y0, x0);
-        if (kWide && n >= p.Nb) continue;   // the second tile of an odd tile count's last item
-        const float* bias = p.bias + g * p.cout_g_pad + n0;
-        const float* alpha = p.alpha + g * p.cout_g_pad + n0;
-        const int och = p.out_ch_off + g * p.cout_g + n0;
-        const bool pair_ok = ((och | p.out_ld) & 1) == 0;
-        if constexpr (kPool) {
-            const int ty0 = row_base + (warp & 3) * 2;   // tile row of accumulator row 0 of this thread (row 8: ty0 + 1)
-            const float (&acc0)[BN / 2] = acc[0];
-            // rows ty0 / ty0 + 1 of this thread, then the column partner lane ^ 4; lanes with an even tile column store the pooled pixel
-            const int py = (y0 + ty0) >> 1, px = (x0 + tx) >> 1;
-            const bool store = (tx & 1) == 0 && py < (p.H >> 1) && px < (p.W >> 1);
-            __half* o = p.out + (((size_t)n * (p.H >> 1) + py) * (p.W >> 1) + px) * p.out_ld + och;
+        for (int j = half, item = blockIdx.x + half * gridDim.x; item < total_items; j += 2, item += 2 * gridDim.x) {
+            int sp, g, n0;
+            decode(item, sp, g, n0);
+            // the tensor pipe is ours once the other warpgroup has issued every MMA of item j - 1
+            if (j > 0) HALO_TIMED(HALO_PH_TURN_WAIT, ptx::mbar_wait(ptx::smem_u32(turn + half), (uint32_t)((j - 1) >> 1) & 1u));
+            int prev_st = 0, prev_bs = 0;
+            for (int c = 0; c < chunks; ++c) {
+                HALO_TIMED(HALO_PH_A_WAIT, ptx::mbar_wait(ptx::smem_u32(a_full + bs), bph));
+                const uint32_t abase = ptx::smem_u32(s_box + (size_t)bs * p.box_bytes);
+                for (int tap = 0; tap < taps; ++tap) {
+                    const int r = tap / p.S, s = tap - r * p.S;
+                    uint64_t da[2];
 #pragma unroll
-            for (int j = 0; j < BN / 8; ++j) {
-                float v0 = fmaxf(acc0[4 * j], acc0[4 * j + 2]), v1 = fmaxf(acc0[4 * j + 1], acc0[4 * j + 3]);
-                v0 = fmaxf(v0, __shfl_xor_sync(0xffffffffu, v0, 4));
-                v1 = fmaxf(v1, __shfl_xor_sync(0xffffffffu, v1, 4));
-                const int c = 8 * j + col0;
-                if (!store) continue;
-                float a0 = v0 + __ldg(bias + c), a1 = v1 + __ldg(bias + c + 1);
-                a0 = a0 > 0.f ? a0 : a0 * __ldg(alpha + c);
-                a1 = a1 > 0.f ? a1 : a1 * __ldg(alpha + c + 1);
-                const __half2 h2 = __floats2half2_rn(a0, a1);
-                if (pair_ok) *(__half2*)(o + c) = h2;
-                else { o[c] = __low2half(h2); o[c + 1] = __high2half(h2); }
-            }
-        } else {
-            const int n_valid = min(BN, p.cout_g - n0);
+                    for (int m = 0; m < 2; ++m) da[m] = ptx::make_sw128_kmajor_desc_at(abase + (uint32_t)(((m * 8 + r) * BW + s) * 128), sbo);
+                    const uint64_t db = ptx::make_sw128_kmajor_desc(ptx::smem_u32(s_b + (size_t)st * B_BYTES));
+                    HALO_TIMED(HALO_PH_B_WAIT, ptx::mbar_wait(ptx::smem_u32(b_full + st), sph));
 #pragma unroll
-            for (int m = 0; m < kTiles; ++m) {
-                const int ty0 = row_base + m * 8 + (warp & 3) * 2;   // tile row of accumulator row 0 of this thread (row 8: ty0 + 1)
+                    for (int m = 0; m < 2; ++m) ptx::fence_acc(acc[m]);
+                    ptx::wgmma_fence();
 #pragma unroll
-                for (int h = 0; h < 2; ++h) {
-                    const int oy = y0 + ty0 + h, ox = x0 + tx;
-                    if (oy >= p.H || ox >= p.W) continue;
-                    __half* o = p.out + (((size_t)n * p.H + oy) * p.W + ox) * p.out_ld + och;
+                    for (int k = 0; k < 4; ++k)
 #pragma unroll
-                    for (int j = 0; j < BN / 8; ++j) {
-                        const int c = 8 * j + col0;
-                        if (c >= n_valid) break;
-                        float a0 = acc[m][4 * j + 2 * h] + __ldg(bias + c), a1 = acc[m][4 * j + 2 * h + 1] + __ldg(bias + c + 1);
-                        a0 = a0 > 0.f ? a0 : a0 * __ldg(alpha + c);
-                        a1 = a1 > 0.f ? a1 : a1 * __ldg(alpha + c + 1);
-                        const __half2 h2 = __floats2half2_rn(a0, a1);
-                        const bool two = c + 1 < n_valid;
-                        if (two && pair_ok) *(__half2*)(o + c) = h2;
-                        else { o[c] = __low2half(h2); if (two) o[c + 1] = __high2half(h2); }
+                        for (int m = 0; m < 2; ++m)
+                            ptx::wgmma<__half, BN>(acc[m], da[m] + (uint64_t)(k * 2), db + (uint64_t)(k * 2), (c | tap | k) != 0 ? 1u : 0u);
+                    ptx::wgmma_commit();
+#pragma unroll
+                    for (int m = 0; m < 2; ++m) ptx::fence_acc(acc[m]);
+                    if ((c | tap) != 0) {
+                        // the previous k-step's MMAs are done: its weight stage, and at a chunk's first tap the previous box, are free
+                        HALO_TIMED(HALO_PH_MMA_WAIT, ptx::wgmma_wait<1>());
+                        if (lane == 0) {
+                            ptx::mbar_arrive(ptx::smem_u32(b_empty + prev_st));
+                            if (tap == 0) ptx::mbar_arrive(ptx::smem_u32(a_empty + prev_bs));
+                        }
                     }
+                    prev_st = st;
+                    if (++st == p.num_stages) { st = 0; sph ^= 1; }
                 }
+                prev_bs = bs;
+                if (++bs == kBoxSlots) { bs = 0; bph ^= 1; }
             }
+            if (lane == 0) ptx::mbar_arrive(ptx::smem_u32(turn + (half ^ 1)));   // every MMA of item j is issued: hand over the pipe
+            HALO_TIMED(HALO_PH_MMA_WAIT, ptx::wgmma_wait<0>());
+#pragma unroll
+            for (int m = 0; m < 2; ++m) ptx::fence_acc(acc[m]);
+            if (lane == 0) {
+                ptx::mbar_arrive(ptx::smem_u32(b_empty + prev_st));
+                ptx::mbar_arrive(ptx::smem_u32(a_empty + prev_bs));
+            }
+            advance(bs, bph, chunks, kBoxSlots);   // item j + 1 is the other warpgroup's
+            advance(st, sph, item_stages, p.num_stages);
+            HALO_PH_MARK(t_epi);
+            int n, y0, x0;
+            tile_pos(sp, n, y0, x0);
+            halo_epilogue<BN, kPool, 2>(acc, p, n, y0, x0, g, n0, 0, warp, lane);
+            HALO_PH_ADD(HALO_PH_EPILOGUE, t_epi);
+        }
+    } else {
+        const int box = kWide ? half : 0;            // this warpgroup's box inside a box slot
+        const int row_base = kWide ? 0 : half * 8;   // tile row of block 0's first accumulator row
+        for (int item = blockIdx.x; item < total_items; item += gridDim.x) {
+            int sp, g, n0;
+            decode(item, sp, g, n0);
+            for (int c = 0; c < chunks; ++c) {
+                HALO_TIMED(HALO_PH_A_WAIT, ptx::mbar_wait(ptx::smem_u32(a_full + bs), bph));
+                const uint32_t abase = ptx::smem_u32(s_box + (size_t)(bs * kTiles + box) * p.box_bytes) + (uint32_t)(row_base * BW * 128);
+                int prev = 0;
+                for (int tap = 0; tap < taps; ++tap) {
+                    const int r = tap / p.S, s = tap - r * p.S;
+                    uint64_t da[kTiles];
+#pragma unroll
+                    for (int m = 0; m < kTiles; ++m) da[m] = ptx::make_sw128_kmajor_desc_at(abase + (uint32_t)(((m * 8 + r) * BW + s) * 128), sbo);
+                    const uint64_t db = ptx::make_sw128_kmajor_desc(ptx::smem_u32(s_b + (size_t)st * B_BYTES));
+                    HALO_TIMED(HALO_PH_B_WAIT, ptx::mbar_wait(ptx::smem_u32(b_full + st), sph));
+#pragma unroll
+                    for (int m = 0; m < kTiles; ++m) ptx::fence_acc(acc[m]);
+                    ptx::wgmma_fence();
+#pragma unroll
+                    for (int k = 0; k < 4; ++k)
+#pragma unroll
+                        for (int m = 0; m < kTiles; ++m)
+                            ptx::wgmma<__half, BN>(acc[m], da[m] + (uint64_t)(k * 2), db + (uint64_t)(k * 2), (c | tap | k) != 0 ? 1u : 0u);
+                    ptx::wgmma_commit();
+#pragma unroll
+                    for (int m = 0; m < kTiles; ++m) ptx::fence_acc(acc[m]);
+                    if (tap > 0) {
+                        HALO_TIMED(HALO_PH_MMA_WAIT, ptx::wgmma_wait<1>());
+                        if (lane == 0) ptx::mbar_arrive(ptx::smem_u32(b_empty + prev));
+                    }
+                    prev = st;
+                    if (++st == p.num_stages) { st = 0; sph ^= 1; }
+                }
+                HALO_TIMED(HALO_PH_MMA_WAIT, ptx::wgmma_wait<0>());   // every tap of this chunk has read the box
+#pragma unroll
+                for (int m = 0; m < kTiles; ++m) ptx::fence_acc(acc[m]);
+                if (lane == 0) {
+                    ptx::mbar_arrive(ptx::smem_u32(b_empty + prev));
+                    ptx::mbar_arrive(ptx::smem_u32(a_empty + bs));
+                }
+                if (++bs == kBoxSlots) { bs = 0; bph ^= 1; }
+            }
+
+            HALO_PH_MARK(t_epi);
+            int n, y0, x0;
+            tile_pos(sp + box, n, y0, x0);
+            if (kWide && n >= p.Nb) continue;   // the second tile of an odd tile count's last item
+            halo_epilogue<BN, kPool, kBlocks>(acc, p, n, y0, x0, g, n0, row_base, warp, lane);
+            HALO_PH_ADD(HALO_PH_EPILOGUE, t_epi);
         }
     }
+#ifdef HPB_HALO_PHASES
+    HALO_PH_ADD(HALO_PH_TOTAL, t_start);
+    if ((threadIdx.x & 127) == 0)
+        for (int i = 0; i < HALO_PH_COUNT; ++i) atomicAdd(g_halo_phases + i, (unsigned long long)ph[i]);
+#endif
 }
 
 inline int halo_box_bytes(int R, int S) { return ((HALO_TH + R - 1) * (HALO_TW + S - 1) * 128 + 1023) & ~1023; }
-// tiles: spatial tiles per work item (1, or 2 for the wide item: two boxes per box slot)
-inline size_t conv_halo_smem_bytes(int R, int S, int BN, int stages, int tiles = 1)
+// the work item of conv_halo_kernel: one 16 x 8 tile on both consumer warpgroups, two tiles (kWide), or one tile on one warpgroup (kPP)
+enum class HaloItem { Narrow, Wide, PingPong };
+inline int halo_box_slots(HaloItem it) { return it == HaloItem::PingPong ? HALO_PP_BOXES : HALO_BOXES; }
+inline int halo_boxes_per_slot(HaloItem it) { return it == HaloItem::Wide ? 2 : 1; }
+inline size_t conv_halo_smem_bytes(int R, int S, int BN, int stages, HaloItem it)
 {
-    return 1024 + (size_t)HALO_BOXES * tiles * halo_box_bytes(R, S) + (size_t)stages * BN * 128 + (2 * HALO_BOXES + 2 * CONV_MAX_STAGES) * 8;
+    return 1024 + (size_t)halo_box_slots(it) * halo_boxes_per_slot(it) * halo_box_bytes(R, S) + (size_t)stages * BN * 128 +
+           (2 * halo_box_slots(it) + 2 * CONV_MAX_STAGES + 2) * 8;
 }
 // as many weight stages as fit, up to CONV_MAX_STAGES (at least 2: a caller that needs more checks the result)
-inline int conv_halo_pick_stages(int R, int S, int BN, int tiles = 1)
+inline int conv_halo_pick_stages(int R, int S, int BN, HaloItem it)
 {
     int s = CONV_MAX_STAGES;
-    while (s > 2 && conv_halo_smem_bytes(R, S, BN, s, tiles) > CONV_SMEM_LIMIT) --s;
+    while (s > 2 && conv_halo_smem_bytes(R, S, BN, s, it) > CONV_SMEM_LIMIT) --s;
     return s;
 }
 

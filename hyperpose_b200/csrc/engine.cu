@@ -623,6 +623,8 @@ enum class Launch : uint8_t {
     Halo,           // conv_halo_kernel: one TMA box per 16 x 8-pixel tile and channel chunk serves every filter tap
     HaloPool,       // conv_halo_kernel with the 2x2 max-pool that follows in its epilogue (hp.out is the POOLED buffer)
     HaloWide,       // conv_halo_kernel with 256-pixel work items: two 16 x 8 tiles share every weight tile
+    HaloPP,         // conv_halo_kernel with ping-pong items: one 16 x 8 tile per consumer warpgroup, the two take turns on the tensor pipe
+    HaloPoolPP,     // HaloPool on ping-pong items
     DwTma,          // dwconv3_tma_kernel<1>
     DwTmaPair,      // dwconv3_tma_kernel<2>: this op and the next one (same input, other filters)
     DwCol,          // dwconv3_col_kernel
@@ -669,7 +671,7 @@ struct EngOp {
 // reference the tests compare the default against.
 struct EngOptions {
     enum { HALO_AUTO, HALO_NONE, HALO_ALL } halo = HALO_AUTO;   // HPB_HALO=all | anything else; unset: build_conv_plan's rule
-    bool halo_wide = true;       // HPB_HALO_NARROW: every halo layer takes the 128-pixel work item
+    bool halo_wide = true;       // HPB_HALO_NARROW: every halo layer takes the 128-pixel work item (neither wide nor ping-pong)
     bool stem3 = true;           // fused 3x3 stem; HPB_NO_STEM3 keeps the im2col buffer
     bool pool_fuse = true;       // HPB_NO_POOL_FUSE
     bool dw1_fuse = true;        // HPB_NO_DW1_FUSE
@@ -776,14 +778,24 @@ inline float tf32_round(float x)
     return x;
 }
 
-// The halo plan's work item: one 16 x 8 tile (128 pixels), or two tiles sharing every weight tile (conv_halo_kernel<128, false, true>)
-void set_halo_item(EngOp& op, bool wide)
+bool is_halo(Launch k)
+{
+    return k == Launch::Halo || k == Launch::HaloPool || k == Launch::HaloWide || k == Launch::HaloPP || k == Launch::HaloPoolPP;
+}
+HaloItem halo_item_of(Launch k)
+{
+    return k == Launch::HaloWide ? HaloItem::Wide : k == Launch::HaloPP || k == Launch::HaloPoolPP ? HaloItem::PingPong : HaloItem::Narrow;
+}
+
+// The halo plan's work item: one 16 x 8 tile (128 pixels) on both consumer warpgroups, two tiles sharing every weight tile
+// (conv_halo_kernel<128, false, true>), or one tile per warpgroup with the two taking turns (conv_halo_kernel<BN, kPool, false, true>)
+void set_halo_item(EngOp& op, HaloItem item, bool pool)
 {
     HaloParams& h = op.plan.hp;
-    const int tiles = wide ? 2 : 1;
-    h.num_stages = conv_halo_pick_stages(h.R, h.S, op.plan.prm.BN, tiles);
-    op.plan.smem = conv_halo_smem_bytes(h.R, h.S, op.plan.prm.BN, h.num_stages, tiles);
-    op.launch = wide ? Launch::HaloWide : Launch::Halo;
+    h.num_stages = conv_halo_pick_stages(h.R, h.S, op.plan.prm.BN, item);
+    op.plan.smem = conv_halo_smem_bytes(h.R, h.S, op.plan.prm.BN, h.num_stages, item);
+    op.launch = item == HaloItem::Wide ? Launch::HaloWide : item == HaloItem::PingPong ? (pool ? Launch::HaloPoolPP : Launch::HaloPP)
+                                                                                   : (pool ? Launch::HaloPool : Launch::Halo);
 }
 
 // Which halo layers take the wide item, from per-layer times of both items at the cfg3 / cfg4 / cfg5 benchmark batch sizes
@@ -794,6 +806,31 @@ void set_halo_item(EngOp& op, bool wide)
 bool halo_wide_faster(int R, long wide_items, int sms)
 {
     return R == 7 && wide_items >= sms;
+}
+
+// The ping-pong item exists for 3x3 layers at BN = 64 and 128 (the VGG trunk's widths).  Which of them take it, from per-layer times
+// of both items at the cfg3 / cfg4 / cfg5 benchmark batch sizes (tools/layer_times.py, DESIGN.md §4): layers of four or more
+// 64-channel chunks (36+ k-steps per item: 12-17 % faster) and layers with the 2x2 max-pool in their epilogue (a quarter of the stores:
+// 14-24 % faster, down to one chunk).  Shorter items with the full epilogue lose up to 14 %: one warpgroup's epilogue of a whole
+// 16 x 8 x BN tile outlasts the other's 9 or 18 k-steps.  Launches of fewer than two items per CTA leave one warpgroup idle; they
+// were not measured and keep the 128-pixel item.
+bool halo_pp_exists(int R, int BN) { return R == 3 && (BN == 64 || BN == 128); }
+bool halo_pp_faster(int chunks, bool pooled, long items, int sms) { return (chunks >= 4 || pooled) && items >= 2L * sms; }
+
+// The halo layer's work item (halo_wide_faster, halo_pp_faster), its pool fused or not.  HPB_HALO=all takes the wide item wherever
+// it exists and the ping-pong item where the wide one does not; HPB_HALO_NARROW=1 the 128-pixel item.
+HaloItem pick_halo_item(const hp_engine* e, const EngOp& op, bool pooled)
+{
+    const HaloParams& h = op.plan.hp;
+    const int BN = op.plan.prm.BN, sms = e->num_sms - e->reserve_sms;
+    const long tiles = (long)h.Nb * h.tiles_x * h.tiles_y, n_tiles = (long)h.groups * (h.cout_g_pad / BN);
+    const bool all = e->opt.halo == EngOptions::HALO_ALL;
+    if (!e->opt.halo_wide) return HaloItem::Narrow;
+    // the wide item: BN = 128 without the pool, and at least 3 weight stages next to its four boxes
+    if (!pooled && BN == 128 && conv_halo_pick_stages(h.R, h.S, BN, HaloItem::Wide) >= 3 && (all || halo_wide_faster(h.R, (tiles + 1) / 2 * n_tiles, sms)))
+        return HaloItem::Wide;
+    if (halo_pp_exists(h.R, BN) && (all || halo_pp_faster(h.cin_g / CONV_BLOCK_K, pooled, tiles * n_tiles, sms))) return HaloItem::PingPong;
+    return HaloItem::Narrow;
 }
 
 // The conv's GEMM operands, epilogue and tensor maps.  data_type::kHALF: fp16 activations and weights, 64-channel chunks;
@@ -950,12 +987,7 @@ int build_conv_plan(hp_engine* e, EngOp& op, const float* blob)
         h.out = ob.d; h.out_ld = ob.channels; h.out_ch_off = (int)po.out_ch_off;
         rc = make_tmap_act_box(&pl.tmap_x, ib.d, e->max_batch, ib.H, ib.W, ib.channels, ib.channels, HALO_TW + eS - 1, HALO_TH + eR - 1, CU_TENSOR_MAP_SWIZZLE_128B);
         if (rc) return rc;
-        // the wide item: BN = 128 only, and at least 3 weight stages next to its four boxes; HPB_HALO=all takes it wherever it exists
-        const bool wide_ok = e->opt.halo_wide && BN == 128 && conv_halo_pick_stages(eR, eS, BN, 2) >= 3;
-        const long wide_items = ((long)e->max_batch * tx * ty + 1) / 2 * G * (cout_pad / BN);
-        const bool wide_want = e->opt.halo == EngOptions::HALO_AUTO ? halo_wide_faster(eR, wide_items, e->num_sms - e->reserve_sms)
-                                                                    : e->opt.halo == EngOptions::HALO_ALL;
-        set_halo_item(op, wide_ok && wide_want);
+        set_halo_item(op, pick_halo_item(e, op, false), false);
     }
     return HP_OK;
 }
@@ -1010,10 +1042,17 @@ const void* halo_kernel_bn(int BN)
     }
     return nullptr;
 }
-// Launch::Halo / HaloPool / HaloWide (the wide item exists for BN = 128 only, see set_halo_item)
+// Launch::Halo / HaloPool / HaloWide / HaloPP / HaloPoolPP (the wide item exists for BN = 128 only, the ping-pong item for BN = 64
+// and 128, see build_conv_plan)
 const void* halo_kernel(Launch k, int BN)
 {
     if (k == Launch::HaloWide) return BN == 128 ? (const void*)conv_halo_kernel<128, false, true> : nullptr;
+    if (k == Launch::HaloPP || k == Launch::HaloPoolPP) {
+        const bool pool = k == Launch::HaloPoolPP;
+        if (BN == 64) return pool ? (const void*)conv_halo_kernel<64, true, false, true> : (const void*)conv_halo_kernel<64, false, false, true>;
+        if (BN == 128) return pool ? (const void*)conv_halo_kernel<128, true, false, true> : (const void*)conv_halo_kernel<128, false, false, true>;
+        return nullptr;
+    }
     return k == Launch::HaloPool ? halo_kernel_bn<true>(BN) : halo_kernel_bn<false>(BN);
 }
 const void* conv_kernel(int dtype, bool res, int BN, int stem_R = 0)
@@ -1044,7 +1083,7 @@ void launch_dw_tma(hp_engine* e, const EngOp& op, const EngOp* pair, int N, cuda
     else      launch_pdl(dwconv3_tma_kernel<1>, grid, DWT_THREADS, op.dwt_smem, st, op.tmap_dw, p);
 }
 
-// conv_wgmma_kernel, or conv_halo_kernel for Launch::Halo / HaloPool / HaloWide
+// conv_wgmma_kernel, or conv_halo_kernel for the Halo* launches
 int launch_conv(hp_engine* e, EngOp& op, int N, cudaStream_t st, bool u8_input)
 {
     ConvPlan& pl = op.plan;
@@ -1052,7 +1091,7 @@ int launch_conv(hp_engine* e, EngOp& op, int N, cudaStream_t st, bool u8_input)
     p.Nb = N;
     const int stem_R = op.launch == Launch::ConvStem && u8_input ? (int)op.po.R : 0;
     p.frames = e->cur_frames ? e->cur_frames : e->d_frames;
-    if (op.launch == Launch::Halo || op.launch == Launch::HaloPool || op.launch == Launch::HaloWide) {
+    if (is_halo(op.launch)) {
         HaloParams h = pl.hp;
         h.Nb = N;
         const int tiles = op.launch == Launch::HaloWide ? 2 : 1;
@@ -1155,7 +1194,7 @@ int run_graph(hp_engine* e, int N, bool u8_input, cudaStream_t st, int first = 0
 #undef HP_IM2COL
             break;
         }
-        case Launch::Conv: case Launch::ConvStem: case Launch::Halo: case Launch::HaloPool: case Launch::HaloWide:
+        case Launch::Conv: case Launch::ConvStem: case Launch::Halo: case Launch::HaloPool: case Launch::HaloWide: case Launch::HaloPP: case Launch::HaloPoolPP:
             launch_conv(e, op, N, st, u8_input);
             break;
         case Launch::DwTma:
@@ -1584,7 +1623,7 @@ int hp_engine_create_ex(hp_engine** out, const void* pack, size_t pack_bytes, in
     // conv (halo kernel) -> 2x2 max-pool: the pool moves into the conv's epilogue when nobody else reads the un-pooled tensor
     for (size_t i = 0; opt.pool_fuse && i + 1 < e->ops.size(); ++i) {
         EngOp& c = e->ops[i]; EngOp& m = e->ops[i + 1];
-        if ((c.launch != Launch::Halo && c.launch != Launch::HaloWide) || !c.plan.monotone_act || m.po.type != OP_MAXPOOL2 || (m.po.R != 0 && m.po.R != 2)) continue;
+        if ((c.launch != Launch::Halo && c.launch != Launch::HaloWide && c.launch != Launch::HaloPP) || !c.plan.monotone_act || m.po.type != OP_MAXPOOL2 || (m.po.R != 0 && m.po.R != 2)) continue;
         const EngBuffer& cb = e->bufs[c.po.out_buf];
         const EngBuffer& pb = e->bufs[m.po.out_buf];
         const int C = (int)c.po.groups * (int)c.po.cout_g;
@@ -1595,8 +1634,9 @@ int hp_engine_create_ex(hp_engine** out, const void* pack, size_t pack_bytes, in
             if (k != i + 1 && reads_buffer(e->ops[k].po, c.po.out_buf)) other_reader = true;
         if (other_reader) continue;
         c.plan.hp.out = pb.d; c.plan.hp.out_ld = pb.channels; c.plan.hp.out_ch_off = (int)m.po.out_ch_off;
-        set_halo_item(c, false);   // the pooled epilogue has the 128-pixel item only; its smem is at most the wide one's
-        c.launch = Launch::HaloPool;
+        // the item is picked again for the pooled epilogue: it has no wide form, and pooled layers take the ping-pong item at any depth
+        set_halo_item(c, pick_halo_item(e, c, true), true);
+        max_smem = std::max(max_smem, c.plan.smem);
         m.launch = Launch::None;
         e->bufs[c.po.out_buf].fused_away = true;
     }
@@ -1684,7 +1724,7 @@ int hp_engine_create_ex(hp_engine** out, const void* pack, size_t pack_bytes, in
     e->use_pdl = dtype == HP_DTYPE_F16 && launches > 0 && per_launch < 10e9;
     for (const EngOp& o : e->ops) {
         if (o.po.type != OP_CONV) continue;
-        if ((o.launch == Launch::Halo || o.launch == Launch::HaloPool || o.launch == Launch::HaloWide) &&
+        if (is_halo(o.launch) &&
             cudaFuncSetAttribute(halo_kernel(o.launch, o.plan.prm.BN), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)max_smem) != cudaSuccess) {
             set_error("engine: cannot opt in to %zu bytes of dynamic shared memory (halo)", max_smem);
             return fail(HP_ERR_CUDA);
@@ -2034,7 +2074,7 @@ int hp_pack_int8_calibrated(const void* pack, size_t pack_bytes)
 }
 
 // test hook: the kernel op `op` launches on the next run over u8 frames, as decided when the engine was created (EngOp::launch and
-// the conv plan's tile width): conv<f16|tf32|i8,BN[,res][,stem3|stem7]>, halo<BN[,pool]>, dw_strip<K,S>, dw_col, dw_tma<1|2>, dw_f32,
+// the conv plan's tile width): conv<f16|tf32|i8,BN[,res][,stem3|stem7]>, halo<BN[,pool|,wide|,pp|,pool,pp]>, dw_strip<K,S>, dw_col, dw_tma<1|2>, dw_f32,
 // dw_i8, maxpool<K>, maxpool_f32, maxpool_i8, im2col, im2col_i8, heads, ppn_head, or none when a neighbouring op's launch covers it
 int hp_engine_debug_op_kernel(const hp_engine* e, int op, char* name, int cap)
 {
@@ -2054,6 +2094,8 @@ int hp_engine_debug_op_kernel(const hp_engine* e, int op, char* name, int cap)
     case Launch::Halo: s = "halo<" + std::to_string(BN) + ">"; break;
     case Launch::HaloPool: s = "halo<" + std::to_string(BN) + ",pool>"; break;
     case Launch::HaloWide: s = "halo<" + std::to_string(BN) + ",wide>"; break;
+    case Launch::HaloPP: s = "halo<" + std::to_string(BN) + ",pp>"; break;
+    case Launch::HaloPoolPP: s = "halo<" + std::to_string(BN) + ",pool,pp>"; break;
     case Launch::DwTma: s = "dw_tma<1>"; break;
     case Launch::DwTmaPair: s = "dw_tma<2>"; break;
     case Launch::DwCol: s = "dw_col"; break;
@@ -2138,6 +2180,22 @@ int hp_pifpaf_process_device(hp_pifpaf* p, const float* d_pif, const float* d_pa
 int hp_pifpaf_pipeline_info(hp_pifpaf* p, void** stream, void** inputs_free_event, int* hcap);
 int hp_pifpaf_copy_results_host_async(hp_pifpaf* p, hp_human* pin_humans, int* pin_counts_flags, int N, void* stream);
 int hp_pifpaf_grow_capacity(hp_pifpaf* p, int flags);
+
+#ifdef HPB_HALO_PHASES
+// instrumented build only (-DHPB_HALO_PHASES, tools/halo_phases.py): the cycle counts conv_halo_kernel has summed since the last
+// reset, in HALO_PH_* order (total, operand A late, operand B late, wgmma wait, epilogue, turn wait); reset != 0 zeroes them after
+int hp_debug_halo_phases(unsigned long long* out, int n, int reset)
+{
+    if (!out || n != HALO_PH_COUNT) { set_error("hp_debug_halo_phases: expected %d counters", (int)HALO_PH_COUNT); return HP_ERR_ARG; }
+    HP_CUDA_TRY(cudaDeviceSynchronize());
+    HP_CUDA_TRY(cudaMemcpyFromSymbol(out, g_halo_phases, sizeof(unsigned long long) * HALO_PH_COUNT));
+    if (reset) {
+        const unsigned long long zero[HALO_PH_COUNT] = {};
+        HP_CUDA_TRY(cudaMemcpyToSymbol(g_halo_phases, zero, sizeof(zero)));
+    }
+    return HP_OK;
+}
+#endif
 
 } // extern "C" (helpers below are C++)
 
