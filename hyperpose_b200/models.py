@@ -452,8 +452,6 @@ def resnet50_lw_openpose(seed: int = 0, weights=None) -> Graph:
     ws = weights
     g = Graph("resnet50_lw_openpose", 19, 38, 3, mean=(0.0, 0.0, 0.0))
     relu = lambda n: np.zeros(n, np.float32)
-    lin = lambda n: np.ones(n, np.float32)
-    b_ = lambda n: (rng.standard_normal(n) * 0.05).astype(np.float32)
 
     col = g.add_buffer(192, 1); g.add_im2col(col, stride=2, ksize=7)
     c1 = g.add_buffer(64, 1)
@@ -465,6 +463,17 @@ def resnet50_lw_openpose(seed: int = 0, weights=None) -> Graph:
     x = g.add_buffer(64, 2); g.add_maxpool(c1, x, 64, "maxpool_1", ksize=3)
     # (n_filter, blocks, stride of the first block) at scale_size 8
     cur, cur_c, cur_d = _resnet50_body(g, rng, ws, x, 64, 2, [(64, 3, 1), (128, 4, 2), (256, 6, 1), (512, 3, 1)])
+    _lw_head(g, rng, ws, cur, cur_c)
+    return g
+
+
+def _lw_head(g, rng, ws, cur, cur_c):
+    """the LightWeightOpenPose head on a stride-8 backbone output `cur` of `cur_c` channels (lw_openpose.py:106-191): CPM, init stage,
+    one refinement stage with residual blocks (relu(bn(conv)) + res in the conv epilogue), conf / paf into the split outputs.
+    Layer names (cpm.*, init.*, ref.b{k}.*) are those of weights._lw_head_order, for every backbone."""
+    relu = lambda n: np.zeros(n, np.float32)
+    lin = lambda n: np.ones(n, np.float32)
+    b_ = lambda n: (rng.standard_normal(n) * 0.05).astype(np.float32)
 
     def lw_conv(in_buf, out_buf, ci, co, k, act=True, name="c", wname=None, **kw):      # Conv2d(+bias, relu)
         if ws:
@@ -496,7 +505,7 @@ def resnet50_lw_openpose(seed: int = 0, weights=None) -> Graph:
         g.add_conv(wide_buf, out_spec[0], w2, b2, lin(57), name=name_out, **out_spec[1])
 
     # ---- CPM (lw_openpose.py:106-121) ----
-    t0 = g.add_buffer(128, 3); lw_conv(cur, t0, 2048, 128, 1, name="cpm_init", wname="cpm.init")
+    t0 = g.add_buffer(128, 3); lw_conv(cur, t0, cur_c, 128, 1, name="cpm_init", wname="cpm.init")
     t1 = g.add_buffer(128, 3); lw_block(t0, t1, 128, 128, 3, "cpm_b1", wname="cpm.b1")
     t2 = g.add_buffer(128, 3); lw_block(t1, t2, 128, 128, 3, "cpm_b2", wname="cpm.b2")
     t3 = g.add_buffer(128, 3); lw_block(t2, t3, 128, 128, 3, "cpm_b3", wname="cpm.b3", res_buf=t0, res_mode=2)          # x + main_block(x)
@@ -523,6 +532,51 @@ def resnet50_lw_openpose(seed: int = 0, weights=None) -> Graph:
         src, ci = r2, 128
     wide2 = g.add_buffer(1024, 3)
     head_pair(src, wide2, (0, dict(out_mode=OUT_F32_NCHW_SPLIT, split=19)), "ref", "ref_4", "ref_out")
+
+
+# (block name, n_filter) of vggtiny_backbone at scale_size 8 (backbones.py:343-365); "pool" is MaxPool2d(2, 2, 'SAME')
+VGGTINY_LAYERS = [("block_1_1", 32), ("block_1_2", 64), "pool", ("block_2_1", 128), ("block_2_2", 128), "pool",
+                  ("block_3_1", 200), ("block_3_2", 200), ("block_3_3", 200), "pool", ("block_4_1", 384), ("block_4_2", 384)]
+
+
+def lw_openpose_vggtiny(seed: int = 0, weights=None) -> Graph:
+    """Lightweight-OpenPose on TinyVGG (the model of the reference's quick start, export_pb.py --model_type=LightweightOpenpose
+    --model_backbone=Vggtiny): vggtiny_backbone(scale_size=8) (backbones.py:343-391: nine 3x3 Conv2d(+bias) + BatchNorm(relu) blocks,
+    three 2x2 'SAME' max-pools with ceil output, 384 channels at stride 8), then the LW head (_lw_head).  BatchNorm folded.
+    A 32- or 200-channel tensor lives in a buffer rounded up to 64 channels, whose zero pad channels the next conv reads as its
+    padded K.  `weights`: a hyperpose_b200.weights.LwVggtinyWeights; default = seeded random values."""
+    rng = np.random.default_rng(seed)
+    ws = weights
+    g = Graph("lw_openpose_vggtiny", 19, 38, 3, mean=(0.0, 0.0, 0.0))
+    col = g.add_buffer(64, 0); g.add_im2col(col)
+    cur, cur_c, cur_d, n_pool = col, 3, 0, 0
+    for layer in VGGTINY_LAYERS:
+        if layer == "pool":
+            n_pool += 1
+            nxt = g.add_buffer(_r64(cur_c), cur_d + 1); g.add_maxpool(cur, nxt, cur_c, f"maxpool_{n_pool}")
+            cur, cur_d = nxt, cur_d + 1
+            continue
+        name, co = layer
+        if ws:
+            w, b = ws.conv(name, co, cur_c, 3); w = w[None]; sc, sh = ws.bn(name + ".bn", co)
+        else:
+            w = _he(rng, 1, co, cur_c, 3, 3); b = (rng.standard_normal(co) * 0.05).astype(np.float32); sc, sh = _bn_fold(rng, co)
+        nxt = g.add_buffer(_r64(co), cur_d)
+        g.add_conv(cur, nxt, w * sc.reshape(1, co, 1, 1, 1), sh + b * sc, np.zeros(co, np.float32), im2col_input=int(cur == col), name=name)
+        cur, cur_c = nxt, co
+    _lw_head(g, rng, ws, cur, cur_c)
+    return g
+
+
+def lw_openpose_resnet18(seed: int = 0, weights=None) -> Graph:
+    """Lightweight-OpenPose on ResNet-18: Resnet18_backbone(scale_size=8) (backbones.py:512-585: 7x7/2 stem, 3x3/2 max-pool, blocks
+    2_1 .. 5_1; at scale 8 blocks 4_1 and 5_1 keep stride 1, so 512 channels at stride 8), then the LW head (_lw_head).  Blocks as in
+    ppn_resnet18 (_resnet18_body).  `weights`: a hyperpose_b200.weights.LwResnet18Weights; default = seeded random values."""
+    rng = np.random.default_rng(seed)
+    ws = weights
+    g = Graph("lw_openpose_resnet18", 19, 38, 3, mean=(0.0, 0.0, 0.0))
+    cur, cur_c, cur_d = _resnet18_body(g, rng, ws, *_ppn_stem(g, rng, ws), RESNET18_STRIDES_8)
+    _lw_head(g, rng, ws, cur, cur_c)
     return g
 
 
@@ -610,6 +664,14 @@ def ppn_resnet18(seed: int = 0, weights=None) -> Graph:
     rng = np.random.default_rng(seed)
     ws = weights
     g = Graph("ppn_resnet18", 6 * PPN_K, PPN_L * PPN_NH * PPN_NW, 5, mean=(0.0, 0.0, 0.0), head_type=2)
+    cur, cur_c, cur_d = _resnet18_body(g, rng, ws, *_ppn_stem(g, rng, ws), [st for _, _, st, _ in RESNET18_BLOCKS])
+    _ppn_head(g, rng, ws, cur, cur_c, cur_d)
+    return g
+
+
+def _resnet18_body(g, rng, ws, cur, cur_c, cur_d, strides):
+    """blocks 2_1 .. 5_1 of Resnet18_backbone (RESNET18_BLOCKS) with the given stride per block, from the stem output `cur`.
+    BatchNorm folded; relu(x + res) in the conv epilogue.  Returns (buffer, channels, down_shift)."""
     relu = lambda n: np.zeros(n, np.float32)
     lin = lambda n: np.ones(n, np.float32)
 
@@ -626,8 +688,7 @@ def ppn_resnet18(seed: int = 0, weights=None) -> Graph:
             w[:, 1, 1] = 1.0
         g.add_dwconv(in_buf, out_buf, w, np.zeros(C, np.float32), lin(C), stride=2, name=name)
 
-    cur, cur_c, cur_d = _ppn_stem(g, rng, ws)
-    for name, nf, st, ds in RESNET18_BLOCKS:
+    for (name, nf, _, ds), st in zip(RESNET18_BLOCKS, strides):
         d_out = cur_d + (1 if st == 2 else 0)
         a = g.add_buffer(nf, cur_d)
         conv_bn(cur, a, cur_c, nf, 3, True, f"{name}_1", 2.0)
@@ -644,13 +705,14 @@ def ppn_resnet18(seed: int = 0, weights=None) -> Graph:
         out = g.add_buffer(nf, d_out)
         conv_bn(a, out, nf, nf, 3, True, f"{name}_2", 0.5, res_buf=res, res_mode=1)    # relu(x + res)
         cur, cur_c, cur_d = out, nf, d_out
-    _ppn_head(g, rng, ws, cur, cur_c, cur_d)
-    return g
+    return cur, cur_c, cur_d
 
 
 # (block name, n_filter, stride, is_down_sample) of Resnet18_backbone(scale_size=32) (backbones.py:529-535)
 RESNET18_BLOCKS = [("block_2_1", 64, 1, False), ("block_2_2", 64, 1, False), ("block_3_1", 128, 2, True), ("block_3_2", 128, 1, False),
                    ("block_4_1", 256, 2, True), ("block_4_2", 256, 1, False), ("block_5_1", 512, 2, True)]
+# the strides at scale_size 8: blocks 4_1 and 5_1 keep stride 1 (backbones.py:520-523)
+RESNET18_STRIDES_8 = (1, 1, 2, 1, 1, 1, 1)
 
 
 def ppn_resnet50(seed: int = 0, weights=None) -> Graph:

@@ -3,6 +3,8 @@
   * OpenPose-VGG19            hyperpose/Model/openpose/model/openpose.py + backbones.py:447-509      -> ListWeights
   * MobilenetThin-OpenPose    openpose/model/mbv2_th_openpose.py + backbones.py:233-297              -> MobilenetThinWeights
   * LW-OpenPose on ResNet-50  openpose/model/lw_openpose.py + backbones.py:587-698                   -> Resnet50LwWeights
+  * LW-OpenPose on TinyVGG    openpose/model/lw_openpose.py + backbones.py:343-391                   -> LwVggtinyWeights
+  * LW-OpenPose on ResNet-18  openpose/model/lw_openpose.py + backbones.py:512-585                   -> LwResnet18Weights
   * PifPaf on ResNet-50       pifpaf/model.py:41-281 + backbones.py:587-698                          -> Resnet50PifPafWeights
   * PPN on ResNet-18 / -50    pose_proposal/model.py:14-119 + backbones.py:512-698                   -> Ppn18Weights / Ppn50Weights
 
@@ -301,14 +303,43 @@ def resnet50_lw_layer_order(n_conf: int = 19, n_paf: int = 38):
     init_stage, refine_stage1; :106-191 for the stages)"""
     order = []
     _resnet50_order(order, [(64, 3, 1), (128, 4, 2), (256, 6, 1), (512, 3, 1)])
+    _lw_head_order(order, 2048, n_conf, n_paf)
+    return order
+
+
+def _lw_head_order(order, cin, n_conf: int = 19, n_paf: int = 38):
+    """cpm_stage, init_stage, refine_stage1 of LightWeightOpenPose (lw_openpose.py:106-191), created after the backbone; `cin` is the
+    backbone's out_channels (the CPM init_layer's input)"""
     blk = lambda name, ci, co, k: [("conv", name, co, ci, k), ("bn", name + ".bn", co, 0, 0)]   # conv_block: Conv2d(+bias) + BatchNorm
-    order += [("conv", "cpm.init", 128, 2048, 1)] + blk("cpm.b1", 128, 128, 3) + blk("cpm.b2", 128, 128, 3) + blk("cpm.b3", 128, 128, 3)
+    order += [("conv", "cpm.init", 128, cin, 1)] + blk("cpm.b1", 128, 128, 3) + blk("cpm.b2", 128, 128, 3) + blk("cpm.b3", 128, 128, 3)
     order += [("conv", "cpm.end", 128, 128, 3)]
     order += [("conv", f"init.{i}", 128, 128, 3) for i in (1, 2, 3)]
     order += [("conv", "init.conf.1", 512, 128, 1), ("conv", "init.conf.2", n_conf, 512, 1), ("conv", "init.paf.1", 512, 128, 1), ("conv", "init.paf.2", n_paf, 512, 1)]
     for k in range(1, 6):
         order += [("conv", f"ref.b{k}.init", 128, 128 + n_conf + n_paf if k == 1 else 128, 1)] + blk(f"ref.b{k}.c1", 128, 128, 3) + blk(f"ref.b{k}.c2", 128, 128, 3)
     order += [("conv", "ref.conf.1", 512, 128, 1), ("conv", "ref.conf.2", n_conf, 512, 1), ("conv", "ref.paf.1", 512, 128, 1), ("conv", "ref.paf.2", n_paf, 512, 1)]
+
+
+def lw_vggtiny_layer_order(n_conf: int = 19, n_paf: int = 38):
+    """all_weights order of LightWeightOpenPose(backbone=vggtiny_backbone) (lw_openpose.py:33-45): vggtiny_backbone(scale_size=8)
+    (backbones.py:343-391: per block a Conv2d with biases, then its BatchNorm), cpm_stage on 384 channels, init_stage, refine_stage1"""
+    from .models import VGGTINY_LAYERS
+    order, cin = [], 3
+    for layer in VGGTINY_LAYERS:
+        if layer != "pool":
+            name, co = layer
+            order += [("conv", name, co, cin, 3), ("bn", name + ".bn", co, 0, 0)]
+            cin = co
+    _lw_head_order(order, cin, n_conf, n_paf)
+    return order
+
+
+def lw_resnet18_layer_order(n_conf: int = 19, n_paf: int = 38):
+    """all_weights order of LightWeightOpenPose(backbone=Resnet18_backbone) (lw_openpose.py:33-45): Resnet18_backbone(scale_size=8)
+    (the stride does not change a weight: the same arrays as _resnet18_order), cpm_stage on 512 channels, init_stage, refine_stage1"""
+    order = []
+    _resnet18_order(order)
+    _lw_head_order(order, 512, n_conf, n_paf)
     return order
 
 
@@ -328,11 +359,11 @@ def _ppn_head_order(order, cin, K: int = 18, L: int = 17, nh: int = 9, nw: int =
               ("conv", "add3", 6 * K + L * nh * nw, 512, 1)]
 
 
-def ppn_resnet18_layer_order():
-    """all_weights order of PoseProposal on Resnet18_backbone(scale_size=32) (backbones.py:512-585): conv_1_1 (no bias), bn_1_1, then
-    the blocks; inside a Res_block `main_block` is created before `down_sample` (:564-576), so the shortcut's conv / bn come last"""
+def _resnet18_order(order):
+    """Resnet18_backbone (backbones.py:512-585): conv_1_1 (no bias), bn_1_1, then the blocks; inside a Res_block `main_block` is
+    created before `down_sample` (:564-576), so the shortcut's conv / bn come last"""
     from .models import RESNET18_BLOCKS
-    order = [("conv_nobias", "conv1", 64, 3, 7), ("bn", "bn1", 64, 0, 0)]
+    order += [("conv_nobias", "conv1", 64, 3, 7), ("bn", "bn1", 64, 0, 0)]
     cin = 64
     for name, nf, _, ds in RESNET18_BLOCKS:
         order += [("conv_nobias", f"{name}_1.conv", nf, cin, 3), ("bn", f"{name}_1.bn", nf, 0, 0),
@@ -340,6 +371,12 @@ def ppn_resnet18_layer_order():
         if ds:
             order += [("conv_nobias", f"{name}_ds.conv", nf, cin, 1), ("bn", f"{name}_ds.bn", nf, 0, 0)]
         cin = nf
+
+
+def ppn_resnet18_layer_order():
+    """all_weights order of PoseProposal on Resnet18_backbone(scale_size=32) (backbones.py:512-585), then the PPN head"""
+    order = []
+    _resnet18_order(order)
     _ppn_head_order(order, 512)
     return order
 
@@ -373,6 +410,24 @@ class Ppn50Weights(BnNetWeights):
 class Resnet50LwWeights(BnNetWeights):
     def __init__(self, arrays):
         super().__init__(arrays, resnet50_lw_layer_order())
+
+    @classmethod
+    def from_npz(cls, path: str):
+        return cls(load_params_npz(path))
+
+
+class LwVggtinyWeights(BnNetWeights):
+    def __init__(self, arrays):
+        super().__init__(arrays, lw_vggtiny_layer_order())
+
+    @classmethod
+    def from_npz(cls, path: str):
+        return cls(load_params_npz(path))
+
+
+class LwResnet18Weights(BnNetWeights):
+    def __init__(self, arrays):
+        super().__init__(arrays, lw_resnet18_layer_order())
 
     @classmethod
     def from_npz(cls, path: str):
