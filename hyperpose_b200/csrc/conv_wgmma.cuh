@@ -749,16 +749,22 @@ constexpr int HALO_WIDE_PRODUCER_REGS = 40, HALO_WIDE_CONSUMER_REGS = 232;
 constexpr int HALO_PP_BOXES = 4;
 
 #ifdef HPB_HALO_PHASES
-// instrumented build (tools/halo_phases.py): clock64 cycles of every consumer warpgroup, summed over the CTAs of all halo launches
-enum { HALO_PH_TOTAL, HALO_PH_A_WAIT, HALO_PH_B_WAIT, HALO_PH_MMA_WAIT, HALO_PH_EPILOGUE, HALO_PH_TURN_WAIT, HALO_PH_COUNT };
+// instrumented build (tools/halo_phases.py): clock64 cycles of every consumer warpgroup, summed over the CTAs of all halo launches.
+// HALO_PH_EPILOGUE: accumulators -> output (registers -> global, or -> the staging buffer and the TMA store's issue);
+// HALO_PH_STAGE_WAIT: waiting for the staging buffer's previous TMA store to have read it
+enum { HALO_PH_TOTAL, HALO_PH_A_WAIT, HALO_PH_B_WAIT, HALO_PH_MMA_WAIT, HALO_PH_EPILOGUE, HALO_PH_TURN_WAIT, HALO_PH_STAGE_WAIT, HALO_PH_COUNT };
 __device__ unsigned long long g_halo_phases[HALO_PH_COUNT];
 #define HALO_PH_MARK(t) const long long t = clock64()
 #define HALO_TIMED(i, ...) do { const long long t0_ = clock64(); __VA_ARGS__; ph[i] += clock64() - t0_; } while (0)
 #define HALO_PH_ADD(i, t) (ph[i] += clock64() - (t))
+#define HALO_PH_PARAM , long long (&ph)[HALO_PH_COUNT]
+#define HALO_PH_ARG , ph
 #else
 #define HALO_PH_MARK(t) do {} while (0)
 #define HALO_TIMED(i, ...) do { __VA_ARGS__; } while (0)
 #define HALO_PH_ADD(i, t) do {} while (0)
+#define HALO_PH_PARAM
+#define HALO_PH_ARG
 #endif
 
 struct HaloParams {
@@ -771,7 +777,17 @@ struct HaloParams {
     int num_stages;             // weight ring depth
     const float* bias; const float* alpha;
     __half* out; int out_ld, out_ch_off;   // NHWC output (kPool: the pooled tensor, [Nb, H/2, W/2, out_ld])
+    int tma_store;              // 1: the epilogue stages the fp16 tile in shared memory and TMA-stores it (halo_epilogue_tma)
+    int stage_bytes;            // tma_store: each consumer warpgroup's staging region (halo_stage_bytes; 0 on the wide item)
 };
+
+// the work item of conv_halo_kernel: one 16 x 8 tile on both consumer warpgroups, two tiles (kWide), or one tile on one warpgroup (kPP)
+enum class HaloItem { Narrow, Wide, PingPong };
+// staging slots of one consumer warpgroup for the TMA-store epilogue, BN x 128 B each (one m64 block): the wide item stages its two
+// blocks in its own box of the item's last chunk; the ping-pong item at BN = 128 stores its two blocks through one 16 KiB slot in
+// turn (a full 32 KiB per warpgroup would cost two more of its weight stages)
+__host__ __device__ constexpr int halo_stage_slots(int BN, HaloItem it) { return it == HaloItem::Wide || (it == HaloItem::PingPong && BN == 64) ? 2 : 1; }
+inline int halo_stage_bytes(int BN, HaloItem it) { return it == HaloItem::Wide ? 0 : halo_stage_slots(BN, it) * BN * 128; }
 
 namespace ptx {
 // K-major 128B-swizzled operand whose 8-row groups are `sbo` bytes apart and whose start need not be 1024-byte aligned.  The swizzle
@@ -788,6 +804,24 @@ __device__ __forceinline__ uint64_t make_sw128_kmajor_desc_at(uint32_t smem_addr
 }
 template <uint32_t N> __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
 template <uint32_t N> __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+// four 8 x 8 fp16 matrices, one per register: the thread holds row lane / 4, columns 2 (lane % 4) + {0, 1} of each (the accumulator
+// fragment's layout); lane 8 i + r gives the address of row r of matrix i
+__device__ __forceinline__ void stmatrix_x4(uint32_t addr, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3)
+{
+    asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(r0), "r"(r1), "r"(r2), "r"(r3) : "memory");
+}
+__device__ __forceinline__ void st_shared_u32(uint32_t addr, uint32_t v) { asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v) : "memory"); }
+__device__ __forceinline__ void named_barrier_sync(int id, int threads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory"); }
+__device__ __forceinline__ void tma_store_4d(const CUtensorMap* m, uint32_t src, int c0, int c1, int c2, int c3)
+{
+    asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];"
+                 ::"l"(m), "r"(src), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// the thread's bulk groups but the newest N have finished reading shared memory / have completed (their writes are performed)
+template <int N> __device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
+template <int N> __device__ __forceinline__ void bulk_wait() { asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory"); }
+__device__ __forceinline__ uint32_t half2_bits(__half2 h) { return *reinterpret_cast<uint32_t*>(&h); }
 } // namespace ptx
 
 // Stores m64 blocks 0 .. kBlocks - 1 of one warpgroup's accumulators: block m holds tile rows row_base + 8 m .. row_base + 8 m + 7 of
@@ -853,9 +887,96 @@ __device__ __forceinline__ void halo_epilogue(const float (&acc)[kBlocks][BN / 2
     }
 }
 
+// halo_epilogue with the same fp32 arithmetic, written through shared memory: block m's fp16 outputs go into staging slot m % kSlots
+// (BN / 64 slices of {64 channels x 8 x 8 pixels}, pooled {64 x 4 x 4}, each in the 128B-swizzled layout of one TMA box: pixel row q,
+// 16-byte chunk j at q * 128 + ((j ^ q % 8) * 16)), and the warpgroup's leader thread stores each slice with one TMA box of tmap_o and
+// commits one bulk group per block.  The tensor map clips what lies past the image's right / bottom edge (or the floor-pooled map)
+// and past the layer's last channel.  kWait: before a slot is written again, the leader waits until the group that read it last is
+// done reading (the wide item stages into its own box instead, which its caller hands back to the producer once that store has read it).
+template <int BN, bool kPool, int kBlocks, int kSlots, bool kWait>
+__device__ __forceinline__ void halo_epilogue_tma(const float (&acc)[kBlocks][BN / 2], const HaloParams& p, const CUtensorMap* tmap_o, uint32_t stage,
+                                                  int n, int y0, int x0, int g, int n0, int row_base, int warp, int lane, bool leader HALO_PH_PARAM)
+{
+    static_assert(BN == 64 || BN == 128, "one TMA box per 64-channel slice, at most two");
+    constexpr int kSliceBytes = (kPool ? 16 : 64) * 128;
+    constexpr int kSlotBytes = BN / 64 * kSliceBytes;
+    const int col0 = 2 * (lane & 3);
+    const float* bias = p.bias + g * p.cout_g_pad + n0;
+    const float* alpha = p.alpha + g * p.cout_g_pad + n0;
+    const int och = p.out_ch_off + g * p.cout_g + n0;
+    const int bar_id = warp >> 2;   // named barrier 1 / 2: consumer warpgroup 1 / 2
+#pragma unroll
+    for (int m = 0; m < kBlocks; ++m) {
+        const uint32_t slot = stage + (uint32_t)((m % kSlots) * kSlotBytes);
+        HALO_PH_MARK(t_wait);
+        if (kWait && leader) ptx::bulk_wait_read<kSlots - 1>();
+        ptx::named_barrier_sync(bar_id, 128);   // the slot is free, and the whole warpgroup is past its last wgmma
+#ifdef HPB_HALO_PHASES
+        { const long long d = clock64() - t_wait; ph[HALO_PH_STAGE_WAIT] += d; ph[HALO_PH_EPILOGUE] -= d; }
+#endif
+        const int ty0 = row_base + m * 8;   // tile row of the block's first pixel row
+        if constexpr (kPool) {
+            // the pooled pixel of this thread's rows (ty0 + 2 (warp % 4), + 1) and columns (tx, tx ^ 1): slot row (warp % 4) * 4 + tx / 2
+            const int q = (warp & 3) * 4 + (lane >> 3);
+            const bool store = ((lane >> 2) & 1) == 0;
+#pragma unroll
+            for (int j = 0; j < BN / 8; ++j) {
+                float v0 = fmaxf(acc[m][4 * j], acc[m][4 * j + 2]), v1 = fmaxf(acc[m][4 * j + 1], acc[m][4 * j + 3]);
+                v0 = fmaxf(v0, __shfl_xor_sync(0xffffffffu, v0, 4));
+                v1 = fmaxf(v1, __shfl_xor_sync(0xffffffffu, v1, 4));
+                if (!store) continue;
+                const int c = 8 * j + col0;
+                const float2 b = __ldg((const float2*)(bias + c)), a = __ldg((const float2*)(alpha + c));
+                float a0 = v0 + b.x, a1 = v1 + b.y;
+                a0 = a0 > 0.f ? a0 : a0 * a.x;
+                a1 = a1 > 0.f ? a1 : a1 * a.y;
+                ptx::st_shared_u32(slot + (uint32_t)((j >> 3) * kSliceBytes + q * 128 + (((j & 7) ^ (q & 7)) << 4) + (lane & 3) * 4),
+                                   ptx::half2_bits(__floats2half2_rn(a0, a1)));
+            }
+        } else {
+            // stmatrix: register i of a thread holds rows lane / 4 (+ 8 h) and channels 8 (4 jb + i) + col0 + {0, 1}; lane 8 i + r
+            // addresses pixel row r of matrix i, so (row % 8) == r
+            const int r = lane & 7, i = lane >> 3;
+#pragma unroll
+            for (int jb = 0; jb < BN / 32; ++jb) {
+                float2 b[4], a[4];
+#pragma unroll
+                for (int k = 0; k < 4; ++k) {
+                    const int c = 8 * (4 * jb + k) + col0;
+                    b[k] = __ldg((const float2*)(bias + c));
+                    a[k] = __ldg((const float2*)(alpha + c));
+                }
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    uint32_t v[4];
+#pragma unroll
+                    for (int k = 0; k < 4; ++k) {
+                        float a0 = acc[m][4 * (4 * jb + k) + 2 * h] + b[k].x, a1 = acc[m][4 * (4 * jb + k) + 2 * h + 1] + b[k].y;
+                        a0 = a0 > 0.f ? a0 : a0 * a[k].x;
+                        a1 = a1 > 0.f ? a1 : a1 * a[k].y;
+                        v[k] = ptx::half2_bits(__floats2half2_rn(a0, a1));
+                    }
+                    const int j = 4 * jb + i, row = (warp & 3) * 16 + 8 * h + r;
+                    ptx::stmatrix_x4(slot + (uint32_t)((j >> 3) * kSliceBytes + row * 128 + (((j & 7) ^ r) << 4)), v[0], v[1], v[2], v[3]);
+                }
+            }
+        }
+        ptx::fence_proxy_async();   // the generic-proxy writes -> visible to the TMA store
+        ptx::named_barrier_sync(bar_id, 128);
+        if (leader) {
+            const int x = kPool ? x0 >> 1 : x0, y = kPool ? (y0 + ty0) >> 1 : y0 + ty0;
+            ptx::tma_store_4d(tmap_o, slot, och, x, y, n);
+            if (BN == 128 && n0 + 64 < p.cout_g)   // (not a slice of padding channels only)
+                ptx::tma_store_4d(tmap_o, slot + (uint32_t)kSliceBytes, och + 64, x, y, n);
+            ptx::bulk_commit();
+        }
+    }
+}
+
 template <int BN, bool kPool, bool kWide = false, bool kPP = false>
 __global__ void __launch_bounds__(CONV_THREADS, 1)
-conv_halo_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_b, const HaloParams p)
+conv_halo_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_b, const __grid_constant__ CUtensorMap tmap_o,
+                 const HaloParams p)
 {
     static_assert(!(kWide && kPool), "the pooled epilogue pairs pixel rows of one m64 block; it has no wide form");
     static_assert(!(kWide && kPP), "an item is either two tiles on two warpgroups or one tile on one warpgroup");
@@ -865,12 +986,16 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_consta
     constexpr int kBlocks = kWide || kPP ? 2 : 1;   // m64 accumulator blocks per warpgroup
     constexpr int kBoxSlots = kPP ? HALO_PP_BOXES : HALO_BOXES;
     constexpr int kWarpsPerSlot = kPP ? 4 : 8;   // consumer warps that read (and release) one box slot / weight stage
+    constexpr int kStageSlots = halo_stage_slots(BN, kWide ? HaloItem::Wide : kPP ? HaloItem::PingPong : HaloItem::Narrow);
+    // the TMA-store epilogue (p.tma_store) exists for BN = 64 and 128; other widths always take halo_epilogue
+    constexpr bool kTmaForm = BN % 64 == 0;
     extern __shared__ uint8_t smem_raw[];
     ptx::pdl_launch_dependents();
     uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
     uint8_t* s_box = smem;                                                   // [kBoxSlots][kTiles][box_bytes]
     uint8_t* s_b = s_box + (size_t)kBoxSlots * kTiles * p.box_bytes;         // [num_stages][BN x 128 B]
-    uint64_t* a_full = (uint64_t*)(s_b + (size_t)p.num_stages * B_BYTES);    // [kBoxSlots]
+    uint8_t* s_stage = s_b + (size_t)p.num_stages * B_BYTES;                 // [2][stage_bytes]: TMA-store staging per consumer warpgroup
+    uint64_t* a_full = (uint64_t*)(s_stage + 2 * (size_t)p.stage_bytes);     // [kBoxSlots]
     uint64_t* a_empty = a_full + kBoxSlots;
     uint64_t* b_full = a_empty + kBoxSlots;                                  // [CONV_MAX_STAGES]
     uint64_t* b_empty = b_full + CONV_MAX_STAGES;
@@ -888,6 +1013,7 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_consta
     if (threadIdx.x == 0) {
         ptx::prefetch_tmap(&tmap_x);
         ptx::prefetch_tmap(&tmap_b);
+        if (kTmaForm && p.tma_store) ptx::prefetch_tmap(&tmap_o);
         for (int i = 0; i < kBoxSlots; ++i) {
             ptx::mbar_init(ptx::smem_u32(a_full + i), 1);
             ptx::mbar_init(ptx::smem_u32(a_empty + i), kWarpsPerSlot);   // one arrive per consumer warp that reads it
@@ -967,6 +1093,9 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_consta
     if constexpr (kWide || kPP) ptx::setmaxnreg_inc<HALO_WIDE_CONSUMER_REGS>();
     const int half = wg - 1;
     const uint32_t sbo = (uint32_t)BW * 128u;
+    const bool tma = kTmaForm && p.tma_store;
+    const bool leader = (threadIdx.x & 127) == 0;   // issues (and waits for) the warpgroup's TMA stores
+    const uint32_t stage = ptx::smem_u32(s_stage + (size_t)half * p.stage_bytes);
     float acc[kBlocks][BN / 2];
     int bs = 0, st = 0;
     uint32_t bph = 0, sph = 0;
@@ -1036,12 +1165,20 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_consta
             HALO_PH_MARK(t_epi);
             int n, y0, x0;
             tile_pos(sp, n, y0, x0);
-            halo_epilogue<BN, kPool, 2>(acc, p, n, y0, x0, g, n0, 0, warp, lane);
+            if constexpr (kTmaForm) {
+                if (tma) halo_epilogue_tma<BN, kPool, 2, kStageSlots, true>(acc, p, &tmap_o, stage, n, y0, x0, g, n0, 0, warp, lane, leader HALO_PH_ARG);
+                else halo_epilogue<BN, kPool, 2>(acc, p, n, y0, x0, g, n0, 0, warp, lane);
+            } else {
+                halo_epilogue<BN, kPool, 2>(acc, p, n, y0, x0, g, n0, 0, warp, lane);
+            }
             HALO_PH_ADD(HALO_PH_EPILOGUE, t_epi);
         }
     } else {
         const int box = kWide ? half : 0;            // this warpgroup's box inside a box slot
         const int row_base = kWide ? 0 : half * 8;   // tile row of block 0's first accumulator row
+        // wide item, TMA store: the box slot the leader has not released yet -- the previous item's last chunk, which holds its staged
+        // tile until the store has read it (the producer's next load into it is a chunk away)
+        int held = -1;
         for (int item = blockIdx.x; item < total_items; item += gridDim.x) {
             int sp, g, n0;
             decode(item, sp, g, n0);
@@ -1071,6 +1208,11 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_consta
                         HALO_TIMED(HALO_PH_MMA_WAIT, ptx::wgmma_wait<1>());
                         if (lane == 0) ptx::mbar_arrive(ptx::smem_u32(b_empty + prev));
                     }
+                    if (kWide && held >= 0 && tap == taps / 2) {
+                        HALO_TIMED(HALO_PH_STAGE_WAIT, ptx::bulk_wait_read<0>());
+                        ptx::mbar_arrive(ptx::smem_u32(a_empty + held));
+                        held = -1;
+                    }
                     prev = st;
                     if (++st == p.num_stages) { st = 0; sph ^= 1; }
                 }
@@ -1079,7 +1221,8 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_consta
                 for (int m = 0; m < kTiles; ++m) ptx::fence_acc(acc[m]);
                 if (lane == 0) {
                     ptx::mbar_arrive(ptx::smem_u32(b_empty + prev));
-                    ptx::mbar_arrive(ptx::smem_u32(a_empty + bs));
+                    if (kWide && tma && leader && c == chunks - 1) held = bs;   // this box stages the tile's outputs
+                    else ptx::mbar_arrive(ptx::smem_u32(a_empty + bs));
                 }
                 if (++bs == kBoxSlots) { bs = 0; bph ^= 1; }
             }
@@ -1087,11 +1230,33 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_consta
             HALO_PH_MARK(t_epi);
             int n, y0, x0;
             tile_pos(sp + box, n, y0, x0);
-            if (kWide && n >= p.Nb) continue;   // the second tile of an odd tile count's last item
-            halo_epilogue<BN, kPool, kBlocks>(acc, p, n, y0, x0, g, n0, row_base, warp, lane);
+            if (kWide && n >= p.Nb) {   // the second tile of an odd tile count's last item
+                if (held >= 0) { ptx::mbar_arrive(ptx::smem_u32(a_empty + held)); held = -1; }
+                continue;
+            }
+            if constexpr (kTmaForm) {
+                if (tma && !kWide) {
+                    halo_epilogue_tma<BN, kPool, kBlocks, kStageSlots, true>(acc, p, &tmap_o, stage, n, y0, x0, g, n0, row_base, warp, lane,
+                                                                          leader HALO_PH_ARG);
+                } else if (tma) {
+                    // wide item: the box this warpgroup has just finished with; a 7x7 box (39 KiB) holds both m64 blocks at once, a
+                    // smaller one (3x3: 23 KiB) one block at a time
+                    const int last_bs = (bs + kBoxSlots - 1) % kBoxSlots;
+                    const uint32_t dst = ptx::smem_u32(s_box + (size_t)(last_bs * kTiles + box) * p.box_bytes);
+                    if (p.box_bytes >= kBlocks * B_BYTES)
+                        halo_epilogue_tma<BN, kPool, kBlocks, kBlocks, false>(acc, p, &tmap_o, dst, n, y0, x0, g, n0, row_base, warp, lane, leader HALO_PH_ARG);
+                    else
+                        halo_epilogue_tma<BN, kPool, kBlocks, 1, true>(acc, p, &tmap_o, dst, n, y0, x0, g, n0, row_base, warp, lane, leader HALO_PH_ARG);
+                } else {
+                    halo_epilogue<BN, kPool, kBlocks>(acc, p, n, y0, x0, g, n0, row_base, warp, lane);
+                }
+            } else {
+                halo_epilogue<BN, kPool, kBlocks>(acc, p, n, y0, x0, g, n0, row_base, warp, lane);
+            }
             HALO_PH_ADD(HALO_PH_EPILOGUE, t_epi);
         }
     }
+    if (tma && leader) ptx::bulk_wait<0>();   // every store has completed before the CTA exits (the next kernel reads them)
 #ifdef HPB_HALO_PHASES
     HALO_PH_ADD(HALO_PH_TOTAL, t_start);
     if ((threadIdx.x & 127) == 0)
@@ -1100,20 +1265,19 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_consta
 }
 
 inline int halo_box_bytes(int R, int S) { return ((HALO_TH + R - 1) * (HALO_TW + S - 1) * 128 + 1023) & ~1023; }
-// the work item of conv_halo_kernel: one 16 x 8 tile on both consumer warpgroups, two tiles (kWide), or one tile on one warpgroup (kPP)
-enum class HaloItem { Narrow, Wide, PingPong };
 inline int halo_box_slots(HaloItem it) { return it == HaloItem::PingPong ? HALO_PP_BOXES : HALO_BOXES; }
 inline int halo_boxes_per_slot(HaloItem it) { return it == HaloItem::Wide ? 2 : 1; }
-inline size_t conv_halo_smem_bytes(int R, int S, int BN, int stages, HaloItem it)
+// tma_store: with the staging regions of the TMA-store epilogue (halo_stage_bytes per consumer warpgroup)
+inline size_t conv_halo_smem_bytes(int R, int S, int BN, int stages, HaloItem it, bool tma_store)
 {
     return 1024 + (size_t)halo_box_slots(it) * halo_boxes_per_slot(it) * halo_box_bytes(R, S) + (size_t)stages * BN * 128 +
-           (2 * halo_box_slots(it) + 2 * CONV_MAX_STAGES + 2) * 8;
+           (tma_store ? 2 * (size_t)halo_stage_bytes(BN, it) : 0) + (2 * halo_box_slots(it) + 2 * CONV_MAX_STAGES + 2) * 8;
 }
 // as many weight stages as fit, up to CONV_MAX_STAGES (at least 2: a caller that needs more checks the result)
-inline int conv_halo_pick_stages(int R, int S, int BN, HaloItem it)
+inline int conv_halo_pick_stages(int R, int S, int BN, HaloItem it, bool tma_store)
 {
     int s = CONV_MAX_STAGES;
-    while (s > 2 && conv_halo_smem_bytes(R, S, BN, s, it) > CONV_SMEM_LIMIT) --s;
+    while (s > 2 && conv_halo_smem_bytes(R, S, BN, s, it, tma_store) > CONV_SMEM_LIMIT) --s;
     return s;
 }
 

@@ -603,6 +603,7 @@ struct ConvPlan {
     ConvParams prm;
     CUtensorMap tmap_a, tmap_b;
     CUtensorMap tmap_x;          // halo plan: the input as a 4-D tensor with a (16+R-1) x (8+S-1)-pixel box
+    CUtensorMap tmap_o;          // halo plan, hp.tma_store: the output's channels [0, out_ch_off + groups * cout_g) with an 8 x 8-pixel box (pooled 4 x 4)
     void* d_w = nullptr;         // K-major weights: fp16, or fp32 rounded to TF32 (the engine's dtype)
     bool monotone_act = false;   // every PReLU slope of the layer is >= 0
     HaloParams hp;               // halo plan: conv_halo_kernel's parameters
@@ -672,6 +673,7 @@ struct EngOp {
 struct EngOptions {
     enum { HALO_AUTO, HALO_NONE, HALO_ALL } halo = HALO_AUTO;   // HPB_HALO=all | anything else; unset: build_conv_plan's rule
     bool halo_wide = true;       // HPB_HALO_NARROW: every halo layer takes the 128-pixel work item (neither wide nor ping-pong)
+    bool halo_tma_store = true;  // HPB_HALO_REG_EPILOGUE: the halo kernel stores its outputs from registers, not through TMA
     bool stem3 = true;           // fused 3x3 stem; HPB_NO_STEM3 keeps the im2col buffer
     bool pool_fuse = true;       // HPB_NO_POOL_FUSE
     bool dw1_fuse = true;        // HPB_NO_DW1_FUSE
@@ -787,15 +789,33 @@ HaloItem halo_item_of(Launch k)
     return k == Launch::HaloWide ? HaloItem::Wide : k == Launch::HaloPP || k == Launch::HaloPoolPP ? HaloItem::PingPong : HaloItem::Narrow;
 }
 
+// Can the halo plan's epilogue TMA-store its tile?  One box per 64-channel slice (BN = 64 or 128) at a 16-byte aligned channel
+// offset and pixel stride, a channel extent of whole 16-byte units (the TMA store clips a box at the extent in 16-byte units, so
+// 57 channels would also write the 58th to 64th), and no box reaching into another n-tile's channels: a grouped layer's groups must
+// be whole n-tiles (the map's channel extent clips only the last group's padding).  Other plans keep halo_epilogue's per-thread stores.
+bool halo_tma_store_ok(const HaloParams& h, int BN)
+{
+    return BN % 64 == 0 && h.out_ld % 8 == 0 && h.out_ch_off % 8 == 0 && (h.groups * h.cout_g) % 8 == 0 &&
+           (h.groups == 1 || h.cout_g % BN == 0);
+}
+
 // The halo plan's work item: one 16 x 8 tile (128 pixels) on both consumer warpgroups, two tiles sharing every weight tile
-// (conv_halo_kernel<128, false, true>), or one tile per warpgroup with the two taking turns (conv_halo_kernel<BN, kPool, false, true>)
-void set_halo_item(EngOp& op, HaloItem item, bool pool)
+// (conv_halo_kernel<128, false, true>), or one tile per warpgroup with the two taking turns (conv_halo_kernel<BN, kPool, false, true>);
+// with the TMA-store epilogue where the plan allows it, its output tensor map and staging regions
+int set_halo_item(const hp_engine* e, EngOp& op, HaloItem item, bool pool)
 {
     HaloParams& h = op.plan.hp;
-    h.num_stages = conv_halo_pick_stages(h.R, h.S, op.plan.prm.BN, item);
-    op.plan.smem = conv_halo_smem_bytes(h.R, h.S, op.plan.prm.BN, h.num_stages, item);
+    const int BN = op.plan.prm.BN;
+    h.tma_store = e->opt.halo_tma_store && halo_tma_store_ok(h, BN);
+    h.stage_bytes = h.tma_store ? halo_stage_bytes(BN, item) : 0;
+    h.num_stages = conv_halo_pick_stages(h.R, h.S, BN, item, h.tma_store);
+    op.plan.smem = conv_halo_smem_bytes(h.R, h.S, BN, h.num_stages, item, h.tma_store);
     op.launch = item == HaloItem::Wide ? Launch::HaloWide : item == HaloItem::PingPong ? (pool ? Launch::HaloPoolPP : Launch::HaloPP)
                                                                                    : (pool ? Launch::HaloPool : Launch::Halo);
+    if (!h.tma_store) return HP_OK;
+    const int oh = pool ? h.H / 2 : h.H, ow = pool ? h.W / 2 : h.W, box = pool ? HALO_TW / 2 : HALO_TW;
+    return make_tmap_act_box(&op.plan.tmap_o, h.out, e->max_batch, oh, ow, h.out_ch_off + h.groups * h.cout_g, h.out_ld, box, box,
+                             CU_TENSOR_MAP_SWIZZLE_128B);
 }
 
 // Which halo layers take the wide item, from per-layer times of both items at the cfg3 / cfg4 / cfg5 benchmark batch sizes
@@ -827,7 +847,7 @@ HaloItem pick_halo_item(const hp_engine* e, const EngOp& op, bool pooled)
     const bool all = e->opt.halo == EngOptions::HALO_ALL;
     if (!e->opt.halo_wide) return HaloItem::Narrow;
     // the wide item: BN = 128 without the pool, and at least 3 weight stages next to its four boxes
-    if (!pooled && BN == 128 && conv_halo_pick_stages(h.R, h.S, BN, HaloItem::Wide) >= 3 && (all || halo_wide_faster(h.R, (tiles + 1) / 2 * n_tiles, sms)))
+    if (!pooled && BN == 128 && conv_halo_pick_stages(h.R, h.S, BN, HaloItem::Wide, false) >= 3 && (all || halo_wide_faster(h.R, (tiles + 1) / 2 * n_tiles, sms)))
         return HaloItem::Wide;
     if (halo_pp_exists(h.R, BN) && (all || halo_pp_faster(h.cin_g / CONV_BLOCK_K, pooled, tiles * n_tiles, sms))) return HaloItem::PingPong;
     return HaloItem::Narrow;
@@ -987,7 +1007,8 @@ int build_conv_plan(hp_engine* e, EngOp& op, const float* blob)
         h.out = ob.d; h.out_ld = ob.channels; h.out_ch_off = (int)po.out_ch_off;
         rc = make_tmap_act_box(&pl.tmap_x, ib.d, e->max_batch, ib.H, ib.W, ib.channels, ib.channels, HALO_TW + eS - 1, HALO_TH + eR - 1, CU_TENSOR_MAP_SWIZZLE_128B);
         if (rc) return rc;
-        set_halo_item(op, pick_halo_item(e, op, false), false);
+        rc = set_halo_item(e, op, pick_halo_item(e, op, false), false);
+        if (rc) return rc;
     }
     return HP_OK;
 }
@@ -1098,7 +1119,7 @@ int launch_conv(hp_engine* e, EngOp& op, int N, cudaStream_t st, bool u8_input)
         const long items = ((long)N * h.tiles_x * h.tiles_y + tiles - 1) / tiles * h.groups * (h.cout_g_pad / p.BN);
         cudaLaunchAttribute at[1];
         const cudaLaunchConfig_t cfg = pdl_config((int)std::min<long>(e->num_sms - e->reserve_sms, items), CONV_THREADS, pl.smem, st, at);
-        void* args[] = { (void*)&pl.tmap_x, (void*)&pl.tmap_b, (void*)&h };
+        void* args[] = { (void*)&pl.tmap_x, (void*)&pl.tmap_b, (void*)&pl.tmap_o, (void*)&h };
         HP_CUDA_TRY(cudaLaunchKernelExC(&cfg, halo_kernel(op.launch, p.BN), args));
         return HP_OK;
     }
@@ -1466,6 +1487,7 @@ int hp_engine_create_ex(hp_engine** out, const void* pack, size_t pack_bytes, in
     EngOptions& opt = e->opt;
     if (const char* v = getenv("HPB_HALO")) opt.halo = strcmp(v, "all") == 0 ? EngOptions::HALO_ALL : EngOptions::HALO_NONE;
     opt.halo_wide = !getenv("HPB_HALO_NARROW");
+    opt.halo_tma_store = !getenv("HPB_HALO_REG_EPILOGUE");
     opt.stem3 = !getenv("HPB_NO_STEM3");
     opt.pool_fuse = !getenv("HPB_NO_POOL_FUSE");
     opt.dw1_fuse = !getenv("HPB_NO_DW1_FUSE");
@@ -1635,7 +1657,7 @@ int hp_engine_create_ex(hp_engine** out, const void* pack, size_t pack_bytes, in
         if (other_reader) continue;
         c.plan.hp.out = pb.d; c.plan.hp.out_ld = pb.channels; c.plan.hp.out_ch_off = (int)m.po.out_ch_off;
         // the item is picked again for the pooled epilogue: it has no wide form, and pooled layers take the ping-pong item at any depth
-        set_halo_item(c, pick_halo_item(e, c, true), true);
+        if (int rc = set_halo_item(e, c, pick_halo_item(e, c, true), true)) return fail(rc);
         max_smem = std::max(max_smem, c.plan.smem);
         m.launch = Launch::None;
         e->bufs[c.po.out_buf].fused_away = true;
@@ -2114,6 +2136,16 @@ int hp_engine_debug_op_kernel(const hp_engine* e, int op, char* name, int cap)
     return HP_OK;
 }
 
+// test hook: *tma_store = 1 when op `op` runs conv_halo_kernel with the TMA-store epilogue (halo_epilogue_tma), 0 for every other op
+// (a halo plan the TMA store cannot express, or HPB_HALO_REG_EPILOGUE=1)
+int hp_engine_debug_op_epilogue(const hp_engine* e, int op, int* tma_store)
+{
+    if (!e || op < 0 || op >= (int)e->ops.size() || !tma_store) { set_error("hp_engine_debug_op_epilogue: bad argument"); return HP_ERR_ARG; }
+    const EngOp& o = e->ops[op];
+    *tma_store = is_halo(o.launch) && o.plan.hp.tma_store ? 1 : 0;
+    return HP_OK;
+}
+
 long long hp_engine_launch_count(const hp_engine* e) { return e ? e->launches : 0; }
 
 int hp_engine_set_output_override(hp_engine* e, const float* d_conf, const float* d_paf)
@@ -2183,7 +2215,8 @@ int hp_pifpaf_grow_capacity(hp_pifpaf* p, int flags);
 
 #ifdef HPB_HALO_PHASES
 // instrumented build only (-DHPB_HALO_PHASES, tools/halo_phases.py): the cycle counts conv_halo_kernel has summed since the last
-// reset, in HALO_PH_* order (total, operand A late, operand B late, wgmma wait, epilogue, turn wait); reset != 0 zeroes them after
+// reset, in HALO_PH_* order (total, operand A late, operand B late, wgmma wait, epilogue, turn wait, staging wait); reset != 0 zeroes
+// them after
 int hp_debug_halo_phases(unsigned long long* out, int n, int reset)
 {
     if (!out || n != HALO_PH_COUNT) { set_error("hp_debug_halo_phases: expected %d counters", (int)HALO_PH_COUNT); return HP_ERR_ARG; }

@@ -249,6 +249,9 @@ int hp_engine_debug_run_ops(hp_engine* e, int first_op, int last_op, int N);
  * name[cap]: "conv<f16|tf32|i8,BN[,res][,stem3|stem7]>", "halo<BN[,pool]>", "dw_strip<K,S>", "dw_col", "dw_tma<1|2>", "dw_f32", "dw_i8",
  * "maxpool<K>", "maxpool_f32", "maxpool_i8", "im2col", "im2col_i8", "heads", or "none" for an op that a neighbouring op's launch covers */
 int hp_engine_debug_op_kernel(const hp_engine* e, int op, char* name, int cap);
+/* test hook: *tma_store = 1 when op `op` runs the halo conv kernel with its TMA-store epilogue, 0 otherwise (HPB_HALO_REG_EPILOGUE=1
+ * or a plan the TMA store cannot express: per-thread stores from registers) */
+int hp_engine_debug_op_epilogue(const hp_engine* e, int op, int* tma_store);
 
 /* benchmark hook (SURVEY 8d): after the last conv of every run, copy these DEVICE tensors over the engine's
  * conf/paf outputs, so that random-init weights still give the parser a realistic load.  NULL disables it. */

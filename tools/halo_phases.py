@@ -1,8 +1,9 @@
-"""Where the halo kernel's time goes on cfg3's 3x3 layers (the VGG trunk, cpm_* and init_*), from an instrumented build: builds the
-library with -DHPB_HALO_PHASES into a temporary directory, runs every 3x3 halo layer of bench.py's cfg3 graph on its own at the
-benchmark batch, and prints per layer the consumer warpgroups' clock64 cycles split into waiting for the halo box (A late), waiting for
-a weight tile (B late), waiting in wgmma_wait, the epilogue, waiting for the other warpgroup's turn (ping-pong item only) and the rest
-(issuing MMAs, descriptors, barrier arrives).  Set HPB_HALO_NARROW=1 for the 128-pixel item."""
+"""Where the halo kernel's time goes on a bench.py graph's halo layers (cfg3: the VGG trunk, cpm_*, init_* and the 7x7 refinement
+convs), from an instrumented build: builds the library with -DHPB_HALO_PHASES into a temporary directory, runs every halo layer of
+the graph on its own at the benchmark batch, and prints per layer the consumer warpgroups' clock64 cycles split into waiting for the
+halo box (A late), waiting for a weight tile (B late), waiting in wgmma_wait, the epilogue (accumulators to the output or to the
+staging buffer), waiting for the other warpgroup's turn (ping-pong item only), waiting for a staging buffer the previous TMA store
+still reads, and the rest (issuing MMAs, descriptors, barrier arrives).  Set HPB_HALO_NARROW=1 for the 128-pixel item."""
 import argparse
 import json
 import os
@@ -18,7 +19,7 @@ sys.path.insert(0, ROOT)
 from bench import WORKLOADS  # noqa: E402
 from hyperpose_b200 import build as hb, capi, models, synthetic as syn  # noqa: E402
 
-PHASES = ["total", "a_wait", "b_wait", "mma_wait", "epilogue", "turn_wait"]   # HALO_PH_* order (conv_wgmma.cuh)
+PHASES = ["total", "a_wait", "b_wait", "mma_wait", "epilogue", "turn_wait", "stage_wait"]   # HALO_PH_* order (conv_wgmma.cuh)
 
 
 def read_phases(L, reset=True):
@@ -47,11 +48,11 @@ def main():
     torch.cuda.synchronize()
     print(f"# {torch.cuda.get_device_name()}, {args.workload} batch {B}, HPB_HALO_NARROW={os.environ.get('HPB_HALO_NARROW')}; "
           "share of consumer-warpgroup cycles")
-    print(f"{'layer':<10} {'kernel':<18} {'k-steps':>7} {'Mclk/wg':>8} " + " ".join(f"{p:>9}" for p in PHASES[1:]) + f" {'rest':>6}")
+    print(f"{'layer':<12} {'kernel':<18} {'k-steps':>7} {'Mclk/wg':>8} " + " ".join(f"{p:>9}" for p in PHASES[1:]) + f" {'rest':>6}")
     rows = []
     for i, o in enumerate(g.ops):
         k = eng.debug_op_kernel(i)
-        if not k.startswith("halo<") or o.R != 3:
+        if not k.startswith("halo<"):
             continue
         eng.debug_run_ops(i, i, B)   # warm
         read_phases(L)
@@ -60,10 +61,10 @@ def main():
         ph = read_phases(L)
         tot = ph[0]
         share = ph[1:] / tot
-        ksteps = 9 * ((o.cin_g + 63) // 64)
+        ksteps = o.R * o.R * ((o.cin_g + 63) // 64)
         ctas = torch.cuda.get_device_properties(0).multi_processor_count
         rows.append({"op": o.name, "kernel": k, "ksteps_per_item": ksteps, **{p: round(float(s), 4) for p, s in zip(PHASES[1:], share)}})
-        print(f"{o.name:<10} {k:<18} {ksteps:>7} {tot / args.reps / (2 * ctas) / 1e6:>8.3f} " +
+        print(f"{o.name:<12} {k:<18} {ksteps:>7} {tot / args.reps / (2 * ctas) / 1e6:>8.3f} " +
               " ".join(f"{s:>9.1%}" for s in share) + f" {1 - share.sum():>6.1%}")
     eng.close()
     print(json.dumps({"workload": args.workload, "HPB_HALO_NARROW": os.environ.get("HPB_HALO_NARROW"), "gpu": torch.cuda.get_device_name(),
