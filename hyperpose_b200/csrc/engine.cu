@@ -1468,6 +1468,13 @@ int hp_engine_create_ex(hp_engine** out, const void* pack, size_t pack_bytes, in
             const uint64_t lim = 1u << 16;   // per-dimension bound: keeps the products below 2^64
             const bool dw = po.type == OP_DWCONV;
             const uint64_t G = dw ? 1 : po.groups, co = po.cout_g, ci = dw ? 1 : po.cin_g, R = po.R, S = po.S;
+            // the conv kernels pad R / 2 rows and S / 2 columns before the image: "SAME" ((R - 1) / 2 before) for odd filters only;
+            // an empty filter or channel range would leave the epilogue with accumulators no k-step wrote
+            if (!dw && (G == 0 || co == 0 || ci == 0 || R % 2 == 0 || S % 2 == 0)) {
+                set_error("hp_engine_create: conv op %u has a %ux%u filter, %u groups of %u -> %u channels (the conv kernels take odd "
+                          "filter sizes and at least one group and channel)", i, po.R, po.S, po.groups, po.cin_g, po.cout_g);
+                return HP_ERR_ARG;
+            }
             if (G == 0 || co == 0 || ci == 0 || R == 0 || S == 0 || G > lim || co > lim || ci > lim || R > 15 || S > 15 ||
                 !in_blob(po.w_off, G * co * ci * R * S) || !in_blob(po.b_off, G * co) || !in_blob(po.a_off, G * co)) {
                 set_error("hp_engine_create: op %u names weights outside the pack (groups %u, cout %u, cin %u, %ux%u)", i, po.groups, po.cout_g, po.cin_g, po.R, po.S);

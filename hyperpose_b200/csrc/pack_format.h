@@ -14,7 +14,7 @@ constexpr uint32_t PACK_VERSION = 2;
 enum PackOpType : uint32_t {
     OP_IM2COL3 = 1, // network input (u8 HWC frames or f32 NCHW) -> [N,OH,OW,roundup(R*R*3,64)] fp16: RxRx3 patches (k = (r*R+s)*3+c) + zeros,
                     // minus mean; R in {3,7}, stride 1/2, TF "SAME" padding
-    OP_CONV = 2,    // stride-1 SAME convolution + bias + PReLU (alpha 0 = ReLU, alpha 1 = linear)
+    OP_CONV = 2,    // stride-1 SAME convolution (odd R and S) + bias + PReLU (alpha 0 = ReLU, alpha 1 = linear)
     OP_MAXPOOL2 = 3, // RxR (R = 2 or 3) stride-2 max-pool, TF "SAME" semantics (out = ceil(in/2), window clipped at the border)
     OP_PIFPAF_HEAD = 5, // OpenPifPaf heads: pixel-shuffle(2) + crop + sigmoid/softplus + index grid of the two raw 1x1-conv outputs
                         // (in_buf = pif raw [.,.,340+], res_buf = paf raw [.,.,684+]) -> engine outputs pif[N,17,5,ho,wo], paf[N,19,9,ho,wo]

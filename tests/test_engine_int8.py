@@ -1,6 +1,10 @@
 """The INT8 engine (HP_DTYPE_INT8, data_type::kINT8) against its CPU model (tests/int8_sim.py), byte for byte: every conv kernel
 instantiation and helper kernel in one- or two-op graphs, four whole networks with scales from Engine.calibrate, the calibration
-itself, the packs an INT8 engine refuses, and the pose paths on an INT8 engine."""
+itself, the packs an INT8 engine refuses, and the pose paths on an INT8 engine.
+
+The one-op cases also run every conv kernel with more work items than CTAs (the persistent kernel carries its stage ring from one item
+to the next), the conf / PAF output conv, and batches shorter than the engine's max_batch: there the frames past N of the input
+buffers hold 127, and every byte past frame N, in every buffer and conf / paf plane, must keep its value."""
 import os
 import struct
 import subprocess
@@ -15,7 +19,7 @@ gpu = pytest.mark.gpu
 
 BNS = (16, 32, 48, 64, 96, 128)
 CONV_KERNELS = {f"conv<i8,{b}>" for b in BNS} | {f"conv<i8,{b},res>" for b in BNS}
-BN_OF = {13: 16, 19: 32, 24: 32, 40: 48, 57: 64, 72: 96, 200: 128, 288: 96, 16: 16, 32: 32, 48: 48, 64: 64, 96: 96, 128: 128}
+BN_OF = {13: 16, 19: 32, 24: 32, 40: 48, 57: 64, 72: 96, 160: 96, 200: 128, 288: 96, 16: 16, 32: 32, 48: 48, 64: 64, 96: 96, 128: 128}
 S1, S2, S3 = (2, 13, 21), (3, 5, 7), (1, 40, 72)
 MEAN = (0.41, 0.52, 0.37)
 
@@ -37,13 +41,16 @@ def _nhwc(a):
 
 
 class Case:
-    def __init__(self, cid, shape, graph, kernels, scales, fill=None, entry=None):
+    def __init__(self, cid, shape, graph, kernels, scales, fill=None, entry=None, max_batch=None):
         self.id, self.shape, self.graph, self.kernels, self.scales = cid, shape, graph, kernels, np.asarray(scales, np.float32)
         self.fill = fill or {}   # {buffer: (first channel, value)}
         self.entry = entry       # None (buffers written directly) | "u8" | "f32"
+        self.max_batch = max_batch or shape[0]   # the engine's max_batch_size; the case runs shape[0] frames
+        if self.max_batch != shape[0]:
+            self.id += f"-max{self.max_batch}"
 
 
-def conv_case(cout, cin=64, G=1, R=3, shape=S1, in_off=0, out_off=0, res_mode=0, res_off=0, pad127=False, seed=0):
+def conv_case(cout, cin=64, G=1, R=3, shape=S1, in_off=0, out_off=0, res_mode=0, res_off=0, pad127=False, seed=0, max_batch=None):
     rng = np.random.default_rng(seed)
     g = _graph("conv")
     b_in = g.add_buffer(_r(in_off + G * cin + (16 if in_off else 0), 16), 0)
@@ -59,10 +66,23 @@ def conv_case(cout, cin=64, G=1, R=3, shape=S1, in_off=0, out_off=0, res_mode=0,
     k = f"conv<i8,{BN_OF[cout]}" + (",res>" if res_mode else ">")
     cid = f"{k}-cout{cout}-cin{cin}-G{G}-{R}x{R}-{'x'.join(map(str, shape))}" + (f"-in{in_off}" if in_off else "") + \
           (f"-out{out_off}" if out_off else "") + (f"-res{res_mode}@{res_off}" if res_mode else "") + ("-pad127" if pad127 else "")
-    return Case(cid, shape, g, [k], scales, fill={b_in: (in_off + G * cin, 127)} if pad127 else None)
+    return Case(cid, shape, g, [k], scales, fill={b_in: (in_off + G * cin, 127)} if pad127 else None, max_batch=max_batch)
 
 
-def stem_case(cout, R, stride, shape, entry):
+def split_case(conf, paf, cin, R, shape, max_batch=None, seed=3):
+    """the output conv: conf / paf planes of fp32 y, conf channels first"""
+    rng = np.random.default_rng(seed)
+    g = models.Graph("split", conf_channels=conf, paf_channels=paf, out_down_shift=0, mean=MEAN)
+    b_in = g.add_buffer(_r(cin, 16), 0)
+    co = conf + paf
+    g.add_conv(b_in, 0, (rng.standard_normal((1, co, cin, R, R)) * np.sqrt(2.0 / (cin * R * R))).astype(np.float32),
+               rng.standard_normal(co).astype(np.float32) * 0.5, rng.uniform(-0.5, 1.0, co).astype(np.float32),
+               out_mode=models.OUT_F32_NCHW_SPLIT, split=conf)
+    k = f"conv<i8,{BN_OF[co]}>"
+    return Case(f"{k}-split{conf}+{paf}-cin{cin}-{R}x{R}-{'x'.join(map(str, shape))}", shape, g, [k], [1 / 64], max_batch=max_batch)
+
+
+def stem_case(cout, R, stride, shape, entry, max_batch=None):
     rng = np.random.default_rng(1)
     g = _graph("stem")
     d = 1 if stride == 2 else 0
@@ -72,26 +92,27 @@ def stem_case(cout, R, stride, shape, entry):
     g.add_conv(col, out, (rng.standard_normal((1, cout, 3, R, R)) * np.sqrt(2.0 / (3 * R * R))).astype(np.float32),
                rng.standard_normal(cout).astype(np.float32) * 0.5, rng.uniform(-0.5, 1.0, cout).astype(np.float32), im2col_input=1)
     k = f"conv<i8,{BN_OF[cout]}>"
-    return Case(f"im2col_i8-{entry}-{R}x{R}-s{stride}-{k}-{'x'.join(map(str, shape))}", shape, g, ["im2col_i8", k], [1 / 127, 3 / 127], entry=entry)
+    return Case(f"im2col_i8-{entry}-{R}x{R}-s{stride}-{k}-{'x'.join(map(str, shape))}", shape, g, ["im2col_i8", k], [1 / 127, 3 / 127], entry=entry,
+                max_batch=max_batch)
 
 
-def dw_case(C, K, stride, shape=S1, in_off=16, out_off=8):
+def dw_case(C, K, stride, shape=S1, in_off=16, out_off=8, max_batch=None):
     rng = np.random.default_rng(2)
     g = _graph("dw")
     b_in = g.add_buffer(_r(in_off + C + 8, 8), 0)
     b_out = g.add_buffer(_r(out_off + C + 8, 8), 1 if stride == 2 else 0)
     g.add_dwconv(b_in, b_out, (rng.standard_normal((C, K, K)) * np.sqrt(2.0 / (K * K))).astype(np.float32), rng.standard_normal(C).astype(np.float32) * 0.5,
                  rng.uniform(-0.5, 1.0, C).astype(np.float32), stride=stride, in_ch_off=in_off, out_ch_off=out_off)
-    return Case(f"dw_i8-C{C}-{K}x{K}-s{stride}-{'x'.join(map(str, shape))}", shape, g, ["dw_i8"], [1 / 64, 3 / 127])
+    return Case(f"dw_i8-C{C}-{K}x{K}-s{stride}-{'x'.join(map(str, shape))}", shape, g, ["dw_i8"], [1 / 64, 3 / 127], max_batch=max_batch)
 
 
-def pool_case(C, K, shape=S1, in_off=8, out_off=16):
+def pool_case(C, K, shape=S1, in_off=8, out_off=16, max_batch=None):
     g = _graph("pool")
     b_in = g.add_buffer(_r(in_off + C + 8, 8), 0)
     b_out = g.add_buffer(_r(out_off + C + 8, 8), 1)
     g.add_maxpool(b_in, b_out, C, ksize=K)
     g.ops[-1].in_ch_off, g.ops[-1].out_ch_off = in_off, out_off
-    return Case(f"maxpool_i8-K{K}-C{C}-{'x'.join(map(str, shape))}", shape, g, ["maxpool_i8"], [0.05, 0.05])
+    return Case(f"maxpool_i8-K{K}-C{C}-{'x'.join(map(str, shape))}", shape, g, ["maxpool_i8"], [0.05, 0.05], max_batch=max_batch)
 
 
 def _cases():
@@ -110,10 +131,33 @@ def _cases():
         cs.append(stem_case(57, 7, 2, (1, 40, 72), entry))
     cs += [dw_case(40, k, s) for k in (1, 3) for s in (1, 2)]
     cs += [pool_case(40, 2), pool_case(24, 3), pool_case(40, 3, shape=S3)]
+    # one frame short of max_batch
+    cs += [conv_case(40, 64, 1, 3, S1, max_batch=4), conv_case(64, 64, 1, 1, S2, res_mode=2, res_off=8, max_batch=5),
+           stem_case(40, 3, 1, (2, 13, 21), "u8", max_batch=3), stem_case(57, 7, 2, (1, 40, 72), "f32", max_batch=2),
+           dw_case(40, 3, 1, max_batch=3), dw_case(40, 1, 2, max_batch=3), pool_case(40, 3, max_batch=3)]
+    # the conf / PAF output conv: the split inside the one BN 64 n-tile, and in the second BN 96 n-tile
+    cs += [split_case(19, 38, 64, 1, S1), split_case(19, 38, 64, 3, S1, max_batch=3), split_case(100, 60, 64, 3, S2, max_batch=4)]
     return cs
 
 
 CASES = _cases()
+
+
+def _multi_round():
+    """more items than CTAs (136 .. 272), one frame short of max_batch: all 12 conv kernels, grouped layers, concat offsets, ragged
+    last n-tiles, odd k-step counts (1 x 1 and 3 x 3 over one 128-channel chunk), and the output conv"""
+    cs = []
+    for bn, cout, G, R, shape, out_off in [(16, 13, 4, 1, (3, 40, 72), 8), (32, 24, 1, 3, (1, 130, 140), 0), (48, 40, 2, 3, (2, 45, 97), 0),
+                                           (64, 57, 1, 1, (2, 97, 99), 8), (96, 288, 1, 1, (1, 70, 97), 0), (128, 200, 1, 1, (1, 60, 149), 8)]:
+        cs.append(conv_case(cout, 64, G, R, shape, out_off=out_off, max_batch=shape[0] + 1))
+    for i, (cout, G, R, shape) in enumerate([(16, 4, 3, (3, 40, 72)), (32, 2, 1, (2, 45, 97)), (48, 1, 3, (1, 130, 140)), (64, 1, 1, (2, 97, 99)),
+                                             (96, 2, 1, (2, 60, 72)), (128, 1, 1, (1, 130, 140))]):
+        cs.append(conv_case(cout, 64, G, R, shape, res_mode=1 + i % 2, res_off=(0, 8, 16)[i % 3], out_off=(0, 8)[i % 2], max_batch=shape[0] + 1))
+    cs.append(split_case(19, 38, 64, 1, (2, 97, 99), max_batch=3))
+    return cs
+
+
+MULTI = _multi_round()
 
 
 def _buf_shape(g, bi, N, H, W):
@@ -128,21 +172,29 @@ def _int8_graph(g, scales):
     return g
 
 
-@gpu
-@pytest.mark.parametrize("case", CASES, ids=[c.id for c in CASES])
-def test_int8_kernel(case):
+def _run_int8_case(case):
     g = _int8_graph(case.graph, case.scales)
     N, H, W = case.shape
-    eng = capi.Engine(g.to_pack(), (W, H), max_batch_size=N, dtype="int8")
+    M = case.max_batch
+    split = any(op.type == models.OP_CONV and op.out_mode == models.OUT_F32_NCHW_SPLIT for op in g.ops)
+    eng = capi.Engine(g.to_pack(), (W, H), max_batch_size=M, dtype="int8")
     try:
         names = [eng.debug_op_kernel(i) for i in range(len(g.ops))]
         assert names == case.kernels, names
         rng = np.random.default_rng(7)
+        if split and N < M:   # the planes' frames past N: what a run over all M frames of other contents left there
+            for bi in range(len(g.buffers)):
+                eng.debug_write_buffer(bi, rng.integers(-127, 128, _buf_shape(g, bi, M, H, W)).astype(np.int8))
+            eng.debug_run_ops(0, len(g.ops) - 1, M)
+            planes_before = eng.read_outputs(M)
+        written = {op.out_buf for op in g.ops if not (op.type == models.OP_CONV and op.out_mode == models.OUT_F32_NCHW_SPLIT)}
         init = {}
         for bi in range(len(g.buffers)):   # every buffer: random bytes (the output channels outside the op must keep theirs)
-            a = rng.integers(-127, 128, _buf_shape(g, bi, N, H, W)).astype(np.int8)
+            a = rng.integers(-127, 128, _buf_shape(g, bi, M, H, W)).astype(np.int8)
             if bi in case.fill:
                 a[..., case.fill[bi][0]:] = case.fill[bi][1]
+            if bi not in written:
+                a[N:] = 127    # input frames past N: an output that reads them comes out wrong
             init[bi] = a
             eng.debug_write_buffer(bi, a)
         if case.entry == "u8":
@@ -156,27 +208,62 @@ def test_int8_kernel(case):
         else:
             eng.debug_run_ops(0, len(g.ops) - 1, N)
             kw = dict(N=N, HW=(H, W))
-        _, _, want = int8_sim.run_graph(g, case.scales, init={b: _nchw(a) for b, a in init.items()}, **kw)
+        conf, paf, want = int8_sim.run_graph(g, case.scales, init={b: _nchw(a[:N]) for b, a in init.items()}, **kw)
         for bi in range(len(g.buffers)):
-            got = eng.debug_read_buffer(bi, N)
-            ref = _nhwc(want[bi])
+            full = eng.debug_read_buffer(bi, M)
+            got, ref = full[:N], _nhwc(want[bi])
             bad = np.argwhere(got != ref)
             assert bad.size == 0, f"buffer {bi}: {len(bad)} bytes differ, first at {bad[0].tolist()}: {got[tuple(bad[0])]} != {ref[tuple(bad[0])]}"
+            assert full[N:].tobytes() == init[bi][N:].tobytes(), f"buffer {bi} written past frame {N}"
+        if split:
+            got = eng.read_outputs(M)
+            for name, a, ref in zip(("conf", "paf"), got, (conf, paf)):
+                bad = np.argwhere(a[:N] != ref)
+                assert bad.size == 0, f"{name}: {len(bad)} values differ, first at {bad[0].tolist()}: {a[:N][tuple(bad[0])]} != {ref[tuple(bad[0])]}"
+            if N < M:
+                for name, a, was in zip(("conf", "paf"), got, planes_before):
+                    assert a[N:].tobytes() == was[N:].tobytes(), f"{name} written past frame {N}"
     finally:
         eng.close()
 
 
 @gpu
+@pytest.mark.parametrize("case", CASES, ids=[c.id for c in CASES])
+def test_int8_kernel(case):
+    _run_int8_case(case)
+
+
+@gpu
+@pytest.mark.parametrize("case", MULTI, ids=[c.id for c in MULTI])
+def test_int8_kernel_multi_round(case):
+    """some CTA runs two or more items, and the item count is not a multiple of the grid"""
+    import torch
+    from tests.test_engine_kernels import work_items
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    op = case.graph.ops[0]
+    _, H, W = case.shape
+    items = work_items(case.kernels[0], op, case.shape[0], H, W)
+    grid = min(sms, items)
+    print(f"[int8 rounds] {case.id}: {items} items on {grid} CTAs")
+    assert items > grid and items % grid
+    _run_int8_case(case)
+
+
+@gpu
 def test_int8_conv_inventory():
     """the cases above reach all 12 int8 conv kernels (each case's engine is created here: independent of test order)"""
-    reached = set()
-    for case in CASES:
+    reached, multi = set(), set()
+    for case in CASES + MULTI:
         g = _int8_graph(case.graph, case.scales)
         N, H, W = case.shape
-        eng = capi.Engine(g.to_pack(), (W, H), max_batch_size=N, dtype="int8")
-        reached.update(n for n in (eng.debug_op_kernel(i) for i in range(len(g.ops))) if n.startswith("conv<"))
+        eng = capi.Engine(g.to_pack(), (W, H), max_batch_size=case.max_batch, dtype="int8")
+        names = {n for n in (eng.debug_op_kernel(i) for i in range(len(g.ops))) if n.startswith("conv<")}
         eng.close()
+        reached |= names
+        if case in MULTI:
+            multi |= names
     assert reached == CONV_KERNELS, sorted(CONV_KERNELS - reached)
+    assert multi == CONV_KERNELS, sorted(CONV_KERNELS - multi)
 
 
 # ---- whole networks -------------------------------------------------------------------------------------------------------

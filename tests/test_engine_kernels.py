@@ -9,9 +9,12 @@ Inputs are random values on the operand grid, of either sign, magnitudes around 
       from a magnitude pass of the reference; 2^-23 mag per addition allows two fp32 ulps for the tensor core's alignment and
       truncation; 2^-24 covers fp16 subnormals;
   (b) the channels of the output buffer outside the op's range -- a partial n-tile's pad channels included -- keep their bits;
+  (b') a case may run N frames on an engine built for max_batch > N (the last, short batch of a video): frames N .. max_batch - 1
+      of every input buffer hold NaN, and every byte of those frames, in every buffer and conf / paf plane, must keep its value;
   (c) the bound rejects a wrong reference: with one filter tap zeroed, and with the last output channel's weights replaced by the
       first's, most outputs the mutation changes must break it;
-  (d) the worst |got - ref| / bound of the case is printed.
+  (d) the worst |got - ref| / bound of the case is printed, with the work items and grid of each conv launch (work_items).
+The conf / paf planes of the output conv (OUT_F32_NCHW_SPLIT) hold the unrounded fp32 result: their bound has no 2^-11 |ref| term.
 Max-pool is exact and compared bit for bit."""
 import copy
 import zlib
@@ -48,8 +51,11 @@ def _r(x, m):
 
 
 class Case:
-    def __init__(self, cid, dtype, shape, graph, kernels, outs, K, env=None, stem=False, mutate=0, twin_env=None, fill=None):
+    def __init__(self, cid, dtype, shape, graph, kernels, outs, K, env=None, stem=False, mutate=0, twin_env=None, fill=None, max_batch=None):
         self.id, self.dtype, self.shape, self.graph, self.kernels, self.outs, self.K = cid, dtype, shape, graph, kernels, outs, K
+        self.max_batch = max_batch or shape[0]   # the engine's max_batch_size; the case runs shape[0] frames
+        assert self.max_batch >= shape[0]
+        # outs: (buffer, first channel, channels), or ("conf" | "paf", 0, channels) for a plane of the split output conv
         self.env = env or {}
         self.stem = stem            # the input is u8 frames (infer_u8, then infer_f32 through the im2col buffer)
         self.mutate = mutate        # op whose weights the wrong references change, or None (max-pool)
@@ -61,8 +67,9 @@ def _graph(name):
     return models.Graph(name, conf_channels=19, paf_channels=38, out_down_shift=0, mean=MEAN)
 
 
-def _conv_w(rng, G, co, ci, R):
-    return (rng.standard_normal((G, co, ci, R, R)) * np.sqrt(2.0 / (ci * R * R))).astype(np.float32)
+def _conv_w(rng, G, co, ci, R, S=None):
+    S = S or R
+    return (rng.standard_normal((G, co, ci, R, S)) * np.sqrt(2.0 / (ci * R * S))).astype(np.float32)
 
 
 def _slopes(rng, n, monotone=False):
@@ -70,7 +77,8 @@ def _slopes(rng, n, monotone=False):
 
 
 def conv_case(dtype, cout, cin=64, G=1, R=3, shape=S1, in_off=0, out_off=0, res_mode=0, res_off=0, pad_value=None, kernel=None,
-              env=None, pool=False, seed=0):
+              env=None, pool=False, seed=0, S=None, max_batch=None):
+    S = S or R
     rng = np.random.default_rng(seed)
     chunk = 64 if dtype == "f16" else 32
     g = _graph("conv")
@@ -80,7 +88,7 @@ def conv_case(dtype, cout, cin=64, G=1, R=3, shape=S1, in_off=0, out_off=0, res_
     kw = {}
     if res_mode:
         kw = dict(res_buf=g.add_buffer(_r(res_off + G * cout + 8, 8), 0), res_ch_off=res_off, res_mode=res_mode)
-    g.add_conv(b_in, b_out, _conv_w(rng, G, cout, cin, R), rng.standard_normal(G * cout).astype(np.float32) * 0.5,
+    g.add_conv(b_in, b_out, _conv_w(rng, G, cout, cin, R, S), rng.standard_normal(G * cout).astype(np.float32) * 0.5,
                _slopes(rng, G * cout, monotone=pool), in_ch_off=in_off, out_ch_off=out_off, **kw)
     kernels, outs = [kernel], [(b_out, out_off, G * cout)]
     if pool:
@@ -88,14 +96,15 @@ def conv_case(dtype, cout, cin=64, G=1, R=3, shape=S1, in_off=0, out_off=0, res_
         g.add_maxpool(b_out, b_pool, G * cout)
         g.ops[-1].in_ch_off = g.ops[-1].out_ch_off = out_off
         kernels, outs = [kernel, "none"], [(b_pool, out_off, G * cout)]
-    cid = f"{dtype}-{kernel}-cout{cout}-cin{cin}-G{G}-{R}x{R}-{'x'.join(map(str, shape))}" + (f"-in{in_off}" if in_off else "") + \
-          (f"-out{out_off}" if out_off else "") + (f"-res{res_mode}@{res_off}" if res_mode else "") + (f"-{','.join(f'{k}={v}' for k, v in env.items())}" if env else "")
+    cid = f"{dtype}-{kernel}-cout{cout}-cin{cin}-G{G}-{R}x{S}-{'x'.join(map(str, shape))}" + (f"-in{in_off}" if in_off else "") + \
+          (f"-out{out_off}" if out_off else "") + (f"-res{res_mode}@{res_off}" if res_mode else "") + (f"-{','.join(f'{k}={v}' for k, v in env.items())}" if env else "") + \
+          (f"-max{max_batch}" if max_batch and max_batch != shape[0] else "")
     fill = {b_in: (in_off + G * cin, 3e4 if dtype == "f16" else 1e30)} if pad_value else None
-    return Case(cid, dtype, shape, g, kernels, outs, R * R * _r(cin, chunk), env=env, mutate=0,
-                twin_env={"HPB_NO_POOL_FUSE": "1"} if pool else None, fill=fill)
+    return Case(cid, dtype, shape, g, kernels, outs, R * S * _r(cin, chunk), env=env, mutate=0,
+                twin_env={"HPB_NO_POOL_FUSE": "1"} if pool else None, fill=fill, max_batch=max_batch)
 
 
-def stem_case(cout, R, stride, shape, out_off=0, seed=0):
+def stem_case(cout, R, stride, shape, out_off=0, seed=0, max_batch=None):
     rng = np.random.default_rng(seed)
     g = _graph("stem")
     d = 1 if stride == 2 else 0
@@ -105,11 +114,11 @@ def stem_case(cout, R, stride, shape, out_off=0, seed=0):
     g.add_conv(col, out, _conv_w(rng, 1, cout, 3, R), rng.standard_normal(cout).astype(np.float32) * 0.5, _slopes(rng, cout),
                im2col_input=1, out_ch_off=out_off)
     k = f"conv<f16,{BN_OF[cout]},stem{R}>"
-    return Case(f"f16-{k}-cout{cout}-s{stride}-{'x'.join(map(str, shape))}", "f16", shape, g, ["none", k], [(out, out_off, cout)],
-                _r(R * R * 3, 64), stem=True, mutate=1)
+    return Case(f"f16-{k}-cout{cout}-s{stride}-{'x'.join(map(str, shape))}" + (f"-max{max_batch}" if max_batch else ""), "f16", shape, g,
+                ["none", k], [(out, out_off, cout)], _r(R * R * 3, 64), stem=True, mutate=1, max_batch=max_batch)
 
 
-def dw_case(dtype, C, K, stride, kernel, shape=S1, in_off=8, out_off=16, pair=False, seed=0):
+def dw_case(dtype, C, K, stride, kernel, shape=S1, in_off=8, out_off=16, pair=False, seed=0, max_batch=None):
     rng = np.random.default_rng(seed)
     g = _graph("dw")
     b_in = g.add_buffer(_r(in_off + C + 8, 8), 0)
@@ -121,16 +130,18 @@ def dw_case(dtype, C, K, stride, kernel, shape=S1, in_off=8, out_off=16, pair=Fa
                      in_ch_off=in_off, out_ch_off=out_off + j * C)
         outs.append((b_out, out_off + j * C, C))
     kernels = [kernel, "none"] if pair else [kernel]
-    return Case(f"{dtype}-{kernel}-C{C}-{K}x{K}-s{stride}-{'x'.join(map(str, shape))}", dtype, shape, g, kernels, outs, K * K, mutate=0)
+    return Case(f"{dtype}-{kernel}-C{C}-{K}x{K}-s{stride}-{'x'.join(map(str, shape))}" + (f"-max{max_batch}" if max_batch else ""), dtype, shape,
+                g, kernels, outs, K * K, mutate=0, max_batch=max_batch)
 
 
-def pool_case(dtype, C, K, kernel, shape=S1, in_off=8, out_off=16):
+def pool_case(dtype, C, K, kernel, shape=S1, in_off=8, out_off=16, max_batch=None):
     g = _graph("pool")
     b_in = g.add_buffer(_r(in_off + C + 8, 8), 0)
     b_out = g.add_buffer(_r(out_off + C + 8, 8), 1)
     g.add_maxpool(b_in, b_out, C, ksize=K)
     g.ops[-1].in_ch_off, g.ops[-1].out_ch_off = in_off, out_off
-    return Case(f"{dtype}-{kernel}-C{C}-{'x'.join(map(str, shape))}", dtype, shape, g, [kernel], [(b_out, out_off, C)], 0, mutate=None)
+    return Case(f"{dtype}-{kernel}-C{C}-{'x'.join(map(str, shape))}" + (f"-max{max_batch}" if max_batch else ""), dtype, shape, g, [kernel],
+                [(b_out, out_off, C)], 0, mutate=None, max_batch=max_batch)
 
 
 def _cases():
@@ -176,24 +187,58 @@ def _engine(case, monkeypatch, env=None):
     for k, v in {**case.env, **(env or {})}.items():
         monkeypatch.setenv(k, v)
     N, H, W = case.shape
-    return capi.Engine(case.graph.to_pack(), (W, H), max_batch_size=N, dtype=case.dtype)
+    return capi.Engine(case.graph.to_pack(), (W, H), max_batch_size=case.max_batch, dtype=case.dtype)
 
 
 def _buf_shape(case, bi):
+    """a buffer's NHWC shape over all max_batch frames"""
     N, H, W = case.shape
     c, d = case.graph.buffers[bi]
     for _ in range(d):
         H, W = (H + 1) // 2, (W + 1) // 2
-    return N, H, W, c
+    return case.max_batch, H, W, c
+
+
+def work_items(kernel, op, N, H, W):
+    """work items of a conv launch over N frames of an H x W input (engine.cu, launch_conv): conv_wgmma_kernel takes
+    ceil(N H W / 128) pixel tiles x groups x n-tiles; the halo kernel T x groups x n-tiles, T = N ceil(H / 16) ceil(W / 8) 16 x 8
+    tiles, or ceil(T / 2) tile pairs for the wide item.  A CTA runs items blockIdx.x, + gridDim.x, ... (the ping-pong item hands them
+    to its two warpgroups in turn)"""
+    args = kernel[kernel.index("<") + 1:-1].split(",")
+    if kernel.startswith("conv<"):
+        bn, m = int(args[1]), -(-N * H * W // 128)
+    else:
+        bn, m = int(args[0]), N * -(-H // 16) * -(-W // 8)
+        if "wide" in args:
+            m = -(-m // 2)
+    return m * op.groups * -(-op.cout_g // bn)
+
+
+def conv_launches(case):
+    """[(op, kernel, items, grid)] of the case's conv launches; grid = min(SMs, items)"""
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    out = []
+    for i, (op, k) in enumerate(zip(case.graph.ops, case.kernels)):
+        if k.startswith(("conv<", "halo<")):
+            _, H, W, _ = _buf_shape(case, op.in_buf)
+            items = work_items(k, op, case.shape[0], H, W)
+            out.append((i, k, items, min(sms, items)))
+    return out
 
 
 def _on_grid(x, dtype):
     return x.astype(np.float16) if dtype == "f16" else torch_backbone.tf32_round(torch.from_numpy(x.astype(np.float32))).numpy()
 
 
-def _inputs(case, rng):
-    """NHWC contents of every buffer: random operands on the grid, sentinels in the output buffers"""
-    written = {o[0] for o in case.outs}
+def _planes(case):
+    return [o for o in case.outs if isinstance(o[0], str)]
+
+
+def _inputs(case, rng, written=None):
+    """NHWC contents of every buffer over all max_batch frames: random operands on the grid, sentinels in the output buffers, NaN in
+    the frames past the run's N of every other buffer"""
+    N = case.shape[0]
+    written = {o[0] for o in case.outs} if written is None else written
     data = {}
     for bi in range(len(case.graph.buffers)):
         shp = _buf_shape(case, bi)
@@ -205,15 +250,33 @@ def _inputs(case, rng):
             x = -np.abs(x) - 0.25       # all negative: a window padded with zeros instead of -inf is caught at the borders
         if bi in case.fill:
             x[..., case.fill[bi][0]:] = case.fill[bi][1]
+        x[N:] = np.nan
         data[bi] = _on_grid(x, case.dtype)
     return data
 
 
+def _read_all(eng, case, n):
+    """n frames of every buffer the engine keeps in memory (a buffer whose consumer runs in the producer's epilogue is never
+    written) and, when the case writes them, of the conf / paf planes (NHWC)"""
+    out = {}
+    for bi in range(len(case.graph.buffers)):
+        try:
+            out[bi] = eng.debug_read_buffer(bi, n)
+        except capi.HyperposeError as e:
+            assert e.status == capi.HP_ERR_UNSUPPORTED and "not materialised" in str(e), str(e)
+    if _planes(case):
+        conf, paf = eng.read_outputs(n)
+        out["conf"], out["paf"] = conf.transpose(0, 2, 3, 1), paf.transpose(0, 2, 3, 1)
+    return out
+
+
 def _reference(case, g, data, frames, magnitude=False):
-    init = {bi: a.astype(np.float64).transpose(0, 3, 1, 2) for bi, a in data.items()}
-    _, _, bufs = torch_backbone.run_graph(g, frames, device="cpu", dtype=torch.float64, init=init,
-                                          rounding="fp16" if case.dtype == "f16" else "tf32", round_stores=False, magnitude=magnitude)
-    return [bufs[b][:, off:off + c].numpy().transpose(0, 2, 3, 1) for b, off, c in case.outs]
+    N = case.shape[0]
+    init = {bi: a[:N].astype(np.float64).transpose(0, 3, 1, 2) for bi, a in data.items()}
+    conf, paf, bufs = torch_backbone.run_graph(g, frames, device="cpu", dtype=torch.float64, init=init,
+                                               rounding="fp16" if case.dtype == "f16" else "tf32", round_stores=False, magnitude=magnitude)
+    src = {"conf": conf, "paf": paf}
+    return [(src[b] if isinstance(b, str) else bufs[b])[:, off:off + c].numpy().transpose(0, 2, 3, 1) for b, off, c in case.outs]
 
 
 def _mutants(case):
@@ -225,10 +288,10 @@ def _mutants(case):
         op = g.ops[case.mutate]
         w = op.weight if op.type == models.OP_CONV else op.weight[None]     # [G, cout, cin, R, S] / [1, C, K, K]
         if kind == "tap":
-            if op.type == models.OP_CONV and op.R == 1:
+            if op.type == models.OP_CONV and w.shape[-2:] == (1, 1):
                 w[:, :, -8:] = 0
             else:
-                w[..., op.R // 2, op.R // 2] = 0
+                w[..., w.shape[-2] // 2, w.shape[-1] // 2] = 0
         else:
             w[-1, -1] = w[-1, 0]
         out.append((kind, g))
@@ -237,12 +300,22 @@ def _mutants(case):
 
 def _run_and_check(case, monkeypatch, rng):
     N, H, W = case.shape
+    M = case.max_batch
     eng = _engine(case, monkeypatch)
     assert [eng.debug_op_kernel(i) for i in range(len(case.graph.ops))] == case.kernels
+    launches = conv_launches(case)
     data = _inputs(case, rng)
     frames = rng.integers(0, 256, (N, H, W, 3), dtype=np.uint8)
+    # the planes' frames past N: what a run over all max_batch frames of other (finite) contents left there
+    before = {bi: _on_grid(rng.standard_normal(_buf_shape(case, bi)), case.dtype) for bi in data} if _planes(case) and N < M else None
 
     def run(entry):
+        planes_before = None
+        if before is not None:
+            for bi, a in before.items():
+                eng.debug_write_buffer(bi, a)
+            eng.debug_run_ops(0, len(case.graph.ops) - 1, M)
+            planes_before = _read_all(eng, case, M)
         for bi, a in data.items():
             eng.debug_write_buffer(bi, a)
         if entry == "u8":
@@ -252,7 +325,13 @@ def _run_and_check(case, monkeypatch, rng):
             eng.infer_f32(np.ascontiguousarray(x))
         else:
             eng.debug_run_ops(0, len(case.graph.ops) - 1, N)
-        return {b: eng.debug_read_buffer(b, N) for b in {o[0] for o in case.outs}}
+        full = _read_all(eng, case, M)
+        # (b') frames N .. max_batch - 1 keep their bytes
+        for b, a in full.items():
+            if N < M:
+                was = planes_before[b] if isinstance(b, str) else data[b]
+                assert a[N:].tobytes() == was[N:].tobytes(), f"{case.id} ({entry}): {b} written past frame {N}"
+        return {o[0]: full[o[0]][:N] for o in case.outs}
 
     runs = {e: run(e) for e in (("u8", "f32") if case.stem else ("ops",))}
     if case.twin_env:
@@ -261,18 +340,21 @@ def _run_and_check(case, monkeypatch, rng):
         eng = twin
         twin_out = run("ops")
         for b, a in runs["ops"].items():
-            assert a.tobytes() == twin_out[b].tobytes(), f"{case.id}: buffer {b} differs under {case.twin_env}"
+            assert a.tobytes() == twin_out[b].tobytes(), f"{case.id}: {b} differs under {case.twin_env}"
     eng.close()
 
     # (b) channels outside the op's range keep their bits
     for entry, got in runs.items():
         for b, a in got.items():
+            if isinstance(b, str):
+                continue
             keep = np.ones(a.shape[-1], bool)
             for ob, off, c in case.outs:
                 if ob == b:
                     keep[off:off + c] = False
-            assert a[..., keep].tobytes() == data[b][..., keep].tobytes(), f"{case.id} ({entry}): channels outside the output range were written"
+            assert a[..., keep].tobytes() == data[b][:N][..., keep].tobytes(), f"{case.id} ({entry}): channels outside the output range were written"
 
+    shown = ", ".join(f"op {i} {k}: {items} items on {grid} CTAs" for i, k, items, grid in launches)
     ref = _reference(case, case.graph, data, frames)
     if case.mutate is None:   # max-pool: exact
         for entry, got in runs.items():
@@ -282,15 +364,17 @@ def _run_and_check(case, monkeypatch, rng):
         print(f"[kernel bound] {case.id}: {case.kernels[0]} bit-exact")
         return 0.0
     mag = _reference(case, case.graph, data, frames, magnitude=True)
-    bound = [2.0 ** -11 * np.abs(r) + (case.K + 2) * 2.0 ** -23 * m + 2.0 ** -24 for r, m in zip(ref, mag)]
+    # the fp16 / TF32 buffers hold the result rounded once more (2^-11 |ref|); the conf / paf planes hold it unrounded
+    bound = [(0.0 if isinstance(o[0], str) else 2.0 ** -11) * np.abs(r) + (case.K + 2) * 2.0 ** -23 * m + 2.0 ** -24
+             for o, r, m in zip(case.outs, ref, mag)]
     worst = 0.0
     for entry, got in runs.items():
         for (b, off, c), r, bd in zip(case.outs, ref, bound):
             g64 = got[b][..., off:off + c].astype(np.float64)
-            assert np.isfinite(g64).all(), f"{case.id} ({entry}): non-finite output"
+            assert np.isfinite(g64).all(), f"{case.id} ({entry}): non-finite output at {np.argwhere(~np.isfinite(g64))[0].tolist()}"
             ratio = np.abs(g64 - r) / bd
             i = np.unravel_index(np.argmax(ratio), ratio.shape)
-            assert ratio[i] <= 1.0, f"{case.id} ({entry}): |got - ref| = {abs(g64[i] - r[i]):.3e} > bound {bd[i]:.3e} at {i} (got {g64[i]}, ref {r[i]})"
+            assert ratio[i] <= 1.0, f"{case.id} ({entry}): {b}: |got - ref| = {abs(g64[i] - r[i]):.3e} > bound {bd[i]:.3e} at {i} (got {g64[i]}, ref {r[i]})"
             worst = max(worst, float(ratio.max()))
         # (c) the bound rejects wrong references
         for kind, mg in _mutants(case):
@@ -303,7 +387,7 @@ def _run_and_check(case, monkeypatch, rng):
                 broken += int((np.abs(g64 - mr) > bd)[ch].sum())
             assert changed > 0, f"{case.id}: the {kind} mutation changes nothing"
             assert broken > 0.5 * changed, f"{case.id} ({entry}): the bound accepts the {kind}-mutated reference on {changed - broken} of {changed} changed outputs"
-    print(f"[kernel bound] {case.id}: {case.kernels} worst |got - ref| / bound {worst:.3f}")
+    print(f"[kernel bound] {case.id}: {case.kernels} worst |got - ref| / bound {worst:.3f}; {shown}")
     return worst
 
 
