@@ -412,6 +412,24 @@ __device__ __forceinline__ PixelPos unflatten(const ConvParams& p, int px)
     return q;
 }
 
+// position in a ring of mbarrier-guarded buffers: the slot, and the parity of the phase its barriers are in.  (The member order
+// steers ptxas's register assignment: phase first compiles conv_wgmma_kernel's producer and consumer loops to the same SASS as two
+// separate counters.)
+struct RingPos {
+    uint32_t phase = 0;
+    int slot = 0;
+    __device__ __forceinline__ void step(int depth)
+    {
+        if (++slot == depth) { slot = 0; phase ^= 1; }
+    }
+    __device__ __forceinline__ void advance(int n, int depth)
+    {
+        slot += n;
+        phase ^= (uint32_t)(slot / depth) & 1u;
+        slot %= depth;
+    }
+};
+
 // One thread per (output pixel, 64-channel chunk): gathers the RxRx3 neighbourhood (k = (r*R+s)*3 + c, c = model channel)
 // into roundup(R*R*3, 64) fp16 channels.  SAME padding pads the *normalised* input with zeros.
 //   u8 path : v = (float)((double)u8 * factor) (data.cpp:48); model channel c reads byte (flip ? 2-c : c)
@@ -499,6 +517,7 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
             // ===================== u8 patch gather (one pixel row of the A tile per thread) + weight TMA =====================
             const int row = threadIdx.x;
             const int total_px = p.Nb * p.H * p.W;
+            // two counters rather than a RingPos: with the struct, ptxas gives conv_wgmma_kernel<__half, 96, false, 3> two more registers
             int stage = 0;
             uint32_t phase = 0;
             for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
@@ -536,8 +555,7 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
     if (wg == 0) {
         // ===================== TMA producer =====================
         if (warp == 0 && ptx::elect_one()) {
-            int stage = 0;
-            uint32_t phase = 0;
+            RingPos ring;
             const int pad_h = p.R / 2, pad_w = p.S / 2;
             for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
                 const ConvTile t = decode_tile(p, tile, n_tiles_g);
@@ -548,13 +566,13 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
                 for (int r = 0; r < p.R; ++r)
                     for (int s = 0; s < p.S; ++s)
                         for (int c = 0; c < chunks; ++c, kcol += BK) {
-                            ptx::mbar_wait(ptx::smem_u32(empty_bar + stage), phase ^ 1);
-                            const uint32_t fb = ptx::smem_u32(full_bar + stage);
-                            uint8_t* sa = smem + (size_t)stage * STAGE_BYTES;
+                            ptx::mbar_wait(ptx::smem_u32(empty_bar + ring.slot), ring.phase ^ 1);
+                            const uint32_t fb = ptx::smem_u32(full_bar + ring.slot);
+                            uint8_t* sa = smem + (size_t)ring.slot * STAGE_BYTES;
                             ptx::mbar_expect_tx(fb, (uint32_t)STAGE_BYTES);
                             ptx::tma_load_im2col_4d(ptx::smem_u32(sa), &tmap_a, fb, a_ch0 + c * BK, q0.w - pad_w, q0.h - pad_h, q0.n, s, r);
                             ptx::tma_load_2d(ptx::smem_u32(sa + CONV_A_BYTES), &tmap_b, fb, kcol, b_row);
-                            if (++stage == p.num_stages) { stage = 0; phase ^= 1; }
+                            ring.step(p.num_stages);
                         }
             }
         }
@@ -568,15 +586,14 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
     const int total_px = p.Nb * p.H * p.W;
     const uint32_t smem0 = ptx::smem_u32(smem);
     typename ConvAcc<T>::type acc[BN / 2];
-    int stage = 0;
-    uint32_t phase = 0;
+    RingPos ring;
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
         const ConvTile t = decode_tile(p, tile, n_tiles_g);
         int prev = 0;
         for (int ks = 0; ks < ksteps; ++ks) {
-            const uint32_t sa = smem0 + (uint32_t)(stage * STAGE_BYTES);
+            const uint32_t sa = smem0 + (uint32_t)(ring.slot * STAGE_BYTES);
             const uint64_t da = ptx::make_sw128_kmajor_desc(sa + (uint32_t)(half * 64 * 128)), db = ptx::make_sw128_kmajor_desc(sa + CONV_A_BYTES);
-            ptx::mbar_wait(ptx::smem_u32(full_bar + stage), phase);
+            ptx::mbar_wait(ptx::smem_u32(full_bar + ring.slot), ring.phase);
             ptx::fence_acc(acc);
             ptx::wgmma_fence();
 #pragma unroll
@@ -588,8 +605,8 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
                 ptx::wgmma_wait<1>();
                 if (lane == 0) ptx::mbar_arrive(ptx::smem_u32(empty_bar + prev));
             }
-            prev = stage;
-            if (++stage == p.num_stages) { stage = 0; phase ^= 1; }
+            prev = ring.slot;
+            ring.step(p.num_stages);
         }
         ptx::wgmma_wait<0>();
         ptx::fence_acc(acc);
@@ -726,9 +743,8 @@ inline int conv_pick_stages(int BN)
 // required), so fp16(act(max(v) + b)) == max(fp16(act(v + b))) bit for bit.
 // ---------------------------------------------------------------------------------------------
 constexpr int HALO_TH = 16, HALO_TW = 8;
-constexpr int HALO_BOXES = 2;
 
-// kWide: a work item is TWO consecutive 16 x 8 tiles of the same grid (tiles 2i and 2i + 1 in (image, ty, tx) order, each with its
+// The wide item (HaloItem::Wide): a work item is TWO consecutive 16 x 8 tiles of the same grid (tiles 2i and 2i + 1 in (image, ty, tx) order, each with its
 // own halo box, so a pair may straddle two rows or two frames) x one n-tile.  Warpgroup 1 computes all 128 pixels of the first tile,
 // warpgroup 2 those of the second (two m64 accumulator blocks each: tile rows 0-7 and 8-15), and both read the same weight stage: one
 // 16 KiB weight tile, one full-barrier wait and one release serve 256 x 128 x 64 MACs instead of 128 x 128 x 64.  Every accumulator
@@ -738,15 +754,14 @@ constexpr int HALO_BOXES = 2;
 // (out-of-tensor rows are zero-filled, or a frame beyond N of the max-batch buffer) and computed, and its epilogue is skipped.
 constexpr int HALO_WIDE_PRODUCER_REGS = 40, HALO_WIDE_CONSUMER_REGS = 232;
 
-// kPP ("ping-pong", 3x3 layers): a work item is one 16 x 8 tile x one n-tile, as in the 128-pixel item, but ONE warpgroup computes
+// The ping-pong item (HaloItem::PingPong, 3x3 layers): a work item is one 16 x 8 tile x one n-tile, as in the 128-pixel item, but ONE warpgroup computes
 // all of it (two m64 blocks, tile rows 0-7 and 8-15, the same accumulators and register split as the wide item).  A CTA's items
 // alternate between warpgroups 1 and 2, and both consume the producer's box and weight rings in the CTA's item order.  Two turn
 // barriers pass the tensor pipe back and forth: a warpgroup starts an item's MMAs once the other has ISSUED (not finished) its
 // previous item's, so the pipe does not drain at the hand-off, and each warpgroup's final wait and epilogue run under the other's
 // main loop.  Within an item nothing drains at a chunk boundary: box c is released after the first wait<1> of chunk c + 1, which
-// has seen every MMA of chunk c complete; the box ring (HALO_PP_BOXES) keeps the producer a chunk ahead.  Every accumulator row sees
+// has seen every MMA of chunk c complete; the box ring's four slots keep the producer a chunk ahead.  Every accumulator row sees
 // the same (chunk, tap, k16) wgmma sequence as in the 128-pixel item, so the outputs are identical.
-constexpr int HALO_PP_BOXES = 4;
 
 #ifdef HPB_HALO_PHASES
 // instrumented build (tools/halo_phases.py): clock64 cycles of every consumer warpgroup, summed over the CTAs of all halo launches.
@@ -781,13 +796,27 @@ struct HaloParams {
     int stage_bytes;            // tma_store: each consumer warpgroup's staging region (halo_stage_bytes; 0 on the wide item)
 };
 
-// the work item of conv_halo_kernel: one 16 x 8 tile on both consumer warpgroups, two tiles (kWide), or one tile on one warpgroup (kPP)
+// the work item of conv_halo_kernel: one 16 x 8 tile on both consumer warpgroups (the 128-pixel item), two tiles (Wide), or one tile
+// on one warpgroup (PingPong)
 enum class HaloItem { Narrow, Wide, PingPong };
-// staging slots of one consumer warpgroup for the TMA-store epilogue, BN x 128 B each (one m64 block): the wide item stages its two
-// blocks in its own box of the item's last chunk; the ping-pong item at BN = 128 stores its two blocks through one 16 KiB slot in
-// turn (a full 32 KiB per warpgroup would cost two more of its weight stages)
-__host__ __device__ constexpr int halo_stage_slots(int BN, HaloItem it) { return it == HaloItem::Wide || (it == HaloItem::PingPong && BN == 64) ? 2 : 1; }
-inline int halo_stage_bytes(int BN, HaloItem it) { return it == HaloItem::Wide ? 0 : halo_stage_slots(BN, it) * BN * 128; }
+// What an item is made of.  The kernel's loops and shared-memory layout and the host's sizing of that memory all read it from here.
+struct HaloShape {
+    int tiles;         // 16 x 8 tiles per item = halo boxes per box slot
+    int blocks;        // m64 accumulator blocks per consumer warpgroup
+    int box_slots;     // box ring depth
+    int slot_warps;    // consumer warps that read (and release) one box slot / weight stage
+    int stage_slots;   // staging slots of one consumer warpgroup for the TMA-store epilogue, BN x 128 B each (one m64 block)
+    bool move_regs;    // setmaxnreg moves registers from the producer warpgroup to the consumers (HALO_WIDE_*_REGS)
+};
+// The wide item stages its two blocks in its own box of the item's last chunk, so it has no staging slots; the ping-pong item at
+// BN = 128 stores its two blocks through one 16 KiB slot in turn (a full 32 KiB per warpgroup would cost two more of its weight stages).
+__host__ __device__ constexpr HaloShape halo_shape(HaloItem it, int BN)
+{
+    return it == HaloItem::Wide       ? HaloShape{ 2, 2, 2, 8, 0, true }
+           : it == HaloItem::PingPong ? HaloShape{ 1, 2, 4, 4, BN == 64 ? 2 : 1, true }
+                                      : HaloShape{ 1, 1, 2, 8, 1, false };
+}
+inline int halo_stage_bytes(int BN, HaloItem it) { return halo_shape(it, BN).stage_slots * BN * 128; }
 
 namespace ptx {
 // K-major 128B-swizzled operand whose 8-row groups are `sbo` bytes apart and whose start need not be 1024-byte aligned.  The swizzle
@@ -973,39 +1002,84 @@ __device__ __forceinline__ void halo_epilogue_tma(const float (&acc)[kBlocks][BN
     }
 }
 
-template <int BN, bool kPool, bool kWide = false, bool kPP = false>
+// One k-step (chunk, tap (r, s)) of a consumer warpgroup: m64 block m, the tile rows 8 m .. 8 m + 7 below the box row at `abase`,
+// times the weight tile in slot b.slot of the ring, once that slot's full barrier has completed phase b.phase.  The first k-step of
+// an item (c | tap == 0) overwrites the accumulators.
+template <int BN, int kBlocks>
+__device__ __forceinline__ void halo_kstep(float (&acc)[kBlocks][BN / 2], uint32_t abase, int r, int s, int BW, uint32_t sbo, const uint8_t* s_b,
+                                           uint64_t* b_full, RingPos b, int c_or_tap HALO_PH_PARAM)
+{
+    uint64_t da[kBlocks];
+#pragma unroll
+    for (int m = 0; m < kBlocks; ++m) da[m] = ptx::make_sw128_kmajor_desc_at(abase + (uint32_t)(((m * 8 + r) * BW + s) * 128), sbo);
+    const uint64_t db = ptx::make_sw128_kmajor_desc(ptx::smem_u32(s_b + (size_t)b.slot * BN * 128));
+    HALO_TIMED(HALO_PH_B_WAIT, ptx::mbar_wait(ptx::smem_u32(b_full + b.slot), b.phase));
+#pragma unroll
+    for (int m = 0; m < kBlocks; ++m) ptx::fence_acc(acc[m]);
+    ptx::wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < 4; ++k)
+#pragma unroll
+        for (int m = 0; m < kBlocks; ++m)
+            ptx::wgmma<__half, BN>(acc[m], da[m] + (uint64_t)(k * 2), db + (uint64_t)(k * 2), (c_or_tap | k) != 0 ? 1u : 0u);
+    ptx::wgmma_commit();
+#pragma unroll
+    for (int m = 0; m < kBlocks; ++m) ptx::fence_acc(acc[m]);
+}
+
+// The epilogue of one warpgroup's share of an item: with `tma` (p.tma_store, at a width with a TMA form) halo_epilogue_tma through
+// the staging slots at `stage`, else halo_epilogue from registers.  The wide item's `stage` is its own box of the item's last chunk:
+// a 7x7 box (39 KiB) holds both m64 blocks at once, a smaller one (3x3: 23 KiB) one block at a time.
+template <int BN, bool kPool, HaloItem kItem>
+__device__ __forceinline__ void halo_store(const float (&acc)[halo_shape(kItem, BN).blocks][BN / 2], const HaloParams& p, const CUtensorMap* tmap_o,
+                                           bool tma, uint32_t stage, int n, int y0, int x0, int g, int n0, int row_base, int warp, int lane,
+                                           bool leader HALO_PH_PARAM)
+{
+    constexpr HaloShape kShape = halo_shape(kItem, BN);
+    if constexpr (BN % 64 == 0) {
+        if (tma) {
+            if constexpr (kItem != HaloItem::Wide)
+                halo_epilogue_tma<BN, kPool, kShape.blocks, kShape.stage_slots, true>(acc, p, tmap_o, stage, n, y0, x0, g, n0, row_base, warp, lane,
+                                                                                     leader HALO_PH_ARG);
+            else if (p.box_bytes >= kShape.blocks * BN * 128)
+                halo_epilogue_tma<BN, kPool, kShape.blocks, kShape.blocks, false>(acc, p, tmap_o, stage, n, y0, x0, g, n0, row_base, warp, lane,
+                                                                                 leader HALO_PH_ARG);
+            else
+                halo_epilogue_tma<BN, kPool, kShape.blocks, 1, true>(acc, p, tmap_o, stage, n, y0, x0, g, n0, row_base, warp, lane, leader HALO_PH_ARG);
+            return;
+        }
+    }
+    halo_epilogue<BN, kPool, kShape.blocks>(acc, p, n, y0, x0, g, n0, row_base, warp, lane);
+}
+
+template <int BN, bool kPool, HaloItem kItem>
 __global__ void __launch_bounds__(CONV_THREADS, 1)
 conv_halo_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_b, const __grid_constant__ CUtensorMap tmap_o,
                  const HaloParams p)
 {
-    static_assert(!(kWide && kPool), "the pooled epilogue pairs pixel rows of one m64 block; it has no wide form");
-    static_assert(!(kWide && kPP), "an item is either two tiles on two warpgroups or one tile on one warpgroup");
-    static_assert(!kPP || BN == 64 || BN == 128, "the ping-pong item is built for the VGG trunk's widths, BN = 64 and 128");
+    static_assert(!(kItem == HaloItem::Wide && kPool), "the pooled epilogue pairs pixel rows of one m64 block; it has no wide form");
+    static_assert(kItem != HaloItem::PingPong || BN == 64 || BN == 128, "the ping-pong item is built for the VGG trunk's widths, BN = 64 and 128");
+    constexpr HaloShape kShape = halo_shape(kItem, BN);
     constexpr int B_BYTES = BN * 128;
-    constexpr int kTiles = kWide ? 2 : 1;   // spatial tiles per item = boxes per box slot
-    constexpr int kBlocks = kWide || kPP ? 2 : 1;   // m64 accumulator blocks per warpgroup
-    constexpr int kBoxSlots = kPP ? HALO_PP_BOXES : HALO_BOXES;
-    constexpr int kWarpsPerSlot = kPP ? 4 : 8;   // consumer warps that read (and release) one box slot / weight stage
-    constexpr int kStageSlots = halo_stage_slots(BN, kWide ? HaloItem::Wide : kPP ? HaloItem::PingPong : HaloItem::Narrow);
     // the TMA-store epilogue (p.tma_store) exists for BN = 64 and 128; other widths always take halo_epilogue
     constexpr bool kTmaForm = BN % 64 == 0;
     extern __shared__ uint8_t smem_raw[];
     ptx::pdl_launch_dependents();
     uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-    uint8_t* s_box = smem;                                                   // [kBoxSlots][kTiles][box_bytes]
-    uint8_t* s_b = s_box + (size_t)kBoxSlots * kTiles * p.box_bytes;         // [num_stages][BN x 128 B]
-    uint8_t* s_stage = s_b + (size_t)p.num_stages * B_BYTES;                 // [2][stage_bytes]: TMA-store staging per consumer warpgroup
-    uint64_t* a_full = (uint64_t*)(s_stage + 2 * (size_t)p.stage_bytes);     // [kBoxSlots]
-    uint64_t* a_empty = a_full + kBoxSlots;
-    uint64_t* b_full = a_empty + kBoxSlots;                                  // [CONV_MAX_STAGES]
+    uint8_t* s_box = smem;                                                           // [box_slots][tiles][box_bytes]
+    uint8_t* s_b = s_box + (size_t)kShape.box_slots * kShape.tiles * p.box_bytes;    // [num_stages][BN x 128 B]
+    uint8_t* s_stage = s_b + (size_t)p.num_stages * B_BYTES;                         // [2][stage_bytes]: TMA-store staging per consumer warpgroup
+    uint64_t* a_full = (uint64_t*)(s_stage + 2 * (size_t)p.stage_bytes);             // [box_slots]
+    uint64_t* a_empty = a_full + kShape.box_slots;
+    uint64_t* b_full = a_empty + kShape.box_slots;                                   // [CONV_MAX_STAGES]
     uint64_t* b_empty = b_full + CONV_MAX_STAGES;
-    uint64_t* turn = b_empty + CONV_MAX_STAGES;                              // kPP: [2], warpgroup 1 + i may start its next item
+    uint64_t* turn = b_empty + CONV_MAX_STAGES;                                      // ping-pong item: [2], warpgroup 1 + i may start its next item
 
     const int wg = threadIdx.x >> 7, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int n_tiles_g = p.cout_g_pad / BN;
     const int nt_total = p.groups * n_tiles_g;
     const int sp_per_img = p.tiles_x * p.tiles_y;
-    const int total_items = (p.Nb * sp_per_img + kTiles - 1) / kTiles * nt_total;
+    const int total_items = (p.Nb * sp_per_img + kShape.tiles - 1) / kShape.tiles * nt_total;
     const int chunks = p.cin_g / CONV_BLOCK_K;
     const int taps = p.R * p.S;
     const int BW = HALO_TW + p.S - 1, BH = HALO_TH + p.R - 1;
@@ -1014,15 +1088,15 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_consta
         ptx::prefetch_tmap(&tmap_x);
         ptx::prefetch_tmap(&tmap_b);
         if (kTmaForm && p.tma_store) ptx::prefetch_tmap(&tmap_o);
-        for (int i = 0; i < kBoxSlots; ++i) {
+        for (int i = 0; i < kShape.box_slots; ++i) {
             ptx::mbar_init(ptx::smem_u32(a_full + i), 1);
-            ptx::mbar_init(ptx::smem_u32(a_empty + i), kWarpsPerSlot);   // one arrive per consumer warp that reads it
+            ptx::mbar_init(ptx::smem_u32(a_empty + i), kShape.slot_warps);   // one arrive per consumer warp that reads it
         }
         for (int i = 0; i < p.num_stages; ++i) {
             ptx::mbar_init(ptx::smem_u32(b_full + i), 1);
-            ptx::mbar_init(ptx::smem_u32(b_empty + i), kWarpsPerSlot);
+            ptx::mbar_init(ptx::smem_u32(b_empty + i), kShape.slot_warps);
         }
-        if constexpr (kPP) {
+        if constexpr (kItem == HaloItem::PingPong) {
             ptx::mbar_init(ptx::smem_u32(turn), 4);       // one arrive per warp of the warpgroup that hands over
             ptx::mbar_init(ptx::smem_u32(turn + 1), 4);
         }
@@ -1034,7 +1108,7 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_consta
     // item -> (first spatial tile, group, n-tile); n-tiles vary fastest so that neighbouring CTAs share a halo box in L2
     auto decode = [&](int item, int& sp, int& g, int& n0) {
         const int nt = item % nt_total;
-        sp = item / nt_total * kTiles;
+        sp = item / nt_total * kShape.tiles;
         g = nt / n_tiles_g;
         n0 = (nt - g * n_tiles_g) * BN;
     };
@@ -1051,34 +1125,33 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_consta
     long long ph[HALO_PH_COUNT] = {};
     HALO_PH_MARK(t_start);
 #endif
+    RingPos a, b;   // box ring (a_full / a_empty), weight ring (b_full / b_empty)
     if (wg == 0) {
-        if constexpr (kWide || kPP) ptx::setmaxnreg_dec<HALO_WIDE_PRODUCER_REGS>();
-        // ===================== TMA producer: kTiles halo boxes per (item, chunk), one weight tile per (item, chunk, tap) =====================
+        if constexpr (kShape.move_regs) ptx::setmaxnreg_dec<HALO_WIDE_PRODUCER_REGS>();
+        // ===================== TMA producer: kShape.tiles halo boxes per (item, chunk), one weight tile per (item, chunk, tap) =====================
         if (warp == 0 && ptx::elect_one()) {
-            int bs = 0, st = 0;
-            uint32_t bph = 0, sph = 0;
             const int pad_h = p.R / 2, pad_w = p.S / 2;
             for (int item = blockIdx.x; item < total_items; item += gridDim.x) {
                 int sp, g, n0;
                 decode(item, sp, g, n0);
                 for (int c = 0; c < chunks; ++c) {
-                    ptx::mbar_wait(ptx::smem_u32(a_empty + bs), bph ^ 1);
-                    const uint32_t fa = ptx::smem_u32(a_full + bs);
-                    ptx::mbar_expect_tx(fa, (uint32_t)(kTiles * BH * BW * 128));
+                    ptx::mbar_wait(ptx::smem_u32(a_empty + a.slot), a.phase ^ 1);
+                    const uint32_t fa = ptx::smem_u32(a_full + a.slot);
+                    ptx::mbar_expect_tx(fa, (uint32_t)(kShape.tiles * BH * BW * 128));
 #pragma unroll
-                    for (int t = 0; t < kTiles; ++t) {
+                    for (int t = 0; t < kShape.tiles; ++t) {
                         int n, y0, x0;
                         tile_pos(sp + t, n, y0, x0);
-                        ptx::tma_load_4d(ptx::smem_u32(s_box + (size_t)(bs * kTiles + t) * p.box_bytes), &tmap_x, fa,
+                        ptx::tma_load_4d(ptx::smem_u32(s_box + (size_t)(a.slot * kShape.tiles + t) * p.box_bytes), &tmap_x, fa,
                                          p.in_ch_off + g * p.cin_g + c * CONV_BLOCK_K, x0 - pad_w, y0 - pad_h, n);
                     }
-                    if (++bs == kBoxSlots) { bs = 0; bph ^= 1; }
+                    a.step(kShape.box_slots);
                     for (int tap = 0; tap < taps; ++tap) {
-                        ptx::mbar_wait(ptx::smem_u32(b_empty + st), sph ^ 1);
-                        const uint32_t fb = ptx::smem_u32(b_full + st);
+                        ptx::mbar_wait(ptx::smem_u32(b_empty + b.slot), b.phase ^ 1);
+                        const uint32_t fb = ptx::smem_u32(b_full + b.slot);
                         ptx::mbar_expect_tx(fb, (uint32_t)B_BYTES);
-                        ptx::tma_load_2d(ptx::smem_u32(s_b + (size_t)st * B_BYTES), &tmap_b, fb, tap * p.cin_g + c * CONV_BLOCK_K, g * p.cout_g_pad + n0);
-                        if (++st == p.num_stages) { st = 0; sph ^= 1; }
+                        ptx::tma_load_2d(ptx::smem_u32(s_b + (size_t)b.slot * B_BYTES), &tmap_b, fb, tap * p.cin_g + c * CONV_BLOCK_K, g * p.cout_g_pad + n0);
+                        b.step(p.num_stages);
                     }
                 }
             }
@@ -1090,26 +1163,18 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_consta
     // 128-pixel item: warpgroups 1, 2 take tile rows 8 half .. 8 half + 7 of the item's tile (one m64 block each).
     // wide item: warpgroup 1 + half takes tile `half` of the pair, m64 block m = its tile rows 8 m .. 8 m + 7.
     // ping-pong item: warpgroup 1 + half takes the CTA's items half, half + 2, ..., m64 block m = tile rows 8 m .. 8 m + 7.
-    if constexpr (kWide || kPP) ptx::setmaxnreg_inc<HALO_WIDE_CONSUMER_REGS>();
+    if constexpr (kShape.move_regs) ptx::setmaxnreg_inc<HALO_WIDE_CONSUMER_REGS>();
     const int half = wg - 1;
     const uint32_t sbo = (uint32_t)BW * 128u;
     const bool tma = kTmaForm && p.tma_store;
     const bool leader = (threadIdx.x & 127) == 0;   // issues (and waits for) the warpgroup's TMA stores
     const uint32_t stage = ptx::smem_u32(s_stage + (size_t)half * p.stage_bytes);
-    float acc[kBlocks][BN / 2];
-    int bs = 0, st = 0;
-    uint32_t bph = 0, sph = 0;
-    if constexpr (kPP) {
-        // ring position after n more entries
-        auto advance = [](int& slot, uint32_t& phase, int n, int depth) {
-            slot += n;
-            phase ^= (uint32_t)(slot / depth) & 1u;
-            slot %= depth;
-        };
+    float acc[kShape.blocks][BN / 2];
+    if constexpr (kItem == HaloItem::PingPong) {
         const int item_stages = chunks * taps;
         if (half) {   // warpgroup 2 starts behind the CTA's first item
-            advance(bs, bph, chunks, kBoxSlots);
-            advance(st, sph, item_stages, p.num_stages);
+            a.advance(chunks, kShape.box_slots);
+            b.advance(item_stages, p.num_stages);
         }
         for (int j = half, item = blockIdx.x + half * gridDim.x; item < total_items; j += 2, item += 2 * gridDim.x) {
             int sp, g, n0;
@@ -1118,26 +1183,11 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_consta
             if (j > 0) HALO_TIMED(HALO_PH_TURN_WAIT, ptx::mbar_wait(ptx::smem_u32(turn + half), (uint32_t)((j - 1) >> 1) & 1u));
             int prev_st = 0, prev_bs = 0;
             for (int c = 0; c < chunks; ++c) {
-                HALO_TIMED(HALO_PH_A_WAIT, ptx::mbar_wait(ptx::smem_u32(a_full + bs), bph));
-                const uint32_t abase = ptx::smem_u32(s_box + (size_t)bs * p.box_bytes);
+                HALO_TIMED(HALO_PH_A_WAIT, ptx::mbar_wait(ptx::smem_u32(a_full + a.slot), a.phase));
+                const uint32_t abase = ptx::smem_u32(s_box + (size_t)a.slot * p.box_bytes);
                 for (int tap = 0; tap < taps; ++tap) {
                     const int r = tap / p.S, s = tap - r * p.S;
-                    uint64_t da[2];
-#pragma unroll
-                    for (int m = 0; m < 2; ++m) da[m] = ptx::make_sw128_kmajor_desc_at(abase + (uint32_t)(((m * 8 + r) * BW + s) * 128), sbo);
-                    const uint64_t db = ptx::make_sw128_kmajor_desc(ptx::smem_u32(s_b + (size_t)st * B_BYTES));
-                    HALO_TIMED(HALO_PH_B_WAIT, ptx::mbar_wait(ptx::smem_u32(b_full + st), sph));
-#pragma unroll
-                    for (int m = 0; m < 2; ++m) ptx::fence_acc(acc[m]);
-                    ptx::wgmma_fence();
-#pragma unroll
-                    for (int k = 0; k < 4; ++k)
-#pragma unroll
-                        for (int m = 0; m < 2; ++m)
-                            ptx::wgmma<__half, BN>(acc[m], da[m] + (uint64_t)(k * 2), db + (uint64_t)(k * 2), (c | tap | k) != 0 ? 1u : 0u);
-                    ptx::wgmma_commit();
-#pragma unroll
-                    for (int m = 0; m < 2; ++m) ptx::fence_acc(acc[m]);
+                    halo_kstep<BN, kShape.blocks>(acc, abase, r, s, BW, sbo, s_b, b_full, b, c | tap HALO_PH_ARG);
                     if ((c | tap) != 0) {
                         // the previous k-step's MMAs are done: its weight stage, and at a chunk's first tap the previous box, are free
                         HALO_TIMED(HALO_PH_MMA_WAIT, ptx::wgmma_wait<1>());
@@ -1146,36 +1196,31 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_consta
                             if (tap == 0) ptx::mbar_arrive(ptx::smem_u32(a_empty + prev_bs));
                         }
                     }
-                    prev_st = st;
-                    if (++st == p.num_stages) { st = 0; sph ^= 1; }
+                    prev_st = b.slot;
+                    b.step(p.num_stages);
                 }
-                prev_bs = bs;
-                if (++bs == kBoxSlots) { bs = 0; bph ^= 1; }
+                prev_bs = a.slot;
+                a.step(kShape.box_slots);
             }
             if (lane == 0) ptx::mbar_arrive(ptx::smem_u32(turn + (half ^ 1)));   // every MMA of item j is issued: hand over the pipe
             HALO_TIMED(HALO_PH_MMA_WAIT, ptx::wgmma_wait<0>());
 #pragma unroll
-            for (int m = 0; m < 2; ++m) ptx::fence_acc(acc[m]);
+            for (int m = 0; m < kShape.blocks; ++m) ptx::fence_acc(acc[m]);
             if (lane == 0) {
                 ptx::mbar_arrive(ptx::smem_u32(b_empty + prev_st));
                 ptx::mbar_arrive(ptx::smem_u32(a_empty + prev_bs));
             }
-            advance(bs, bph, chunks, kBoxSlots);   // item j + 1 is the other warpgroup's
-            advance(st, sph, item_stages, p.num_stages);
+            a.advance(chunks, kShape.box_slots);   // item j + 1 is the other warpgroup's
+            b.advance(item_stages, p.num_stages);
             HALO_PH_MARK(t_epi);
             int n, y0, x0;
             tile_pos(sp, n, y0, x0);
-            if constexpr (kTmaForm) {
-                if (tma) halo_epilogue_tma<BN, kPool, 2, kStageSlots, true>(acc, p, &tmap_o, stage, n, y0, x0, g, n0, 0, warp, lane, leader HALO_PH_ARG);
-                else halo_epilogue<BN, kPool, 2>(acc, p, n, y0, x0, g, n0, 0, warp, lane);
-            } else {
-                halo_epilogue<BN, kPool, 2>(acc, p, n, y0, x0, g, n0, 0, warp, lane);
-            }
+            halo_store<BN, kPool, kItem>(acc, p, &tmap_o, tma, stage, n, y0, x0, g, n0, 0, warp, lane, leader HALO_PH_ARG);
             HALO_PH_ADD(HALO_PH_EPILOGUE, t_epi);
         }
     } else {
-        const int box = kWide ? half : 0;            // this warpgroup's box inside a box slot
-        const int row_base = kWide ? 0 : half * 8;   // tile row of block 0's first accumulator row
+        const int box = kItem == HaloItem::Wide ? half : 0;            // this warpgroup's box inside a box slot
+        const int row_base = kItem == HaloItem::Wide ? 0 : half * 8;   // tile row of block 0's first accumulator row
         // wide item, TMA store: the box slot the leader has not released yet -- the previous item's last chunk, which holds its staged
         // tile until the store has read it (the producer's next load into it is a chunk away)
         int held = -1;
@@ -1183,76 +1228,46 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_consta
             int sp, g, n0;
             decode(item, sp, g, n0);
             for (int c = 0; c < chunks; ++c) {
-                HALO_TIMED(HALO_PH_A_WAIT, ptx::mbar_wait(ptx::smem_u32(a_full + bs), bph));
-                const uint32_t abase = ptx::smem_u32(s_box + (size_t)(bs * kTiles + box) * p.box_bytes) + (uint32_t)(row_base * BW * 128);
+                HALO_TIMED(HALO_PH_A_WAIT, ptx::mbar_wait(ptx::smem_u32(a_full + a.slot), a.phase));
+                const uint32_t abase = ptx::smem_u32(s_box + (size_t)(a.slot * kShape.tiles + box) * p.box_bytes) + (uint32_t)(row_base * BW * 128);
                 int prev = 0;
                 for (int tap = 0; tap < taps; ++tap) {
                     const int r = tap / p.S, s = tap - r * p.S;
-                    uint64_t da[kTiles];
-#pragma unroll
-                    for (int m = 0; m < kTiles; ++m) da[m] = ptx::make_sw128_kmajor_desc_at(abase + (uint32_t)(((m * 8 + r) * BW + s) * 128), sbo);
-                    const uint64_t db = ptx::make_sw128_kmajor_desc(ptx::smem_u32(s_b + (size_t)st * B_BYTES));
-                    HALO_TIMED(HALO_PH_B_WAIT, ptx::mbar_wait(ptx::smem_u32(b_full + st), sph));
-#pragma unroll
-                    for (int m = 0; m < kTiles; ++m) ptx::fence_acc(acc[m]);
-                    ptx::wgmma_fence();
-#pragma unroll
-                    for (int k = 0; k < 4; ++k)
-#pragma unroll
-                        for (int m = 0; m < kTiles; ++m)
-                            ptx::wgmma<__half, BN>(acc[m], da[m] + (uint64_t)(k * 2), db + (uint64_t)(k * 2), (c | tap | k) != 0 ? 1u : 0u);
-                    ptx::wgmma_commit();
-#pragma unroll
-                    for (int m = 0; m < kTiles; ++m) ptx::fence_acc(acc[m]);
+                    halo_kstep<BN, kShape.blocks>(acc, abase, r, s, BW, sbo, s_b, b_full, b, c | tap HALO_PH_ARG);
                     if (tap > 0) {
                         HALO_TIMED(HALO_PH_MMA_WAIT, ptx::wgmma_wait<1>());
                         if (lane == 0) ptx::mbar_arrive(ptx::smem_u32(b_empty + prev));
                     }
-                    if (kWide && held >= 0 && tap == taps / 2) {
+                    if (kItem == HaloItem::Wide && held >= 0 && tap == taps / 2) {
                         HALO_TIMED(HALO_PH_STAGE_WAIT, ptx::bulk_wait_read<0>());
                         ptx::mbar_arrive(ptx::smem_u32(a_empty + held));
                         held = -1;
                     }
-                    prev = st;
-                    if (++st == p.num_stages) { st = 0; sph ^= 1; }
+                    prev = b.slot;
+                    b.step(p.num_stages);
                 }
                 HALO_TIMED(HALO_PH_MMA_WAIT, ptx::wgmma_wait<0>());   // every tap of this chunk has read the box
 #pragma unroll
-                for (int m = 0; m < kTiles; ++m) ptx::fence_acc(acc[m]);
+                for (int m = 0; m < kShape.blocks; ++m) ptx::fence_acc(acc[m]);
                 if (lane == 0) {
                     ptx::mbar_arrive(ptx::smem_u32(b_empty + prev));
-                    if (kWide && tma && leader && c == chunks - 1) held = bs;   // this box stages the tile's outputs
-                    else ptx::mbar_arrive(ptx::smem_u32(a_empty + bs));
+                    if (kItem == HaloItem::Wide && tma && leader && c == chunks - 1) held = a.slot;   // this box stages the tile's outputs
+                    else ptx::mbar_arrive(ptx::smem_u32(a_empty + a.slot));
                 }
-                if (++bs == kBoxSlots) { bs = 0; bph ^= 1; }
+                a.step(kShape.box_slots);
             }
 
             HALO_PH_MARK(t_epi);
             int n, y0, x0;
             tile_pos(sp + box, n, y0, x0);
-            if (kWide && n >= p.Nb) {   // the second tile of an odd tile count's last item
+            if (kItem == HaloItem::Wide && n >= p.Nb) {   // the second tile of an odd tile count's last item
                 if (held >= 0) { ptx::mbar_arrive(ptx::smem_u32(a_empty + held)); held = -1; }
                 continue;
             }
-            if constexpr (kTmaForm) {
-                if (tma && !kWide) {
-                    halo_epilogue_tma<BN, kPool, kBlocks, kStageSlots, true>(acc, p, &tmap_o, stage, n, y0, x0, g, n0, row_base, warp, lane,
-                                                                          leader HALO_PH_ARG);
-                } else if (tma) {
-                    // wide item: the box this warpgroup has just finished with; a 7x7 box (39 KiB) holds both m64 blocks at once, a
-                    // smaller one (3x3: 23 KiB) one block at a time
-                    const int last_bs = (bs + kBoxSlots - 1) % kBoxSlots;
-                    const uint32_t dst = ptx::smem_u32(s_box + (size_t)(last_bs * kTiles + box) * p.box_bytes);
-                    if (p.box_bytes >= kBlocks * B_BYTES)
-                        halo_epilogue_tma<BN, kPool, kBlocks, kBlocks, false>(acc, p, &tmap_o, dst, n, y0, x0, g, n0, row_base, warp, lane, leader HALO_PH_ARG);
-                    else
-                        halo_epilogue_tma<BN, kPool, kBlocks, 1, true>(acc, p, &tmap_o, dst, n, y0, x0, g, n0, row_base, warp, lane, leader HALO_PH_ARG);
-                } else {
-                    halo_epilogue<BN, kPool, kBlocks>(acc, p, n, y0, x0, g, n0, row_base, warp, lane);
-                }
-            } else {
-                halo_epilogue<BN, kPool, kBlocks>(acc, p, n, y0, x0, g, n0, row_base, warp, lane);
-            }
+            // the wide item stages its outputs in this warpgroup's box of the chunk just read, one ring position back
+            const int last = (a.slot + kShape.box_slots - 1) % kShape.box_slots;
+            const uint32_t dst = kItem == HaloItem::Wide ? ptx::smem_u32(s_box + (size_t)(last * kShape.tiles + box) * p.box_bytes) : stage;
+            halo_store<BN, kPool, kItem>(acc, p, &tmap_o, tma, dst, n, y0, x0, g, n0, row_base, warp, lane, leader HALO_PH_ARG);
             HALO_PH_ADD(HALO_PH_EPILOGUE, t_epi);
         }
     }
@@ -1265,13 +1280,13 @@ conv_halo_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_consta
 }
 
 inline int halo_box_bytes(int R, int S) { return ((HALO_TH + R - 1) * (HALO_TW + S - 1) * 128 + 1023) & ~1023; }
-inline int halo_box_slots(HaloItem it) { return it == HaloItem::PingPong ? HALO_PP_BOXES : HALO_BOXES; }
-inline int halo_boxes_per_slot(HaloItem it) { return it == HaloItem::Wide ? 2 : 1; }
-// tma_store: with the staging regions of the TMA-store epilogue (halo_stage_bytes per consumer warpgroup)
+// conv_halo_kernel's dynamic shared memory: alignment, box ring, weight ring, staging regions (with tma_store: halo_stage_bytes per
+// consumer warpgroup) and barriers
 inline size_t conv_halo_smem_bytes(int R, int S, int BN, int stages, HaloItem it, bool tma_store)
 {
-    return 1024 + (size_t)halo_box_slots(it) * halo_boxes_per_slot(it) * halo_box_bytes(R, S) + (size_t)stages * BN * 128 +
-           (tma_store ? 2 * (size_t)halo_stage_bytes(BN, it) : 0) + (2 * halo_box_slots(it) + 2 * CONV_MAX_STAGES + 2) * 8;
+    const HaloShape sh = halo_shape(it, BN);
+    return 1024 + (size_t)sh.box_slots * sh.tiles * halo_box_bytes(R, S) + (size_t)stages * BN * 128 +
+           (tma_store ? 2 * (size_t)halo_stage_bytes(BN, it) : 0) + (2 * sh.box_slots + 2 * CONV_MAX_STAGES + 2) * 8;
 }
 // as many weight stages as fit, up to CONV_MAX_STAGES (at least 2: a caller that needs more checks the result)
 inline int conv_halo_pick_stages(int R, int S, int BN, HaloItem it, bool tma_store)

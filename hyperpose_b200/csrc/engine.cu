@@ -607,6 +607,8 @@ struct ConvPlan {
     void* d_w = nullptr;         // K-major weights: fp16, or fp32 rounded to TF32 (the engine's dtype)
     bool monotone_act = false;   // every PReLU slope of the layer is >= 0
     HaloParams hp;               // halo plan: conv_halo_kernel's parameters
+    HaloItem halo_item = HaloItem::Narrow;   // halo plan: the work item
+    bool halo_pool = false;      // halo plan: the 2x2 max-pool that follows is taken in the epilogue (hp.out is the POOLED buffer)
     float* d_bias = nullptr;
     float* d_alpha = nullptr;
     float* d_mul = nullptr;      // INT8 engine: s_in * s_w[o] per (padded) output channel
@@ -621,11 +623,7 @@ enum class Launch : uint8_t {
     StemOrIm2col,   // u8 frames: nothing, the consumer conv (ConvStem) gathers its patches from the frames; f32 entry: im2col3_kernel
     Conv,           // conv_wgmma_kernel
     ConvStem,       // u8 frames: conv_wgmma_kernel with the fused R x R stem (R = po.R); f32 entry: as Conv
-    Halo,           // conv_halo_kernel: one TMA box per 16 x 8-pixel tile and channel chunk serves every filter tap
-    HaloPool,       // conv_halo_kernel with the 2x2 max-pool that follows in its epilogue (hp.out is the POOLED buffer)
-    HaloWide,       // conv_halo_kernel with 256-pixel work items: two 16 x 8 tiles share every weight tile
-    HaloPP,         // conv_halo_kernel with ping-pong items: one 16 x 8 tile per consumer warpgroup, the two take turns on the tensor pipe
-    HaloPoolPP,     // HaloPool on ping-pong items
+    Halo,           // conv_halo_kernel: one TMA box per 16 x 8-pixel tile and channel chunk serves every filter tap (plan.halo_item, plan.halo_pool)
     DwTma,          // dwconv3_tma_kernel<1>
     DwTmaPair,      // dwconv3_tma_kernel<2>: this op and the next one (same input, other filters)
     DwCol,          // dwconv3_col_kernel
@@ -780,15 +778,6 @@ inline float tf32_round(float x)
     return x;
 }
 
-bool is_halo(Launch k)
-{
-    return k == Launch::Halo || k == Launch::HaloPool || k == Launch::HaloWide || k == Launch::HaloPP || k == Launch::HaloPoolPP;
-}
-HaloItem halo_item_of(Launch k)
-{
-    return k == Launch::HaloWide ? HaloItem::Wide : k == Launch::HaloPP || k == Launch::HaloPoolPP ? HaloItem::PingPong : HaloItem::Narrow;
-}
-
 // Can the halo plan's epilogue TMA-store its tile?  One box per 64-channel slice (BN = 64 or 128) at a 16-byte aligned channel
 // offset and pixel stride, a channel extent of whole 16-byte units (the TMA store clips a box at the extent in 16-byte units, so
 // 57 channels would also write the 58th to 64th), and no box reaching into another n-tile's channels: a grouped layer's groups must
@@ -800,7 +789,7 @@ bool halo_tma_store_ok(const HaloParams& h, int BN)
 }
 
 // The halo plan's work item: one 16 x 8 tile (128 pixels) on both consumer warpgroups, two tiles sharing every weight tile
-// (conv_halo_kernel<128, false, true>), or one tile per warpgroup with the two taking turns (conv_halo_kernel<BN, kPool, false, true>);
+// (HaloItem::Wide), or one tile per warpgroup with the two taking turns (HaloItem::PingPong), with or without the fused max-pool;
 // with the TMA-store epilogue where the plan allows it, its output tensor map and staging regions
 int set_halo_item(const hp_engine* e, EngOp& op, HaloItem item, bool pool)
 {
@@ -810,8 +799,9 @@ int set_halo_item(const hp_engine* e, EngOp& op, HaloItem item, bool pool)
     h.stage_bytes = h.tma_store ? halo_stage_bytes(BN, item) : 0;
     h.num_stages = conv_halo_pick_stages(h.R, h.S, BN, item, h.tma_store);
     op.plan.smem = conv_halo_smem_bytes(h.R, h.S, BN, h.num_stages, item, h.tma_store);
-    op.launch = item == HaloItem::Wide ? Launch::HaloWide : item == HaloItem::PingPong ? (pool ? Launch::HaloPoolPP : Launch::HaloPP)
-                                                                                   : (pool ? Launch::HaloPool : Launch::Halo);
+    op.plan.halo_item = item;
+    op.plan.halo_pool = pool;
+    op.launch = Launch::Halo;
     if (!h.tma_store) return HP_OK;
     const int oh = pool ? h.H / 2 : h.H, ow = pool ? h.W / 2 : h.W, box = pool ? HALO_TW / 2 : HALO_TW;
     return make_tmap_act_box(&op.plan.tmap_o, h.out, e->max_batch, oh, ow, h.out_ch_off + h.groups * h.cout_g, h.out_ld, box, box,
@@ -1050,31 +1040,26 @@ const void* conv_kernel_bn(int BN)
     }
     return nullptr;
 }
-template <bool kPool>
-const void* halo_kernel_bn(int BN)
+// conv_halo_kernel instantiations: the 128-pixel item at every tile width, the wide item at BN = 128 without the pool, the ping-pong
+// item at BN = 64 and 128 (see pick_halo_item)
+const void* halo_kernel(int BN, HaloItem item, bool pool)
 {
-    switch (BN) {
-    case 16: return (const void*)conv_halo_kernel<16, kPool>;
-    case 32: return (const void*)conv_halo_kernel<32, kPool>;
-    case 48: return (const void*)conv_halo_kernel<48, kPool>;
-    case 64: return (const void*)conv_halo_kernel<64, kPool>;
-    case 96: return (const void*)conv_halo_kernel<96, kPool>;
-    case 128: return (const void*)conv_halo_kernel<128, kPool>;
-    }
-    return nullptr;
-}
-// Launch::Halo / HaloPool / HaloWide / HaloPP / HaloPoolPP (the wide item exists for BN = 128 only, the ping-pong item for BN = 64
-// and 128, see build_conv_plan)
-const void* halo_kernel(Launch k, int BN)
-{
-    if (k == Launch::HaloWide) return BN == 128 ? (const void*)conv_halo_kernel<128, false, true> : nullptr;
-    if (k == Launch::HaloPP || k == Launch::HaloPoolPP) {
-        const bool pool = k == Launch::HaloPoolPP;
-        if (BN == 64) return pool ? (const void*)conv_halo_kernel<64, true, false, true> : (const void*)conv_halo_kernel<64, false, false, true>;
-        if (BN == 128) return pool ? (const void*)conv_halo_kernel<128, true, false, true> : (const void*)conv_halo_kernel<128, false, false, true>;
+    using I = HaloItem;
+    if (item == I::Wide) return BN == 128 && !pool ? (const void*)conv_halo_kernel<128, false, I::Wide> : nullptr;
+    if (item == I::PingPong) {
+        if (BN == 64) return pool ? (const void*)conv_halo_kernel<64, true, I::PingPong> : (const void*)conv_halo_kernel<64, false, I::PingPong>;
+        if (BN == 128) return pool ? (const void*)conv_halo_kernel<128, true, I::PingPong> : (const void*)conv_halo_kernel<128, false, I::PingPong>;
         return nullptr;
     }
-    return k == Launch::HaloPool ? halo_kernel_bn<true>(BN) : halo_kernel_bn<false>(BN);
+    switch (BN) {
+    case 16: return pool ? (const void*)conv_halo_kernel<16, true, I::Narrow> : (const void*)conv_halo_kernel<16, false, I::Narrow>;
+    case 32: return pool ? (const void*)conv_halo_kernel<32, true, I::Narrow> : (const void*)conv_halo_kernel<32, false, I::Narrow>;
+    case 48: return pool ? (const void*)conv_halo_kernel<48, true, I::Narrow> : (const void*)conv_halo_kernel<48, false, I::Narrow>;
+    case 64: return pool ? (const void*)conv_halo_kernel<64, true, I::Narrow> : (const void*)conv_halo_kernel<64, false, I::Narrow>;
+    case 96: return pool ? (const void*)conv_halo_kernel<96, true, I::Narrow> : (const void*)conv_halo_kernel<96, false, I::Narrow>;
+    case 128: return pool ? (const void*)conv_halo_kernel<128, true, I::Narrow> : (const void*)conv_halo_kernel<128, false, I::Narrow>;
+    }
+    return nullptr;
 }
 const void* conv_kernel(int dtype, bool res, int BN, int stem_R = 0)
 {
@@ -1104,7 +1089,7 @@ void launch_dw_tma(hp_engine* e, const EngOp& op, const EngOp* pair, int N, cuda
     else      launch_pdl(dwconv3_tma_kernel<1>, grid, DWT_THREADS, op.dwt_smem, st, op.tmap_dw, p);
 }
 
-// conv_wgmma_kernel, or conv_halo_kernel for the Halo* launches
+// conv_wgmma_kernel, or conv_halo_kernel for Launch::Halo
 int launch_conv(hp_engine* e, EngOp& op, int N, cudaStream_t st, bool u8_input)
 {
     ConvPlan& pl = op.plan;
@@ -1112,15 +1097,15 @@ int launch_conv(hp_engine* e, EngOp& op, int N, cudaStream_t st, bool u8_input)
     p.Nb = N;
     const int stem_R = op.launch == Launch::ConvStem && u8_input ? (int)op.po.R : 0;
     p.frames = e->cur_frames ? e->cur_frames : e->d_frames;
-    if (is_halo(op.launch)) {
+    if (op.launch == Launch::Halo) {
         HaloParams h = pl.hp;
         h.Nb = N;
-        const int tiles = op.launch == Launch::HaloWide ? 2 : 1;
+        const int tiles = halo_shape(pl.halo_item, p.BN).tiles;
         const long items = ((long)N * h.tiles_x * h.tiles_y + tiles - 1) / tiles * h.groups * (h.cout_g_pad / p.BN);
         cudaLaunchAttribute at[1];
         const cudaLaunchConfig_t cfg = pdl_config((int)std::min<long>(e->num_sms - e->reserve_sms, items), CONV_THREADS, pl.smem, st, at);
         void* args[] = { (void*)&pl.tmap_x, (void*)&pl.tmap_b, (void*)&pl.tmap_o, (void*)&h };
-        HP_CUDA_TRY(cudaLaunchKernelExC(&cfg, halo_kernel(op.launch, p.BN), args));
+        HP_CUDA_TRY(cudaLaunchKernelExC(&cfg, halo_kernel(p.BN, pl.halo_item, pl.halo_pool), args));
         return HP_OK;
     }
     p.m_tiles = (int)(((size_t)N * p.H * p.W + CONV_BLOCK_M - 1) / CONV_BLOCK_M);
@@ -1215,7 +1200,7 @@ int run_graph(hp_engine* e, int N, bool u8_input, cudaStream_t st, int first = 0
 #undef HP_IM2COL
             break;
         }
-        case Launch::Conv: case Launch::ConvStem: case Launch::Halo: case Launch::HaloPool: case Launch::HaloWide: case Launch::HaloPP: case Launch::HaloPoolPP:
+        case Launch::Conv: case Launch::ConvStem: case Launch::Halo:
             launch_conv(e, op, N, st, u8_input);
             break;
         case Launch::DwTma:
@@ -1652,7 +1637,7 @@ int hp_engine_create_ex(hp_engine** out, const void* pack, size_t pack_bytes, in
     // conv (halo kernel) -> 2x2 max-pool: the pool moves into the conv's epilogue when nobody else reads the un-pooled tensor
     for (size_t i = 0; opt.pool_fuse && i + 1 < e->ops.size(); ++i) {
         EngOp& c = e->ops[i]; EngOp& m = e->ops[i + 1];
-        if ((c.launch != Launch::Halo && c.launch != Launch::HaloWide && c.launch != Launch::HaloPP) || !c.plan.monotone_act || m.po.type != OP_MAXPOOL2 || (m.po.R != 0 && m.po.R != 2)) continue;
+        if (c.launch != Launch::Halo || c.plan.halo_pool || !c.plan.monotone_act || m.po.type != OP_MAXPOOL2 || (m.po.R != 0 && m.po.R != 2)) continue;
         const EngBuffer& cb = e->bufs[c.po.out_buf];
         const EngBuffer& pb = e->bufs[m.po.out_buf];
         const int C = (int)c.po.groups * (int)c.po.cout_g;
@@ -1753,8 +1738,8 @@ int hp_engine_create_ex(hp_engine** out, const void* pack, size_t pack_bytes, in
     e->use_pdl = dtype == HP_DTYPE_F16 && launches > 0 && per_launch < 10e9;
     for (const EngOp& o : e->ops) {
         if (o.po.type != OP_CONV) continue;
-        if (is_halo(o.launch) &&
-            cudaFuncSetAttribute(halo_kernel(o.launch, o.plan.prm.BN), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)max_smem) != cudaSuccess) {
+        if (o.launch == Launch::Halo &&
+            cudaFuncSetAttribute(halo_kernel(o.plan.prm.BN, o.plan.halo_item, o.plan.halo_pool), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)max_smem) != cudaSuccess) {
             set_error("engine: cannot opt in to %zu bytes of dynamic shared memory (halo)", max_smem);
             return fail(HP_ERR_CUDA);
         }
@@ -2120,11 +2105,10 @@ int hp_engine_debug_op_kernel(const hp_engine* e, int op, char* name, int cap)
         s = std::string("conv<") + dt + std::to_string(BN) + (o.plan.prm.res_mode ? ",res>" : ">");
         break;
     case Launch::ConvStem: s = "conv<f16," + std::to_string(BN) + ",stem" + std::to_string(po.R) + ">"; break;
-    case Launch::Halo: s = "halo<" + std::to_string(BN) + ">"; break;
-    case Launch::HaloPool: s = "halo<" + std::to_string(BN) + ",pool>"; break;
-    case Launch::HaloWide: s = "halo<" + std::to_string(BN) + ",wide>"; break;
-    case Launch::HaloPP: s = "halo<" + std::to_string(BN) + ",pp>"; break;
-    case Launch::HaloPoolPP: s = "halo<" + std::to_string(BN) + ",pool,pp>"; break;
+    case Launch::Halo:
+        s = "halo<" + std::to_string(BN) + (o.plan.halo_pool ? ",pool" : "") +
+            (o.plan.halo_item == HaloItem::Wide ? ",wide" : o.plan.halo_item == HaloItem::PingPong ? ",pp" : "") + ">";
+        break;
     case Launch::DwTma: s = "dw_tma<1>"; break;
     case Launch::DwTmaPair: s = "dw_tma<2>"; break;
     case Launch::DwCol: s = "dw_col"; break;
@@ -2149,7 +2133,7 @@ int hp_engine_debug_op_epilogue(const hp_engine* e, int op, int* tma_store)
 {
     if (!e || op < 0 || op >= (int)e->ops.size() || !tma_store) { set_error("hp_engine_debug_op_epilogue: bad argument"); return HP_ERR_ARG; }
     const EngOp& o = e->ops[op];
-    *tma_store = is_halo(o.launch) && o.plan.hp.tma_store ? 1 : 0;
+    *tma_store = o.launch == Launch::Halo && o.plan.hp.tma_store ? 1 : 0;
     return HP_OK;
 }
 

@@ -28,7 +28,7 @@ from oracle import torch_backbone
 
 gpu = pytest.mark.gpu
 
-# All conv kernels launch_conv can pick: one per tile width in conv_kernel_bn<T, kRes, kStemR> and halo_kernel_bn<kPool>
+# All conv kernels launch_conv can pick: one per tile width in conv_kernel_bn<T, kRes, kStemR> and halo_kernel's 128-pixel item
 # (engine.cu).  A new tile width has to be added here too.
 BNS = (16, 32, 48, 64, 96, 128)
 CONV_KERNELS = ({f"conv<f16,{b}>" for b in BNS} | {f"conv<f16,{b},res>" for b in BNS} | {f"conv<f16,{b},stem3>" for b in BNS} |
