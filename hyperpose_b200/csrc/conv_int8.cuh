@@ -71,11 +71,12 @@ __global__ void __launch_bounds__(256) maxpool_i8_kernel(const int8_t* __restric
     *(unsigned*)(out + (((size_t)n * OH + oh) * OW + ow) * C_out_ld + c4 * 4) = m;
 }
 
-// depthwise KxK conv (K = 1 or 3, stride 1 / 2, TF "SAME") + bias + PReLU, int8 in / out, fp32 weights, 4 channels per thread.
-// Per tap x = q * s_in, acc = acc + x * w from acc = 0, taps row major then by ascending column, each operation rounded on its own.
+// depthwise KxK conv (K = 1 or 3, stride 1 / 2, taps `dil` pixels apart, TF "SAME") + bias + PReLU, int8 in / out, fp32 weights, 4
+// channels per thread.  Per tap x = q * s_in, acc = acc + x * w from acc = 0, taps row major then by ascending column, each operation
+// rounded on its own.
 __global__ void __launch_bounds__(256) dwconv_i8_kernel(const int8_t* __restrict__ in, int in_ld, int8_t* __restrict__ out, int out_ld, const float* __restrict__ w /*[K*K][C]*/,
                                                         const float* __restrict__ bias, const float* __restrict__ alpha, int N, int H, int W, int C, int OH, int OW,
-                                                        int K, int stride, int pad_h, int pad_w, float s_in, float inv_s_out)
+                                                        int K, int stride, int dil, int pad_h, int pad_w, float s_in, float inv_s_out)
 {
     const size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     const int cv = C / 4;
@@ -88,10 +89,10 @@ __global__ void __launch_bounds__(256) dwconv_i8_kernel(const int8_t* __restrict
     const int n = (int)(t / OH);
     float acc[4] = { 0.f, 0.f, 0.f, 0.f };
     for (int r = 0; r < K; ++r) {
-        const int h = oh * stride - pad_h + r;
+        const int h = oh * stride - pad_h + r * dil;
         if (h < 0 || h >= H) continue;
         for (int s = 0; s < K; ++s) {
-            const int x = ow * stride - pad_w + s;
+            const int x = ow * stride - pad_w + s * dil;
             if (x < 0 || x >= W) continue;
             const char4 q = *(const char4*)(in + (((size_t)n * H + h) * W + x) * in_ld + c0);
             const float4 k = __ldg((const float4*)(w + (size_t)(r * K + s) * C + c0));

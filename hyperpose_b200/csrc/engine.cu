@@ -192,28 +192,34 @@ __global__ void __launch_bounds__(256, 3) dwconv_kernel(const __half* __restrict
 // segments; the x-1 / x+1 neighbours are L1 hits of the adjacent columns' threads) and scatters the row into the three
 // output rows it feeds, so per output there are 3 loads + 36 FMAs and the 36 weights stay in registers for the whole run.
 // Accumulation order per output is tap-row major, tap-column ascending -- the same as dwconv_kernel (bit-identical).
+// Dilation D (taps D pixels apart, SAME padding D): output row y reads input rows y - D, y, y + D only, so the rows of one residue
+// mod D form a 3x3 / dilation-1 problem of their own.  A thread marches one residue class ("phase") of its column: rows are
+// counted in that class (H rows -> Hs = ceil((H - phase) / D)), one step is D image rows, the column neighbours are x -/+ D.
+template <int D>
 __global__ void __launch_bounds__(256, 3) dwconv3_col_kernel(const __half* __restrict__ in, int in_ld, __half* __restrict__ out, int out_ld,
                                                           const float* __restrict__ w /*[9][C]*/, const float* __restrict__ bias,
                                                           const float* __restrict__ alpha, int N, int H, int W, int C, int rows_per_chunk, int chunks)
 {
     const size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     const int cv = C / 4;
-    const size_t total = (size_t)N * chunks * W * cv;
+    const size_t total = (size_t)N * D * chunks * W * cv;
     if (idx >= total) return;
     const int c0 = (int)(idx % cv) * 4;
     size_t t = idx / cv;
     const int x = (int)(t % W); t /= W;
-    const int chunk = (int)(t % chunks);
-    const int n = (int)(t / chunks);
-    const int oh0 = chunk * rows_per_chunk, oh1 = min(oh0 + rows_per_chunk, H);
+    const int chunk = (int)(t % chunks); t /= chunks;
+    const int phase = (int)(t % D);
+    const int n = (int)(t / D);
+    const int Hs = (H - phase + D - 1) / D;   // image rows phase, phase + D, ...
+    const int oh0 = chunk * rows_per_chunk, oh1 = min(oh0 + rows_per_chunk, Hs);
     if (oh0 >= oh1) return;
     float4 wt[9];
 #pragma unroll
     for (int k = 0; k < 9; ++k) wt[k] = __ldg((const float4*)(w + (size_t)k * C + c0));
     const float4 bs = __ldg((const float4*)(bias + c0)), al = __ldg((const float4*)(alpha + c0));
-    const bool has_l = x > 0, has_r = x + 1 < W;
-    const __half* colp = in + ((size_t)n * H * W + x) * in_ld + c0;
-    __half* outp = out + ((size_t)n * H * W + x) * out_ld + c0;
+    const bool has_l = x >= D, has_r = x + D < W;
+    const __half* colp = in + (((size_t)n * H + phase) * W + x) * in_ld + c0;
+    __half* outp = out + (((size_t)n * H + phase) * W + x) * out_ld + c0;
     float4 a0 = { 0.f, 0.f, 0.f, 0.f }, a1 = a0, a2 = a0;   // output rows ih-1, ih, ih+1 while input row ih is being read
 #define HP_FMA4(acc, wv, xv) { acc.x = fmaf(xv.x, wv.x, acc.x); acc.y = fmaf(xv.y, wv.y, acc.y); acc.z = fmaf(xv.z, wv.z, acc.z); acc.w = fmaf(xv.w, wv.w, acc.w); }
     // one input row: it is tap row 2 of output ih-1 (A, complete afterwards -> stored), tap row 1 of output ih (B), tap row 0 of
@@ -222,8 +228,8 @@ __global__ void __launch_bounds__(256, 3) dwconv3_col_kernel(const __half* __res
     {                                                                                                                               \
         uint2 ul = { 0u, 0u }, ur = { 0u, 0u };                                                                                      \
         const uint2 uc = *(const uint2*)rp;                                                                                          \
-        if (has_l) ul = *(const uint2*)(rp - in_ld);                                                                                 \
-        if (has_r) ur = *(const uint2*)(rp + in_ld);                                                                                 \
+        if (has_l) ul = *(const uint2*)(rp - D * in_ld);                                                                             \
+        if (has_r) ur = *(const uint2*)(rp + D * in_ld);                                                                             \
         rp += row_in;                                                                                                                \
         const float2 l0 = __half22float2(*(const __half2*)&ul.x), l1 = __half22float2(*(const __half2*)&ul.y);                       \
         const float2 m0 = __half22float2(*(const __half2*)&uc.x), m1 = __half22float2(*(const __half2*)&uc.y);                       \
@@ -245,8 +251,8 @@ __global__ void __launch_bounds__(256, 3) dwconv3_col_kernel(const __half* __res
         *(uint2*)op = ov;                                                                                                            \
         op += row_out;                                                                                                               \
     }
-    const size_t row_in = (size_t)W * in_ld, row_out = (size_t)W * out_ld;
-    const int ih_first = max(oh0 - 1, 0), ih_last = min(oh1, H - 1);   // valid input rows feeding this run
+    const size_t row_in = (size_t)D * W * in_ld, row_out = (size_t)D * W * out_ld;
+    const int ih_first = max(oh0 - 1, 0), ih_last = min(oh1, Hs - 1);   // valid input rows feeding this run
     const __half* rp = colp + (size_t)ih_first * row_in;
     __half* op = outp + (size_t)oh0 * row_out;
     int ih = ih_first;
@@ -273,6 +279,8 @@ __global__ void __launch_bounds__(256, 3) dwconv3_col_kernel(const __half* __res
 // `stages - 1` tiles ahead.  Compute is the column march of dwconv3_col_kernel from shared memory: a lane owns a channel pair (the 32
 // lanes of a warp read one pixel's 128 bytes: conflict-free), a warp a column of the tile; the accumulation order per output is the
 // same (tap-row major, tap-column ascending, absent taps as zeros), as fmas on channel pairs (pair_math.cuh): bit-identical.
+// Dilation D: the halo is D pixels wide ({64, wbo + 2D, hb + 2D} boxes) and, as in dwconv3_col_kernel, a warp marches one residue
+// class of rows mod D of its column (work unit = column x phase), stepping D box rows and reading the box columns col, col + D, col + 2D.
 struct DwTmaParams {
     __half* out0; __half* out1; int out_ld;
     const float* w0; const float* w1;   // [9][C] | bias[C] | alpha[C]
@@ -281,13 +289,14 @@ struct DwTmaParams {
 constexpr int DWT_THREADS = 384;   // 12 warps
 constexpr int DWT_STAGE_MAX = 73728;   // bytes of one tile buffer at most (3 of them + barriers fit 227 KB)
 
-template <int NB>
+template <int NB, int D>
 __global__ void __launch_bounds__(DWT_THREADS, 1) dwconv3_tma_kernel(const __grid_constant__ CUtensorMap tmap_in, const DwTmaParams p)
 {
+    static_assert(NB == 1 || D == 1, "the dual-filter form is for undilated pairs only");
     extern __shared__ uint8_t dwt_smem_raw[];
     const uint32_t base = (ptx::smem_u32(dwt_smem_raw) + 127u) & ~127u;
-    const int bw = p.wbo + 2;
-    const uint32_t stage_bytes = (uint32_t)(p.hb + 2) * (uint32_t)bw * 128u;
+    const int bw = p.wbo + 2 * D;
+    const uint32_t stage_bytes = (uint32_t)(p.hb + 2 * D) * (uint32_t)bw * 128u;
     const uint32_t bars = base + (uint32_t)p.stages * stage_bytes;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     ptx::pdl_launch_dependents();
@@ -313,12 +322,12 @@ __global__ void __launch_bounds__(DWT_THREADS, 1) dwconv3_tma_kernel(const __gri
         tile_of(item, ct, tx, ty, n);
         const int s = k % p.stages;
         ptx::mbar_expect_tx(bars + 8u * s, stage_bytes);
-        ptx::tma_load_4d(base + (uint32_t)s * stage_bytes, &tmap_in, bars + 8u * s, ct * 64, tx * p.wbo - 1, ty * p.hb - 1, n);
+        ptx::tma_load_4d(base + (uint32_t)s * stage_bytes, &tmap_in, bars + 8u * s, ct * 64, tx * p.wbo - D, ty * p.hb - D, n);
     };
     ptx::pdl_wait();   // the prologue above may run under the previous kernel's tail; its results are visible from here on
     if (threadIdx.x == 0)
         for (int k = 0; k < p.stages - 1; ++k) issue(k);
-    const size_t row_out = (size_t)p.W * p.out_ld;
+    const size_t row_out = (size_t)D * p.W * p.out_ld;   // one step of a warp's march: D image rows
     float2 wa[9], wb[9], bsa, ala, bsb, alb;
     int ct_loaded = -1;
     for (int k = 0;; ++k) {
@@ -345,9 +354,13 @@ __global__ void __launch_bounds__(DWT_THREADS, 1) dwconv3_tma_kernel(const __gri
         ptx::mbar_wait(bars + 8u * s, (uint32_t)(k / p.stages) & 1u);
         const uint32_t* tile = (const uint32_t*)(dwt_smem_raw + (base - ptx::smem_u32(dwt_smem_raw)) + (size_t)s * stage_bytes) + lane;
         const int row_words = bw * 32;
-        for (int col = warp; col < ncols; col += (int)(blockDim.x >> 5)) {
-            const uint32_t* sp = tile + col * 32;   // box row 0 (image row y_lo - 1), box columns col, col+1, col+2 = image x-1, x, x+1
-            const size_t o = (((size_t)n * p.H + y_lo) * p.W + x_lo + col) * p.out_ld + c0;
+        for (int u = warp; u < ncols * D; u += (int)(blockDim.x >> 5)) {
+            const int col = u / D, ph = u % D;
+            const int nout = (nrows - ph + D - 1) / D;   // output rows y_lo + ph, + D, ...
+            if (nout <= 0) continue;
+            // box row ph (image row y_lo + ph - D), box columns col, col+D, col+2D = image x-D, x, x+D
+            const uint32_t* sp = tile + ph * row_words + col * 32;
+            const size_t o = (((size_t)n * p.H + y_lo + ph) * p.W + x_lo + col) * p.out_ld + c0;
             __half* opa = p.out0 + o;
             __half* opb = NB == 2 ? p.out1 + o : nullptr;
             float2 a0 = { 0.f, 0.f }, a1 = a0, a2 = a0, b0 = a0, b1 = a0, b2 = a0;
@@ -363,8 +376,8 @@ __global__ void __launch_bounds__(DWT_THREADS, 1) dwconv3_tma_kernel(const __gri
             // box row I: tap row 2 of output row I-2 (A0/B0, complete -> stored), tap row 1 of I-1 (A1/B1), tap row 0 of I (A2/B2, from zero)
 #define HP_DWT_STEP(A0, A1, A2, B0, B1, B2, I)                                                                                     \
             {                                                                                                                       \
-                const uint32_t ul = sp[0], uc = sp[32], ur = sp[64];                                                                 \
-                sp += row_words;                                                                                                     \
+                const uint32_t ul = sp[0], uc = sp[32 * D], ur = sp[64 * D];                                                         \
+                sp += D * row_words;                                                                                                 \
                 const float2 vl = __half22float2(*(const __half2*)&ul), vm = __half22float2(*(const __half2*)&uc), vr = __half22float2(*(const __half2*)&ur); \
                 A0 = ffma2_rn(vl, wa[6], A0); A0 = ffma2_rn(vm, wa[7], A0); A0 = ffma2_rn(vr, wa[8], A0);                      \
                 A1 = ffma2_rn(vl, wa[3], A1); A1 = ffma2_rn(vm, wa[4], A1); A1 = ffma2_rn(vr, wa[5], A1);                      \
@@ -376,7 +389,7 @@ __global__ void __launch_bounds__(DWT_THREADS, 1) dwconv3_tma_kernel(const __gri
                 }                                                                                                                   \
                 if ((I) >= 2) HP_DWT_EMIT(A0, B0);                                                                                   \
             }
-            const int R = nrows + 2;
+            const int R = nout + 2;
             int i = 0;
             for (; i + 2 < R; i += 3) {   // three rows per trip: the accumulators rotate by renaming
                 HP_DWT_STEP(a0, a1, a2, b0, b1, b2, i);
@@ -687,6 +700,9 @@ inline int same_pad_before(int in, int k, int stride)
     const int total = std::max((out - 1) * stride + k - in, 0);
     return total / 2;
 }
+
+// a depthwise op's dilation (the pack's 0 = 1); its SAME window spans (K - 1) * dilation + 1 pixels
+inline int dw_dilation(const PackOp& po) { return po.dilation ? (int)po.dilation : 1; }
 
 struct EngBuffer {
     bool fused_away = false;   // never written: its only consumer (a 2x2 max-pool / 1x1 depthwise op) runs inside the producing conv's epilogue
@@ -1085,8 +1101,9 @@ void launch_dw_tma(hp_engine* e, const EngOp& op, const EngOp* pair, int N, cuda
     p.tiles_x = op.dwt_tiles_x; p.tiles_y = op.dwt_tiles_y; p.wbo = op.dwt_wbo; p.hb = op.dwt_hb; p.stages = op.dwt_stages;
     p.n_items = N * p.tiles_y * p.tiles_x * p.ctiles;
     const int grid = std::min(p.n_items, std::max(1, e->num_sms - e->reserve_sms));
-    if (pair) launch_pdl(dwconv3_tma_kernel<2>, grid, DWT_THREADS, op.dwt_smem, st, op.tmap_dw, p);
-    else      launch_pdl(dwconv3_tma_kernel<1>, grid, DWT_THREADS, op.dwt_smem, st, op.tmap_dw, p);
+    if (pair)                     launch_pdl(dwconv3_tma_kernel<2, 1>, grid, DWT_THREADS, op.dwt_smem, st, op.tmap_dw, p);
+    else if (dw_dilation(po) == 2) launch_pdl(dwconv3_tma_kernel<1, 2>, grid, DWT_THREADS, op.dwt_smem, st, op.tmap_dw, p);
+    else                          launch_pdl(dwconv3_tma_kernel<1, 1>, grid, DWT_THREADS, op.dwt_smem, st, op.tmap_dw, p);
 }
 
 // conv_wgmma_kernel, or conv_halo_kernel for Launch::Halo
@@ -1210,18 +1227,20 @@ int run_graph(hp_engine* e, int N, bool u8_input, cudaStream_t st, int first = 0
             launch_dw_tma(e, op, &e->ops[oi + 1], N, st);
             break;
         case Launch::DwCol: {
-            // column-marching kernel: enough row chunks to give every SM a few blocks
+            // column-marching kernel: enough row chunks to give every SM a few blocks (rows of one phase of a dilated op: ceil(H / D))
             const EngBuffer& ib = e->bufs[po.in_buf];
             const EngBuffer& ob = e->bufs[po.out_buf];
-            const int C = (int)po.cout_g;
-            const size_t base = ((size_t)N * ib.W * (C / 4) + 255) / 256;
+            const int C = (int)po.cout_g, D = dw_dilation(po), Hs = (ib.H + D - 1) / D;
+            const size_t base = ((size_t)N * D * ib.W * (C / 4) + 255) / 256;
             int chunks = (int)((4 * (size_t)e->num_sms + base - 1) / base);
-            chunks = std::max(1, std::min(chunks, std::max(1, ib.H / 4)));
-            const int rows = (ib.H + chunks - 1) / chunks;
-            chunks = (ib.H + rows - 1) / rows;
-            const size_t tot = (size_t)N * chunks * ib.W * (C / 4);
-            dwconv3_col_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, st>>>(ib.d + po.in_ch_off, ib.channels, ob.d + po.out_ch_off, ob.channels, op.d_dw,
-                op.d_dw + (size_t)9 * C, op.d_dw + (size_t)9 * C + C, N, ib.H, ib.W, C, rows, chunks);
+            chunks = std::max(1, std::min(chunks, std::max(1, Hs / 4)));
+            const int rows = (Hs + chunks - 1) / chunks;
+            chunks = (Hs + rows - 1) / rows;
+            const size_t tot = (size_t)N * D * chunks * ib.W * (C / 4);
+#define HP_DWCOL(DD) dwconv3_col_kernel<DD><<<(unsigned)((tot + 255) / 256), 256, 0, st>>>(ib.d + po.in_ch_off, ib.channels, ob.d + po.out_ch_off, \
+                ob.channels, op.d_dw, op.d_dw + (size_t)9 * C, op.d_dw + (size_t)9 * C + C, N, ib.H, ib.W, C, rows, chunks)
+            if (D == 2) HP_DWCOL(2); else HP_DWCOL(1);
+#undef HP_DWCOL
             break;
         }
         case Launch::DwStrip: {   // 3x3 / stride 2 and 1x1
@@ -1272,8 +1291,10 @@ int run_graph(hp_engine* e, int N, bool u8_input, cudaStream_t st, int first = 0
             const int C = (int)po.cout_g;
             const size_t total = (size_t)N * ob.H * ob.W * (C / 4);
             const float* dw = op.d_dw;
+            const int D = dw_dilation(po), span = (K - 1) * D + 1;
             dwconv_f32_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>((const float*)ib.d + po.in_ch_off, ib.channels, (float*)ob.d + po.out_ch_off, ob.channels, dw,
-                dw + (size_t)K * K * C, dw + (size_t)K * K * C + C, N, ib.H, ib.W, C, ob.H, ob.W, K, stride, same_pad_before(ib.H, K, stride), same_pad_before(ib.W, K, stride));
+                dw + (size_t)K * K * C, dw + (size_t)K * K * C + C, N, ib.H, ib.W, C, ob.H, ob.W, K, stride, D, same_pad_before(ib.H, span, stride),
+                same_pad_before(ib.W, span, stride));
             break;
         }
         case Launch::MaxPoolF32: {
@@ -1312,9 +1333,10 @@ int run_graph(hp_engine* e, int N, bool u8_input, cudaStream_t st, int first = 0
             const int C = (int)po.cout_g;
             const size_t total = (size_t)N * ob.H * ob.W * (C / 4);
             const float* dw = op.d_dw;
+            const int D = dw_dilation(po), span = (K - 1) * D + 1;
             dwconv_i8_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>((const int8_t*)ib.d + po.in_ch_off, ib.channels, (int8_t*)ob.d + po.out_ch_off, ob.channels, dw,
-                dw + (size_t)K * K * C, dw + (size_t)K * K * C + C, N, ib.H, ib.W, C, ob.H, ob.W, K, stride, same_pad_before(ib.H, K, stride), same_pad_before(ib.W, K, stride),
-                e->act_scale[po.in_buf], 1.0f / e->act_scale[po.out_buf]);
+                dw + (size_t)K * K * C, dw + (size_t)K * K * C + C, N, ib.H, ib.W, C, ob.H, ob.W, K, stride, D, same_pad_before(ib.H, span, stride),
+                same_pad_before(ib.W, span, stride), e->act_scale[po.in_buf], 1.0f / e->act_scale[po.out_buf]);
             break;
         }
         case Launch::MaxPoolI8: {
@@ -1449,6 +1471,19 @@ int hp_engine_create_ex(hp_engine** out, const void* pack, size_t pack_bytes, in
         for (uint32_t i = 0; i < hdr.n_ops; ++i) {
             PackOp po;
             memcpy(&po, vops + i, sizeof(po));
+            // dilation: depthwise 3x3 at stride 1 takes 1 or 2 (the dilated kernels' halo and the planner are sized for 2 at most); every
+            // other op ignores the field, so a nonzero value there is a malformed pack, not a request to be dropped silently
+            if (po.type == OP_DWCONV) {
+                const uint32_t D = po.dilation ? po.dilation : 1;   // unsigned: the field is untrusted
+                if (D > 2 || (D == 2 && (po.R != 3 || po.S != 3 || (po.stride ? po.stride : 1) != 1))) {
+                    set_error("hp_engine_create: depthwise op %u has dilation %u with a %ux%u filter at stride %u (dilation 2 needs 3x3 at stride 1; "
+                              "otherwise 0 or 1)", i, po.dilation, po.R, po.S, po.stride ? po.stride : 1);
+                    return HP_ERR_ARG;
+                }
+            } else if (po.dilation != 0) {
+                set_error("hp_engine_create: op %u (type %u) has dilation %u; only depthwise ops take one", i, po.type, po.dilation);
+                return HP_ERR_ARG;
+            }
             if (po.type != OP_CONV && po.type != OP_DWCONV) continue;
             const uint64_t lim = 1u << 16;   // per-dimension bound: keeps the products below 2^64
             const bool dw = po.type == OP_DWCONV;
@@ -1564,6 +1599,7 @@ int hp_engine_create_ex(hp_engine** out, const void* pack, size_t pack_bytes, in
                 return fail(HP_ERR_CUDA);
             }
             e->flops_per_frame += 2.0 * ob.H * ob.W * C * K * K;
+            // (a dilated op is 3x3 / stride 1, validated above: never DwStrip)
             op.launch = tf32 ? Launch::DwF32 : i8 ? Launch::DwI8 : K == 3 && stride == 1 ? Launch::DwCol : Launch::DwStrip;
         } else if (po.type == OP_MAXPOOL2) {
             // 8 channels per 16-byte load (fp16) / two float4 loads (fp32): both offsets aligned, both channel ranges inside their buffers
@@ -1694,36 +1730,38 @@ int hp_engine_create_ex(hp_engine** out, const void* pack, size_t pack_bytes, in
         const PackOp& po = a.po;
         if (!opt.dw_tma || a.launch != Launch::DwCol || po.cout_g % 64 || po.in_buf == po.out_buf) continue;
         const EngBuffer& ib = e->bufs[po.in_buf];
-        const int C = (int)po.cout_g;
-        const int nx = (ib.W + 61) / 62, wbo = (ib.W + nx - 1) / nx, bw = wbo + 2;
+        const int C = (int)po.cout_g, halo = 2 * dw_dilation(po);   // box = tile + a D-pixel halo on every side, at most 64 columns
+        const int nx = (ib.W + 63 - halo) / (64 - halo), wbo = (ib.W + nx - 1) / nx, bw = wbo + halo;
         // tile height: the tallest of 8 / 6 / 4 / 3 / 2 rows that fits a buffer and still gives every SM two tiles at the full batch
         int hb = 2;
         for (int cand : { 8, 6, 4, 3, 2 }) {
-            if (cand > std::max(2, ib.H) || (size_t)(cand + 2) * bw * 128 > (size_t)DWT_STAGE_MAX) continue;
+            if (cand > std::max(2, ib.H) || (size_t)(cand + halo) * bw * 128 > (size_t)DWT_STAGE_MAX) continue;
             const size_t items = (size_t)e->max_batch * ((ib.H + cand - 1) / cand) * nx * (C / 64);
             hb = cand;
             if (items >= 2 * (size_t)e->num_sms) break;
         }
-        const size_t stage = (size_t)(hb + 2) * bw * 128;
+        const size_t stage = (size_t)(hb + halo) * bw * 128;
         if (stage > (size_t)DWT_STAGE_MAX) continue;
         a.dwt_stages = (int)std::min<size_t>(4, (200 * 1024) / stage);
         if (a.dwt_stages < 2) continue;
         a.dwt_wbo = wbo; a.dwt_hb = hb; a.dwt_tiles_x = nx; a.dwt_tiles_y = (ib.H + hb - 1) / hb;
         a.dwt_smem = a.dwt_stages * stage + 128 + 64;
-        if (make_tmap_act_box(&a.tmap_dw, ib.d + po.in_ch_off, e->max_batch, ib.H, ib.W, C, ib.channels, bw, hb + 2, CU_TENSOR_MAP_SWIZZLE_NONE) != HP_OK) return fail(HP_ERR_CUDA);
+        if (make_tmap_act_box(&a.tmap_dw, ib.d + po.in_ch_off, e->max_batch, ib.H, ib.W, C, ib.channels, bw, hb + halo, CU_TENSOR_MAP_SWIZZLE_NONE) != HP_OK) return fail(HP_ERR_CUDA);
         a.launch = Launch::DwTma;
         dwt_max = std::max(dwt_max, a.dwt_smem);
     }
-    if (dwt_max > 0 && (cudaFuncSetAttribute(dwconv3_tma_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dwt_max) != cudaSuccess ||
-                        cudaFuncSetAttribute(dwconv3_tma_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dwt_max) != cudaSuccess)) {
+    if (dwt_max > 0 && (cudaFuncSetAttribute(dwconv3_tma_kernel<1, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dwt_max) != cudaSuccess ||
+                        cudaFuncSetAttribute(dwconv3_tma_kernel<2, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dwt_max) != cudaSuccess ||
+                        cudaFuncSetAttribute(dwconv3_tma_kernel<1, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dwt_max) != cudaSuccess)) {
         set_error("engine: cannot opt in to %zu bytes of dynamic shared memory (depthwise)", dwt_max);
         return fail(HP_ERR_CUDA);
     }
-    // two TMA depthwise convs of the same input (the conf / paf branch of a MobilenetThin stage): one launch with both filter sets
+    // two TMA depthwise convs of the same input (the conf / paf branch of a MobilenetThin stage): one launch with both filter sets.
+    // The dual-filter kernel marches undilated tiles: a dilated op always launches alone.
     for (size_t i = 0; opt.dw_pair && i + 1 < e->ops.size(); ++i) {
         EngOp& a = e->ops[i]; EngOp& b = e->ops[i + 1];
         if (a.launch != Launch::DwTma || b.launch != Launch::DwTma || a.po.in_buf != b.po.in_buf || a.po.in_ch_off != b.po.in_ch_off ||
-            a.po.cout_g != b.po.cout_g || a.po.out_buf != b.po.out_buf) continue;
+            a.po.cout_g != b.po.cout_g || a.po.out_buf != b.po.out_buf || dw_dilation(a.po) != 1 || dw_dilation(b.po) != 1) continue;
         a.launch = Launch::DwTmaPair;
         b.launch = Launch::None;
     }
@@ -2089,7 +2127,8 @@ int hp_pack_int8_calibrated(const void* pack, size_t pack_bytes)
 
 // test hook: the kernel op `op` launches on the next run over u8 frames, as decided when the engine was created (EngOp::launch and
 // the conv plan's tile width): conv<f16|tf32|i8,BN[,res][,stem3|stem7]>, halo<BN[,pool|,wide|,pp|,pool,pp]>, dw_strip<K,S>, dw_col, dw_tma<1|2>, dw_f32,
-// dw_i8, maxpool<K>, maxpool_f32, maxpool_i8, im2col, im2col_i8, heads, ppn_head, or none when a neighbouring op's launch covers it
+// dw_i8, maxpool<K>, maxpool_f32, maxpool_i8, im2col, im2col_i8, heads, ppn_head, or none when a neighbouring op's launch covers it.
+// A dilated depthwise op names its dilation: dw_tma<1,d2>, dw_col<d2>, dw_f32<d2>, dw_i8<d2>.
 int hp_engine_debug_op_kernel(const hp_engine* e, int op, char* name, int cap)
 {
     if (!e || op < 0 || op >= (int)e->ops.size() || !name || cap <= 0) { set_error("hp_engine_debug_op_kernel: bad argument"); return HP_ERR_ARG; }
@@ -2121,6 +2160,10 @@ int hp_engine_debug_op_kernel(const hp_engine* e, int op, char* name, int cap)
     case Launch::Im2colI8: s = "im2col_i8"; break;
     case Launch::DwI8: s = "dw_i8"; break;
     case Launch::MaxPoolI8: s = "maxpool_i8"; break;
+    }
+    if (po.type == OP_DWCONV && o.launch != Launch::None && dw_dilation(po) != 1) {   // a dilated op: dw_tma<1,d2>, dw_col<d2>, dw_f32<d2>, dw_i8<d2>
+        const std::string d = "d" + std::to_string(dw_dilation(po));
+        s = s.back() == '>' ? s.substr(0, s.size() - 1) + "," + d + ">" : s + "<" + d + ">";
     }
     if ((int)s.size() >= cap) { set_error("hp_engine_debug_op_kernel: %zu-character name, capacity %d", s.size(), cap); return HP_ERR_CAPACITY; }
     memcpy(name, s.c_str(), s.size() + 1);

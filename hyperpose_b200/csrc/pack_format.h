@@ -18,7 +18,8 @@ enum PackOpType : uint32_t {
     OP_MAXPOOL2 = 3, // RxR (R = 2 or 3) stride-2 max-pool, TF "SAME" semantics (out = ceil(in/2), window clipped at the border)
     OP_PIFPAF_HEAD = 5, // OpenPifPaf heads: pixel-shuffle(2) + crop + sigmoid/softplus + index grid of the two raw 1x1-conv outputs
                         // (in_buf = pif raw [.,.,340+], res_buf = paf raw [.,.,684+]) -> engine outputs pif[N,17,5,ho,wo], paf[N,19,9,ho,wo]
-    OP_DWCONV = 4,   // depthwise KxK (K = 1 or 3) conv, stride 1/2, TF "SAME" padding, + bias + PReLU; HBM-bound CUDA-core kernel
+    OP_DWCONV = 4,   // depthwise KxK (K = 1 or 3) conv, stride 1/2, dilation 1 (or 2 for 3x3 / stride 1), TF "SAME" padding,
+                     // + bias + PReLU; HBM-bound CUDA-core kernel
     OP_PPN_HEAD = 6  // Pose Proposal Network head: sigmoid + restore_coor of one raw 1x1-conv output (in_buf [.,.,6K + L*nh*nw+]) ->
                      // engine outputs conf[N,6,K,gh,gw] (conf_point, conf_iou, x, y, w, h) and paf[N,L,nh,nw,gh,gw];
                      // cout_g = K, groups = L, R x S = nh x nw
@@ -54,7 +55,8 @@ struct PackOp {
     uint32_t stride;                // OP_IM2COL3 / OP_DWCONV: 1 or 2 (0 = 1)
     uint32_t res_buf, res_ch_off;   // OP_CONV residual input (fp16 NHWC buffer of the output's geometry)
     uint32_t res_mode;              // 0 none | 1 y = act(conv + bias + res) (ResNet) | 2 y = act(conv + bias) + res (LW-OpenPose blocks)
-    uint32_t reserved2;
+    uint32_t dilation;              // OP_DWCONV: 1 or 2 (0 = 1), 2 only for 3x3 at stride 1 (SAME pads (3-1)*2/2 = 2 per side);
+                                    // 0 for every other op
     uint64_t w_off, b_off, a_off;   // float offsets into the blob: W[G][cout_g][cin_g][R][S], bias[G*cout_g], alpha[G*cout_g]
                                     // OP_DWCONV: W[C][R][S], bias[C], alpha[C] with C = cout_g
 };

@@ -4,7 +4,7 @@
                                     [--int8-calibration frames.npy [--factor F] [--no-flip-rgb]]
 
 `--weights` is a TensorLayer `save_weights(format="npz")` file of the reference's model of that architecture -- OpenPose-VGG19 (also
-the name-keyed `npz_dict` form), MobilenetThin-OpenPose, LightWeightOpenPose on ResNet-50 / TinyVGG / ResNet-18, PifPaf on ResNet-50, Pose Proposal Networks
+the name-keyed `npz_dict` form), MobilenetThin-OpenPose, LightWeightOpenPose on ResNet-50 / TinyVGG / ResNet-18 / MobilenetDilated, PifPaf on ResNet-50, Pose Proposal Networks
 on ResNet-18 / ResNet-50; hyperpose_b200/weights.py
 spells out the all_weights order of each, BatchNorm statistics are folded.  Without it the pack holds seeded random weights, which is
 what the benchmarks and tests use (no trained model can be downloaded offline).  Replaces the .onnx / .uff / .trt files of
@@ -28,7 +28,7 @@ def main(argv=None) -> int:
     ap = argparse.ArgumentParser(description=__doc__.split("\n")[0])
     ap.add_argument("--model", default="openpose_vgg19",
                     choices=["openpose_vgg19", "mobilenet_thin_openpose", "resnet50_lw_openpose", "lw_openpose_vggtiny", "lw_openpose_resnet18",
-                             "resnet50_pifpaf", "ppn_resnet18", "ppn_resnet50", "tiny_test_net"])
+                             "lw_openpose_mobilenet_dilated", "resnet50_pifpaf", "ppn_resnet18", "ppn_resnet50", "tiny_test_net"])
     ap.add_argument("--out", required=True)
     ap.add_argument("--weights", default=None, help="TensorLayer save_weights(format='npz') file of the same architecture")
     ap.add_argument("--seed", type=int, default=0)
@@ -41,7 +41,8 @@ def main(argv=None) -> int:
     if a.weights:
         loaders = {"openpose_vgg19": weights.ListWeights, "mobilenet_thin_openpose": weights.MobilenetThinWeights,
                    "resnet50_lw_openpose": weights.Resnet50LwWeights, "lw_openpose_vggtiny": weights.LwVggtinyWeights,
-                   "lw_openpose_resnet18": weights.LwResnet18Weights, "resnet50_pifpaf": weights.Resnet50PifPafWeights,
+                   "lw_openpose_resnet18": weights.LwResnet18Weights, "lw_openpose_mobilenet_dilated": weights.LwMobilenetDilatedWeights,
+                   "resnet50_pifpaf": weights.Resnet50PifPafWeights,
                    "ppn_resnet18": weights.Ppn18Weights, "ppn_resnet50": weights.Ppn50Weights}
         if a.model not in loaders:
             ap.error(f"--weights: no trained-weight layout for {a.model}")

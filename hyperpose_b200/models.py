@@ -44,10 +44,22 @@ class Op:
     res_buf: int = 0
     res_ch_off: int = 0
     res_mode: int = 0                  # 1: act(conv + res)   2: act(conv) + res
-    weight: np.ndarray | None = None   # [G, cout_g, cin_g, R, S] float32 (OP_DWCONV: [C, K, K])
+    weight: np.ndarray | None = None   # [G, cout_g, cin_g, R, S] float32 (OP_DWCONV: [C, K, K]; dilated: the window, see add_dwconv)
     bias: np.ndarray | None = None     # [G*cout_g]
     alpha: np.ndarray | None = None    # [G*cout_g]  PReLU slope; 0 = ReLU, 1 = linear
     name: str = ""
+    dilation: int = 1                  # OP_DWCONV: taps this many pixels apart (2 only for 3x3 at stride 1); written as 0 when 1
+
+    def taps(self) -> np.ndarray:
+        """the filter as the pack stores it: [G, cout_g, cin_g, R, S], or a depthwise op's [C, K, K] taps (every dilation-th element of
+        a dilated op's window)"""
+        d = self.dilation
+        if self.type != OP_DWCONV or d == 1:
+            return self.weight
+        off = self.weight.copy()
+        off[:, ::d, ::d] = 0
+        assert not off.any(), f"{self.name}: a dilated depthwise window holds nonzero values between its taps"
+        return self.weight[:, ::d, ::d]
 
 
 @dataclass
@@ -71,13 +83,22 @@ class Graph:
     def add_im2col(self, out_buf: int, stride: int = 1, ksize: int = 3, name="im2col") -> None:
         self.ops.append(Op(OP_IM2COL3, out_buf=out_buf, R=ksize, S=ksize, stride=stride, name=name))
 
-    def add_dwconv(self, in_buf, out_buf, weight, bias, alpha, stride=1, in_ch_off=0, out_ch_off=0, name="dw") -> None:
-        """depthwise KxK conv (K in {1,3}) + bias + PReLU; weight [C, K, K]"""
+    def add_dwconv(self, in_buf, out_buf, weight, bias, alpha, stride=1, in_ch_off=0, out_ch_off=0, name="dw", dilation=1) -> None:
+        """depthwise KxK conv (K in {1,3}) + bias + PReLU; weight [C, K, K].  dilation 2 (3x3, stride 1): taps 2 pixels apart, TF 'SAME'
+        over the 5 x 5 window (2 pixels of padding per side).  A dilated op keeps its filter as that window, [C, (K-1)d+1, (K-1)d+1] with
+        zeros between the taps: anything that reads Op.weight as a dense depthwise filter (the CPU references of oracle/ and tests/)
+        computes the dilated convolution.  The pack stores the K x K taps and the dilation (Op.taps)."""
         C, K, K2 = weight.shape
         assert K == K2 and K in (1, 3) and C % 8 == 0
+        assert dilation == 1 or (dilation == 2 and K == 3 and stride == 1), (dilation, K, stride)
+        w = np.ascontiguousarray(weight, np.float32)
+        if dilation != 1:
+            win = np.zeros((C, (K - 1) * dilation + 1, (K - 1) * dilation + 1), np.float32)
+            win[:, ::dilation, ::dilation] = w
+            w = win
         self.ops.append(Op(OP_DWCONV, in_buf, out_buf, in_ch_off, out_ch_off, K, K, 1, C, C, stride=stride,
-                           weight=np.ascontiguousarray(weight, np.float32), bias=np.ascontiguousarray(bias, np.float32).reshape(-1),
-                           alpha=np.ascontiguousarray(alpha, np.float32).reshape(-1), name=name))
+                           weight=w, bias=np.ascontiguousarray(bias, np.float32).reshape(-1),
+                           alpha=np.ascontiguousarray(alpha, np.float32).reshape(-1), name=name, dilation=dilation))
 
     def add_maxpool(self, in_buf: int, out_buf: int, channels: int, name="pool", ksize: int = 2) -> None:
         self.ops.append(Op(OP_MAXPOOL2, in_buf=in_buf, out_buf=out_buf, R=ksize, S=ksize, cout_g=channels, name=name))
@@ -121,12 +142,13 @@ class Graph:
         for op in self.ops:
             w_off = b_off = a_off = 0
             if op.type in (OP_CONV, OP_DWCONV):
-                w_off = off; blob.append(op.weight.reshape(-1)); off += op.weight.size
+                w = op.taps()
+                w_off = off; blob.append(w.reshape(-1)); off += w.size
                 b_off = off; blob.append(op.bias); off += op.bias.size
                 a_off = off; blob.append(op.alpha); off += op.alpha.size
             op_recs.append(struct.pack("<18I3Q", op.type, op.in_buf, op.out_buf, op.in_ch_off, op.out_ch_off, op.R, op.S, op.groups,
                                        op.cin_g, op.cout_g, op.out_mode, op.split, op.im2col_input, op.stride,
-                                       op.res_buf, op.res_ch_off, op.res_mode, 0, w_off, b_off, a_off))
+                                       op.res_buf, op.res_ch_off, op.res_mode, 0 if op.dilation == 1 else op.dilation, w_off, b_off, a_off))
         blob_arr = np.concatenate(blob).astype("<f4") if blob else np.zeros(0, "<f4")
         table = b""
         if self.act_scales is not None:
@@ -277,56 +299,8 @@ def mobilenet_thin_openpose(seed: int = 0, n_stages: int = 6, weights=None) -> G
     g = Graph("mobilenet_thin_openpose", 19, 38, 3, mean=(0.0, 0.0, 0.0))
     relu = lambda n: np.zeros(n, np.float32)
     lin = lambda n: np.ones(n, np.float32)
-
-    # every tensor comes from `ws` by name when a trained model is imported, else from the seeded generator (same draw order as ever)
-    def dw_w(name, C, K):
-        return ws.dwconv(name, C, K) if ws else (rng.standard_normal((C, K, K)) * np.sqrt(2.0 / (K * K))).astype(np.float32)
-
-    def bn(name, C):
-        return ws.bn(name, C) if ws else _bn_fold(rng, C)
-
-    def dw(in_buf, out_buf, C, K, stride=1, in_off=0, out_off=0, name="dw", act=True, wname=None):
-        """wname: one weight name, or a list of (name, channels) whose depthwise filters / BatchNorms are laid side by side"""
-        parts = wname if isinstance(wname, list) else [(wname or name, C)]
-        if ws:
-            w = np.concatenate([dw_w(n_ + ".dw", c_, K) for n_, c_ in parts])
-            sc, sh = (np.concatenate(x) for x in zip(*[bn(n_ + ".dwbn", c_) for n_, c_ in parts]))
-        else:
-            w = dw_w(name, C, K); sc, sh = bn(name, C)
-        g.add_dwconv(in_buf, out_buf, w * sc[:, None, None], sh, relu(C) if act else lin(C), stride=stride, in_ch_off=in_off, out_ch_off=out_off, name=name)
-
-    def pw(in_buf, out_buf, groups, cin_g, cout_g, act=True, out_off=0, cin_real=None, name="pw", wname=None, **kw):
-        """wname: None (random), one name (groups == 1) or one name per group"""
-        if ws:
-            names = wname if isinstance(wname, list) else [wname]
-            w = np.zeros((groups, cout_g, cin_g, 1, 1), np.float32)
-            scs, shs = [], []
-            for gi, n_ in enumerate(names):
-                ci = cin_real if cin_real is not None else cin_g
-                w[gi, :, :ci] = ws.conv(n_ + ".pw", cout_g, ci, 1)[0]
-                sc_, sh_ = bn(n_ + ".pwbn", cout_g); scs.append(sc_); shs.append(sh_)
-            sc, sh = np.concatenate(scs), np.concatenate(shs)
-        else:
-            w = _he(rng, groups, cout_g, cin_g, 1, 1, 2.0 if act else 1.0)
-            if cin_real is not None:
-                w[:, :, cin_real:] = 0
-            sc, sh = bn(name, groups * cout_g)
-        w = w * sc.reshape(groups, cout_g, 1, 1, 1)
-        g.add_conv(in_buf, out_buf, w, sh, relu(groups * cout_g) if act else lin(groups * cout_g), out_ch_off=out_off, name=name, **kw)
-
-    # ---- stem: conv 3x3/2 3->32 (+bias, ReLU), BN, ReLU ----
-    b_col = g.add_buffer(64, 1); g.add_im2col(b_col, stride=2)
-    b0 = g.add_buffer(64, 1)
-    if ws:
-        w0, bias0 = ws.conv("convblock_0.conv", 32, 3, 3)
-        w0 = w0[None]
-    else:
-        w0, bias0 = _he(rng, 1, 32, 3, 3, 3), (rng.standard_normal(32) * 0.05).astype(np.float32)
-    g.add_conv(b_col, b0, w0, bias0, relu(32), im2col_input=1, name="convblock_0")
-    sc, sh = bn("convblock_0.bn", 32)
-    b0b = g.add_buffer(64, 1)
-    g.add_dwconv(b0, b0b, sc.reshape(32, 1, 1), sh, relu(32), name="convblock_0_bn")
-    cur, cur_off, cur_c, cur_d = b0b, 0, 32, 1
+    dw_w, bn, dw, pw = _sep_helpers(g, rng, ws)
+    cur, cur_off, cur_c, cur_d = _mobilenet_stem(g, rng, ws, bn), 0, 32, 1
     cat_c = _r64(1152 + 57)
     cat = g.add_buffer(cat_c, 3)   # [maxpool(block3) 128 | block7 512 | block11 512 | conf 19 | paf 38 | 7 zero]
     # (n_filter, stride) of convblock_1..11 at scale_size 8 (backbones.py:264-275)
@@ -390,6 +364,71 @@ def mobilenet_thin_openpose(seed: int = 0, n_stages: int = 6, weights=None) -> G
     for s_ in range(1, n_stages):
         stage(1209, 128, s_ == n_stages - 1, f"ref{s_}")
     return g
+
+
+def _sep_helpers(g, rng, ws):
+    """the builders of MobileNet separable blocks (BatchNorm folded) on graph `g` -> (dw_w, bn, dw, pw).  Every tensor comes from `ws` by
+    name when a trained model is imported (weights.BnNetWeights), else from the seeded generator `rng`, drawn in call order."""
+    relu = lambda n: np.zeros(n, np.float32)
+    lin = lambda n: np.ones(n, np.float32)
+
+    def dw_w(name, C, K):
+        return ws.dwconv(name, C, K) if ws else (rng.standard_normal((C, K, K)) * np.sqrt(2.0 / (K * K))).astype(np.float32)
+
+    def bn(name, C):
+        return ws.bn(name, C) if ws else _bn_fold(rng, C)
+
+    def dw(in_buf, out_buf, C, K, stride=1, in_off=0, out_off=0, name="dw", act=True, wname=None, dilation=1):
+        """depthwise conv + BN (+ReLU).  wname: one weight name, or a list of (name, channels) whose depthwise filters / BatchNorms are
+        laid side by side"""
+        parts = wname if isinstance(wname, list) else [(wname or name, C)]
+        if ws:
+            w = np.concatenate([dw_w(n_ + ".dw", c_, K) for n_, c_ in parts])
+            sc, sh = (np.concatenate(x) for x in zip(*[bn(n_ + ".dwbn", c_) for n_, c_ in parts]))
+        else:
+            w = dw_w(name, C, K); sc, sh = bn(name, C)
+        g.add_dwconv(in_buf, out_buf, w * sc[:, None, None], sh, relu(C) if act else lin(C), stride=stride, in_ch_off=in_off, out_ch_off=out_off,
+                     name=name, dilation=dilation)
+
+    def pw(in_buf, out_buf, groups, cin_g, cout_g, act=True, out_off=0, cin_real=None, name="pw", wname=None, **kw):
+        """wname: None (random), one name (groups == 1) or one name per group"""
+        if ws:
+            names = wname if isinstance(wname, list) else [wname]
+            w = np.zeros((groups, cout_g, cin_g, 1, 1), np.float32)
+            scs, shs = [], []
+            for gi, n_ in enumerate(names):
+                ci = cin_real if cin_real is not None else cin_g
+                w[gi, :, :ci] = ws.conv(n_ + ".pw", cout_g, ci, 1)[0]
+                sc_, sh_ = bn(n_ + ".pwbn", cout_g); scs.append(sc_); shs.append(sh_)
+            sc, sh = np.concatenate(scs), np.concatenate(shs)
+        else:
+            w = _he(rng, groups, cout_g, cin_g, 1, 1, 2.0 if act else 1.0)
+            if cin_real is not None:
+                w[:, :, cin_real:] = 0
+            sc, sh = bn(name, groups * cout_g)
+        w = w * sc.reshape(groups, cout_g, 1, 1, 1)
+        g.add_conv(in_buf, out_buf, w, sh, relu(groups * cout_g) if act else lin(groups * cout_g), out_ch_off=out_off, name=name, **kw)
+
+    return dw_w, bn, dw, pw
+
+
+def _mobilenet_stem(g, rng, ws, bn):
+    """conv_block(32, 3, strides=2) of MobilenetThin / MobilenetDilated (the second `conv_block` of backbones.py, :234-239): conv 3x3/2
+    3->32 (+bias, ReLU), then BatchNorm(ReLU) as a 1x1 depthwise affine.  `bn`: _sep_helpers' BatchNorm source.  -> the 32-channel
+    output buffer at stride 2 (64 channels wide)"""
+    relu = lambda n: np.zeros(n, np.float32)
+    b_col = g.add_buffer(64, 1); g.add_im2col(b_col, stride=2)
+    b0 = g.add_buffer(64, 1)
+    if ws:
+        w0, bias0 = ws.conv("convblock_0.conv", 32, 3, 3)
+        w0 = w0[None]
+    else:
+        w0, bias0 = _he(rng, 1, 32, 3, 3, 3), (rng.standard_normal(32) * 0.05).astype(np.float32)
+    g.add_conv(b_col, b0, w0, bias0, relu(32), im2col_input=1, name="convblock_0")
+    sc, sh = bn("convblock_0.bn", 32)
+    b0b = g.add_buffer(64, 1)
+    g.add_dwconv(b0, b0b, sc.reshape(32, 1, 1), sh, relu(32), name="convblock_0_bn")
+    return b0b
 
 
 def _resnet50_body(g, rng, ws, cur, cur_c, cur_d, layout):
@@ -576,6 +615,33 @@ def lw_openpose_resnet18(seed: int = 0, weights=None) -> Graph:
     ws = weights
     g = Graph("lw_openpose_resnet18", 19, 38, 3, mean=(0.0, 0.0, 0.0))
     cur, cur_c, cur_d = _resnet18_body(g, rng, ws, *_ppn_stem(g, rng, ws), RESNET18_STRIDES_8)
+    _lw_head(g, rng, ws, cur, cur_c)
+    return g
+
+
+# (n_filter, stride, dilation) of the eleven dw_conv_blocks of MobilenetDilated_backbone (backbones.py:201-229; scale_size is forced to 8,
+# so the two `strides` variables there are (1, 1))
+MOBILENET_DILATED_BLOCKS = [(64, 1, 1), (128, 2, 1), (128, 1, 1), (256, 2, 1), (256, 1, 1), (512, 1, 1), (512, 1, 2), (512, 1, 1),
+                            (512, 1, 1), (512, 1, 1), (512, 1, 1)]
+
+
+def lw_openpose_mobilenet_dilated(seed: int = 0, weights=None) -> Graph:
+    """Lightweight-OpenPose on its default backbone, MobilenetDilated_backbone (lw_openpose.py:33-37, backbones.py:201-229): the
+    MobilenetThin stem (_mobilenet_stem), eleven dw_conv_blocks -- DepthwiseConv2d (no bias) + BatchNorm(relu), Conv2d 1x1 (no bias) +
+    BatchNorm(relu) -- down to stride 8 with 512 channels, the first 512 -> 512 block's depthwise conv dilated by 2, then the LW head
+    (_lw_head).  BatchNorm folded.  `weights`: a hyperpose_b200.weights.LwMobilenetDilatedWeights; default = seeded random values."""
+    rng = np.random.default_rng(seed)
+    ws = weights
+    g = Graph("lw_openpose_mobilenet_dilated", 19, 38, 3, mean=(0.0, 0.0, 0.0))
+    _, bn, dw, pw = _sep_helpers(g, rng, ws)
+    cur, cur_c, cur_d = _mobilenet_stem(g, rng, ws, bn), 32, 1
+    for i, (co, st, dil) in enumerate(MOBILENET_DILATED_BLOCKS, start=1):
+        d_out = cur_d + (1 if st == 2 else 0)
+        t = g.add_buffer(_r64(cur_c), d_out)
+        dw(cur, t, cur_c, 3, stride=st, name=f"convblock_{i}_dw", wname=f"convblock_{i}", dilation=dil)
+        nxt = g.add_buffer(_r64(co), d_out)
+        pw(t, nxt, 1, _r64(cur_c), co, cin_real=cur_c, name=f"convblock_{i}_pw", wname=f"convblock_{i}")
+        cur, cur_c, cur_d = nxt, co, d_out
     _lw_head(g, rng, ws, cur, cur_c)
     return g
 

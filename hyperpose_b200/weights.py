@@ -5,6 +5,7 @@
   * LW-OpenPose on ResNet-50  openpose/model/lw_openpose.py + backbones.py:587-698                   -> Resnet50LwWeights
   * LW-OpenPose on TinyVGG    openpose/model/lw_openpose.py + backbones.py:343-391                   -> LwVggtinyWeights
   * LW-OpenPose on ResNet-18  openpose/model/lw_openpose.py + backbones.py:512-585                   -> LwResnet18Weights
+  * LW-OpenPose on MobilenetDilated (its default backbone) lw_openpose.py + backbones.py:201-229  -> LwMobilenetDilatedWeights
   * PifPaf on ResNet-50       pifpaf/model.py:41-281 + backbones.py:587-698                          -> Resnet50PifPafWeights
   * PPN on ResNet-18 / -50    pose_proposal/model.py:14-119 + backbones.py:512-698                   -> Ppn18Weights / Ppn50Weights
 
@@ -343,6 +344,20 @@ def lw_resnet18_layer_order(n_conf: int = 19, n_paf: int = 38):
     return order
 
 
+def lw_mobilenet_dilated_layer_order(n_conf: int = 19, n_paf: int = 38):
+    """all_weights order of LightWeightOpenPose on its default MobilenetDilated_backbone (lw_openpose.py:33-37, backbones.py:201-229):
+    conv_block(32, 3) -- Conv2d(+bias) then BatchNorm --, eleven dw_conv_blocks as separable blocks (the dilation changes no weight's
+    shape), cpm_stage on 512 channels, init_stage, refine_stage1"""
+    from .models import MOBILENET_DILATED_BLOCKS
+    order = [("conv", "convblock_0.conv", 32, 3, 3), ("bn", "convblock_0.bn", 32, 0, 0)]
+    cin = 32
+    for i, (co, _, _) in enumerate(MOBILENET_DILATED_BLOCKS, start=1):
+        _sep_block(order, f"convblock_{i}", cin, co, 3)
+        cin = co
+    _lw_head_order(order, 512, n_conf, n_paf)
+    return order
+
+
 def resnet50_pifpaf_layer_order(n_pos: int = 17, n_limbs: int = 19):
     """all_weights order of the PifPaf model (pifpaf/model.py:41-51): Resnet50_backbone(use_pool=False, scale_size=32), pif_head, paf_head
     (one 1x1 Conv2d with bias each, :229,:262)"""
@@ -428,6 +443,15 @@ class LwVggtinyWeights(BnNetWeights):
 class LwResnet18Weights(BnNetWeights):
     def __init__(self, arrays):
         super().__init__(arrays, lw_resnet18_layer_order())
+
+    @classmethod
+    def from_npz(cls, path: str):
+        return cls(load_params_npz(path))
+
+
+class LwMobilenetDilatedWeights(BnNetWeights):
+    def __init__(self, arrays):
+        super().__init__(arrays, lw_mobilenet_dilated_layer_order())
 
     @classmethod
     def from_npz(cls, path: str):

@@ -1,5 +1,6 @@
-"""Lightweight-OpenPose throughput on TinyVGG and ResNet-18: lw_openpose_vggtiny at 256 x 384 (the reference's published size) and
-342 x 368 (the model zoo's TinyVGG-V2-HW=342x368), lw_openpose_resnet18 at 368 x 432; fp16 engine, batch 16.
+"""Lightweight-OpenPose throughput on TinyVGG, ResNet-18 and MobilenetDilated: lw_openpose_vggtiny at 256 x 384 (the reference's
+published size) and 342 x 368 (the model zoo's TinyVGG-V2-HW=342x368), lw_openpose_resnet18 and lw_openpose_mobilenet_dilated (the
+published "LightweightOpenPose (Dilated MobileNet)") at 368 x 432; fp16 engine, batch 16.
 
 The path is device-resident and pipelined: u8 frames already in HBM -> hp_pose_submit_u8_device / hp_pose_collect (CUDA-graph replay
 of convs + PAF parse + record copy, two batches in flight).  Random weights give structureless maps, so synthetic crowd tensors
@@ -8,10 +9,12 @@ of convs + PAF parse + record copy, two batches in flight).  Random weights give
 One JSON line per workload: frames/s of three rounds (CUDA events around `--steps` steps after a >= 2 s warm-up; the workloads
 alternate inside a round), conv ms per step (the engine's per-op CUDA-event profile, a separate run), the algorithmic GFLOP per
 frame from the graph, and the card, its power limit and the SM clock read by nvidia-smi right after the timed rounds.
---per-op adds every op's kernel (Engine.debug_op_kernel) and its time per step.
+--per-op adds every op's kernel (Engine.debug_op_kernel) and its time per step.  The MobilenetDilated line also carries the time of its
+dilated depthwise layer next to the same layer run undilated (the same graph with dilation 1, profiled on its own engine).
 
     python tools/bench_lw.py [--steps 50] [--per-op]"""
 import argparse
+import copy
 import json
 import os
 import subprocess
@@ -27,7 +30,7 @@ from hyperpose_b200 import capi, models, synthetic as syn  # noqa: E402
 B = 16
 HCAP = 64
 WORKLOADS = [("lw_vggtiny", "lw_openpose_vggtiny", 256, 384), ("lw_vggtiny", "lw_openpose_vggtiny", 342, 368),
-             ("lw_resnet18", "lw_openpose_resnet18", 368, 432)]
+             ("lw_resnet18", "lw_openpose_resnet18", 368, 432), ("lw_mobilenet_dilated", "lw_openpose_mobilenet_dilated", 368, 432)]
 
 
 def smi():
@@ -39,9 +42,9 @@ def smi():
 
 
 class Workload:
-    def __init__(self, label, net, H, W, seed):
+    def __init__(self, label, net, H, W, seed, graph=None):
         self.label, self.H, self.W = label, H, W
-        self.g = getattr(models, net)(0)
+        self.g = graph if graph is not None else getattr(models, net)(0)
         self.eng = capi.Engine(self.g.to_pack(), (W, H), max_batch_size=B)
         self.parser = capi.PafParser(0.05, 0.05)
         self.parser.set_capacity(peaks_per_part=128, candidates_per_limb=2048, humans=HCAP)
@@ -120,6 +123,16 @@ def main():
                "fps": fps[k], "fps_median": float(np.median(fps[k])), "humans_per_frame": [min(humans[k]), max(humans[k])],
                "conv_ms_per_step": round(float(ms[ty == models.OP_CONV].sum()), 3), "engine_ms_per_step": round(float(ms.sum()), 3),
                "gflop_per_frame": round(w.g.flops_per_frame(w.H, w.W) / 1e9, 2), **clocks}
+        dilated = [i for i, op in enumerate(w.g.ops) if op.dilation != 1]
+        if dilated:
+            plain = copy.deepcopy(w.g)
+            for op in plain.ops:
+                op.weight, op.dilation = op.taps(), 1
+            pw = Workload(w.label, None, w.H, w.W, 900, graph=plain)
+            pms, _ = pw.profile()
+            res["dilated_layers"] = [{"op": w.g.ops[i].name, "kernel": w.eng.debug_op_kernel(i), "ms": round(float(ms[i]), 4),
+                                      "undilated_kernel": pw.eng.debug_op_kernel(i), "undilated_ms": round(float(pms[i]), 4)} for i in dilated]
+            pw.close()
         if a.per_op:
             res["per_op"] = [{"op": op.name, "kernel": w.eng.debug_op_kernel(i), "ms": round(float(ms[i]), 4)} for i, op in enumerate(w.g.ops)]
         print(json.dumps(res))
