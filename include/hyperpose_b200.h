@@ -246,8 +246,10 @@ int hp_engine_debug_read_buffer(hp_engine* e, int buf, void* out_f16, int N, int
 int hp_engine_debug_write_buffer(hp_engine* e, int buf, const void* in_f16, int N);
 int hp_engine_debug_run_ops(hp_engine* e, int first_op, int last_op, int N);
 /* test hook: the kernel op `op` launches on the next run over u8 frames, fixed at creation, as a NUL-terminated name in
- * name[cap]: "conv<f16|tf32|i8,BN[,res][,stem3|stem7]>", "halo<BN[,pool]>", "dw_strip<K,S>", "dw_col", "dw_tma<1|2>", "dw_f32", "dw_i8",
- * "maxpool<K>", "maxpool_f32", "maxpool_i8", "im2col", "im2col_i8", "heads", or "none" for an op that a neighbouring op's launch covers */
+ * name[cap]: "conv<f16|tf32|i8,BN[,res][,stem3|stem7]>", "halo<BN[,pool|,wide|,pp|,pool,pp]>", "dw_strip<K,S>", "dw_col", "dw_tma<1|2>",
+ * "dw_f32", "dw_i8", "maxpool<K>", "maxpool_f32", "maxpool_i8", "im2col" (fp16 and TF32), "im2col_i8", "heads", "ppn_head", or "none" for
+ * an op that a neighbouring op's launch covers.  A dilated depthwise op adds its dilation: "dw_tma<1,d2>", "dw_col<d2>", "dw_f32<d2>",
+ * "dw_i8<d2>". */
 int hp_engine_debug_op_kernel(const hp_engine* e, int op, char* name, int cap);
 /* test hook: *tma_store = 1 when op `op` runs the halo conv kernel with its TMA-store epilogue, 0 otherwise (HPB_HALO_REG_EPILOGUE=1
  * or a plan the TMA store cannot express: per-thread stores from registers) */

@@ -264,7 +264,7 @@ def test_dilated_kernel_against_fp64(case, monkeypatch):
 @gpu
 @pytest.mark.parametrize("C,shape", [(512, (B, 46, 54)), (512, (5, 46, 54)), (64, (2, 13, 21)), (72, (2, 13, 21)), (64, (3, 3, 5))])
 def test_dilated_int8_kernel_matches_model(C, shape):
-    """dwconv_i8_kernel with dilation 2, byte for byte against tests/int8_sim.py (batch-16 engine)"""
+    """dwconv_c4_kernel<int8_t> with dilation 2, byte for byte against tests/int8_sim.py (batch-16 engine)"""
     from hyperpose_b200 import capi
     from tests import int8_sim
     from tests.test_engine_kernels import _graph, _slopes
