@@ -211,7 +211,7 @@ EXPORTS += [
     "hp_paf_grow_capacity", "hp_pool_create", "hp_pool_destroy", "hp_pool_size", "hp_pool_set_capacity", "hp_pool_run_u8_host",
     "hp_pool_set_output_override", "hp_pool_launch_count", "hp_default_device", "hp_handoff_device_of",
     "hp_engine_create_ex", "hp_engine_dtype", "hp_pose_submit_u8_device", "hp_engine_debug_op_kernel",
-    "hp_engine_debug_op_epilogue",
+    "hp_engine_debug_op_epilogue", "hp_engine_debug_op_conv_epilogue",
     "hp_engine_calibrate_u8", "hp_pack_int8_calibrated",
 ]
 
@@ -238,6 +238,7 @@ def _bind_engine(L):
     L.hp_engine_debug_run_ops.argtypes = [vp, C.c_int, C.c_int, C.c_int]
     L.hp_engine_debug_op_kernel.argtypes = [vp, C.c_int, C.c_char_p, C.c_int]
     L.hp_engine_debug_op_epilogue.argtypes = [vp, C.c_int, ip]
+    L.hp_engine_debug_op_conv_epilogue.argtypes = [vp, C.c_int, ip]
     L.hp_engine_calibrate_u8.argtypes = [vp, vp, C.c_int, vp, C.c_int]
     L.hp_pack_int8_calibrated.argtypes = [vp, C.c_size_t]
     L.hp_pose_run_u8_host.argtypes = [vp, vp, vp, C.c_int, vp, C.c_int, ip]
@@ -425,6 +426,12 @@ class Engine:
         """"tma" when op `op` runs the halo kernel with its TMA-store epilogue, "reg" otherwise"""
         v = C.c_int(0)
         check(lib().hp_engine_debug_op_epilogue(self._h, op, C.byref(v)))
+        return "tma" if v.value else "reg"
+
+    def debug_op_conv_epilogue(self, op: int) -> str:
+        """"tma" when op `op` runs the im2col conv kernel with its TMA-store epilogue, "reg" otherwise"""
+        v = C.c_int(0)
+        check(lib().hp_engine_debug_op_conv_epilogue(self._h, op, C.byref(v)))
         return "tma" if v.value else "reg"
 
     def set_output_override(self, d_conf_ptr: int, d_paf_ptr: int):

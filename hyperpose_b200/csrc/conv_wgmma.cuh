@@ -16,7 +16,8 @@
 // * persistent CTAs (one per SM), warp-specialised: one thread of warpgroup 0 issues the TMA loads into a ring of
 //   mbarrier-guarded stages; warpgroups 1 and 2 each own 64 of the 128 pixel rows, run wgmma.mma_async m64nBN with the fp32
 //   accumulators in registers, and apply the epilogue (bias (+ residual) + PReLU -> fp16 / TF32 NHWC, or fp32 NCHW planes for
-//   the parser) straight from those registers while the producer already streams the next tile.
+//   the parser) while the producer already streams the next tile: fp16 NHWC outputs at BN = 64 / 128 go through a shared-memory
+//   staging slot and TMA stores (conv_epilogue_tma), everything else straight from the registers.
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -72,6 +73,7 @@ struct ConvParams {
     float out_inv_scale, res_scale;
     int in_g_stride;           // input channels between groups (the real cin_g: a group's padded last k-step reads on into the next
                                // group's channels, or past the buffer's end as zeros, against zero weights)
+    int tma_store;             // 1: fp16 NHWC outputs go through shared memory and TMA stores (conv_epilogue_tma, BN = 64 or 128)
 };
 
 // accumulator element of conv_wgmma_kernel<T, ...>: fp32 for the fp16 / TF32 engines, s32 for the INT8 engine
@@ -155,6 +157,18 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* m, 
         ::"r"(dst), "l"(m), "r"(bar), "r"(c0), "r"(c1)
         : "memory");
 }
+// four 8 x 8 fp16 matrices, one per register: the thread holds row lane / 4, columns 2 (lane % 4) + {0, 1} of each (the accumulator
+// fragment's layout); lane 8 i + r gives the address of row r of matrix i
+__device__ __forceinline__ void stmatrix_x4(uint32_t addr, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3)
+{
+    asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(r0), "r"(r1), "r"(r2), "r"(r3) : "memory");
+}
+__device__ __forceinline__ void named_barrier_sync(int id, int threads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory"); }
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// the thread's bulk groups but the newest N have finished reading shared memory / have completed (their writes are performed)
+template <int N> __device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
+template <int N> __device__ __forceinline__ void bulk_wait() { asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory"); }
+__device__ __forceinline__ uint32_t half2_bits(__half2 h) { return *reinterpret_cast<uint32_t*>(&h); }
 // programmatic dependent launch (no-ops when the kernel was launched without the attribute)
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
@@ -480,18 +494,93 @@ __device__ __forceinline__ int8_t quantize_i8(float y, float inv_s)
     return (int8_t)min(max(__float2int_rn(__fmul_rn(y, inv_s)), -127), 127);
 }
 
+// The fp16 epilogue of one consumer warpgroup's m64 block (tile pixels p0 + 64 half .. + 63, all inside the batch) written through
+// shared memory: the arithmetic of conv_wgmma_kernel's register epilogue, operation for operation, then the fp16 block goes into the
+// warpgroup's staging slot (BN / 64 slices of {64 channels x 64 pixels}, each in the 128B-swizzled layout of one TMA box: pixel row q,
+// 16-byte chunk j at q * 128 + ((j ^ q % 8) * 16)) and the leader thread stores each slice with one box of tmap_o, a 2-D map over
+// [pixels of max_batch frames, the output's channels up to the layer's last].  The map clips the padding channels of a partial
+// n-tile; the caller keeps pixels past the batch (a partial last tile, or N < max_batch) on the register epilogue.
+template <int BN, bool kRes>
+__device__ __forceinline__ void conv_epilogue_tma(const float (&acc)[BN / 2], const ConvParams& p, const ConvTile& t, const CUtensorMap* tmap_o,
+                                                  uint32_t slot, int half, int warp, int lane)
+{
+    static_assert(BN == 64 || BN == 128, "one TMA box per 64-channel slice, at most two");
+    constexpr int kSliceBytes = 64 * 128;
+    const bool leader = (threadIdx.x & 127) == 0;
+    const int bar_id = 1 + half;   // named barrier 1 / 2: consumer warpgroup 1 / 2
+    const int col0 = 2 * (lane & 3);
+    const float* bias = p.bias + t.g * p.cout_g_pad + t.n0;
+    const float* alpha = p.alpha + t.g * p.cout_g_pad + t.n0;
+    const int n_valid = min(BN, p.cout_g - t.n0);   // a multiple of 8: both channels of a pair are real, or neither
+    const int och = p.out_ch_off + t.g * p.cout_g + t.n0;
+    const int px0 = t.p0 + half * 64;
+    if (leader) ptx::bulk_wait_read<0>();
+    ptx::named_barrier_sync(bar_id, 128);   // the previous tile's store has read the slot
+    // stmatrix: register i of a thread holds rows lane / 4 (+ 8 h) and channels 8 (4 jb + i) + col0 + {0, 1}; lane 8 i + r addresses
+    // pixel row r of matrix i, so (row % 8) == r
+    const int r = lane & 7, i = lane >> 3;
+#pragma unroll
+    for (int jb = 0; jb < BN / 32; ++jb) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const size_t pix = (size_t)(px0 + (warp & 3) * 16 + 8 * h + (lane >> 2));
+            uint32_t v[4];
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+                const int j = 4 * jb + k, c = 8 * j + col0;
+                const bool real = c < n_valid;
+                float a0 = acc[4 * j + 2 * h] + __ldg(bias + c), a1 = acc[4 * j + 2 * h + 1] + __ldg(bias + c + 1);
+                float r0 = 0.f, r1 = 0.f;
+                if (kRes && p.res_mode && real) {
+                    const size_t ri = pix * p.res_ld + p.res_ch_off + t.g * p.cout_g + t.n0 + c;
+                    const float2 rf = __half22float2(*((const __half2*)p.res + ri / 2)); r0 = rf.x; r1 = rf.y;
+                }
+                if (kRes && p.res_mode == 1) { a0 += r0; a1 += r1; }
+                a0 = a0 > 0.f ? a0 : a0 * __ldg(alpha + c);
+                a1 = a1 > 0.f ? a1 : a1 * __ldg(alpha + c + 1);
+                if (kRes && p.res_mode == 2) { a0 += r0; a1 += r1; }
+                __half2 h2 = __floats2half2_rn(a0, a1);
+                if (p.post_w && real) {   // the fused 1x1 depthwise stage, as in the register epilogue
+                    const int pc = t.g * p.cout_g + t.n0 + c;
+                    const float2 x = __half22float2(h2);
+                    float y0 = fmaf(x.x, __ldg(p.post_w + pc), 0.f) + __ldg(p.post_b + pc);
+                    float y1 = fmaf(x.y, __ldg(p.post_w + pc + 1), 0.f) + __ldg(p.post_b + pc + 1);
+                    y0 = y0 > 0.f ? y0 : y0 * __ldg(p.post_a + pc);
+                    y1 = y1 > 0.f ? y1 : y1 * __ldg(p.post_a + pc + 1);
+                    h2 = __floats2half2_rn(y0, y1);
+                }
+                v[k] = ptx::half2_bits(h2);
+            }
+            const int j = 4 * jb + i, row = (warp & 3) * 16 + 8 * h + r;
+            ptx::stmatrix_x4(slot + (uint32_t)((j >> 3) * kSliceBytes + row * 128 + (((j & 7) ^ r) << 4)), v[0], v[1], v[2], v[3]);
+        }
+    }
+    ptx::fence_proxy_async();   // the generic-proxy writes -> visible to the TMA store
+    ptx::named_barrier_sync(bar_id, 128);
+    if (leader) {
+        ptx::tma_store_2d(tmap_o, slot, och, px0);
+        if (BN == 128 && t.n0 + 64 < p.cout_g)   // (not a slice of padding channels only)
+            ptx::tma_store_2d(tmap_o, slot + (uint32_t)kSliceBytes, och + 64, px0);
+        ptx::bulk_commit();
+    }
+}
+
 template <typename T, int BN, bool kRes, int kStemR = 0>
 __global__ void __launch_bounds__(CONV_THREADS, 1)
-conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b, const ConvParams p)
+conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b, const __grid_constant__ CUtensorMap tmap_o,
+                  const ConvParams p)
 {
     constexpr bool kF16 = std::is_same<T, __half>::value;
     constexpr bool kI8 = std::is_same<T, int8_t>::value;
     constexpr int BK = 128 / (int)sizeof(T);                 // channels per k-step
     constexpr int STAGE_BYTES = CONV_A_BYTES + BN * 128;      // a multiple of 1024: every tile stays aligned to the swizzle atom
+    // the TMA-store epilogue (p.tma_store) exists for fp16 at BN = 64 and 128; other kernels always store from registers
+    constexpr bool kTmaForm = kF16 && (BN == 64 || BN == 128);
     extern __shared__ uint8_t smem_raw[];
     ptx::pdl_launch_dependents();   // the next kernel may start its prologue on every SM this grid has left
     uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-    uint64_t* full_bar = (uint64_t*)(smem + (size_t)p.num_stages * STAGE_BYTES);   // [stages]  TMA -> wgmma
+    uint8_t* s_stage = smem + (size_t)p.num_stages * STAGE_BYTES;                  // tma_store: [2][BN x 128 B], one slot per consumer warpgroup
+    uint64_t* full_bar = (uint64_t*)(s_stage + (p.tma_store ? 2 * BN * 128 : 0)); // [stages]  TMA -> wgmma
     uint64_t* empty_bar = full_bar + CONV_MAX_STAGES;                             // [stages]  wgmma -> TMA
 
     const int wg = threadIdx.x >> 7, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -503,6 +592,7 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
     if (threadIdx.x == 0) {
         ptx::prefetch_tmap(&tmap_a);
         ptx::prefetch_tmap(&tmap_b);
+        if (kTmaForm && p.tma_store) ptx::prefetch_tmap(&tmap_o);
         for (int i = 0; i < p.num_stages; ++i) {
             ptx::mbar_init(ptx::smem_u32(full_bar + i), kStemR ? 129 : 1);   // stem: 128 gathering threads + the weight load
             ptx::mbar_init(ptx::smem_u32(empty_bar + i), 8);   // one arrive per consumer warp
@@ -585,6 +675,7 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
     const int col0 = 2 * (lane & 3);                           // columns col0 + 8 j + {0, 1}
     const int total_px = p.Nb * p.H * p.W;
     const uint32_t smem0 = ptx::smem_u32(smem);
+    const bool tma = kTmaForm && p.tma_store;
     typename ConvAcc<T>::type acc[BN / 2];
     RingPos ring;
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
@@ -612,6 +703,12 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
         ptx::fence_acc(acc);
         if (lane == 0) ptx::mbar_arrive(ptx::smem_u32(empty_bar + prev));
 
+        if constexpr (kTmaForm) {
+            if (tma && t.p0 + half * 64 + 64 <= total_px) {   // (the tensor map spans max_batch frames: a block past the batch stays below)
+                conv_epilogue_tma<BN, kRes>(acc, p, t, &tmap_o, ptx::smem_u32(s_stage + (size_t)half * BN * 128), half, warp, lane);
+                continue;
+            }
+        }
         // epilogue: this thread holds rows row0 / row0 + 8, columns col0 + 8 j + {0, 1}: acc[4 j + 2 h + {0, 1}]
         const float* bias = p.bias + t.g * p.cout_g_pad + t.n0;
         const float* alpha = p.alpha + t.g * p.cout_g_pad + t.n0;
@@ -715,15 +812,21 @@ conv_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
             }
         }
     }
+    if (tma && (threadIdx.x & 127) == 0) ptx::bulk_wait<0>();   // every store has completed before the CTA exits (the next kernel reads them)
 }
 
 constexpr size_t CONV_SMEM_FIXED = 1024 /*base alignment*/ + 2 * CONV_MAX_STAGES * 8;
-inline size_t conv_smem_bytes(int BN, int stages) { return CONV_SMEM_FIXED + (size_t)stages * (CONV_A_BYTES + BN * 128); }
+// conv_wgmma_kernel's dynamic shared memory: alignment, the A/B ring, with tma_store the two consumer warpgroups' staging slots
+// (BN x 128 B each), and the barriers
+inline size_t conv_smem_bytes(int BN, int stages, bool tma_store)
+{
+    return CONV_SMEM_FIXED + (size_t)stages * (CONV_A_BYTES + BN * 128) + (tma_store ? 2 * (size_t)BN * 128 : 0);
+}
 // as many stages as fit, up to CONV_MAX_STAGES
-inline int conv_pick_stages(int BN)
+inline int conv_pick_stages(int BN, bool tma_store)
 {
     int s = CONV_MAX_STAGES;
-    while (s > 2 && conv_smem_bytes(BN, s) > CONV_SMEM_LIMIT) --s;
+    while (s > 2 && conv_smem_bytes(BN, s, tma_store) > CONV_SMEM_LIMIT) --s;
     return s;
 }
 
@@ -833,24 +936,12 @@ __device__ __forceinline__ uint64_t make_sw128_kmajor_desc_at(uint32_t smem_addr
 }
 template <uint32_t N> __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
 template <uint32_t N> __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
-// four 8 x 8 fp16 matrices, one per register: the thread holds row lane / 4, columns 2 (lane % 4) + {0, 1} of each (the accumulator
-// fragment's layout); lane 8 i + r gives the address of row r of matrix i
-__device__ __forceinline__ void stmatrix_x4(uint32_t addr, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3)
-{
-    asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(r0), "r"(r1), "r"(r2), "r"(r3) : "memory");
-}
 __device__ __forceinline__ void st_shared_u32(uint32_t addr, uint32_t v) { asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v) : "memory"); }
-__device__ __forceinline__ void named_barrier_sync(int id, int threads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory"); }
 __device__ __forceinline__ void tma_store_4d(const CUtensorMap* m, uint32_t src, int c0, int c1, int c2, int c3)
 {
     asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];"
                  ::"l"(m), "r"(src), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
 }
-__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-// the thread's bulk groups but the newest N have finished reading shared memory / have completed (their writes are performed)
-template <int N> __device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
-template <int N> __device__ __forceinline__ void bulk_wait() { asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory"); }
-__device__ __forceinline__ uint32_t half2_bits(__half2 h) { return *reinterpret_cast<uint32_t*>(&h); }
 } // namespace ptx
 
 // Stores m64 blocks 0 .. kBlocks - 1 of one warpgroup's accumulators: block m holds tile rows row_base + 8 m .. row_base + 8 m + 7 of

@@ -594,6 +594,22 @@ int make_tmap_act_box(CUtensorMap* m, const __half* base, int N, int H, int W, i
     return HP_OK;
 }
 
+// a C-channel view (channel stride ld) of fp16 activations as a 2-D tensor (C, pixels), box {64 channels, 64 pixels}, 128B swizzle:
+// the TMA stores of conv_wgmma_kernel's epilogue (conv_epilogue_tma)
+int make_tmap_pixel_rows(CUtensorMap* m, const __half* base, long pixels, int C, int ld)
+{
+    const auto enc = (PFN_encodeTiled)driver_entry_point("cuTensorMapEncodeTiled");
+    if (!enc) { set_error("cuTensorMapEncodeTiled entry point not available"); return HP_ERR_CUDA; }
+    cuuint64_t dims[2] = { (cuuint64_t)C, (cuuint64_t)pixels };
+    cuuint64_t strides[1] = { (cuuint64_t)ld * 2 };
+    cuuint32_t box[2] = { 64, 64 };
+    cuuint32_t estr[2] = { 1, 1 };
+    CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, (void*)base, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                     CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled(pixel rows) failed: %d (pixels=%ld C=%d ld=%d)", (int)r, pixels, C, ld); return HP_ERR_CUDA; }
+    return HP_OK;
+}
+
 int round_up(int a, int b) { return (a + b - 1) / b * b; }
 
 int pick_bn(int cout_g)
@@ -616,7 +632,8 @@ struct ConvPlan {
     ConvParams prm;
     CUtensorMap tmap_a, tmap_b;
     CUtensorMap tmap_x;          // halo plan: the input as a 4-D tensor with a (16+R-1) x (8+S-1)-pixel box
-    CUtensorMap tmap_o;          // halo plan, hp.tma_store: the output's channels [0, out_ch_off + groups * cout_g) with an 8 x 8-pixel box (pooled 4 x 4)
+    CUtensorMap tmap_o;          // the output's channels [0, out_ch_off + groups * cout_g): halo plan, hp.tma_store: with an 8 x 8-pixel box
+                                 // (pooled 4 x 4); im2col plan, prm.tma_store: as [pixels, channels] rows with a 64 x 64 box
     void* d_w = nullptr;         // K-major weights: fp16, or fp32 rounded to TF32 (the engine's dtype)
     bool monotone_act = false;   // every PReLU slope of the layer is >= 0
     HaloParams hp;               // halo plan: conv_halo_kernel's parameters
@@ -685,6 +702,7 @@ struct EngOptions {
     enum { HALO_AUTO, HALO_NONE, HALO_ALL } halo = HALO_AUTO;   // HPB_HALO=all | anything else; unset: build_conv_plan's rule
     bool halo_wide = true;       // HPB_HALO_NARROW: every halo layer takes the 128-pixel work item (neither wide nor ping-pong)
     bool halo_tma_store = true;  // HPB_HALO_REG_EPILOGUE: the halo kernel stores its outputs from registers, not through TMA
+    bool conv_tma_store = true;  // HPB_CONV_REG_EPILOGUE: so does conv_wgmma_kernel
     bool stem3 = true;           // fused 3x3 stem; HPB_NO_STEM3 keeps the im2col buffer
     bool pool_fuse = true;       // HPB_NO_POOL_FUSE
     bool dw1_fuse = true;        // HPB_NO_DW1_FUSE
@@ -824,6 +842,21 @@ int set_halo_item(const hp_engine* e, EngOp& op, HaloItem item, bool pool)
                              CU_TENSOR_MAP_SWIZZLE_128B);
 }
 
+// conv_wgmma_kernel's epilogue: the TMA store (conv_epilogue_tma) where the plan allows it -- the fp16 engine's NHWC outputs at
+// BN = 64 or 128, under the same alignment and channel-extent conditions as the halo kernel's (halo_tma_store_ok: a 57-channel
+// concat write keeps the per-thread stores) -- with its output tensor map, staging slots and ring depth; else the register epilogue.
+// Called once the fusion passes have settled the conv's output (a fused 1x1 depthwise stage moves it).
+int set_conv_tma_store(const hp_engine* e, EngOp& op)
+{
+    ConvParams& p = op.plan.prm;
+    p.tma_store = e->opt.conv_tma_store && e->dtype == HP_DTYPE_F16 && p.out_mode == OUT_F16_NHWC && (p.BN == 64 || p.BN == 128) &&
+                  p.out_ld % 8 == 0 && p.out_ch_off % 8 == 0 && (p.groups * p.cout_g) % 8 == 0 && (p.groups == 1 || p.cout_g % p.BN == 0);
+    p.num_stages = conv_pick_stages(p.BN, p.tma_store);
+    op.plan.smem = conv_smem_bytes(p.BN, p.num_stages, p.tma_store);
+    if (!p.tma_store) return HP_OK;
+    return make_tmap_pixel_rows(&op.plan.tmap_o, (const __half*)p.out, (long)e->max_batch * p.H * p.W, p.out_ch_off + p.groups * p.cout_g, p.out_ld);
+}
+
 // Which halo layers take the wide item, from per-layer times of both items at the cfg3 / cfg4 / cfg5 benchmark batch sizes
 // (tools/layer_times.py with and without HPB_HALO_NARROW, DESIGN.md §4): OpenPose's 7x7 refinement convs, 49 weight tiles per box,
 // run 13-15 % faster.  The 3x3 layers gain at most 5 % (cin 512 at 46x82 and 46x54) and lose up to 46 % where a launch is a few
@@ -948,7 +981,7 @@ int build_conv_plan(hp_engine* e, EngOp& op, const float* blob)
     p.cout_g = cout_g; p.cout_g_pad = cout_pad; p.BN = BN;
     p.m_tiles = (int)(((size_t)e->max_batch * p.H * p.W + CONV_BLOCK_M - 1) / CONV_BLOCK_M);
     p.in_ch_off = (int)po.in_ch_off;
-    p.num_stages = conv_pick_stages(BN);
+    p.num_stages = conv_pick_stages(BN, false);   // (set_conv_tma_store settles the epilogue once the fusion passes are done)
     p.bias = pl.d_bias; p.alpha = pl.d_alpha;
     p.out_mode = (int)po.out_mode;
     if (po.out_mode == OUT_F32_NCHW_SPLIT) {
@@ -981,7 +1014,7 @@ int build_conv_plan(hp_engine* e, EngOp& op, const float* blob)
     if (rc) return rc;
     rc = make_tmap_wgt(&pl.tmap_b, pl.d_w, G * cout_pad, K, BN, e->dtype);
     if (rc) return rc;
-    pl.smem = conv_smem_bytes(BN, p.num_stages);
+    pl.smem = conv_smem_bytes(BN, p.num_stages, false);
     pl.flops_per_frame = 2.0 * ib.H * ib.W * (double)G * cout_g * cin_g * R * S;
     op.launch = Launch::Conv;
     if (e->dtype != HP_DTYPE_F16) return HP_OK;   // the TF32 and INT8 engines have no halo kernel
@@ -1130,7 +1163,7 @@ int launch_conv(hp_engine* e, EngOp& op, int N, cudaStream_t st, bool u8_input)
     const int grid = std::min(e->num_sms - e->reserve_sms, n_tiles);
     cudaLaunchAttribute at[1];
     const cudaLaunchConfig_t cfg = pdl_config(grid, CONV_THREADS, pl.smem, st, at);
-    void* args[] = { (void*)&pl.tmap_a, (void*)&pl.tmap_b, (void*)&p };
+    void* args[] = { (void*)&pl.tmap_a, (void*)&pl.tmap_b, (void*)&pl.tmap_o, (void*)&p };
     HP_CUDA_TRY(cudaLaunchKernelExC(&cfg, conv_kernel(e->dtype, p.res_mode != 0, p.BN, stem_R), args));
     return HP_OK;
 }
@@ -1496,6 +1529,7 @@ int hp_engine_create_ex(hp_engine** out, const void* pack, size_t pack_bytes, in
     if (const char* v = getenv("HPB_HALO")) opt.halo = strcmp(v, "all") == 0 ? EngOptions::HALO_ALL : EngOptions::HALO_NONE;
     opt.halo_wide = !getenv("HPB_HALO_NARROW");
     opt.halo_tma_store = !getenv("HPB_HALO_REG_EPILOGUE");
+    opt.conv_tma_store = !getenv("HPB_CONV_REG_EPILOGUE");
     opt.stem3 = !getenv("HPB_NO_STEM3");
     opt.pool_fuse = !getenv("HPB_NO_POOL_FUSE");
     opt.dw1_fuse = !getenv("HPB_NO_DW1_FUSE");
@@ -1705,6 +1739,11 @@ int hp_engine_create_ex(hp_engine** out, const void* pack, size_t pack_bytes, in
         c.plan.prm.post_w = d.d_dw; c.plan.prm.post_b = d.d_dw + Ctot; c.plan.prm.post_a = d.d_dw + 2 * (size_t)Ctot;
         d.launch = Launch::None;
         if (!rewritten) e->bufs[c.po.out_buf].fused_away = true;   // its final content would have been this conv's output
+    }
+    for (EngOp& c : e->ops) {
+        if (c.launch != Launch::Conv && c.launch != Launch::ConvStem) continue;
+        if (int rc = set_conv_tma_store(e, c)) return fail(rc);
+        max_smem = std::max(max_smem, c.plan.smem);
     }
     // depthwise 3x3 / stride 1 on a multiple of 64 channels: input tiles through TMA (dwconv3_tma_kernel)
     size_t dwt_max = 0;
@@ -2159,6 +2198,16 @@ int hp_engine_debug_op_epilogue(const hp_engine* e, int op, int* tma_store)
     if (!e || op < 0 || op >= (int)e->ops.size() || !tma_store) { set_error("hp_engine_debug_op_epilogue: bad argument"); return HP_ERR_ARG; }
     const EngOp& o = e->ops[op];
     *tma_store = o.launch == Launch::Halo && o.plan.hp.tma_store ? 1 : 0;
+    return HP_OK;
+}
+
+// test hook: *tma_store = 1 when op `op` runs conv_wgmma_kernel with the TMA-store epilogue (conv_epilogue_tma), 0 for every other op
+// (a plan the TMA store cannot express, another engine precision, or HPB_CONV_REG_EPILOGUE=1)
+int hp_engine_debug_op_conv_epilogue(const hp_engine* e, int op, int* tma_store)
+{
+    if (!e || op < 0 || op >= (int)e->ops.size() || !tma_store) { set_error("hp_engine_debug_op_conv_epilogue: bad argument"); return HP_ERR_ARG; }
+    const EngOp& o = e->ops[op];
+    *tma_store = (o.launch == Launch::Conv || o.launch == Launch::ConvStem) && o.plan.prm.tma_store ? 1 : 0;
     return HP_OK;
 }
 

@@ -254,6 +254,10 @@ int hp_engine_debug_op_kernel(const hp_engine* e, int op, char* name, int cap);
 /* test hook: *tma_store = 1 when op `op` runs the halo conv kernel with its TMA-store epilogue, 0 otherwise (HPB_HALO_REG_EPILOGUE=1
  * or a plan the TMA store cannot express: per-thread stores from registers) */
 int hp_engine_debug_op_epilogue(const hp_engine* e, int op, int* tma_store);
+/* test hook: the same for the im2col conv kernel ("conv<f16,...>"): *tma_store = 1 when op `op` stages its fp16 outputs in shared
+ * memory and TMA-stores them, 0 otherwise (HPB_CONV_REG_EPILOGUE=1, the TF32 / INT8 engines, the fp32 conf / PAF output, or a plan
+ * the TMA store cannot express: per-thread stores from registers) */
+int hp_engine_debug_op_conv_epilogue(const hp_engine* e, int op, int* tma_store);
 
 /* benchmark hook (SURVEY 8d): after the last conv of every run, copy these DEVICE tensors over the engine's
  * conf/paf outputs, so that random-init weights still give the parser a realistic load.  NULL disables it. */
