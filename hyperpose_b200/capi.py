@@ -211,7 +211,8 @@ EXPORTS += [
     "hp_paf_grow_capacity", "hp_pool_create", "hp_pool_destroy", "hp_pool_size", "hp_pool_set_capacity", "hp_pool_run_u8_host",
     "hp_pool_set_output_override", "hp_pool_launch_count", "hp_default_device", "hp_handoff_device_of",
     "hp_engine_create_ex", "hp_engine_dtype", "hp_pose_submit_u8_device", "hp_engine_debug_op_kernel",
-    "hp_engine_debug_op_epilogue", "hp_engine_debug_op_conv_epilogue",
+    "hp_engine_debug_op_epilogue", "hp_engine_debug_op_conv_epilogue", "hp_engine_debug_uses_pdl",
+    "hp_engine_debug_read_buffer_raw", "hp_engine_debug_write_outputs",
     "hp_engine_calibrate_u8", "hp_pack_int8_calibrated",
 ]
 
@@ -239,6 +240,9 @@ def _bind_engine(L):
     L.hp_engine_debug_op_kernel.argtypes = [vp, C.c_int, C.c_char_p, C.c_int]
     L.hp_engine_debug_op_epilogue.argtypes = [vp, C.c_int, ip]
     L.hp_engine_debug_op_conv_epilogue.argtypes = [vp, C.c_int, ip]
+    L.hp_engine_debug_uses_pdl.argtypes = [vp, ip]
+    L.hp_engine_debug_read_buffer_raw.argtypes = [vp, C.c_int, vp, C.c_int]
+    L.hp_engine_debug_write_outputs.argtypes = [vp, vp, vp, C.c_int]
     L.hp_engine_calibrate_u8.argtypes = [vp, vp, C.c_int, vp, C.c_int]
     L.hp_pack_int8_calibrated.argtypes = [vp, C.c_size_t]
     L.hp_pose_run_u8_host.argtypes = [vp, vp, vp, C.c_int, vp, C.c_int, ip]
@@ -387,12 +391,24 @@ class Engine:
     def launch_count(self) -> int:
         return int(lib().hp_engine_launch_count(self._h))
 
-    def debug_read_buffer(self, buf: int, n: int) -> np.ndarray:
+    def debug_read_buffer(self, buf: int, n: int, raw: bool = False) -> np.ndarray:
+        """n frames of buffer `buf` (NHWC).  raw=True reads its memory as it stands, also when its final content is never stored
+        (a buffer whose last reader runs in its producer's epilogue) and the plain read refuses"""
         H, W, Cc = C.c_int(), C.c_int(), C.c_int()
         check(lib().hp_engine_debug_read_buffer(self._h, buf, None, n, C.byref(H), C.byref(W), C.byref(Cc)))
         out = np.empty((n, H.value, W.value, Cc.value), self._elem)
-        check(lib().hp_engine_debug_read_buffer(self._h, buf, out.ctypes.data, n, C.byref(H), C.byref(W), C.byref(Cc)))
+        if raw:
+            check(lib().hp_engine_debug_read_buffer_raw(self._h, buf, out.ctypes.data, n))
+        else:
+            check(lib().hp_engine_debug_read_buffer(self._h, buf, out.ctypes.data, n, C.byref(H), C.byref(W), C.byref(Cc)))
         return out
+
+    def debug_write_outputs(self, conf: np.ndarray, paf: np.ndarray):
+        """write frames of the fp32 conf / paf outputs (the arrays read_outputs returns)"""
+        conf, paf = np.ascontiguousarray(conf, np.float32), np.ascontiguousarray(paf, np.float32)
+        assert conf.shape[0] == paf.shape[0]
+        assert conf.shape[1:] == (self.c_conf, self.out_h, self.out_w) and paf.shape[1:] == (self.c_paf, self.out_h, self.out_w)
+        check(lib().hp_engine_debug_write_outputs(self._h, conf.ctypes.data, paf.ctypes.data, conf.shape[0]))
 
     def debug_write_buffer(self, buf: int, arr: np.ndarray):
         arr = np.ascontiguousarray(arr, self._elem)
@@ -433,6 +449,12 @@ class Engine:
         v = C.c_int(0)
         check(lib().hp_engine_debug_op_conv_epilogue(self._h, op, C.byref(v)))
         return "tma" if v.value else "reg"
+
+    def debug_uses_pdl(self) -> bool:
+        """True when the engine launches its conv and depthwise kernels with programmatic dependent launch"""
+        v = C.c_int(0)
+        check(lib().hp_engine_debug_uses_pdl(self._h, C.byref(v)))
+        return bool(v.value)
 
     def set_output_override(self, d_conf_ptr: int, d_paf_ptr: int):
         check(lib().hp_engine_set_output_override(self._h, d_conf_ptr, d_paf_ptr))

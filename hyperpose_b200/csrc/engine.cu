@@ -2076,6 +2076,30 @@ int hp_engine_debug_read_buffer(hp_engine* e, int buf, void* out_f16, int N, int
     return HP_OK;
 }
 
+// test hook: the memory of buffer `buf` as it stands, N frames, also for a buffer hp_engine_debug_read_buffer refuses because its
+// final content is never stored: such a buffer may still hold what earlier ops wrote there (MobilenetThin's ping-pong buffers)
+int hp_engine_debug_read_buffer_raw(hp_engine* e, int buf, void* out, int N)
+{
+    if (!e || buf < 0 || buf >= (int)e->bufs.size() || !out || N <= 0 || N > e->max_batch) { set_error("hp_engine_debug_read_buffer_raw: bad argument"); return HP_ERR_ARG; }
+    HP_CUDA_TRY(cudaSetDevice(e->device));
+    const EngBuffer& b = e->bufs[buf];
+    HP_CUDA_TRY(cudaStreamSynchronize(e->stream));
+    HP_CUDA_TRY(cudaMemcpy(out, b.d, (size_t)N * b.H * b.W * b.channels * elem_bytes(e->dtype), cudaMemcpyDeviceToHost));
+    return HP_OK;
+}
+
+// test hook: N frames of the conf / paf outputs (fp32, the layout hp_engine_read_outputs_host reads), e.g. a sentinel before a replay
+int hp_engine_debug_write_outputs(hp_engine* e, const float* conf, const float* paf, int N)
+{
+    if (!e || !conf || !paf || N <= 0 || N > e->max_batch) { set_error("hp_engine_debug_write_outputs: bad argument"); return HP_ERR_ARG; }
+    HP_CUDA_TRY(cudaSetDevice(e->device));
+    const size_t plane = (size_t)e->out_h * e->out_w;
+    HP_CUDA_TRY(cudaStreamSynchronize(e->stream));
+    HP_CUDA_TRY(cudaMemcpy(e->d_conf, conf, N * e->hdr.conf_channels * plane * sizeof(float), cudaMemcpyHostToDevice));
+    HP_CUDA_TRY(cudaMemcpy(e->d_paf, paf, N * e->hdr.paf_channels * plane * sizeof(float), cudaMemcpyHostToDevice));
+    return HP_OK;
+}
+
 int hp_engine_debug_write_buffer(hp_engine* e, int buf, const void* in_f16, int N)
 {
     if (!e || buf < 0 || buf >= (int)e->bufs.size() || !in_f16 || N <= 0 || N > e->max_batch) { set_error("hp_engine_debug_write_buffer: bad argument"); return HP_ERR_ARG; }
@@ -2208,6 +2232,15 @@ int hp_engine_debug_op_conv_epilogue(const hp_engine* e, int op, int* tma_store)
     if (!e || op < 0 || op >= (int)e->ops.size() || !tma_store) { set_error("hp_engine_debug_op_conv_epilogue: bad argument"); return HP_ERR_ARG; }
     const EngOp& o = e->ops[op];
     *tma_store = (o.launch == Launch::Conv || o.launch == Launch::ConvStem) && o.plan.prm.tma_store ? 1 : 0;
+    return HP_OK;
+}
+
+// test hook: *pdl = 1 when the engine launches its conv / depthwise kernels with programmatic dependent launch (hp_engine::use_pdl,
+// decided at creation from the work per launch), 0 otherwise
+int hp_engine_debug_uses_pdl(const hp_engine* e, int* pdl)
+{
+    if (!e || !pdl) { set_error("hp_engine_debug_uses_pdl: bad argument"); return HP_ERR_ARG; }
+    *pdl = e->use_pdl ? 1 : 0;
     return HP_OK;
 }
 

@@ -245,6 +245,10 @@ long long hp_engine_launch_count(const hp_engine* e);
 int hp_engine_debug_read_buffer(hp_engine* e, int buf, void* out_f16, int N, int* H, int* W, int* C);
 int hp_engine_debug_write_buffer(hp_engine* e, int buf, const void* in_f16, int N);
 int hp_engine_debug_run_ops(hp_engine* e, int first_op, int last_op, int N);
+/* test hooks: read a buffer's memory as it stands, including a buffer hp_engine_debug_read_buffer refuses because its final
+ * content is never stored (earlier ops may still use it); write N frames of the fp32 conf / paf outputs */
+int hp_engine_debug_read_buffer_raw(hp_engine* e, int buf, void* out, int N);
+int hp_engine_debug_write_outputs(hp_engine* e, const float* conf, const float* paf, int N);
 /* test hook: the kernel op `op` launches on the next run over u8 frames, fixed at creation, as a NUL-terminated name in
  * name[cap]: "conv<f16|tf32|i8,BN[,res][,stem3|stem7]>", "halo<BN[,pool|,wide|,pp|,pool,pp]>", "dw_strip<K,S>", "dw_col", "dw_tma<1|2>",
  * "dw_f32", "dw_i8", "maxpool<K>", "maxpool_f32", "maxpool_i8", "im2col" (fp16 and TF32), "im2col_i8", "heads", "ppn_head", or "none" for
@@ -258,6 +262,9 @@ int hp_engine_debug_op_epilogue(const hp_engine* e, int op, int* tma_store);
  * memory and TMA-stores them, 0 otherwise (HPB_CONV_REG_EPILOGUE=1, the TF32 / INT8 engines, the fp32 conf / PAF output, or a plan
  * the TMA store cannot express: per-thread stores from registers) */
 int hp_engine_debug_op_conv_epilogue(const hp_engine* e, int op, int* tma_store);
+/* test hook: *pdl = 1 when the engine launches its conv and depthwise kernels with programmatic dependent launch, each kernel's
+ * prologue running under its predecessor's tail, 0 otherwise.  Decided at creation from the work per launch at max_batch. */
+int hp_engine_debug_uses_pdl(const hp_engine* e, int* pdl);
 
 /* benchmark hook (SURVEY 8d): after the last conv of every run, copy these DEVICE tensors over the engine's
  * conf/paf outputs, so that random-init weights still give the parser a realistic load.  NULL disables it. */
