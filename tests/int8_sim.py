@@ -3,7 +3,9 @@
 Symmetric quantization: buffer b holds int8 q in [-127, 127] standing for q * s_b.  Every step is the engine's, in the same order and
 with the same rounding:
   * weights: s_w[o] = max |W[o]| / 127 (1 for an all-zero row), q_w = clamp(rint(W / s_w), -127, 127), mul[o] = s_in * s_w[o];
-  * conv: the integer convolution in float64 (exact: |products| <= 127^2, sums far below 2^53), cast to float32, then
+  * conv: the integer convolution in float64 (exact: every operand and every partial sum is an integer of magnitude at most
+    127^2 K < 2^31 < 2^53, so any summation order gives the same sum; run_graph(device="cuda") computes it there as an
+    im2col + DGEMM with cuDNN off, since cuDNN's FFT and Winograd algorithms are not exact), cast to float32, then
     v = acc * mul + bias, residual r = q_r * s_res (mode 1: act(v + r), mode 2: act(v) + r), act(y) = y > 0 ? y : y * alpha, each a
     separately rounded float32 operation; NHWC outputs store clamp(rint(y * (1 / s_out)), -127, 127), the conf / PAF outputs y;
   * im2col: the fp32 normalised input (u8 * factor in double, to float32, minus the mean; or the f32 entry minus the mean), quantized
@@ -36,6 +38,19 @@ def quantize_weights(weight):
     return q.reshape(w.shape), sw
 
 
+def float_absmax(g: models.Graph, frames_u8, factor=1.0 / 255):
+    """per-buffer max |x| of a float32 run of g (oracle/torch_backbone, CPU), for Graph.set_int8_scales where no GPU calibrates: the
+    final buffer contents, and for the im2col buffer (which that run does not fill with patches) max |x| of the normalised frames"""
+    from oracle import torch_backbone
+    _, _, bufs = torch_backbone.run_graph(g, frames_u8, factor=factor, device="cpu", rounding="tf32")
+    a = np.array([float(b.abs().max()) for b in bufs], f32)
+    x = (frames_u8.astype(np.float64) * factor).astype(f32)[..., ::-1] - np.asarray(g.mean, f32)
+    for op in g.ops:
+        if op.type == models.OP_IM2COL3:
+            a[op.out_buf] = np.abs(x).max()
+    return a
+
+
 def _same_pad_before(n, k, stride):
     out = (n + stride - 1) // stride
     return max((out - 1) * stride + k - n, 0) // 2
@@ -48,9 +63,24 @@ def _shape(g, bi, H, W):
     return c, H, W
 
 
-def run_graph(g: models.Graph, act_scales, frames_u8=None, f32_input=None, factor=1.0 / 255, flip_rgb=True, init=None, N=None, HW=None):
+def _int_conv(x, qw, G, R, S, im2col, device):
+    """the integer convolution of int8 x [N, C, H, W] (for im2col: [N, R S cin, H, W], k = (r S + s) cin + c) with int8 qw
+    [G co, ci, R, S] in float64 on `device` -> float64 numpy [N, G co, H, W]"""
+    w = torch.from_numpy(qw.astype(np.float64)).to(device)
+    with torch.backends.cudnn.flags(enabled=False):
+        if im2col:
+            xt = torch.from_numpy(x.astype(np.float64)).to(device)
+            acc = torch.einsum("nkhw,ok->nohw", xt, w.permute(0, 2, 3, 1).reshape(w.shape[0], -1))
+        else:
+            acc = F.conv2d(torch.from_numpy(x.astype(np.float64)).to(device), w, padding=(R // 2, S // 2), groups=G)
+    return acc.cpu().numpy()
+
+
+def run_graph(g: models.Graph, act_scales, frames_u8=None, f32_input=None, factor=1.0 / 255, flip_rgb=True, init=None, N=None, HW=None,
+              device="cpu"):
     """-> (conf, paf, bufs).  Input: u8 frames [N, H, W, 3] (BGR), or f32_input [N, 3, H, W] (the f32 entry: already scaled), or
-    neither (graphs without an im2col op: N and HW=(H, W) give the geometry).  init: {buffer: int8 [N, C, H, W]} starting contents."""
+    neither (graphs without an im2col op: N and HW=(H, W) give the geometry).  init: {buffer: int8 [N, C, H, W]} starting contents.
+    device: where the integer convolutions run (the rest stays on the CPU); the result is the same bytes on any device."""
     s = np.asarray(act_scales, f32)
     if frames_u8 is not None:
         N, H, W, _ = frames_u8.shape
@@ -100,13 +130,9 @@ def run_graph(g: models.Graph, act_scales, frames_u8=None, f32_input=None, facto
             qw, sw = quantize_weights(op.weight.reshape(G * co, ci, R, S))
             mul = (s[op.in_buf] * sw).astype(f32)
             if op.im2col_input:
-                k = R * S * ci
-                x = bufs[op.in_buf][:, :k].astype(np.float64)
-                wm = qw.transpose(0, 2, 3, 1).reshape(G * co, k).astype(np.float64)   # k = (r * S + s) * cin + c
-                acc = np.einsum("nkhw,ok->nohw", x, wm)
+                acc = _int_conv(bufs[op.in_buf][:, :R * S * ci], qw, G, R, S, True, device)
             else:
-                x = torch.from_numpy(bufs[op.in_buf][:, op.in_ch_off:op.in_ch_off + G * ci].astype(np.float64))
-                acc = F.conv2d(x, torch.from_numpy(qw.astype(np.float64)), padding=(R // 2, S // 2), groups=G).numpy()
+                acc = _int_conv(bufs[op.in_buf][:, op.in_ch_off:op.in_ch_off + G * ci], qw, G, R, S, False, device)
             v = acc.astype(f32) * mul.reshape(1, -1, 1, 1)
             v = (v + op.bias.astype(f32).reshape(1, -1, 1, 1)).astype(f32)
             if op.res_mode:

@@ -1,6 +1,7 @@
 """The INT8 engine (HP_DTYPE_INT8, data_type::kINT8) against its CPU model (tests/int8_sim.py), byte for byte: every conv kernel
 instantiation and helper kernel in one- or two-op graphs, four whole networks with scales from Engine.calibrate, the calibration
-itself, the packs an INT8 engine refuses, and the pose paths on an INT8 engine.
+itself (bit for bit against an op-by-op replay at the benchmark batches, short chunks and chunk sums included), the packs an INT8
+engine refuses, and the pose paths on an INT8 engine.  The networks at the benchmarks' plans are in tests/test_network_ops.py.
 
 The one-op cases also run every conv kernel with more work items than CTAs (the persistent kernel carries its stage ring from one item
 to the next), the conf / PAF output conv, and batches shorter than the engine's max_batch: there the frames past N of the input
@@ -313,6 +314,25 @@ def test_int8_network_matches_model(net):
         eng.close()
 
 
+@gpu
+def test_int8_model_on_the_gpu_matches_the_cpu():
+    """int8_sim.run_graph(device="cuda") runs the integer convolutions there (im2col + DGEMM, cuDNN off) and gives the CPU run's
+    bytes: MobilenetThin (the im2col stem, grouped convs) and ResNet-50-LW (residual convs) at 64 x 96"""
+    kinds = set()
+    for name in ("mobilenet_thin_openpose", "resnet50_lw_openpose"):
+        g = getattr(models, name)(0)
+        frames = syn.make_frames_u8(3, 2, 64, 96)
+        g.set_int8_scales(int8_sim.float_absmax(g, frames))
+        c0, p0, b0 = int8_sim.run_graph(g, g.act_scales, frames_u8=frames)
+        c1, p1, b1 = int8_sim.run_graph(g, g.act_scales, frames_u8=frames, device="cuda")
+        for bi, (x, y) in enumerate(zip(b0, b1)):
+            assert x.tobytes() == y.tobytes(), f"{name}: buffer {bi}: {int((x != y).sum())} bytes differ"
+        assert c0.tobytes() == c1.tobytes() and p0.tobytes() == p1.tobytes(), name
+        kinds |= {k for op in g.ops if op.type == models.OP_CONV for k, on in (("grouped", op.groups > 1), ("residual", op.res_mode),
+                                                                               ("im2col", op.im2col_input)) if on}
+    assert kinds == {"grouped", "residual", "im2col"}, kinds
+
+
 # ---- calibration ----------------------------------------------------------------------------------------------------------
 @gpu
 def test_calibration_matches_fp32_reference_and_is_a_running_max():
@@ -334,6 +354,70 @@ def test_calibration_matches_fp32_reference_and_is_a_running_max():
         _, _, bufs = torch_backbone.run_graph(g, fa, rounding="tf32", device="cpu", upto=oi)
         ref[op.out_buf] = max(ref[op.out_buf], float(bufs[op.out_buf].abs().max()))
     assert np.all(np.abs(a - ref) <= 6e-3 * ref + 1e-3), (a, ref)
+
+
+CAL_NETS = {"cfg3": ("openpose_vgg19", 368, 656, 16), "cfg4": ("resnet50_lw_openpose", 368, 432, 32),
+            "cfg2": ("mobilenet_thin_openpose", 368, 432, 8)}   # tools/bench_int8.py's workloads: graph, H, W, max_batch
+
+
+def _replay_absmax(g, eng, frames):
+    """what calibrate folds, op by op: max |x| of each op's whole output buffer over the frames (infer_u8 first, so that the channels
+    other ops write hold what they held when calibrate ran; heads and the split output conv skipped)"""
+    n = frames.shape[0]
+    eng.infer_u8(frames)
+    amax = np.zeros(len(g.buffers), np.float32)
+    for i, op in enumerate(g.ops):
+        eng.debug_run_ops(i, i, n)
+        if op.type in (models.OP_PIFPAF_HEAD, models.OP_PPN_HEAD) or (op.type == models.OP_CONV and op.out_mode == models.OUT_F32_NCHW_SPLIT):
+            continue
+        amax[op.out_buf] = max(amax[op.out_buf], np.abs(eng.debug_read_buffer(op.out_buf, n, raw=True)).max())
+    return amax
+
+
+def _same_bits(a, b):
+    return np.asarray(a, np.float32).tobytes() == np.asarray(b, np.float32).tobytes()
+
+
+@gpu
+@pytest.mark.parametrize("cfg", sorted(CAL_NETS))
+def test_calibration_at_benchmark_batch_is_exact(cfg):
+    """calibrate on a TF32 engine at the benchmark's max_batch, bit for bit: (a) one full chunk equals the running max of an op-by-op
+    replay; (b) a short chunk of n = B - 3 frames ignores frames >= n (they hold 1e30); (c) 2B - 3 frames, a full chunk and a short
+    one, equal the element-wise max of the two calibrated apart.  Calibration folds whole buffers, so channels other ops write count
+    too: each compared run starts from the buffer contents the other started from."""
+    name, H, W, B = CAL_NETS[cfg]
+    g = getattr(models, name)(0)
+    eng = capi.Engine(g.to_pack(), (W, H), max_batch_size=B, dtype="tf32")
+    try:
+        frames = syn.make_frames_u8(500, 2 * B - 3, H, W)
+        full, n = frames[:B], B - 3
+        eng.infer_u8(full)
+        a = eng.calibrate(full)
+        ra = _replay_absmax(g, eng, full)
+        assert _same_bits(a, ra), f"{cfg}: calibrate differs from the replay at buffers {np.flatnonzero(a != ra).tolist()}"
+        # (b)
+        saved = [eng.debug_read_buffer(bi, B, raw=True) for bi in range(len(g.buffers))]
+        for bi, x in enumerate(saved):
+            y = x.copy()
+            y[n:] = 1e30
+            eng.debug_write_buffer(bi, y)
+        b = eng.calibrate(full[:n])
+        assert (b < 1e29).all(), f"{cfg}: the {n}-frame calibration read frames >= {n} of buffers {np.flatnonzero(b >= 1e29).tolist()}"
+        rb = _replay_absmax(g, eng, full[:n])
+        assert _same_bits(b, rb), f"{cfg}: the {n}-frame calibration differs from the replay at buffers {np.flatnonzero(b != rb).tolist()}"
+        # (c), from the contents (a) started from (channels no op writes, such as a buffer's pad channels, still held 1e30)
+        for bi, x in enumerate(saved):
+            eng.debug_write_buffer(bi, x)
+        first = eng.calibrate(full)
+        assert _same_bits(first, a), f"{cfg}: calibrating the same frames from the same contents differs at buffers {np.flatnonzero(first != a).tolist()}"
+        last = eng.calibrate(frames[B:])
+        assert not _same_bits(last, first), f"{cfg}: two frame sets calibrate alike"
+        for bi, x in enumerate(saved):
+            eng.debug_write_buffer(bi, x)
+        both = eng.calibrate(frames)
+        assert _same_bits(both, np.maximum(first, last)), f"{cfg}: chunks combine wrongly at buffers {np.flatnonzero(both != np.maximum(first, last)).tolist()}"
+    finally:
+        eng.close()
 
 
 @gpu

@@ -35,8 +35,20 @@ dependent launch), so the launch sequence the benchmarks time is only seen at th
      every buffer and both outputs byte for byte as infer_u8 does.
   4. the frame resize at camera sizes: every case of make_golden.RESIZE_CASES, with and without keep_ratio, bit-exact against the
      oracle (pinned to cv2 by sha), and a mixed batch whose staging regions grow between frames.
-The CPU test at the end checks the harness itself: chaining the per-group references over the reference's own buffers reproduces
-run_graph of the whole graph exactly."""
+The INT8 configs are tools/bench_int8.py's engines (cfg3, cfg4, cfg2 at their batches), with the scales it uses: a TF32 engine of
+the same max_batch calibrates one batch of seed-500 frames.  The INT8 engine launches every op on its own (its im2col op is a group,
+whose patch buffer, pad channels included, is an output; the stem conv reads the patches), and its kernels are specified to the
+byte, so tests 1 and 2 hold it to tests/int8_sim.py exactly rather than within a bound:
+  1. the sentinel is -128 (quantize_i8 clamps to +-127, so no kernel stores it; the conf / PAF planes keep NaN), and
+       (a) every output byte and every conf / PAF value of frames 0, 1 and B - 1 equals int8_sim.run_graph on the group's ops, from
+           the engine's own inputs and the buffers' scales (the integer convolutions on the GPU: float64, exact in any order);
+       (c) an exact comparison passes vacuously only on outputs that do not depend on the inputs: every output holds >= 16
+           distinct values, and for the first op of every conv kernel name the tap-mutated reference changes >= 1 % of frame 0's
+           outputs.  The printed line gives the distinct values and the fraction of int8 outputs at +-127.
+     (b) and the whole-run identity are as above.
+  2. frames >= N' hold -128.
+The CPU tests at the end check the harness itself: chaining the per-group references over the reference's own buffers reproduces
+run_graph of the whole graph exactly, and the per-group int8_sim references reproduce int8_sim.run_graph byte for byte."""
 import copy
 import hashlib
 import os
@@ -49,6 +61,7 @@ import torch
 import oracle
 from hyperpose_b200 import capi, models, synthetic as syn
 from oracle import torch_backbone
+from tests import int8_sim
 from tests.golden.make_golden import RESIZE_CASES, sha
 from tests.ppn_head_ref import ppn_head_ref
 from tests.test_engine_kernels import _r, work_items
@@ -64,17 +77,23 @@ CONFIGS = [("cfg3", "openpose_vgg19", 368, 656, 16, "f16"), ("cfg3-tf32", "openp
            ("lw_resnet18", "lw_openpose_resnet18", 368, 432, 16, "f16"),
            ("lw_mobilenet_dilated", "lw_openpose_mobilenet_dilated", 368, 432, 16, "f16"),
            ("ppn_resnet18", "ppn_resnet18", 384, 384, 16, "f16"), ("ppn_resnet18-tf32", "ppn_resnet18", 384, 384, 16, "tf32"),
-           ("ppn_resnet50", "ppn_resnet50", 384, 384, 16, "f16"), ("ppn_resnet50-tf32", "ppn_resnet50", 384, 384, 16, "tf32")]
+           ("ppn_resnet50", "ppn_resnet50", 384, 384, 16, "f16"), ("ppn_resnet50-tf32", "ppn_resnet50", 384, 384, 16, "tf32"),
+           # tools/bench_int8.py: the INT8 engine, its scales calibrated on seed-500 frames by a TF32 engine of the same max_batch
+           ("cfg3-int8", "openpose_vgg19", 368, 656, 16, "int8"), ("cfg4-int8", "resnet50_lw_openpose", 368, 432, 32, "int8"),
+           ("cfg2-int8", "mobilenet_thin_openpose", 368, 432, 8, "int8")]
 CFG = {c[0]: c for c in CONFIGS}
+INT8 = [c[0] for c in CONFIGS if c[5] == "int8"]
 FRAME_SEED = 2
+CAL_SEED = 500
 HEADS = (models.OP_PIFPAF_HEAD, models.OP_PPN_HEAD)
 
 
 # ---- launch groups and their float64 reference (no GPU) ---------------------------------------------------------------------
 def _op_reads(op):
-    """[(buffer, first channel, channels)] op reads from activation buffers (an im2col op reads the frames)"""
+    """[(buffer, first channel, channels)] op reads from activation buffers (an im2col op reads the frames; the conv after it, the
+    patches)"""
     if op.type == models.OP_CONV:
-        out = [] if op.im2col_input else [(op.in_buf, op.in_ch_off, op.groups * op.cin_g)]
+        out = [(op.in_buf, 0, op.R * op.S * op.cin_g)] if op.im2col_input else [(op.in_buf, op.in_ch_off, op.groups * op.cin_g)]
         return out + ([(op.res_buf, op.res_ch_off, op.groups * op.cout_g)] if op.res_mode else [])
     if op.type in (models.OP_DWCONV, models.OP_MAXPOOL2):
         return [(op.in_buf, op.in_ch_off, op.cout_g)]
@@ -95,7 +114,7 @@ def _op_writes(op):
 
 
 class Group:
-    """ops first .. last of graph g: one launch (and on the TF32 engine, the im2col op with the conv that reads it)"""
+    """ops first .. last of graph g: one launch (and on the f16 / TF32 engines, the im2col op with the conv that reads it)"""
 
     def __init__(self, g, first, last, dtype):
         self.first, self.last, self.dtype = first, last, dtype
@@ -106,11 +125,10 @@ class Group:
             self.reads += [r for r in _op_reads(op) if r[0] not in made and r not in self.reads]
             made |= {w[0] for w in _op_writes(op)}
         self.in_bufs = sorted({r[0] for r in self.reads})
-        # checked outputs: what no later op of the group reads (a fused op's input is never stored), never the im2col patches
+        # checked outputs: what no later op of the group reads (a fused op's input is never stored, nor the patches of a fused stem);
+        # on the INT8 engine the im2col op is a group of its own, and its patch buffer, pad channels included, is an output
         self.outs = []
         for i, op in enumerate(self.ops):
-            if op.type == models.OP_IM2COL3:
-                continue
             later = {r[0] for o in self.ops[i + 1:] for r in _op_reads(o)}
             self.outs += [w for w in _op_writes(op) if w[0] not in later]
         self.out_bufs = sorted({o[0] for o in self.outs if not isinstance(o[0], str)})
@@ -119,7 +137,7 @@ class Group:
         self.pool = self.ops[-1].type == models.OP_MAXPOOL2 and len(self.ops) == 1
         self.conv = next((i for i, op in enumerate(self.ops) if op.type == models.OP_CONV), None)
         self.dw1 = self.conv is not None and self.ops[-1].type == models.OP_DWCONV   # a 1x1 depthwise op in a conv's epilogue (a stem's too)
-        chunk = 64 if dtype == "f16" else 32
+        chunk = {"f16": 64, "tf32": 32, "int8": 128}[dtype]
         lead = self.ops[self.conv] if self.conv is not None else self.ops[0]
         if self.conv is not None and lead.im2col_input:   # the patch channels, as the kernel suite's stem cases count them
             self.K = _r(lead.R * lead.S * 3, 64)
@@ -147,12 +165,22 @@ class Group:
                                                    rounding="fp16" if self.dtype == "f16" else "tf32", round_stores=False, magnitude=magnitude)
         return {b: bufs[i] for i, b in enumerate(self.used)}, conf, paf
 
+    def reference_int8(self, scales, init, frames, graph=None, device="cpu"):
+        """the INT8 engine's arithmetic (tests/int8_sim.py) on the group's ops from int8 buffer contents init {buffer: [N, C, H, W]}
+        and u8 frames [N, H, W, 3] (the patches of an im2col op; the geometry of the others), with the graph's scale table `scales`
+        -> ({buffer: int8 [N, C, H, W]} of every buffer the ops touch, conf, paf)"""
+        init = {self.used.index(b): a for b, a in init.items() if b in self.used}
+        conf, paf, bufs = int8_sim.run_graph(graph or self.graph, np.asarray(scales, np.float32)[self.used], frames_u8=frames, init=init,
+                                             device=device)
+        return {b: bufs[i] for i, b in enumerate(self.used)}, conf, paf
+
 
 def launch_groups(g, kernels, dtype):
-    """the graph's launch groups from the kernel names of its ops (Engine.debug_op_kernel)"""
+    """the graph's launch groups from the kernel names of its ops (Engine.debug_op_kernel).  The INT8 engine launches every op on
+    its own (no fusion, no halo kernel, no PDL): its im2col op (im2col_i8) is a group, and so is the conv that reads the patches."""
     spans = []
     for i, (op, k) in enumerate(zip(g.ops, kernels)):
-        if op.type == models.OP_CONV and op.im2col_input:
+        if op.type == models.OP_CONV and op.im2col_input and dtype != "int8":
             assert spans and g.ops[spans[-1][0]].type == models.OP_IM2COL3 and spans[-1][1] == i - 1 and g.ops[i - 1].out_buf == op.in_buf, \
                 f"op {i}: a conv on im2col patches that does not follow its im2col op"
             spans[-1][1] = i
@@ -193,6 +221,10 @@ def _build(cid, monkeypatch):
     _, name, H, W, B, dtype = CFG[cid]
     _clean_env(monkeypatch)
     g = getattr(models, name)(seed=0)
+    if dtype == "int8":   # as tools/bench_int8.py: one max_batch of calibration frames through a TF32 engine
+        cal = capi.Engine(g.to_pack(), (W, H), max_batch_size=B, dtype="tf32")
+        g.set_int8_scales(cal.calibrate(syn.make_frames_u8(CAL_SEED, B, H, W)))
+        cal.close()
     eng = capi.Engine(g.to_pack(), (W, H), max_batch_size=B, dtype=dtype)
     return g, eng, syn.make_frames_u8(FRAME_SEED, B, H, W)
 
@@ -342,12 +374,58 @@ def _check_group(grp, eng, g, ins, got, planes, frames, sel, mutate, dev):
     return worst
 
 
+def _check_group_int8(grp, g, ins, got, planes, frames, sel, mutate, dev):
+    """(a) and (c) for one group of the INT8 engine -> (fewest distinct values in one of its outputs, fraction of its int8 outputs
+    at +-127)"""
+    fr = frames[sel]
+    init = {b: np.ascontiguousarray(a[sel].transpose(0, 3, 1, 2)) for b, a in ins.items()}
+    ref, rconf, rpaf = grp.reference_int8(g.act_scales, init, fr, device=dev)
+
+    def pick(res, conf, paf, o):
+        b, off, c = o
+        if isinstance(b, str):
+            return conf if b == "conf" else paf
+        return res[b][:, off:None if c is None else off + c]
+
+    def mine(o):
+        b, off, c = o
+        return planes[b][sel] if isinstance(b, str) else got[b][sel][..., off:None if c is None else off + c].transpose(0, 3, 1, 2)
+
+    def bits(a):   # int8 bytes as they are, fp32 planes by their bit patterns
+        return a.view(np.uint32) if a.dtype == np.float32 else a
+
+    distinct, sat, n = [], 0, 0
+    for o in grp.outs:
+        r, gv = np.ascontiguousarray(pick(ref, rconf, rpaf, o)), np.ascontiguousarray(mine(o))
+        bad = np.argwhere(bits(gv) != bits(r))
+        assert bad.size == 0, (f"ops {grp.first}..{grp.last} ({grp.ops[-1].name}): {o[0]}: {len(bad)} of {r.size} values differ from the INT8 model, "
+                               f"first at frame {sel[bad[0][0]]}, channel {bad[0][1]}, pixel {bad[0][2:].tolist()}: got {gv[tuple(bad[0])]}, "
+                               f"want {r[tuple(bad[0])]}")
+        distinct.append(len(np.unique(gv)))
+        if gv.dtype == np.int8:
+            sat += int(((gv == 127) | (gv == -127)).sum())
+            n += gv.size
+    assert min(distinct) >= 16, f"ops {grp.first}..{grp.last}: an output holds {min(distinct)} distinct values: the exact comparison says little"
+    if mutate:   # (c) on frame 0: the reference depends on the taps
+        mg = _tap_mutant(grp.graph, grp.conv)
+        mref, mconf, mpaf = grp.reference_int8(g.act_scales, {b: a[:1] for b, a in init.items()}, fr[:1], graph=mg, device=dev)
+        changed = total = 0
+        for o in grp.outs:
+            r, mr = pick(ref, rconf, rpaf, o)[:1], pick(mref, mconf, mpaf, o)
+            changed += int((bits(np.ascontiguousarray(mr)) != bits(np.ascontiguousarray(r))).sum())
+            total += r.size
+        assert changed >= 0.01 * total, f"ops {grp.first}..{grp.last}: the tap mutation changes {changed} of {total} outputs of frame 0"
+    return min(distinct), sat / n if n else 0.0
+
+
 def _replay(g, eng, frames, groups, B, dev, cid):
-    """steps 3 .. 5 of test 1 for every group, in order -> worst ratio of the network"""
+    """steps 3 .. 5 of test 1 for every group, in order -> worst ratio of the network (0 on the INT8 engine: every group is exact)"""
     H, W = frames.shape[1:3]
     sel = sorted({0, 1, B - 1})
     sms = torch.cuda.get_device_properties(0).multi_processor_count
-    nan = np.float16(np.nan) if eng.dtype == "f16" else np.float32(np.nan)
+    int8 = eng.dtype == "int8"
+    # the sentinel: NaN, or on the INT8 engine -128, which no kernel stores (quantize_i8 clamps to +-127)
+    nan = np.float16(np.nan) if eng.dtype == "f16" else np.int8(-128) if int8 else np.float32(np.nan)
     mutated, worst = set(), 0.0
     for grp in groups:
         ins = {b: _read(eng, b, B) for b in grp.in_bufs}
@@ -355,13 +433,14 @@ def _replay(g, eng, frames, groups, B, dev, cid):
         written = {b: np.zeros(before[b].shape[-1], bool) for b in grp.out_bufs}
         for b, off, c in grp.outs:
             if not isinstance(b, str):
-                written[b][off:off + c] = True
+                written[b][off:None if c is None else off + c] = True
         for b in grp.out_bufs:
             s = before[b].copy()
             keep = ~written[b]
-            for rb, off, c in grp.reads:   # channels the group also reads, up to its padded K chunks, keep their contents
-                if rb == b:
-                    keep[off:off + _r(c if c is not None else s.shape[-1], 64)] = True
+            for rb, off, c in grp.reads:   # channels the group also reads, up to its padded K chunks, keep their contents (an INT8
+                if rb == b:                # k-step past the channels read meets zero weights: -128 there adds nothing)
+                    c = c if c is not None else s.shape[-1]
+                    keep[off:off + (c if int8 else _r(c, 64))] = True
             s[..., ~keep] = nan
             eng.debug_write_buffer(b, s)
         writes_planes = any(isinstance(o[0], str) for o in grp.outs)
@@ -380,9 +459,15 @@ def _replay(g, eng, frames, groups, B, dev, cid):
         mutate = conv_k is not None and conv_k not in mutated and grp.conv is not None
         if mutate:
             mutated.add(conv_k)
+        info = _launch_info(eng, g, grp, B, H, W, sms) or kernels[0]
+        if int8:
+            distinct, sat = _check_group_int8(grp, g, ins, got, planes, frames, sel, mutate, dev)
+            print(f"[network ops] {cid} ops {grp.first}..{grp.last} {grp.ops[-1].name}: {info}; byte-exact, {distinct} distinct values, "
+                  f"{sat:.4f} at +-127" + (" (the tap mutation changes the reference)" if mutate else ""))
+            continue
         w = _check_group(grp, eng, g, ins, got, planes, frames, sel, mutate, dev)
         worst = max(worst, w)
-        print(f"[network ops] {cid} ops {grp.first}..{grp.last} {grp.ops[-1].name}: {_launch_info(eng, g, grp, B, H, W, sms) or kernels[0]}; "
+        print(f"[network ops] {cid} ops {grp.first}..{grp.last} {grp.ops[-1].name}: {info}; "
               f"worst |got - ref| / bound {w:.3f}" + (" (bound rejects the tap mutation)" if mutate else ""))
     return worst, mutated
 
@@ -408,8 +493,8 @@ def test_network_ops_against_fp64_and_replay(cid, monkeypatch):
     bad = _diff_state(whole, replay)
     assert not bad, f"{cid}: the op-by-op replay differs from the whole run at (buffer, frame) {bad[:8]} ({len(bad)} in all)"
     assert mutated, f"{cid}: no conv kernel"
-    print(f"[network ops] {cid}: {len(groups)} launch groups, PDL {eng.debug_uses_pdl()}, conv kernels {sorted(mutated)}; "
-          f"worst |got - ref| / bound {worst:.3f}; {time.time() - t0:.1f} s")
+    print(f"[network ops] {cid}: {len(groups)} launch groups, PDL {eng.debug_uses_pdl()}, conv kernels {sorted(mutated)}; " +
+          ("every group byte-exact" if eng.dtype == "int8" else f"worst |got - ref| / bound {worst:.3f}") + f"; {time.time() - t0:.1f} s")
     eng.close()
 
 
@@ -441,7 +526,7 @@ def test_short_batch_at_benchmark_plans(cid, monkeypatch):
     sentinel = {}
     for bi in bufs:
         a = _read(eng, bi, B)
-        a[n:] = np.nan
+        a[n:] = -128 if eng.dtype == "int8" else np.nan
         eng.debug_write_buffer(bi, a)
         sentinel[bi] = _frame_hashes(a)
     eng.infer_u8(frames[:n])
@@ -455,7 +540,7 @@ def test_short_batch_at_benchmark_plans(cid, monkeypatch):
 
 
 @gpu
-@pytest.mark.parametrize("cid", ["cfg3", "cfg5"])
+@pytest.mark.parametrize("cid", ["cfg3", "cfg5", "cfg3-int8"])
 def test_pipelined_pose_call_matches_infer(cid, monkeypatch):
     """test 3: submit_pose / collect_pose (a captured CUDA graph for the PAF parser; for OpenPifPaf, conv grids narrowed by the SMs
     reserved for the decoder) compute every buffer and both outputs as infer_u8 does.  The parsers only read the outputs."""
@@ -567,3 +652,29 @@ def test_group_references_chain_to_the_whole_graph(name):
         assert torch.equal(x, y), f"{name}: buffer {b} differs"
     if conf is not None:
         assert torch.equal(conf, cc) and torch.equal(paf, pc)
+
+
+@pytest.mark.parametrize("name", sorted({CFG[c][1] for c in INT8}))
+def test_int8_group_references_chain_to_the_whole_graph(name):
+    """the same for the INT8 engine's groups (one per op, the im2col op on its own): the per-group int8_sim references, chained over
+    their own buffers, reproduce int8_sim.run_graph of the whole graph byte for byte.  Scales: set_int8_scales on per-buffer max |x|
+    of a float run of the graph."""
+    H, W = CPU_SIZES.get(name, (64, 96))
+    g = getattr(models, name)(seed=0)
+    frames = syn.make_frames_u8(3, 2, H, W)
+    g.set_int8_scales(int8_sim.float_absmax(g, frames))
+    groups = launch_groups(g, ["op"] * len(g.ops), "int8")
+    assert len(groups) == len(g.ops) and groups[0].ops[0].type == models.OP_IM2COL3 and groups[0].outs == [(g.ops[0].out_buf, 0, None)]
+    conf, paf, whole = int8_sim.run_graph(g, g.act_scales, frames_u8=frames)
+    state = [np.zeros_like(b) for b in whole]
+    cc = pc = None
+    for grp in groups:
+        bufs, c, p = grp.reference_int8(g.act_scales, {b: state[b] for b in grp.used}, frames)
+        for b, a in bufs.items():
+            state[b] = a
+        if c is not None:
+            cc, pc = c, p
+    for b, (x, y) in enumerate(zip(whole, state)):
+        assert x.tobytes() == y.tobytes(), f"{name}: buffer {b} differs"
+    assert all(len(np.unique(whole[b])) >= 16 for b in (g.ops[0].out_buf, g.ops[-1].in_buf))   # the patches and the last features
+    assert conf.tobytes() == cc.tobytes() and paf.tobytes() == pc.tobytes()
