@@ -214,7 +214,14 @@ EXPORTS += [
     "hp_engine_debug_op_epilogue", "hp_engine_debug_op_conv_epilogue", "hp_engine_debug_uses_pdl",
     "hp_engine_debug_read_buffer_raw", "hp_engine_debug_write_outputs",
     "hp_engine_calibrate_u8", "hp_pack_int8_calibrated",
+    "hp_pose_submit_frames_u8_host", "hp_pose_submit_frames_u8_device", "hp_pose_submit_pifpaf_frames_u8_host",
+    "hp_pose_submit_pifpaf_frames_u8_device", "hp_pose_debug_read_slot_frames",
 ]
+
+
+class FrameU8(C.Structure):
+    """hp_frame_u8: one HWC BGR frame of any size, rows packed"""
+    _fields_ = [("data", C.c_void_p), ("height", C.c_int32), ("width", C.c_int32)]
 
 
 def _bind_engine(L):
@@ -259,6 +266,10 @@ def _bind_engine(L):
     L.hp_pose_submit_u8_host.argtypes = [vp, vp, vp, C.c_int, ip]
     L.hp_pose_submit_u8_device.argtypes = [vp, vp, vp, C.c_int, ip]
     L.hp_pose_collect.argtypes = [vp, C.c_int, vp, C.c_int, ip]
+    for f in (L.hp_pose_submit_frames_u8_host, L.hp_pose_submit_frames_u8_device, L.hp_pose_submit_pifpaf_frames_u8_host,
+              L.hp_pose_submit_pifpaf_frames_u8_device):
+        f.argtypes = [vp, vp, C.POINTER(FrameU8), C.c_int, C.c_int, ip]
+    L.hp_pose_debug_read_slot_frames.argtypes = [vp, C.c_int, vp, C.c_int]
     L.hp_pose_stats.argtypes = [vp, C.POINTER(C.c_longlong), C.POINTER(C.c_longlong)]
     L.hp_pool_create.argtypes = [C.POINTER(vp), ip, C.c_int, vp, C.c_size_t, C.c_int, C.c_int, C.c_int, C.c_double, C.c_int, C.c_float, C.c_float]
     L.hp_pool_destroy.argtypes = [vp]
@@ -506,11 +517,53 @@ class Engine:
         self._ticket_n[t.value] = n
         return t.value
 
+    def _submit_frame_table(self, parser, table, keep_ratio, device: bool) -> int:
+        t = C.c_int(-1)
+        L = lib()
+        if isinstance(parser, PifPafParser):
+            fn = L.hp_pose_submit_pifpaf_frames_u8_device if device else L.hp_pose_submit_pifpaf_frames_u8_host
+        else:
+            fn = L.hp_pose_submit_frames_u8_device if device else L.hp_pose_submit_frames_u8_host
+        check(fn(self._h, parser._h, table, len(table), 1 if keep_ratio else 0, C.byref(t)))
+        self._ticket_n = getattr(self, "_ticket_n", {})
+        self._ticket_n[t.value] = len(table)
+        return t.value
+
+    def submit_pose_frames(self, parser, frames, keep_ratio: bool = False) -> int:
+        """hp_pose_submit_frames_u8_host (hp_pose_submit_pifpaf_frames_u8_host for a PifPafParser): a list of u8 HWC3 BGR frames of
+        any sizes, resized on the GPU as cv::resize / non_scaling_resize (keep_ratio) do; returns the ticket for collect_pose.
+        Page-locked frames are read by DMA after submit returns: they are kept referenced here until the ticket is collected."""
+        for i, f in enumerate(frames):
+            if not isinstance(f, np.ndarray) or f.dtype != np.uint8 or f.ndim != 3 or f.shape[2] != 3:
+                raise HyperposeError(HP_ERR_ARG, f"frame {i}: expected a uint8 HWC array with 3 channels, got "
+                                                 f"{getattr(f, 'dtype', type(f).__name__)} {getattr(f, 'shape', '')}")
+        frames = [np.ascontiguousarray(f) for f in frames]
+        table = (FrameU8 * len(frames))(*[FrameU8(f.ctypes.data, f.shape[0], f.shape[1]) for f in frames])
+        t = self._submit_frame_table(parser, table, keep_ratio, device=False)
+        self._ticket_frames = getattr(self, "_ticket_frames", {})
+        self._ticket_frames[t] = frames
+        return t
+
+    def submit_pose_frames_device(self, parser, frames, keep_ratio: bool = False) -> int:
+        """the same for frames in device memory, given as [(ptr, h, w), ...] (u8 HWC3, rows packed).  The resize kernel reads them in
+        place: they must stay valid and unchanged until the ticket is collected."""
+        table = (FrameU8 * len(frames))(*[FrameU8(int(p), int(h), int(w)) for p, h, w in frames])
+        return self._submit_frame_table(parser, table, keep_ratio, device=True)
+
+    def debug_read_slot_frames(self, ticket: int, n: int) -> np.ndarray:
+        """the first n resized network-size frames u8[n,in_h,in_w,3] of a ticket in flight or collected"""
+        out = np.empty((n, self.in_h, self.in_w, 3), np.uint8)
+        check(lib().hp_pose_debug_read_slot_frames(self._h, ticket, out.ctypes.data, n))
+        return out
+
     def collect_pose(self, ticket: int, cap: int = 128):
         N = self._ticket_n[ticket]
         out = np.zeros((N, cap), HUMAN_DT)
         n = (C.c_int * N)()
-        check(lib().hp_pose_collect(self._h, ticket, out.ctypes.data, cap, n))
+        try:
+            check(lib().hp_pose_collect(self._h, ticket, out.ctypes.data, cap, n))
+        finally:   # (the batch has been waited for: its source frames may go)
+            getattr(self, "_ticket_frames", {}).pop(ticket, None)
         return [out[i, :n[i]].copy() for i in range(N)]
 
     def pose_stats(self):

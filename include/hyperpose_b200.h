@@ -295,6 +295,23 @@ int hp_pose_stats(const hp_engine* e, long long* graph_captures, long long* grap
  * been consumed (decoder kernels P1-P3), not for the growth.  Tickets / hp_pose_collect as above. */
 int hp_pose_submit_pifpaf_u8_host(hp_engine* e, hp_pifpaf* decoder, const uint8_t* frames, int N, int* ticket);
 int hp_pose_submit_pifpaf_u8_device(hp_engine* e, hp_pifpaf* decoder, const uint8_t* d_frames, int N, int* ticket);
+/* The pipelined calls for frames of ANY size (cameras, video files: 640x360, 1280x720, 1920x1080 ...): each frame goes through the
+ * reference's resize step -- cv::resize(INTER_LINEAR) or, with keep_ratio, non_scaling_resize (src/tensorrt.cpp:446-451,
+ * src/data.cpp:53-69) -- bit-exact with OpenCV, in ONE batched kernel on the engine stream ahead of the network; the frames of a batch
+ * may all differ in size.  Results by hp_pose_collect, as above.  N > max_batch is HP_ERR_BATCH, a null frame or a size <= 0
+ * HP_ERR_ARG; packs the network-size calls refuse are refused alike.
+ * _host: the source pixels are copied on the copy stream (overlapping the previous batch's convolutions): page-locked frames by DMA
+ * straight from them (keep them alive until collect), pageable ones through pinned staging before submit returns.  Page-locked
+ * frames save a host memcpy of every frame.
+ * _device: the frames are read in place from device memory by the resize kernel: they must stay valid and unchanged until the
+ * ticket is collected. */
+typedef struct hp_frame_u8 { const uint8_t* data; int32_t height, width; } hp_frame_u8;   /* HWC BGR, rows packed */
+int hp_pose_submit_frames_u8_host(hp_engine* e, hp_paf* parser, const hp_frame_u8* frames, int N, int keep_ratio, int* ticket);
+int hp_pose_submit_frames_u8_device(hp_engine* e, hp_paf* parser, const hp_frame_u8* frames, int N, int keep_ratio, int* ticket);
+int hp_pose_submit_pifpaf_frames_u8_host(hp_engine* e, hp_pifpaf* decoder, const hp_frame_u8* frames, int N, int keep_ratio, int* ticket);
+int hp_pose_submit_pifpaf_frames_u8_device(hp_engine* e, hp_pifpaf* decoder, const hp_frame_u8* frames, int N, int keep_ratio, int* ticket);
+/* test hook: the first N resized network-size frames [N,in_h,in_w,3] of an in-flight or collected ticket */
+int hp_pose_debug_read_slot_frames(hp_engine* e, int ticket, uint8_t* out, int N);
 int hp_pifpaf_pipeline_info(hp_pifpaf* p, void** stream, void** inputs_free_event, int* hcap);
 int hp_pifpaf_copy_results_host_async(hp_pifpaf* p, hp_human* pin_humans, int* pin_counts_flags, int N, void* stream);
 int hp_pifpaf_grow_capacity(hp_pifpaf* p, int flags);
