@@ -267,8 +267,10 @@ def _bind_engine(L):
     L.hp_pose_submit_u8_device.argtypes = [vp, vp, vp, C.c_int, ip]
     L.hp_pose_collect.argtypes = [vp, C.c_int, vp, C.c_int, ip]
     for f in (L.hp_pose_submit_frames_u8_host, L.hp_pose_submit_frames_u8_device, L.hp_pose_submit_pifpaf_frames_u8_host,
-              L.hp_pose_submit_pifpaf_frames_u8_device):
+              L.hp_pose_submit_pifpaf_frames_u8_device, L.hp_pose_submit_ppn_frames_u8_host, L.hp_pose_submit_ppn_frames_u8_device):
         f.argtypes = [vp, vp, C.POINTER(FrameU8), C.c_int, C.c_int, ip]
+    L.hp_pose_submit_ppn_u8_host.argtypes = [vp, vp, vp, C.c_int, ip]
+    L.hp_pose_submit_ppn_u8_device.argtypes = [vp, vp, vp, C.c_int, ip]
     L.hp_pose_debug_read_slot_frames.argtypes = [vp, C.c_int, vp, C.c_int]
     L.hp_pose_stats.argtypes = [vp, C.POINTER(C.c_longlong), C.POINTER(C.c_longlong)]
     L.hp_pool_create.argtypes = [C.POINTER(vp), ip, C.c_int, vp, C.c_size_t, C.c_int, C.c_int, C.c_int, C.c_double, C.c_int, C.c_float, C.c_float]
@@ -492,13 +494,16 @@ class Engine:
 
 
     def submit_pose(self, parser: "PafParser", frames: np.ndarray) -> int:
-        """hp_pose_submit_u8_host: enqueue one batch (H2D on the copy stream, graph replay, record D2H); returns the ticket.
+        """hp_pose_submit_u8_host (the _pifpaf_ / _ppn_ form for a PifPafParser / PoseProposalParser): enqueue one batch (H2D on the
+        copy stream, graph replay, record D2H); returns the ticket.
         `frames` must stay alive until collect_pose when it is page-locked memory (DMA reads it directly)."""
         assert frames.dtype == np.uint8 and frames.flags["C_CONTIGUOUS"]
         t = C.c_int(-1)
         if isinstance(parser, PifPafParser):   # OpenPifPaf pack: decoder on its own stream underneath the next batch's convs
             lib().hp_pose_submit_pifpaf_u8_host.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.POINTER(C.c_int)]
             check(lib().hp_pose_submit_pifpaf_u8_host(self._h, parser._h, frames.ctypes.data, frames.shape[0], C.byref(t)))
+        elif isinstance(parser, PoseProposalParser):   # PPN pack: the parse is part of the captured graph on the engine stream
+            check(lib().hp_pose_submit_ppn_u8_host(self._h, parser._h, frames.ctypes.data, frames.shape[0], C.byref(t)))
         else:
             check(lib().hp_pose_submit_u8_host(self._h, parser._h, frames.ctypes.data, frames.shape[0], C.byref(t)))
         self._ticket_n = getattr(self, "_ticket_n", {})
@@ -511,6 +516,8 @@ class Engine:
         if isinstance(parser, PifPafParser):
             lib().hp_pose_submit_pifpaf_u8_device.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.POINTER(C.c_int)]
             check(lib().hp_pose_submit_pifpaf_u8_device(self._h, parser._h, d_frames_ptr, n, C.byref(t)))
+        elif isinstance(parser, PoseProposalParser):
+            check(lib().hp_pose_submit_ppn_u8_device(self._h, parser._h, d_frames_ptr, n, C.byref(t)))
         else:
             check(lib().hp_pose_submit_u8_device(self._h, parser._h, d_frames_ptr, n, C.byref(t)))
         self._ticket_n = getattr(self, "_ticket_n", {})
@@ -522,6 +529,8 @@ class Engine:
         L = lib()
         if isinstance(parser, PifPafParser):
             fn = L.hp_pose_submit_pifpaf_frames_u8_device if device else L.hp_pose_submit_pifpaf_frames_u8_host
+        elif isinstance(parser, PoseProposalParser):
+            fn = L.hp_pose_submit_ppn_frames_u8_device if device else L.hp_pose_submit_ppn_frames_u8_host
         else:
             fn = L.hp_pose_submit_frames_u8_device if device else L.hp_pose_submit_frames_u8_host
         check(fn(self._h, parser._h, table, len(table), 1 if keep_ratio else 0, C.byref(t)))
@@ -530,7 +539,8 @@ class Engine:
         return t.value
 
     def submit_pose_frames(self, parser, frames, keep_ratio: bool = False) -> int:
-        """hp_pose_submit_frames_u8_host (hp_pose_submit_pifpaf_frames_u8_host for a PifPafParser): a list of u8 HWC3 BGR frames of
+        """hp_pose_submit_frames_u8_host (hp_pose_submit_pifpaf_frames_u8_host for a PifPafParser, hp_pose_submit_ppn_frames_u8_host for a
+        PoseProposalParser): a list of u8 HWC3 BGR frames of
         any sizes, resized on the GPU as cv::resize / non_scaling_resize (keep_ratio) do; returns the ticket for collect_pose.
         Page-locked frames are read by DMA after submit returns: they are kept referenced here until the ticket is collected."""
         for i, f in enumerate(frames):
@@ -700,7 +710,10 @@ class PifPafParser:
 
 
 EXPORTS += ["hp_ppn_create", "hp_ppn_destroy", "hp_ppn_set_point_thresh", "hp_ppn_set_limb_thresh", "hp_ppn_set_nms_thresh",
-            "hp_ppn_process_host", "hp_ppn_process_device", "hp_ppn_process_device_strided", "hp_ppn_fetch", "hp_ppn_launch_count"]
+            "hp_ppn_process_host", "hp_ppn_process_device", "hp_ppn_process_device_strided", "hp_ppn_fetch", "hp_ppn_launch_count",
+            "hp_ppn_prepare", "hp_ppn_state", "hp_ppn_copy_results_host_async", "hp_ppn_grow_capacity",
+            "hp_pose_submit_ppn_u8_host", "hp_pose_submit_ppn_u8_device", "hp_pose_submit_ppn_frames_u8_host",
+            "hp_pose_submit_ppn_frames_u8_device"]
 
 
 class PoseProposalParser:

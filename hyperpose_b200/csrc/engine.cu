@@ -808,6 +808,7 @@ struct hp_engine {
     float* d_conf = nullptr;
     float* d_paf = nullptr;
     int out_h = 0, out_w = 0;
+    int ppn_K = 0, ppn_E = 0, ppn_nh = 0, ppn_nw = 0;   // PPN packs: key points, limbs and neighbourhood of the head op's outputs
     uint8_t* d_frames = nullptr;   // [max_batch, in_h, in_w, 3]
     float* d_input_f32 = nullptr;  // [max_batch, 3, in_h, in_w] (lazily)
     uint8_t* pin_frames = nullptr;
@@ -850,10 +851,12 @@ struct hp_engine {
         bool busy = false;
         int N = 0, hcap = 0;
         hp_paf* parser = nullptr;
+        hp_ppn* ppn = nullptr;             // Pose Proposal Network packs: parsed on the engine stream, like the PAF parser
         hp_pifpaf* decoder = nullptr;      // OpenPifPaf packs: the slot's batch is decoded on the decoder's stream
         cudaEvent_t conv_done = nullptr;   // (pifpaf) the engine's kernels of this slot have finished: the decoder may start
         cudaGraphExec_t graph = nullptr;   // captured launch sequence (convs + parse + result D2H) of this slot
-        float key_f[2] = { 0, 0 }; int key_i[6] = { 0, 0, 0, 0, 0, 0 }; int key_N = 0; const void* key_parser = nullptr;
+        // the parser's hp_paf_state / hp_ppn_state when the graph was captured
+        float key_f[3] = { 0, 0, 0 }; int key_i[6] = { 0, 0, 0, 0, 0, 0 }; int key_N = 0; const void* key_parser = nullptr;
         const void* key_ovr[2] = { nullptr, nullptr };
     } slots[2];
     int next_slot = 0;
@@ -1728,6 +1731,7 @@ int hp_engine_create_ex(hp_engine** out, const void* pack, size_t pack_bytes, in
                 return fail(HP_ERR_ARG);
             }
             op.launch = Launch::PpnHead;
+            e->ppn_K = (int)K; e->ppn_E = (int)po.groups; e->ppn_nh = (int)po.R; e->ppn_nw = (int)po.S;
         } else {
             set_error("engine: unknown op type %u", po.type);
             return fail(HP_ERR_UNSUPPORTED);
@@ -2387,16 +2391,29 @@ int hp_debug_halo_phases(unsigned long long* out, int n, int reset)
 
 namespace {
 
+// the network of the slot's frames, the parse of its outputs and the record D2H, all on `st`
 int pose_enqueue_compute(hp_engine* e, hp_engine::PoseSlot& sl, cudaStream_t st)
 {
     e->cur_frames = sl.d_frames;
     int rc = run_graph(e, sl.N, true, st);
     e->cur_frames = nullptr;
     if (rc) return rc;
+    if (sl.ppn) {
+        // the PPN outputs parse in place: conf slot [N,6,K,gh,gw] = conf_point, conf_iou, x, y, w, h; paf slot [N,E,nh,nw,gh,gw] = edges
+        const size_t KG = (size_t)e->ppn_K * e->out_h * e->out_w;
+        rc = hp_ppn_process_device_strided(sl.ppn, e->d_conf, e->d_conf + 2 * KG, e->d_conf + 3 * KG, e->d_conf + 4 * KG, e->d_conf + 5 * KG,
+                                           e->d_paf, sl.N, e->ppn_K, e->out_h, e->out_w, e->ppn_E, e->ppn_nh, e->ppn_nw, 6 * KG,
+                                           (size_t)e->hdr.paf_channels * e->out_h * e->out_w, (void*)st);
+        if (rc) return rc;
+        return hp_ppn_copy_results_host_async(sl.ppn, sl.pin_humans, sl.pin_counts, sl.N, (void*)st);
+    }
     rc = hp_paf_process_device(sl.parser, e->d_conf, e->d_paf, sl.N, (int)e->hdr.conf_channels, (int)e->hdr.paf_channels, e->out_h, e->out_w, (void*)st);
     if (rc) return rc;
     return hp_paf_copy_results_host_async(sl.parser, sl.pin_humans, sl.pin_counts, sl.N, (void*)st);
 }
+
+// kernels the slot's parse launches per batch (what the parser's own launch count adds on the direct path)
+int parse_kernels(const hp_engine::PoseSlot& sl) { return sl.ppn ? 1 : 2; }
 
 // what both pipelined calls need in a slot: its own frame buffer (the plain entry points keep hp_engine::d_frames), the upload and
 // completion events, and pinned record buffers for hcap humans per frame.  A captured graph holds their addresses: it goes when they move.
@@ -2500,21 +2517,32 @@ int slot_upload_frames(hp_engine* e, hp_engine::PoseSlot& sl, FrameDesc* descs, 
     return launch_resize(e, sl.d_desc, sl.d_frames, N);
 }
 
-int pose_slot_prepare(hp_engine* e, hp_engine::PoseSlot& sl, hp_paf* parser, int N)
+// the parser's state a captured graph bakes in (hp_paf_state / hp_ppn_state), and the capacity of records per frame in it
+void parser_state(const hp_paf* parser, const hp_ppn* ppn, float kf[3], int ki[6], int* hcap)
 {
-    int rc = hp_paf_prepare(parser, N, (int)e->hdr.conf_channels, (int)e->hdr.paf_channels, e->out_h, e->out_w);
+    kf[2] = 0.f;
+    if (ppn) { hp_ppn_state(ppn, kf, ki); *hcap = ki[2]; }
+    else { hp_paf_state(parser, kf, ki); *hcap = ki[4]; }
+}
+
+// one of parser / ppn: allocate for a batch of N with it, and drop the slot's graph when anything it bakes in has changed
+int pose_slot_prepare(hp_engine* e, hp_engine::PoseSlot& sl, hp_paf* parser, hp_ppn* ppn, int N)
+{
+    int rc = ppn ? hp_ppn_prepare(ppn, N, e->ppn_K, e->out_h, e->out_w, e->ppn_E, e->ppn_nh, e->ppn_nw)
+                 : hp_paf_prepare(parser, N, (int)e->hdr.conf_channels, (int)e->hdr.paf_channels, e->out_h, e->out_w);
     if (rc) return rc;
-    float kf[2]; int ki[6];
-    hp_paf_state(parser, kf, ki);
-    rc = slot_alloc(e, sl, ki[4]);
+    float kf[3]; int ki[6]; int hcap = 0;
+    parser_state(parser, ppn, kf, ki, &hcap);
+    rc = slot_alloc(e, sl, hcap);
     if (rc) return rc;
+    const void* handle = ppn ? (const void*)ppn : (const void*)parser;
     // anything the captured sequence bakes in
-    const bool same = sl.graph && sl.key_N == N && sl.key_parser == (const void*)parser && memcmp(sl.key_f, kf, sizeof(kf)) == 0 && memcmp(sl.key_i, ki, sizeof(ki)) == 0 &&
+    const bool same = sl.graph && sl.key_N == N && sl.key_parser == handle && memcmp(sl.key_f, kf, sizeof(kf)) == 0 && memcmp(sl.key_i, ki, sizeof(ki)) == 0 &&
                       sl.key_ovr[0] == (const void*)e->override_conf && sl.key_ovr[1] == (const void*)e->override_paf;
     if (!same && sl.graph) { cudaGraphExecDestroy(sl.graph); sl.graph = nullptr; }
-    sl.key_N = N; sl.key_parser = parser; memcpy(sl.key_f, kf, sizeof(kf)); memcpy(sl.key_i, ki, sizeof(ki));
+    sl.key_N = N; sl.key_parser = handle; memcpy(sl.key_f, kf, sizeof(kf)); memcpy(sl.key_i, ki, sizeof(ki));
     sl.key_ovr[0] = e->override_conf; sl.key_ovr[1] = e->override_paf;
-    sl.N = N; sl.parser = parser; sl.decoder = nullptr;
+    sl.N = N; sl.parser = parser; sl.ppn = ppn; sl.decoder = nullptr;
     return HP_OK;
 }
 
@@ -2528,7 +2556,7 @@ int pose_launch(hp_engine* e, hp_engine::PoseSlot& sl)
                 const long long l0 = e->launches;
                 const int rc = pose_enqueue_compute(e, sl, e->stream);
                 const cudaError_t ce = cudaStreamEndCapture(e->stream, &g);
-                e->launches = l0 - 2;   // capturing launches nothing (the parser counted its two kernels: taken back here)
+                e->launches = l0 - parse_kernels(sl);   // capturing launches nothing (the parser counted its kernels: taken back here)
                 if (rc == HP_OK && ce == cudaSuccess && g && cudaGraphInstantiate(&sl.graph, g, 0) == cudaSuccess) e->graph_captures++;
                 else { sl.graph = nullptr; e->graphs_ok = false; cudaGetLastError(); }
                 if (g) cudaGraphDestroy(g);
@@ -2537,7 +2565,7 @@ int pose_launch(hp_engine* e, hp_engine::PoseSlot& sl)
         if (sl.graph) {
             HP_CUDA_TRY(cudaGraphLaunch(sl.graph, e->stream));
             e->graph_launches++;
-            e->launches += e->step_kernels + 2;   // the replay runs what the direct path counts: the engine's step + the parser's two kernels
+            e->launches += e->step_kernels + parse_kernels(sl);   // the replay runs what the direct path counts: the engine's step + the parse
             return HP_OK;
         }
     }
@@ -2557,7 +2585,7 @@ static int pifpaf_slot_prepare(hp_engine* e, hp_engine::PoseSlot& sl, hp_pifpaf*
     const int rc = slot_alloc(e, sl, hcap);
     if (rc) return rc;
     if (!sl.conv_done) HP_CUDA_TRY(cudaEventCreateWithFlags(&sl.conv_done, cudaEventDisableTiming));
-    sl.N = N; sl.parser = nullptr; sl.decoder = dec;
+    sl.N = N; sl.parser = nullptr; sl.ppn = nullptr; sl.decoder = dec;
     return HP_OK;
 }
 
@@ -2607,20 +2635,34 @@ static int pose_submit_pifpaf(hp_engine* e, hp_pifpaf* dec, const uint8_t* frame
     return HP_OK;
 }
 
-static int pose_submit(hp_engine* e, hp_paf* parser, const uint8_t* frames, FrameDesc* descs, int N, int* ticket, bool device_src)
+// the PAF-parser calls (ppn_call false: `parser` is an hp_paf) and the Pose Proposal Network calls (true: an hp_ppn)
+static int pose_submit(hp_engine* e, void* parser, bool ppn_call, const uint8_t* frames, FrameDesc* descs, int N, int* ticket, bool device_src)
 {
-    if (!e || !parser || (!frames && !descs) || !ticket) { set_error("hp_pose_submit: null argument"); return HP_ERR_ARG; }
+    const char* fn = ppn_call ? "hp_pose_submit_ppn" : "hp_pose_submit";
+    if (!e || !parser || (!frames && !descs) || !ticket) { set_error("%s: null argument", fn); return HP_ERR_ARG; }
     if (N <= 0 || N > e->max_batch) { set_error("Input batch size overflow: Yours@%d Max@%d", N, e->max_batch); return HP_ERR_BATCH; }
-    if (e->hdr.head_type == 1) { set_error("hp_pose_submit: the model pack has OpenPifPaf heads (use hp_engine_infer_u8_host + hp_pifpaf_process_device)"); return HP_ERR_UNSUPPORTED; }
-    if (e->hdr.head_type != 0) {
-        set_error("hp_pose_submit: the model pack has Pose Proposal Network heads (use hp_engine_infer_u8_device + hp_ppn_process_device_strided on the engine's outputs)");
-        return HP_ERR_UNSUPPORTED;
+    hp_paf* paf = ppn_call ? nullptr : (hp_paf*)parser;
+    hp_ppn* ppn = ppn_call ? (hp_ppn*)parser : nullptr;
+    if (ppn) {
+        if (e->hdr.head_type != 2) {
+            set_error("hp_pose_submit_ppn: the model pack has no Pose Proposal Network heads (head_type %u)", e->hdr.head_type);
+            return HP_ERR_UNSUPPORTED;
+        }
+        int ki[6];
+        hp_ppn_state(ppn, nullptr, ki);
+        if (ki[5] != e->device) { set_error("hp_pose_submit_ppn: the parser is on device %d but the engine on device %d", ki[5], e->device); return HP_ERR_ARG; }
+    } else {
+        if (e->hdr.head_type == 1) { set_error("hp_pose_submit: the model pack has OpenPifPaf heads (use hp_engine_infer_u8_host + hp_pifpaf_process_device)"); return HP_ERR_UNSUPPORTED; }
+        if (e->hdr.head_type != 0) {
+            set_error("hp_pose_submit: the model pack has Pose Proposal Network heads (use hp_pose_submit_ppn_* with a Pose Proposal Network parser)");
+            return HP_ERR_UNSUPPORTED;
+        }
     }
     HP_CUDA_TRY(cudaSetDevice(e->device));
     const int idx = e->next_slot;
     hp_engine::PoseSlot& sl = e->slots[idx];
-    if (sl.busy) { set_error("hp_pose_submit: two batches are already in flight -- collect ticket %d first", idx); return HP_ERR_ARG; }
-    int rc = pose_slot_prepare(e, sl, parser, N);
+    if (sl.busy) { set_error("%s: two batches are already in flight -- collect ticket %d first", fn, idx); return HP_ERR_ARG; }
+    int rc = pose_slot_prepare(e, sl, paf, ppn, N);
     if (rc) return rc;
     rc = descs ? slot_upload_frames(e, sl, descs, N, device_src)   // (the captured graph reads the slot's buffer)
                : slot_upload(e, sl, frames, N, device_src);
@@ -2636,13 +2678,13 @@ static int pose_submit(hp_engine* e, hp_paf* parser, const uint8_t* frames, Fram
 
 int hp_pose_submit_u8_host(hp_engine* e, hp_paf* parser, const uint8_t* frames, int N, int* ticket)
 {
-    return pose_submit(e, parser, frames, nullptr, N, ticket, false);
+    return pose_submit(e, parser, false, frames, nullptr, N, ticket, false);
 }
 
 // the same with the frames already resident in device memory (what a decoder / capture pipeline on the GPU hands over)
 int hp_pose_submit_u8_device(hp_engine* e, hp_paf* parser, const uint8_t* d_frames, int N, int* ticket)
 {
-    return pose_submit(e, parser, d_frames, nullptr, N, ticket, true);
+    return pose_submit(e, parser, false, d_frames, nullptr, N, ticket, true);
 }
 
 int hp_pose_submit_pifpaf_u8_host(hp_engine* e, hp_pifpaf* decoder, const uint8_t* frames, int N, int* ticket)
@@ -2676,14 +2718,14 @@ int hp_pose_submit_frames_u8_host(hp_engine* e, hp_paf* parser, const hp_frame_u
 {
     std::vector<FrameDesc> d;
     const int rc = frame_descs(e, frames, N, keep_ratio, d);
-    return rc ? rc : pose_submit(e, parser, nullptr, d.data(), N, ticket, false);
+    return rc ? rc : pose_submit(e, parser, false, nullptr, d.data(), N, ticket, false);
 }
 
 int hp_pose_submit_frames_u8_device(hp_engine* e, hp_paf* parser, const hp_frame_u8* frames, int N, int keep_ratio, int* ticket)
 {
     std::vector<FrameDesc> d;
     const int rc = frame_descs(e, frames, N, keep_ratio, d);
-    return rc ? rc : pose_submit(e, parser, nullptr, d.data(), N, ticket, true);
+    return rc ? rc : pose_submit(e, parser, false, nullptr, d.data(), N, ticket, true);
 }
 
 int hp_pose_submit_pifpaf_frames_u8_host(hp_engine* e, hp_pifpaf* decoder, const hp_frame_u8* frames, int N, int keep_ratio, int* ticket)
@@ -2698,6 +2740,31 @@ int hp_pose_submit_pifpaf_frames_u8_device(hp_engine* e, hp_pifpaf* decoder, con
     std::vector<FrameDesc> d;
     const int rc = frame_descs(e, frames, N, keep_ratio, d);
     return rc ? rc : pose_submit_pifpaf(e, decoder, nullptr, d.data(), N, ticket, true);
+}
+
+// ---- Pose Proposal Network packs: network, parse and record D2H in one captured graph on the engine stream, as for the PAF parser ----
+int hp_pose_submit_ppn_u8_host(hp_engine* e, hp_ppn* parser, const uint8_t* frames, int N, int* ticket)
+{
+    return pose_submit(e, parser, true, frames, nullptr, N, ticket, false);
+}
+
+int hp_pose_submit_ppn_u8_device(hp_engine* e, hp_ppn* parser, const uint8_t* d_frames, int N, int* ticket)
+{
+    return pose_submit(e, parser, true, d_frames, nullptr, N, ticket, true);
+}
+
+int hp_pose_submit_ppn_frames_u8_host(hp_engine* e, hp_ppn* parser, const hp_frame_u8* frames, int N, int keep_ratio, int* ticket)
+{
+    std::vector<FrameDesc> d;
+    const int rc = frame_descs(e, frames, N, keep_ratio, d);
+    return rc ? rc : pose_submit(e, parser, true, nullptr, d.data(), N, ticket, false);
+}
+
+int hp_pose_submit_ppn_frames_u8_device(hp_engine* e, hp_ppn* parser, const hp_frame_u8* frames, int N, int keep_ratio, int* ticket)
+{
+    std::vector<FrameDesc> d;
+    const int rc = frame_descs(e, frames, N, keep_ratio, d);
+    return rc ? rc : pose_submit(e, parser, true, nullptr, d.data(), N, ticket, true);
 }
 
 // test hook: the first N resized network-size frames of ticket `ticket` (in flight or collected)
@@ -2738,14 +2805,37 @@ int hp_pose_collect(hp_engine* e, int ticket, hp_human* out, int cap, int* n_out
         if (rc) return rc;
         HP_CUDA_TRY(cudaEventSynchronize(sl.done));
     }
-    for (int attempt = 0; !sl.decoder && attempt < 8; ++attempt) {
+    for (int attempt = 0; sl.ppn && attempt < 8; ++attempt) {
+        int flags = 0, max_count = 0;
+        for (int f = 0; f < N; ++f) { flags |= sl.pin_counts[N + f]; max_count = std::max(max_count, sl.pin_counts[f]); }
+        if (!flags) break;
+        // the reference is unbounded: grow the capacity that overflowed and run this slot's frames again (they are still in its
+        // device buffer), synchronously and outside the graph.  The other ticket may be in flight, and growing reallocates the
+        // parser's buffers its graph writes: it is waited for first.  It keeps its own record capacity and results.
+        HP_CUDA_TRY(cudaStreamSynchronize(e->stream));
+        float kf[3]; int ki[6];
+        hp_ppn_state(sl.ppn, kf, ki);
+        if (ki[2] == sl.key_i[2] && ki[3] == sl.key_i[3]) {   // (else the other ticket's collect has grown the parser since: just run again)
+            const int rc = hp_ppn_grow_capacity(sl.ppn, flags, max_count);
+            if (rc) return rc;
+        }
+        // (with the output override the batch was submitted with: the caller may have set another since)
+        const float* ovr_now[2] = { e->override_conf, e->override_paf };
+        e->override_conf = (const float*)sl.key_ovr[0]; e->override_paf = (const float*)sl.key_ovr[1];
+        int rc = pose_slot_prepare(e, sl, nullptr, sl.ppn, N);
+        if (rc == HP_OK) rc = pose_enqueue_compute(e, sl, e->stream);
+        e->override_conf = ovr_now[0]; e->override_paf = ovr_now[1];
+        if (rc) return rc;
+        HP_CUDA_TRY(cudaStreamSynchronize(e->stream));
+    }
+    for (int attempt = 0; sl.parser && attempt < 8; ++attempt) {
         int flags = 0;
         for (int f = 0; f < N; ++f) flags |= sl.pin_counts[N + f];
         if (!flags) break;
         // the reference is unbounded: grow the parser capacity that overflowed and run this slot's frames again (they are still
         // in its device buffer), synchronously and outside the graph
         if (hp_paf_grow_capacity(sl.parser, flags) != HP_OK) { set_error("hp_pose_collect: parser capacity limit reached (flags=%d)", flags); return HP_ERR_CAPACITY; }
-        int rc = pose_slot_prepare(e, sl, sl.parser, N);
+        int rc = pose_slot_prepare(e, sl, sl.parser, nullptr, N);
         if (rc) return rc;
         rc = pose_enqueue_compute(e, sl, e->stream);
         if (rc) return rc;

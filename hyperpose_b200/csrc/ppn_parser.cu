@@ -391,7 +391,59 @@ struct hp_ppn {
     std::vector<hp_human> host_h; std::vector<int> host_c;
     long long launches = 0;
     int last_N = 0;
+    int prep_N = 0;          // frames humans / counters / spill are allocated for (they only grow)
 };
+
+namespace {
+
+// the launch shape of a grid: candidate-key capacity (a power of two) and dynamic shared memory, or a refusal
+int launch_config(const hp_ppn* p, int gh, int gw, int nh, int nw, int* cap_c, size_t* smem)
+{
+    const int G = gh * gw;
+    if (G > 16384) { hpb::set_error("hp_ppn: %dx%d grid not supported", gh, gw); return HP_ERR_UNSUPPORTED; }
+    // candidate capacity: worst case one per (from box, neighbour) = G * nh * nw, rounded up to a power of two,
+    // bounded by the shared memory left (the phase-D tables alias the same region)
+    const size_t fixed = fixed_smem(G);
+    const size_t tables = p->use_spill ? (size_t)2 * HASH * HASH * sizeof(int) : (size_t)(2 * HASH * HASH + 2 * CAP_ENT) * sizeof(short);
+    size_t want = 1;
+    while (want < (size_t)G * nh * nw) want <<= 1;
+    const size_t budget = (size_t)p->smem_optin - 1024;
+    if (fixed + tables > budget) { hpb::set_error("hp_ppn: %dx%d grid needs %zu B of shared memory (> %zu)", gh, gw, fixed + tables, budget); return HP_ERR_UNSUPPORTED; }
+    while (want > 1 && fixed + want * 8 > budget) want >>= 1;
+    size_t dyn = want * 8;
+    if (dyn < tables) dyn = tables;
+    *cap_c = (int)want;
+    *smem = fixed + dyn;
+    return HP_OK;
+}
+
+// the device buffers a launch of N frames writes, for at least every N prepared so far at the current capacities
+int ensure_buffers(hp_ppn* p, int N)
+{
+    if (N > p->prep_N) p->prep_N = N;
+    if (p->use_spill) HP_CUDA_TRY(p->spill.ensure((size_t)p->prep_N * spill_bytes()));
+    HP_CUDA_TRY(p->humans.ensure((size_t)p->prep_N * p->hcap));
+    HP_CUDA_TRY(p->counters.ensure((size_t)p->prep_N * 2));
+    return HP_OK;
+}
+
+// after a batch whose flags (OR over its frames) report an overflow, in the order hp_ppn_fetch has always grown: the record buffer to
+// the largest frame's count first, else the sticky global-scratch variant; anything else cannot grow
+int grow_after_overflow(hp_ppn* p, int flags, int max_count)
+{
+    if (flags & F_OUT) {
+        if (max_count > p->hcap) p->hcap = max_count;
+        return HP_OK;
+    }
+    if ((flags & (F_HUMANS | F_ENTRIES)) && !p->use_spill) {
+        p->use_spill = true;
+        return HP_OK;
+    }
+    if (flags) { hpb::set_error("hp_ppn: internal capacity exceeded (flags=%d: 1 limb candidates, 2 humans>%d, 4 hash registrations>%d)", flags, SPILL_CAP_H, SPILL_CAP_ENT); return HP_ERR_CAPACITY; }
+    return HP_OK;
+}
+
+} // namespace
 
 extern "C" {
 
@@ -464,30 +516,19 @@ int hp_ppn_process_device_strided(hp_ppn* p, const float* d_conf, const float* d
                        box_frame_stride, edge_frame_stride, K, E * nh * nw, gh, gw);
         return HP_ERR_ARG;
     }
-    const int G = gh * gw;
-    if (G > 16384) { hpb::set_error("hp_ppn: %dx%d grid not supported", gh, gw); return HP_ERR_UNSUPPORTED; }
+    int cap_c = 0;
+    size_t smem = 0;
+    int rc = launch_config(p, gh, gw, nh, nw, &cap_c, &smem);
+    if (rc) return rc;
     HP_CUDA_TRY(cudaSetDevice(p->device));
     cudaStream_t st = stream ? (cudaStream_t)stream : p->stream;
-    // candidate capacity: worst case one per (from box, neighbour) = G * nh * nw, rounded up to a power of two,
-    // bounded by the shared memory left (the phase-D tables alias the same region)
-    const size_t fixed = fixed_smem(G);
-    const size_t tables = p->use_spill ? (size_t)2 * HASH * HASH * sizeof(int) : (size_t)(2 * HASH * HASH + 2 * CAP_ENT) * sizeof(short);
-    size_t want = 1;
-    while (want < (size_t)G * nh * nw) want <<= 1;
-    const size_t budget = (size_t)p->smem_optin - 1024;
-    if (fixed + tables > budget) { hpb::set_error("hp_ppn: %dx%d grid needs %zu B of shared memory (> %zu)", gh, gw, fixed + tables, budget); return HP_ERR_UNSUPPORTED; }
-    while (want > 1 && fixed + want * 8 > budget) want >>= 1;
-    size_t dyn = want * 8;
-    if (dyn < tables) dyn = tables;
-    const size_t smem = fixed + dyn;
-    if (p->use_spill) HP_CUDA_TRY(p->spill.ensure((size_t)N * spill_bytes()));
-    HP_CUDA_TRY(p->humans.ensure((size_t)N * p->hcap));
-    HP_CUDA_TRY(p->counters.ensure((size_t)N * 2));
+    rc = ensure_buffers(p, N);   // (after hp_ppn_prepare for this N: allocates nothing, synchronises nothing)
+    if (rc) return rc;
     PpnParams P;
     P.conf = d_conf; P.x = d_x; P.y = d_y; P.w = d_w; P.h = d_h; P.edge = d_edge;
     P.K = K; P.gh = gh; P.gw = gw; P.E = E; P.nh = nh; P.nw = nw; P.net_w = p->net_w; P.net_h = p->net_h;
     P.box_stride = box_frame_stride; P.edge_stride = edge_frame_stride;
-    P.pt = p->pt; P.lt = p->lt; P.nt = p->nt; P.cap_c = (int)want;
+    P.pt = p->pt; P.lt = p->lt; P.nt = p->nt; P.cap_c = cap_c;
     P.humans = p->humans.p; P.hcap = p->hcap; P.human_cnt = p->counters.p; P.flags = p->counters.p + N;
     P.spill = p->spill.p;
     if (p->use_spill) ppn_parse_kernel<true><<<N, THREADS, smem, st>>>(P);
@@ -506,22 +547,17 @@ int hp_ppn_fetch(hp_ppn* p, hp_human* out, int cap, int* n_out, int N)
     p->host_h.resize((size_t)N * p->hcap); p->host_c.resize((size_t)N * 2);
     HP_CUDA_TRY(cudaMemcpy(p->host_c.data(), p->counters.p, sizeof(int) * 2 * N, cudaMemcpyDeviceToHost));
     HP_CUDA_TRY(cudaMemcpy(p->host_h.data(), p->humans.p, sizeof(hp_human) * (size_t)N * p->hcap, cudaMemcpyDeviceToHost));
-    int fl = 0;
-    for (int f = 0; f < N; ++f) fl |= p->host_c[N + f];
-    if (fl & F_OUT) {
-        // more humans than the device record buffer: grow it for the next call and tell the caller to retry
-        int mx = 0;
-        for (int f = 0; f < N; ++f) mx = p->host_c[f] > mx ? p->host_c[f] : mx;
-        p->hcap = mx;
-        hpb::set_error("hp_ppn: %d humans in one frame; record buffer grown, call again", mx);
+    int fl = 0, mx = 0;
+    for (int f = 0; f < N; ++f) { fl |= p->host_c[N + f]; mx = p->host_c[f] > mx ? p->host_c[f] : mx; }
+    if (fl) {
+        // grow what overflowed for the next call and tell the caller to retry
+        const int hcap_before = p->hcap;
+        const int rc = grow_after_overflow(p, fl, mx);
+        if (rc) return rc;
+        if (p->hcap != hcap_before) hpb::set_error("hp_ppn: %d humans in one frame; record buffer grown, call again", mx);
+        else hpb::set_error("hp_ppn: a frame overflowed the shared-memory human/hash capacities (%d / %d); switched to the global-scratch variant, call again", CAP_H, CAP_ENT);
         return HP_ERR_CAPACITY;
     }
-    if ((fl & (F_HUMANS | F_ENTRIES)) && !p->use_spill) {
-        p->use_spill = true;
-        hpb::set_error("hp_ppn: a frame overflowed the shared-memory human/hash capacities (%d / %d); switched to the global-scratch variant, call again", CAP_H, CAP_ENT);
-        return HP_ERR_CAPACITY;
-    }
-    if (fl) { hpb::set_error("hp_ppn: internal capacity exceeded (flags=%d: 1 limb candidates, 2 humans>%d, 4 hash registrations>%d)", fl, SPILL_CAP_H, SPILL_CAP_ENT); return HP_ERR_CAPACITY; }
     for (int f = 0; f < N; ++f) {
         const int n = p->host_c[f];
         if (n > cap) { hpb::set_error("hp_ppn: frame %d has %d humans but the caller's capacity is %d", f, n, cap); return HP_ERR_CAPACITY; }
@@ -557,5 +593,48 @@ int hp_ppn_process_host(hp_ppn* p, const float* conf_point, const float* x, cons
 }
 
 long long hp_ppn_launch_count(const hp_ppn* p) { return p ? p->launches : 0; }
+
+// ---- building blocks of the pipelined end-to-end call (engine.cu: hp_pose_submit_ppn_* / hp_pose_collect) -------------------
+// Checks the geometry and allocates everything a launch of N frames needs: hp_ppn_process_device_strided for this geometry then
+// allocates nothing and synchronises nothing, so it can be captured into a CUDA graph.
+int hp_ppn_prepare(hp_ppn* p, int N, int K, int gh, int gw, int E, int nh, int nw)
+{
+    if (!p || N <= 0 || gh <= 0 || gw <= 0 || E < 0 || nh <= 0 || nw <= 0) { hpb::set_error("hp_ppn_prepare: bad argument"); return HP_ERR_ARG; }
+    if (K < NPARTS) { hpb::set_error("hp_ppn: K=%d key-point maps, the COCO limb table needs 18", K); return HP_ERR_ARG; }
+    int cap_c = 0;
+    size_t smem = 0;
+    const int rc = launch_config(p, gh, gw, nh, nw, &cap_c, &smem);
+    if (rc) return rc;
+    HP_CUDA_TRY(cudaSetDevice(p->device));
+    return ensure_buffers(p, N);
+}
+// Everything a captured launch bakes in (a change invalidates the graph): point / limb / NMS thresholds, then net_w, net_h, hcap,
+// use_spill, the prepared N (the buffers' frame capacity), and the device.
+int hp_ppn_state(const hp_ppn* p, float* thresholds3, int* ints6)
+{
+    if (!p) return HP_ERR_ARG;
+    if (thresholds3) { thresholds3[0] = p->pt; thresholds3[1] = p->lt; thresholds3[2] = p->nt; }
+    if (ints6) { ints6[0] = p->net_w; ints6[1] = p->net_h; ints6[2] = p->hcap; ints6[3] = p->use_spill ? 1 : 0; ints6[4] = p->prep_N; ints6[5] = p->device; }
+    return HP_OK;
+}
+// Enqueues the D2H of the last launch's results on `stream` (NULL = the parser's own) into caller-owned PINNED host memory:
+// counts_flags[2N] (N counts, then N overflow flags, the layout of hp_paf_copy_results_host_async) and humans[N * hcap]; no
+// synchronisation.
+int hp_ppn_copy_results_host_async(hp_ppn* p, hp_human* pin_humans, int* pin_counts_flags, int N, void* stream)
+{
+    if (!p || !pin_humans || !pin_counts_flags || N <= 0 || N != p->last_N) { hpb::set_error("hp_ppn_copy_results_host_async: bad argument"); return HP_ERR_ARG; }
+    cudaStream_t st = stream ? (cudaStream_t)stream : p->stream;
+    HP_CUDA_TRY(cudaMemcpyAsync(pin_counts_flags, p->counters.p, sizeof(int) * 2 * N, cudaMemcpyDeviceToHost, st));
+    HP_CUDA_TRY(cudaMemcpyAsync(pin_humans, p->humans.p, sizeof(hp_human) * (size_t)N * p->hcap, cudaMemcpyDeviceToHost, st));
+    return HP_OK;
+}
+// After a launch whose flags (OR over its frames) report an overflow, max_count being its largest per-frame count: F_OUT raises hcap
+// to max_count; F_HUMANS / F_ENTRIES switch to the global-scratch variant (sticky); F_CAND, or the global-scratch variant overflowing,
+// is HP_ERR_CAPACITY.  Call hp_ppn_prepare before the next launch.
+int hp_ppn_grow_capacity(hp_ppn* p, int flags, int max_count)
+{
+    if (!p) return HP_ERR_ARG;
+    return grow_after_overflow(p, flags, max_count);
+}
 
 } // extern "C"

@@ -229,8 +229,8 @@ int hp_engine_read_outputs_host(hp_engine* e, float* conf, float* paf, int N);
 int hp_engine_read_outputs_frames(hp_engine* e, float* const* conf_frames, float* const* paf_frames, int N, int publish);
 /* 0: conf/paf maps for hyperpose::parser::paf; 1: OpenPifPaf fields (pif, paf) for hyperpose::parser::pifpaf;
  * 2: Pose Proposal Network outputs for hyperpose::parser::pose_proposal -- conf slot [6,K,gh,gw] (conf_point, conf_iou, x, y, w, h;
- * boxes in network-input pixels), paf slot [L,nh,nw,gh,gw] (edges), c_conf = 6K, c_paf = L*nh*nw.  The hp_pose_* calls refuse it:
- * parse with hp_ppn_process_device_strided on the engine's device outputs. */
+ * boxes in network-input pixels), paf slot [L,nh,nw,gh,gw] (edges), c_conf = 6K, c_paf = L*nh*nw.  The PAF-parser hp_pose_* calls
+ * refuse it: use hp_pose_submit_ppn_* (below), or parse with hp_ppn_process_device_strided on the engine's device outputs. */
 int hp_engine_head_type(const hp_engine* e);
 /* the publication mechanism above: global switch (default on; env HPB_NO_HANDOFF disables) and counters
  * (batches published, process() calls served from a device snapshot, batched parses run, look-ups that fell back) */
@@ -310,6 +310,18 @@ int hp_pose_submit_frames_u8_host(hp_engine* e, hp_paf* parser, const hp_frame_u
 int hp_pose_submit_frames_u8_device(hp_engine* e, hp_paf* parser, const hp_frame_u8* frames, int N, int keep_ratio, int* ticket);
 int hp_pose_submit_pifpaf_frames_u8_host(hp_engine* e, hp_pifpaf* decoder, const hp_frame_u8* frames, int N, int keep_ratio, int* ticket);
 int hp_pose_submit_pifpaf_frames_u8_device(hp_engine* e, hp_pifpaf* decoder, const hp_frame_u8* frames, int N, int keep_ratio, int* ticket);
+/* The pipelined calls for Pose Proposal Network packs (head_type 2): engine.inference(batch) + pose_proposal.process(packet) per image
+ * (examples/operator_api_batched_images_pose_proposal.example.cpp), two batches in flight, frames at the network size or (_frames_)
+ * of any size as above.  The parse of a batch runs on the engine stream right behind its network, reading the engine's outputs in
+ * place (the pointers and strides of hp_ppn_process_device_strided, with K, E, nh, nw from the pack's PPN head op), and the network,
+ * the parse and the record D2H are replayed from one CUDA graph per ticket.  The records are byte-identical to hp_engine_infer_u8_device
+ * + hp_ppn_process_device_strided + hp_ppn_fetch (retried on HP_ERR_CAPACITY).  A pack without PPN heads is HP_ERR_UNSUPPORTED, a
+ * parser on another device than the engine HP_ERR_ARG.  Tickets / hp_pose_collect as above: a parser capacity that overflows is grown
+ * in collect and the ticket's frames run again, so HP_ERR_CAPACITY there means the CALLER's `cap`. */
+int hp_pose_submit_ppn_u8_host(hp_engine* e, hp_ppn* parser, const uint8_t* frames, int N, int* ticket);
+int hp_pose_submit_ppn_u8_device(hp_engine* e, hp_ppn* parser, const uint8_t* d_frames, int N, int* ticket);
+int hp_pose_submit_ppn_frames_u8_host(hp_engine* e, hp_ppn* parser, const hp_frame_u8* frames, int N, int keep_ratio, int* ticket);
+int hp_pose_submit_ppn_frames_u8_device(hp_engine* e, hp_ppn* parser, const hp_frame_u8* frames, int N, int keep_ratio, int* ticket);
 /* test hook: the first N resized network-size frames [N,in_h,in_w,3] of an in-flight or collected ticket */
 int hp_pose_debug_read_slot_frames(hp_engine* e, int ticket, uint8_t* out, int N);
 int hp_pifpaf_pipeline_info(hp_pifpaf* p, void** stream, void** inputs_free_event, int* hcap);
@@ -321,6 +333,13 @@ int hp_paf_prepare(hp_paf* p, int N, int c_conf, int c_paf, int H, int W);
 int hp_paf_state(const hp_paf* p, float* thresholds2, int* ints6);
 int hp_paf_copy_results_host_async(hp_paf* p, hp_human* pin_humans, int* pin_counts_flags, int N, void* stream);
 int hp_paf_grow_capacity(hp_paf* p, int flags);
+/* the same for the Pose Proposal Network parser: prepare checks the geometry and allocates for N frames; state gives the point / limb /
+ * NMS thresholds and {net_w, net_h, hcap, use_spill, prepared N, device}; the D2H writes counts_flags[2N] ([N counts | N flags]) and
+ * humans[N * hcap]; grow takes the flags OR-ed over the batch and its largest per-frame count (HP_ERR_CAPACITY: nothing left to grow) */
+int hp_ppn_prepare(hp_ppn* p, int N, int K, int gh, int gw, int E, int nh, int nw);
+int hp_ppn_state(const hp_ppn* p, float* thresholds3, int* ints6);
+int hp_ppn_copy_results_host_async(hp_ppn* p, hp_human* pin_humans, int* pin_counts_flags, int N, void* stream);
+int hp_ppn_grow_capacity(hp_ppn* p, int flags, int max_count);
 
 /* ------------------------------------------------------------------------------------------
  * Multi-GPU (SURVEY 8e): frames are independent, so they shard across the GPUs of one box with no data-path collective.
