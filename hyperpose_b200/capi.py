@@ -216,12 +216,34 @@ EXPORTS += [
     "hp_engine_calibrate_u8", "hp_pack_int8_calibrated",
     "hp_pose_submit_frames_u8_host", "hp_pose_submit_frames_u8_device", "hp_pose_submit_pifpaf_frames_u8_host",
     "hp_pose_submit_pifpaf_frames_u8_device", "hp_pose_debug_read_slot_frames",
+    "hp_pose_submit_frames_yuv420_host", "hp_pose_submit_frames_yuv420_device", "hp_pose_submit_pifpaf_frames_yuv420_host",
+    "hp_pose_submit_pifpaf_frames_yuv420_device", "hp_pose_submit_ppn_frames_yuv420_host", "hp_pose_submit_ppn_frames_yuv420_device",
 ]
 
 
 class FrameU8(C.Structure):
     """hp_frame_u8: one HWC BGR frame of any size, rows packed"""
     _fields_ = [("data", C.c_void_p), ("height", C.c_int32), ("width", C.c_int32)]
+
+
+class FrameYUV420(C.Structure):
+    """hp_frame_yuv420: one YUV 4:2:0 frame (BT.601 limited range) of any even size, planes pitched.  uv_step 2: semi-planar
+    (NV12: v = u + 1, NV21: u = v + 1); 1: planar (I420, YV12)"""
+    _fields_ = [("y", C.c_void_p), ("u", C.c_void_p), ("v", C.c_void_p), ("height", C.c_int32), ("width", C.c_int32),
+                ("pitch_y", C.c_int32), ("pitch_uv", C.c_int32), ("uv_step", C.c_int32)]
+
+
+# cv2's packed (3H/2, W) layouts: byte offsets of the U and V planes after the H x W luma plane, chroma pitch, chroma step
+YUV420_LAYOUTS = {"nv12": lambda H, W: (H * W, H * W + 1, W, 2), "nv21": lambda H, W: (H * W + 1, H * W, W, 2),
+                  "i420": lambda H, W: (H * W, H * W + H * W // 4, W // 2, 1), "yv12": lambda H, W: (H * W + H * W // 4, H * W, W // 2, 1)}
+
+
+def yuv420_record(frame: np.ndarray, layout: str) -> FrameYUV420:
+    """the FrameYUV420 of a host frame in cv2's packed layout: uint8 (3H/2, W), C-contiguous"""
+    H, W = frame.shape[0] * 2 // 3, frame.shape[1]
+    u, v, pitch_uv, step = YUV420_LAYOUTS[layout](H, W)
+    p = frame.ctypes.data
+    return FrameYUV420(p, p + u, p + v, H, W, W, pitch_uv, step)
 
 
 def _bind_engine(L):
@@ -269,6 +291,9 @@ def _bind_engine(L):
     for f in (L.hp_pose_submit_frames_u8_host, L.hp_pose_submit_frames_u8_device, L.hp_pose_submit_pifpaf_frames_u8_host,
               L.hp_pose_submit_pifpaf_frames_u8_device, L.hp_pose_submit_ppn_frames_u8_host, L.hp_pose_submit_ppn_frames_u8_device):
         f.argtypes = [vp, vp, C.POINTER(FrameU8), C.c_int, C.c_int, ip]
+    for f in (L.hp_pose_submit_frames_yuv420_host, L.hp_pose_submit_frames_yuv420_device, L.hp_pose_submit_pifpaf_frames_yuv420_host,
+              L.hp_pose_submit_pifpaf_frames_yuv420_device, L.hp_pose_submit_ppn_frames_yuv420_host, L.hp_pose_submit_ppn_frames_yuv420_device):
+        f.argtypes = [vp, vp, C.POINTER(FrameYUV420), C.c_int, C.c_int, ip]
     L.hp_pose_submit_ppn_u8_host.argtypes = [vp, vp, vp, C.c_int, ip]
     L.hp_pose_submit_ppn_u8_device.argtypes = [vp, vp, vp, C.c_int, ip]
     L.hp_pose_debug_read_slot_frames.argtypes = [vp, C.c_int, vp, C.c_int]
@@ -524,15 +549,11 @@ class Engine:
         self._ticket_n[t.value] = n
         return t.value
 
-    def _submit_frame_table(self, parser, table, keep_ratio, device: bool) -> int:
+    def _submit_frame_table(self, parser, table, keep_ratio, device: bool, fmt: str = "u8") -> int:
+        """hp_pose_submit{,_pifpaf,_ppn}_frames_{fmt}_{host,device}, chosen by the parser's type"""
         t = C.c_int(-1)
-        L = lib()
-        if isinstance(parser, PifPafParser):
-            fn = L.hp_pose_submit_pifpaf_frames_u8_device if device else L.hp_pose_submit_pifpaf_frames_u8_host
-        elif isinstance(parser, PoseProposalParser):
-            fn = L.hp_pose_submit_ppn_frames_u8_device if device else L.hp_pose_submit_ppn_frames_u8_host
-        else:
-            fn = L.hp_pose_submit_frames_u8_device if device else L.hp_pose_submit_frames_u8_host
+        head = "_pifpaf" if isinstance(parser, PifPafParser) else "_ppn" if isinstance(parser, PoseProposalParser) else ""
+        fn = getattr(lib(), f"hp_pose_submit{head}_frames_{fmt}_{'device' if device else 'host'}")
         check(fn(self._h, parser._h, table, len(table), 1 if keep_ratio else 0, C.byref(t)))
         self._ticket_n = getattr(self, "_ticket_n", {})
         self._ticket_n[t.value] = len(table)
@@ -559,6 +580,34 @@ class Engine:
         place: they must stay valid and unchanged until the ticket is collected."""
         table = (FrameU8 * len(frames))(*[FrameU8(int(p), int(h), int(w)) for p, h, w in frames])
         return self._submit_frame_table(parser, table, keep_ratio, device=True)
+
+    def submit_pose_yuv420(self, parser, frames, layout, keep_ratio: bool = False) -> int:
+        """hp_pose_submit{,_pifpaf,_ppn}_frames_yuv420_host, by the parser's type: a list of YUV 4:2:0 frames, each uint8 (3H/2, W) in
+        cv2's packed layout for `layout` (nv12, nv21, i420 or yv12; or a list of those, one per frame), converted as cv::cvtColor does
+        and resized on the GPU as submit_pose_frames resizes BGR frames; returns the ticket for collect_pose.  Page-locked frames are
+        kept referenced until the ticket is collected."""
+        layouts = [layout] * len(frames) if isinstance(layout, str) else list(layout)
+        if len(layouts) != len(frames) or any(lay not in YUV420_LAYOUTS for lay in layouts):
+            raise HyperposeError(HP_ERR_ARG, f"layout {layout!r}: expected one of {sorted(YUV420_LAYOUTS)}, or one per frame")
+        for i, f in enumerate(frames):
+            if not isinstance(f, np.ndarray) or f.dtype != np.uint8 or f.ndim != 2 or f.shape[0] % 3 or f.shape[0] == 0:
+                raise HyperposeError(HP_ERR_ARG, f"frame {i}: expected a uint8 (3H/2, W) YUV 4:2:0 array, got "
+                                                 f"{getattr(f, 'dtype', type(f).__name__)} {getattr(f, 'shape', '')}")
+        frames = [np.ascontiguousarray(f) for f in frames]
+        table = (FrameYUV420 * len(frames))(*[yuv420_record(f, lay) for f, lay in zip(frames, layouts)])
+        t = self._submit_frame_table(parser, table, keep_ratio, device=False, fmt="yuv420")
+        self._ticket_frames = getattr(self, "_ticket_frames", {})
+        self._ticket_frames[t] = frames
+        return t
+
+    def submit_pose_yuv420_device(self, parser, frames, keep_ratio: bool = False) -> int:
+        """the same for YUV 4:2:0 frames in device memory, given as FrameYUV420 records (device plane pointers and pitches, e.g. an
+        NVDEC surface).  The resize kernel reads them in place: they must stay valid and unchanged until the ticket is collected."""
+        for i, f in enumerate(frames):
+            if not isinstance(f, FrameYUV420):
+                raise HyperposeError(HP_ERR_ARG, f"frame {i}: expected a FrameYUV420, got {type(f).__name__}")
+        table = (FrameYUV420 * len(frames))(*frames)
+        return self._submit_frame_table(parser, table, keep_ratio, device=True, fmt="yuv420")
 
     def debug_read_slot_frames(self, ticket: int, n: int) -> np.ndarray:
         """the first n resized network-size frames u8[n,in_h,in_w,3] of a ticket in flight or collected"""

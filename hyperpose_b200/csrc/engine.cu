@@ -105,16 +105,59 @@ __device__ __forceinline__ int rz_coef(int d, double scale, int src, bool clamp,
     return s;
 }
 
+// One YUV 4:2:0 frame of a resize launch (NV12 / NV21 / I420 / YV12): luma and chroma planes, pitched, each chroma sample covering its
+// 2x2 luma block; converted to BGR per source pixel as cv::cvtColor does, then resized exactly as a FrameDesc frame of the luma size.
+struct YuvFrameDesc {
+    const uint8_t *y, *u, *v;
+    int sh, sw;                    // luma size (both even)
+    int rh, rw;                    // resized region
+    int mode;                      // RZ_*
+    int pitch_y, pitch_uv;         // bytes from one row to the next
+    int uv_step;                   // bytes from one chroma sample to the next: 2 semi-planar, 1 planar
+    int pad[2];
+};
+static_assert(sizeof(YuvFrameDesc) == 64, "YuvFrameDesc is uploaded as raw bytes");
+
+// Source fetches of the resize: byte c (B, G, R) of source pixel x of one source row.
+struct BgrRow {
+    const uint8_t* p;
+    __device__ __forceinline__ int px(int x, int c) const { return p[3 * x + c]; }
+    __device__ __forceinline__ int byte(int b) const { return p[b]; }
+};
+__device__ __forceinline__ BgrRow src_row(const FrameDesc& d, int sy) { return BgrRow{ d.src + (size_t)sy * d.sw * 3 }; }
+
+// OpenCV's YUV420sp2RGB / YUV420p2RGB fixed point (color_yuv.simd.hpp: ITUR_BT_601_CY .. _CVR, ITUR_BT_601_SHIFT = 20), BT.601
+// limited range.  Every sum stays below 2^30 in magnitude.
+struct YuvRow {
+    const uint8_t *y, *u, *v;
+    int step;
+    __device__ __forceinline__ int px(int x, int c) const
+    {
+        const int yy = max(y[x] - 16, 0) * 1220542 + (1 << 19);
+        const int k = (x >> 1) * step;
+        const int cu = u[k] - 128, cv = v[k] - 128;
+        const int s = c == 0 ? yy + 2116026 * cu : (c == 1 ? yy - 852492 * cv - 409993 * cu : yy + 1673527 * cv);
+        return min(max(s >> 20, 0), 255);
+    }
+    __device__ __forceinline__ int byte(int b) const { const int x = b / 3; return px(x, b - 3 * x); }
+};
+__device__ __forceinline__ YuvRow src_row(const YuvFrameDesc& d, int sy)
+{
+    const size_t c = (size_t)(sy >> 1) * d.pitch_uv;
+    return YuvRow{ d.y + (size_t)sy * d.pitch_y, d.u + c, d.v + c, d.uv_step };
+}
+
 // cv::resize(INTER_LINEAR) on CV_8UC3 frames (src/tensorrt.cpp:451) for the N frames of a batch in one launch, each frame read
-// through its own FrameDesc (blockIdx.y), RZ_ROWS destination rows per CTA (blockIdx.x).  OpenCV's 11-bit fixed-point bilinear:
+// through its own descriptor (blockIdx.y), RZ_ROWS destination rows per CTA (blockIdx.x).  OpenCV's 11-bit fixed-point bilinear:
 //   rows: S = src[sx]*a0 + src[sx+1]*a1; out = (((b0*(S0>>4))>>16) + ((b1*(S1>>4))>>16) + 2) >> 2
 // An exact 2x reduction is INTER_AREA in OpenCV: (a+b+c+d+2)>>2; a frame of the network size is copied.  Pixels outside the resized
 // region (letterbox, non_scaling_resize src/data.cpp:53-69) are 0.  One thread per destination BYTE, so a warp stores 32
 // consecutive bytes of the interleaved rows whatever the row or frame alignment.  Dynamic shared memory: 8 * dw bytes.
-__global__ void __launch_bounds__(256) resize_frames_u8c3_kernel(const FrameDesc* __restrict__ desc, uint8_t* __restrict__ dst, int dh, int dw)
+// Desc's src_row gives the fetch of source bytes: packed BGR rows, or YUV 4:2:0 planes converted per source pixel.
+template <class Desc>
+__device__ __forceinline__ void resize_frames(const Desc& d, uint8_t* __restrict__ dst, int dh, int dw)
 {
     extern __shared__ int2 rz_xtab[];   // per destination column: source column, a0 | a1 << 16
-    const FrameDesc d = desc[blockIdx.y];
     uint8_t* out = dst + (size_t)blockIdx.y * dh * dw * 3;
     const int y_begin = blockIdx.x * RZ_ROWS, row_bytes = dw * 3;
     if (d.mode == RZ_LINEAR) {
@@ -127,7 +170,6 @@ __global__ void __launch_bounds__(256) resize_frames_u8c3_kernel(const FrameDesc
         __syncthreads();
     }
     const double yscale = d.mode == RZ_LINEAR ? __ddiv_rn(1.0, __ddiv_rn((double)d.rh, (double)d.sh)) : 0.0;
-    const size_t src_row = (size_t)d.sw * 3;
     for (int y = y_begin; y < y_begin + RZ_ROWS && y < dh; ++y) {
         uint8_t* o = out + (size_t)y * row_bytes;
         if (y >= d.rh) {
@@ -135,40 +177,51 @@ __global__ void __launch_bounds__(256) resize_frames_u8c3_kernel(const FrameDesc
             continue;
         }
         if (d.mode == RZ_COPY) {
-            const uint8_t* r = d.src + y * src_row;
-            for (int b = threadIdx.x; b < row_bytes; b += blockDim.x) o[b] = r[b];
+            const auto r = src_row(d, y);
+            for (int b = threadIdx.x; b < row_bytes; b += blockDim.x) o[b] = (uint8_t)r.byte(b);
         } else if (d.mode == RZ_AREA2X) {
-            const uint8_t* r0 = d.src + (size_t)(2 * y) * src_row;
-            const uint8_t* r1 = r0 + src_row;
+            const auto r0 = src_row(d, 2 * y), r1 = src_row(d, 2 * y + 1);
             for (int b = threadIdx.x; b < row_bytes; b += blockDim.x) {
                 const int x = b / 3, c = b - 3 * x;
                 uint8_t v = 0;
-                if (x < d.rw) {
-                    const int i = 6 * x + c;
-                    v = (uint8_t)((r0[i] + r0[i + 3] + r1[i] + r1[i + 3] + 2) >> 2);
-                }
+                if (x < d.rw) v = (uint8_t)((r0.px(2 * x, c) + r0.px(2 * x + 1, c) + r1.px(2 * x, c) + r1.px(2 * x + 1, c) + 2) >> 2);
                 o[b] = v;
             }
         } else {
             int b0, b1;
             const int sy = rz_coef(y, yscale, d.sh, false, b0, b1);
-            const uint8_t* r0 = d.src + (size_t)min(max(sy, 0), d.sh - 1) * src_row;
-            const uint8_t* r1 = d.src + (size_t)min(max(sy + 1, 0), d.sh - 1) * src_row;
+            const auto r0 = src_row(d, min(max(sy, 0), d.sh - 1));
+            const auto r1 = src_row(d, min(max(sy + 1, 0), d.sh - 1));
             for (int b = threadIdx.x; b < row_bytes; b += blockDim.x) {
                 const int x = b / 3, c = b - 3 * x;
                 int v = 0;
                 if (x < d.rw) {
                     const int2 t = rz_xtab[x];
-                    const int i0 = t.x * 3 + c, i1 = min(t.x + 1, d.sw - 1) * 3 + c;
+                    const int x0 = t.x, x1 = min(t.x + 1, d.sw - 1);
                     const int a0 = t.y & 0xffff, a1 = t.y >> 16;
-                    const int S0 = r0[i0] * a0 + r0[i1] * a1;
-                    const int S1 = r1[i0] * a0 + r1[i1] * a1;
+                    const int S0 = r0.px(x0, c) * a0 + r0.px(x1, c) * a1;
+                    const int S1 = r1.px(x0, c) * a0 + r1.px(x1, c) * a1;
                     v = min(max((((b0 * (S0 >> 4)) >> 16) + ((b1 * (S1 >> 4)) >> 16) + 2) >> 2, 0), 255);
                 }
                 o[b] = (uint8_t)v;
             }
         }
     }
+}
+
+// packed BGR frames (hp_frame_u8)
+__global__ void __launch_bounds__(256) resize_frames_u8c3_kernel(const FrameDesc* __restrict__ desc, uint8_t* __restrict__ dst, int dh, int dw)
+{
+    const FrameDesc d = desc[blockIdx.y];
+    resize_frames(d, dst, dh, dw);
+}
+
+// YUV 4:2:0 frames (hp_frame_yuv420): the conversion is fused into the fetch, so nothing is ever interpolated in YUV.  Two rows of
+// three plane pointers need more than the 32 registers of 8 CTAs per SM: 6 CTAs leave it 40, with no spills.
+__global__ void __launch_bounds__(256, 6) resize_frames_yuv420_kernel(const YuvFrameDesc* __restrict__ desc, uint8_t* __restrict__ dst, int dh, int dw)
+{
+    const YuvFrameDesc d = desc[blockIdx.y];
+    resize_frames(d, dst, dh, dw);
 }
 
 // depthwise KxK conv (K in {1,3}) + bias + PReLU on fp16 NHWC, 8 channels per thread (one 16-byte load per tap),
@@ -845,6 +898,7 @@ struct hp_engine {
         uint8_t* d_src = nullptr; size_t d_src_bytes = 0;
         uint8_t* pin_src = nullptr; size_t pin_src_bytes = 0;
         FrameDesc* d_desc = nullptr; FrameDesc* pin_desc = nullptr;   // [max_batch]
+        YuvFrameDesc* d_ydesc = nullptr; YuvFrameDesc* pin_ydesc = nullptr;   // [max_batch] (hp_pose_submit_*frames_yuv420_*)
         hp_human* pin_humans = nullptr; size_t pin_humans_n = 0;
         int* pin_counts = nullptr; size_t pin_counts_n = 0;   // [N counts | N flags]
         cudaEvent_t h2d_done = nullptr, done = nullptr;
@@ -1479,6 +1533,8 @@ void free_engine(hp_engine* e)
         if (sl.pin_src) cudaFreeHost(sl.pin_src);
         if (sl.d_desc) cudaFree(sl.d_desc);
         if (sl.pin_desc) cudaFreeHost(sl.pin_desc);
+        if (sl.d_ydesc) cudaFree(sl.d_ydesc);
+        if (sl.pin_ydesc) cudaFreeHost(sl.pin_ydesc);
         if (sl.pin_humans) cudaFreeHost(sl.pin_humans);
         if (sl.pin_counts) cudaFreeHost(sl.pin_counts);
         if (sl.h2d_done) cudaEventDestroy(sl.h2d_done);
@@ -1970,6 +2026,15 @@ static int launch_resize(hp_engine* e, const FrameDesc* d_desc, uint8_t* dst, in
 {
     const dim3 grid((e->in_h + RZ_ROWS - 1) / RZ_ROWS, N);
     resize_frames_u8c3_kernel<<<grid, 256, (size_t)e->in_w * sizeof(int2), e->stream>>>(d_desc, dst, e->in_h, e->in_w);
+    e->launches++;
+    HP_CUDA_TRY(cudaGetLastError());
+    return HP_OK;
+}
+
+static int launch_resize_yuv(hp_engine* e, const YuvFrameDesc* d_desc, uint8_t* dst, int N)
+{
+    const dim3 grid((e->in_h + RZ_ROWS - 1) / RZ_ROWS, N);
+    resize_frames_yuv420_kernel<<<grid, 256, (size_t)e->in_w * sizeof(int2), e->stream>>>(d_desc, dst, e->in_h, e->in_w);
     e->launches++;
     HP_CUDA_TRY(cudaGetLastError());
     return HP_OK;
@@ -2517,6 +2582,80 @@ int slot_upload_frames(hp_engine* e, hp_engine::PoseSlot& sl, FrameDesc* descs, 
     return launch_resize(e, sl.d_desc, sl.d_frames, N);
 }
 
+// The same for YUV 4:2:0 frames.  A host frame is copied row-compacted into the slot's source buffer: its luma plane with pitch
+// width, then the interleaved UV plane (semi-planar, copied once) or the U and V planes (planar), 1.5 bytes per pixel.  Each plane goes
+// by a pitched DMA from the caller when it is page-locked, else through the slot's pinned staging.  Device frames are read in place.
+int slot_upload_yuv(hp_engine* e, hp_engine::PoseSlot& sl, YuvFrameDesc* descs, int N, bool device_src)
+{
+    if (!sl.d_ydesc) {
+        HP_CUDA_TRY(cudaMalloc(&sl.d_ydesc, e->max_batch * sizeof(YuvFrameDesc)));
+        HP_CUDA_TRY(cudaMallocHost(&sl.pin_ydesc, e->max_batch * sizeof(YuvFrameDesc)));
+    }
+    if (!device_src) {
+        std::vector<size_t> off(N + 1, 0);
+        for (int f = 0; f < N; ++f) off[f + 1] = off[f] + (((size_t)descs[f].sh * descs[f].sw * 3 / 2 + 255) & ~(size_t)255);
+        if (sl.d_src_bytes < off[N]) {
+            if (sl.d_src) cudaFree(sl.d_src);
+            sl.d_src = nullptr; sl.d_src_bytes = 0;
+            HP_CUDA_TRY(cudaMalloc(&sl.d_src, off[N]));
+            sl.d_src_bytes = off[N];
+        }
+        // one plane: rows x width bytes at `src` with pitch `pitch` into the compacted region at byte offset `at`
+        auto copy_plane = [&](const uint8_t* src, int pitch, int rows, int width, size_t at) -> int {
+            cudaPointerAttributes attr;
+            const bool pinned = cudaPointerGetAttributes(&attr, src) == cudaSuccess && attr.type == cudaMemoryTypeHost;
+            if (pinned) {
+                HP_CUDA_TRY(cudaMemcpy2DAsync(sl.d_src + at, width, src, pitch, width, rows, cudaMemcpyHostToDevice, e->copy_stream));
+                return HP_OK;
+            }
+            cudaGetLastError();
+            if (sl.pin_src_bytes < off[N]) {
+                if (sl.pin_src) cudaFreeHost(sl.pin_src);
+                sl.pin_src = nullptr; sl.pin_src_bytes = 0;
+                HP_CUDA_TRY(cudaMallocHost(&sl.pin_src, off[N]));
+                sl.pin_src_bytes = off[N];
+            }
+            for (int r = 0; r < rows; ++r) memcpy(sl.pin_src + at + (size_t)r * width, src + (size_t)r * pitch, width);
+            HP_CUDA_TRY(cudaMemcpyAsync(sl.d_src + at, sl.pin_src + at, (size_t)rows * width, cudaMemcpyHostToDevice, e->copy_stream));
+            return HP_OK;
+        };
+        for (int f = 0; f < N; ++f) {
+            YuvFrameDesc& d = descs[f];
+            const size_t luma = (size_t)d.sh * d.sw, at = off[f] + luma;
+            int rc = copy_plane(d.y, d.pitch_y, d.sh, d.sw, off[f]);
+            if (rc) return rc;
+            if (d.uv_step == 2) {   // one interleaved plane starting at the lower of u, v
+                const uint8_t* base = d.u < d.v ? d.u : d.v;
+                if ((rc = copy_plane(base, d.pitch_uv, d.sh / 2, d.sw, at))) return rc;
+                d.u = sl.d_src + at + (d.u - base);
+                d.v = sl.d_src + at + (d.v - base);
+                d.pitch_uv = d.sw;
+            } else {
+                const size_t chroma = luma / 4;
+                if ((rc = copy_plane(d.u, d.pitch_uv, d.sh / 2, d.sw / 2, at))) return rc;
+                if ((rc = copy_plane(d.v, d.pitch_uv, d.sh / 2, d.sw / 2, at + chroma))) return rc;
+                d.u = sl.d_src + at;
+                d.v = sl.d_src + at + chroma;
+                d.pitch_uv = d.sw / 2;
+            }
+            d.y = sl.d_src + off[f];
+            d.pitch_y = d.sw;
+        }
+    }
+    memcpy(sl.pin_ydesc, descs, N * sizeof(YuvFrameDesc));
+    HP_CUDA_TRY(cudaMemcpyAsync(sl.d_ydesc, sl.pin_ydesc, N * sizeof(YuvFrameDesc), cudaMemcpyHostToDevice, e->copy_stream));
+    HP_CUDA_TRY(cudaEventRecord(sl.h2d_done, e->copy_stream));
+    HP_CUDA_TRY(cudaStreamWaitEvent(e->stream, sl.h2d_done, 0));
+    return launch_resize_yuv(e, sl.d_ydesc, sl.d_frames, N);
+}
+
+// a submitted batch into the slot's device buffer: network-size frames, or frames of any size (BGR descs or YUV ydescs) resized there
+int slot_upload_batch(hp_engine* e, hp_engine::PoseSlot& sl, const uint8_t* frames, FrameDesc* descs, YuvFrameDesc* ydescs, int N, bool device_src)
+{
+    if (ydescs) return slot_upload_yuv(e, sl, ydescs, N, device_src);
+    return descs ? slot_upload_frames(e, sl, descs, N, device_src) : slot_upload(e, sl, frames, N, device_src);
+}
+
 // the parser's state a captured graph bakes in (hp_paf_state / hp_ppn_state), and the capacity of records per frame in it
 void parser_state(const hp_paf* parser, const hp_ppn* ppn, float kf[3], int ki[6], int* hcap)
 {
@@ -2611,11 +2750,12 @@ static int pifpaf_enqueue(hp_engine* e, hp_engine::PoseSlot& sl)
     return HP_OK;
 }
 
-// frames: N network-size frames, or -- descs != NULL -- N frames of any size described by descs (their sources are rewritten to
-// the slot's copies of host frames)
-static int pose_submit_pifpaf(hp_engine* e, hp_pifpaf* dec, const uint8_t* frames, FrameDesc* descs, int N, int* ticket, bool device_src)
+// frames: N network-size frames, or -- descs / ydescs != NULL -- N BGR / YUV 4:2:0 frames of any size described by them (their
+// sources are rewritten to the slot's copies of host frames)
+static int pose_submit_pifpaf(hp_engine* e, hp_pifpaf* dec, const uint8_t* frames, FrameDesc* descs, YuvFrameDesc* ydescs, int N, int* ticket,
+                              bool device_src)
 {
-    if (!e || !dec || (!frames && !descs) || !ticket) { set_error("hp_pose_submit_pifpaf: null argument"); return HP_ERR_ARG; }
+    if (!e || !dec || (!frames && !descs && !ydescs) || !ticket) { set_error("hp_pose_submit_pifpaf: null argument"); return HP_ERR_ARG; }
     if (N <= 0 || N > e->max_batch) { set_error("Input batch size overflow: Yours@%d Max@%d", N, e->max_batch); return HP_ERR_BATCH; }
     if (e->hdr.head_type != 1) { set_error("hp_pose_submit_pifpaf: the model pack has no OpenPifPaf heads (head_type %u)", e->hdr.head_type); return HP_ERR_UNSUPPORTED; }
     HP_CUDA_TRY(cudaSetDevice(e->device));
@@ -2625,7 +2765,7 @@ static int pose_submit_pifpaf(hp_engine* e, hp_pifpaf* dec, const uint8_t* frame
     int rc = pifpaf_slot_prepare(e, sl, dec, N);
     if (rc) return rc;
     e->reserve_sms = e->opt.pifpaf_reserve_sms;   // the decoder's growth kernel (one warp per frame) runs underneath the next batch's convolutions
-    rc = descs ? slot_upload_frames(e, sl, descs, N, device_src) : slot_upload(e, sl, frames, N, device_src);
+    rc = slot_upload_batch(e, sl, frames, descs, ydescs, N, device_src);
     if (rc) return rc;
     rc = pifpaf_enqueue(e, sl);
     if (rc) return rc;
@@ -2636,10 +2776,11 @@ static int pose_submit_pifpaf(hp_engine* e, hp_pifpaf* dec, const uint8_t* frame
 }
 
 // the PAF-parser calls (ppn_call false: `parser` is an hp_paf) and the Pose Proposal Network calls (true: an hp_ppn)
-static int pose_submit(hp_engine* e, void* parser, bool ppn_call, const uint8_t* frames, FrameDesc* descs, int N, int* ticket, bool device_src)
+static int pose_submit(hp_engine* e, void* parser, bool ppn_call, const uint8_t* frames, FrameDesc* descs, YuvFrameDesc* ydescs, int N,
+                       int* ticket, bool device_src)
 {
     const char* fn = ppn_call ? "hp_pose_submit_ppn" : "hp_pose_submit";
-    if (!e || !parser || (!frames && !descs) || !ticket) { set_error("%s: null argument", fn); return HP_ERR_ARG; }
+    if (!e || !parser || (!frames && !descs && !ydescs) || !ticket) { set_error("%s: null argument", fn); return HP_ERR_ARG; }
     if (N <= 0 || N > e->max_batch) { set_error("Input batch size overflow: Yours@%d Max@%d", N, e->max_batch); return HP_ERR_BATCH; }
     hp_paf* paf = ppn_call ? nullptr : (hp_paf*)parser;
     hp_ppn* ppn = ppn_call ? (hp_ppn*)parser : nullptr;
@@ -2664,8 +2805,7 @@ static int pose_submit(hp_engine* e, void* parser, bool ppn_call, const uint8_t*
     if (sl.busy) { set_error("%s: two batches are already in flight -- collect ticket %d first", fn, idx); return HP_ERR_ARG; }
     int rc = pose_slot_prepare(e, sl, paf, ppn, N);
     if (rc) return rc;
-    rc = descs ? slot_upload_frames(e, sl, descs, N, device_src)   // (the captured graph reads the slot's buffer)
-               : slot_upload(e, sl, frames, N, device_src);
+    rc = slot_upload_batch(e, sl, frames, descs, ydescs, N, device_src);   // (the captured graph reads the slot's buffer)
     if (rc) return rc;
     rc = pose_launch(e, sl);
     if (rc) return rc;
@@ -2678,23 +2818,23 @@ static int pose_submit(hp_engine* e, void* parser, bool ppn_call, const uint8_t*
 
 int hp_pose_submit_u8_host(hp_engine* e, hp_paf* parser, const uint8_t* frames, int N, int* ticket)
 {
-    return pose_submit(e, parser, false, frames, nullptr, N, ticket, false);
+    return pose_submit(e, parser, false, frames, nullptr, nullptr, N, ticket, false);
 }
 
 // the same with the frames already resident in device memory (what a decoder / capture pipeline on the GPU hands over)
 int hp_pose_submit_u8_device(hp_engine* e, hp_paf* parser, const uint8_t* d_frames, int N, int* ticket)
 {
-    return pose_submit(e, parser, false, d_frames, nullptr, N, ticket, true);
+    return pose_submit(e, parser, false, d_frames, nullptr, nullptr, N, ticket, true);
 }
 
 int hp_pose_submit_pifpaf_u8_host(hp_engine* e, hp_pifpaf* decoder, const uint8_t* frames, int N, int* ticket)
 {
-    return pose_submit_pifpaf(e, decoder, frames, nullptr, N, ticket, false);
+    return pose_submit_pifpaf(e, decoder, frames, nullptr, nullptr, N, ticket, false);
 }
 
 int hp_pose_submit_pifpaf_u8_device(hp_engine* e, hp_pifpaf* decoder, const uint8_t* d_frames, int N, int* ticket)
 {
-    return pose_submit_pifpaf(e, decoder, d_frames, nullptr, N, ticket, true);
+    return pose_submit_pifpaf(e, decoder, d_frames, nullptr, nullptr, N, ticket, true);
 }
 
 // the resize descriptors of a frame list, refused before any work is enqueued
@@ -2718,53 +2858,122 @@ int hp_pose_submit_frames_u8_host(hp_engine* e, hp_paf* parser, const hp_frame_u
 {
     std::vector<FrameDesc> d;
     const int rc = frame_descs(e, frames, N, keep_ratio, d);
-    return rc ? rc : pose_submit(e, parser, false, nullptr, d.data(), N, ticket, false);
+    return rc ? rc : pose_submit(e, parser, false, nullptr, d.data(), nullptr, N, ticket, false);
 }
 
 int hp_pose_submit_frames_u8_device(hp_engine* e, hp_paf* parser, const hp_frame_u8* frames, int N, int keep_ratio, int* ticket)
 {
     std::vector<FrameDesc> d;
     const int rc = frame_descs(e, frames, N, keep_ratio, d);
-    return rc ? rc : pose_submit(e, parser, false, nullptr, d.data(), N, ticket, true);
+    return rc ? rc : pose_submit(e, parser, false, nullptr, d.data(), nullptr, N, ticket, true);
 }
 
 int hp_pose_submit_pifpaf_frames_u8_host(hp_engine* e, hp_pifpaf* decoder, const hp_frame_u8* frames, int N, int keep_ratio, int* ticket)
 {
     std::vector<FrameDesc> d;
     const int rc = frame_descs(e, frames, N, keep_ratio, d);
-    return rc ? rc : pose_submit_pifpaf(e, decoder, nullptr, d.data(), N, ticket, false);
+    return rc ? rc : pose_submit_pifpaf(e, decoder, nullptr, d.data(), nullptr, N, ticket, false);
 }
 
 int hp_pose_submit_pifpaf_frames_u8_device(hp_engine* e, hp_pifpaf* decoder, const hp_frame_u8* frames, int N, int keep_ratio, int* ticket)
 {
     std::vector<FrameDesc> d;
     const int rc = frame_descs(e, frames, N, keep_ratio, d);
-    return rc ? rc : pose_submit_pifpaf(e, decoder, nullptr, d.data(), N, ticket, true);
+    return rc ? rc : pose_submit_pifpaf(e, decoder, nullptr, d.data(), nullptr, N, ticket, true);
 }
 
 // ---- Pose Proposal Network packs: network, parse and record D2H in one captured graph on the engine stream, as for the PAF parser ----
 int hp_pose_submit_ppn_u8_host(hp_engine* e, hp_ppn* parser, const uint8_t* frames, int N, int* ticket)
 {
-    return pose_submit(e, parser, true, frames, nullptr, N, ticket, false);
+    return pose_submit(e, parser, true, frames, nullptr, nullptr, N, ticket, false);
 }
 
 int hp_pose_submit_ppn_u8_device(hp_engine* e, hp_ppn* parser, const uint8_t* d_frames, int N, int* ticket)
 {
-    return pose_submit(e, parser, true, d_frames, nullptr, N, ticket, true);
+    return pose_submit(e, parser, true, d_frames, nullptr, nullptr, N, ticket, true);
 }
 
 int hp_pose_submit_ppn_frames_u8_host(hp_engine* e, hp_ppn* parser, const hp_frame_u8* frames, int N, int keep_ratio, int* ticket)
 {
     std::vector<FrameDesc> d;
     const int rc = frame_descs(e, frames, N, keep_ratio, d);
-    return rc ? rc : pose_submit(e, parser, true, nullptr, d.data(), N, ticket, false);
+    return rc ? rc : pose_submit(e, parser, true, nullptr, d.data(), nullptr, N, ticket, false);
 }
 
 int hp_pose_submit_ppn_frames_u8_device(hp_engine* e, hp_ppn* parser, const hp_frame_u8* frames, int N, int keep_ratio, int* ticket)
 {
     std::vector<FrameDesc> d;
     const int rc = frame_descs(e, frames, N, keep_ratio, d);
-    return rc ? rc : pose_submit(e, parser, true, nullptr, d.data(), N, ticket, true);
+    return rc ? rc : pose_submit(e, parser, true, nullptr, d.data(), nullptr, N, ticket, true);
+}
+
+// the resize descriptors of a YUV 4:2:0 frame list, refused before any work is enqueued; the regime comes from the luma size
+static int yuv_frame_descs(const hp_engine* e, const hp_frame_yuv420* frames, int N, int keep_ratio, std::vector<YuvFrameDesc>& descs)
+{
+    if (!e || !frames) { set_error("hp_pose_submit_frames_yuv420: null argument"); return HP_ERR_ARG; }
+    if (N <= 0 || N > e->max_batch) { set_error("Input batch size overflow: Yours@%d Max@%d", N, e->max_batch); return HP_ERR_BATCH; }
+    descs.resize(N);
+    for (int f = 0; f < N; ++f) {
+        const hp_frame_yuv420& fr = frames[f];
+        const char* bad = nullptr;
+        if (!fr.y || !fr.u || !fr.v) bad = "has a null plane";
+        else if (fr.height <= 0 || fr.width <= 0 || (fr.height & 1) || (fr.width & 1)) bad = "has a size that is not positive and even";
+        else if (fr.uv_step != 1 && fr.uv_step != 2) bad = "has a uv_step other than 1 (planar) or 2 (semi-planar)";
+        else if (fr.pitch_y < fr.width || fr.pitch_uv < fr.width / 2 * fr.uv_step) bad = "has a pitch shorter than its row";
+        else if (fr.uv_step == 2 && fr.u - fr.v != 1 && fr.v - fr.u != 1) bad = "is semi-planar but its u and v are not one byte apart";
+        if (bad) {
+            set_error("hp_pose_submit_frames_yuv420: frame %d %s (%dx%d, pitches %d / %d, uv_step %d)", f, bad, fr.height, fr.width,
+                      fr.pitch_y, fr.pitch_uv, fr.uv_step);
+            return HP_ERR_ARG;
+        }
+        FrameDesc d;
+        const int rc = frame_desc(e, nullptr, fr.height, fr.width, keep_ratio, d);
+        if (rc) return rc;
+        descs[f] = YuvFrameDesc{ fr.y, fr.u, fr.v, fr.height, fr.width, d.rh, d.rw, d.mode, fr.pitch_y, fr.pitch_uv, fr.uv_step, { 0, 0 } };
+    }
+    return HP_OK;
+}
+
+int hp_pose_submit_frames_yuv420_host(hp_engine* e, hp_paf* parser, const hp_frame_yuv420* frames, int N, int keep_ratio, int* ticket)
+{
+    std::vector<YuvFrameDesc> d;
+    const int rc = yuv_frame_descs(e, frames, N, keep_ratio, d);
+    return rc ? rc : pose_submit(e, parser, false, nullptr, nullptr, d.data(), N, ticket, false);
+}
+
+int hp_pose_submit_frames_yuv420_device(hp_engine* e, hp_paf* parser, const hp_frame_yuv420* frames, int N, int keep_ratio, int* ticket)
+{
+    std::vector<YuvFrameDesc> d;
+    const int rc = yuv_frame_descs(e, frames, N, keep_ratio, d);
+    return rc ? rc : pose_submit(e, parser, false, nullptr, nullptr, d.data(), N, ticket, true);
+}
+
+int hp_pose_submit_pifpaf_frames_yuv420_host(hp_engine* e, hp_pifpaf* decoder, const hp_frame_yuv420* frames, int N, int keep_ratio, int* ticket)
+{
+    std::vector<YuvFrameDesc> d;
+    const int rc = yuv_frame_descs(e, frames, N, keep_ratio, d);
+    return rc ? rc : pose_submit_pifpaf(e, decoder, nullptr, nullptr, d.data(), N, ticket, false);
+}
+
+int hp_pose_submit_pifpaf_frames_yuv420_device(hp_engine* e, hp_pifpaf* decoder, const hp_frame_yuv420* frames, int N, int keep_ratio, int* ticket)
+{
+    std::vector<YuvFrameDesc> d;
+    const int rc = yuv_frame_descs(e, frames, N, keep_ratio, d);
+    return rc ? rc : pose_submit_pifpaf(e, decoder, nullptr, nullptr, d.data(), N, ticket, true);
+}
+
+int hp_pose_submit_ppn_frames_yuv420_host(hp_engine* e, hp_ppn* parser, const hp_frame_yuv420* frames, int N, int keep_ratio, int* ticket)
+{
+    std::vector<YuvFrameDesc> d;
+    const int rc = yuv_frame_descs(e, frames, N, keep_ratio, d);
+    return rc ? rc : pose_submit(e, parser, true, nullptr, nullptr, d.data(), N, ticket, false);
+}
+
+int hp_pose_submit_ppn_frames_yuv420_device(hp_engine* e, hp_ppn* parser, const hp_frame_yuv420* frames, int N, int keep_ratio, int* ticket)
+{
+    std::vector<YuvFrameDesc> d;
+    const int rc = yuv_frame_descs(e, frames, N, keep_ratio, d);
+    return rc ? rc : pose_submit(e, parser, true, nullptr, nullptr, d.data(), N, ticket, true);
 }
 
 // test hook: the first N resized network-size frames of ticket `ticket` (in flight or collected)

@@ -322,6 +322,28 @@ int hp_pose_submit_ppn_u8_host(hp_engine* e, hp_ppn* parser, const uint8_t* fram
 int hp_pose_submit_ppn_u8_device(hp_engine* e, hp_ppn* parser, const uint8_t* d_frames, int N, int* ticket);
 int hp_pose_submit_ppn_frames_u8_host(hp_engine* e, hp_ppn* parser, const hp_frame_u8* frames, int N, int keep_ratio, int* ticket);
 int hp_pose_submit_ppn_frames_u8_device(hp_engine* e, hp_ppn* parser, const hp_frame_u8* frames, int N, int keep_ratio, int* ticket);
+/* The same calls for YUV 4:2:0 video frames (NVDEC's NV12, libavcodec's I420, camera NV12 / NV21, YV12), for all three head types.
+ * Each source pixel is converted to BGR as cv::cvtColor(COLOR_YUV2BGR_NV12 / _NV21 / _I420 / _YV12) does -- BT.601 limited range,
+ * OpenCV's 20-bit fixed point, each chroma sample covering its 2x2 luma block -- inside the batched resize's fetch, before any
+ * interpolation: the network-size frame is byte-identical to cv::resize(cv::cvtColor(src, code), ...) (or non_scaling_resize of it),
+ * the regime chosen from the luma size as for BGR frames.  No extra pass and no extra buffer.  The frames of a batch may mix layouts
+ * and sizes.  N > max_batch is HP_ERR_BATCH.  HP_ERR_ARG, before anything is enqueued: a null plane, a height or width <= 0 or odd,
+ * pitch_y < width, pitch_uv < (width / 2) * uv_step, uv_step not 1 or 2, semi-planar u and v not one byte apart.
+ * _host: each plane is copied row-compacted (1.5 bytes per pixel; a semi-planar UV plane once), by DMA from page-locked planes,
+ * through pinned staging from pageable ones.  _device: the planes are read in place with the given pitches (an NVDEC surface as it
+ * stands) and must stay valid and unchanged until the ticket is collected. */
+typedef struct hp_frame_yuv420 {
+    const uint8_t *y, *u, *v;
+    int32_t height, width;       /* luma size, both even */
+    int32_t pitch_y, pitch_uv;   /* bytes from one row to the next */
+    int32_t uv_step;             /* 2: semi-planar (NV12 v = u + 1, NV21 u = v + 1); 1: planar (I420, YV12) */
+} hp_frame_yuv420;
+int hp_pose_submit_frames_yuv420_host(hp_engine* e, hp_paf* parser, const hp_frame_yuv420* frames, int N, int keep_ratio, int* ticket);
+int hp_pose_submit_frames_yuv420_device(hp_engine* e, hp_paf* parser, const hp_frame_yuv420* frames, int N, int keep_ratio, int* ticket);
+int hp_pose_submit_pifpaf_frames_yuv420_host(hp_engine* e, hp_pifpaf* decoder, const hp_frame_yuv420* frames, int N, int keep_ratio, int* ticket);
+int hp_pose_submit_pifpaf_frames_yuv420_device(hp_engine* e, hp_pifpaf* decoder, const hp_frame_yuv420* frames, int N, int keep_ratio, int* ticket);
+int hp_pose_submit_ppn_frames_yuv420_host(hp_engine* e, hp_ppn* parser, const hp_frame_yuv420* frames, int N, int keep_ratio, int* ticket);
+int hp_pose_submit_ppn_frames_yuv420_device(hp_engine* e, hp_ppn* parser, const hp_frame_yuv420* frames, int N, int keep_ratio, int* ticket);
 /* test hook: the first N resized network-size frames [N,in_h,in_w,3] of an in-flight or collected ticket */
 int hp_pose_debug_read_slot_frames(hp_engine* e, int ticket, uint8_t* out, int N);
 int hp_pifpaf_pipeline_info(hp_pifpaf* p, void** stream, void** inputs_free_event, int* hcap);
