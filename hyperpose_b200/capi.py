@@ -218,6 +218,9 @@ EXPORTS += [
     "hp_pose_submit_pifpaf_frames_u8_device", "hp_pose_debug_read_slot_frames",
     "hp_pose_submit_frames_yuv420_host", "hp_pose_submit_frames_yuv420_device", "hp_pose_submit_pifpaf_frames_yuv420_host",
     "hp_pose_submit_pifpaf_frames_yuv420_device", "hp_pose_submit_ppn_frames_yuv420_host", "hp_pose_submit_ppn_frames_yuv420_device",
+    "hp_pose_submit_frames_interleaved_host", "hp_pose_submit_frames_interleaved_device", "hp_pose_submit_pifpaf_frames_interleaved_host",
+    "hp_pose_submit_pifpaf_frames_interleaved_device", "hp_pose_submit_ppn_frames_interleaved_host",
+    "hp_pose_submit_ppn_frames_interleaved_device",
 ]
 
 
@@ -244,6 +247,22 @@ def yuv420_record(frame: np.ndarray, layout: str) -> FrameYUV420:
     u, v, pitch_uv, step = YUV420_LAYOUTS[layout](H, W)
     p = frame.ctypes.data
     return FrameYUV420(p, p + u, p + v, H, W, W, pitch_uv, step)
+
+
+class FrameInterleaved(C.Structure):
+    """hp_frame_interleaved: one interleaved frame of any size (width even for 4:2:2), rows `pitch` bytes apart; `format` is a
+    PIXEL_FORMATS value"""
+    _fields_ = [("data", C.c_void_p), ("height", C.c_int32), ("width", C.c_int32), ("pitch", C.c_int32), ("format", C.c_int32)]
+
+
+# hp_pixel_format: the value and the trailing dimension of a uint8 frame array ((H, W) for gray)
+PIXEL_FORMATS = {"bgr": 0, "rgb": 1, "bgra": 2, "rgba": 3, "gray": 4, "yuyv": 5, "uyvy": 6, "yvyu": 7}
+PIXEL_CHANNELS = {"bgr": 3, "rgb": 3, "bgra": 4, "rgba": 4, "gray": None, "yuyv": 2, "uyvy": 2, "yvyu": 2}
+
+
+def interleaved_record(frame: np.ndarray, fmt: str) -> FrameInterleaved:
+    """the FrameInterleaved of a host frame: uint8 (H, W, C) or (H, W) for gray, each row's bytes contiguous; the pitch is strides[0]"""
+    return FrameInterleaved(frame.ctypes.data, frame.shape[0], frame.shape[1], frame.strides[0], PIXEL_FORMATS[fmt])
 
 
 def _bind_engine(L):
@@ -294,6 +313,10 @@ def _bind_engine(L):
     for f in (L.hp_pose_submit_frames_yuv420_host, L.hp_pose_submit_frames_yuv420_device, L.hp_pose_submit_pifpaf_frames_yuv420_host,
               L.hp_pose_submit_pifpaf_frames_yuv420_device, L.hp_pose_submit_ppn_frames_yuv420_host, L.hp_pose_submit_ppn_frames_yuv420_device):
         f.argtypes = [vp, vp, C.POINTER(FrameYUV420), C.c_int, C.c_int, ip]
+    for f in (L.hp_pose_submit_frames_interleaved_host, L.hp_pose_submit_frames_interleaved_device,
+              L.hp_pose_submit_pifpaf_frames_interleaved_host, L.hp_pose_submit_pifpaf_frames_interleaved_device,
+              L.hp_pose_submit_ppn_frames_interleaved_host, L.hp_pose_submit_ppn_frames_interleaved_device):
+        f.argtypes = [vp, vp, C.POINTER(FrameInterleaved), C.c_int, C.c_int, ip]
     L.hp_pose_submit_ppn_u8_host.argtypes = [vp, vp, vp, C.c_int, ip]
     L.hp_pose_submit_ppn_u8_device.argtypes = [vp, vp, vp, C.c_int, ip]
     L.hp_pose_debug_read_slot_frames.argtypes = [vp, C.c_int, vp, C.c_int]
@@ -608,6 +631,42 @@ class Engine:
                 raise HyperposeError(HP_ERR_ARG, f"frame {i}: expected a FrameYUV420, got {type(f).__name__}")
         table = (FrameYUV420 * len(frames))(*frames)
         return self._submit_frame_table(parser, table, keep_ratio, device=True, fmt="yuv420")
+
+    def submit_pose_interleaved(self, parser, frames, format, keep_ratio: bool = False) -> int:
+        """hp_pose_submit{,_pifpaf,_ppn}_frames_interleaved_host, by the parser's type: a list of uint8 frames, (H, W, 3) for bgr / rgb,
+        (H, W, 4) for bgra / rgba, (H, W) for gray, (H, W, 2) for yuyv / uyvy / yvyu; `format` is one of those names or a list of them,
+        one per frame.  Each frame is converted as cv::cvtColor(..., COLOR_<format>2BGR) does and resized on the GPU as
+        submit_pose_frames resizes BGR frames; returns the ticket for collect_pose.  A frame whose rows are contiguous but strided (a
+        crop view of a larger frame) is passed with strides[0] as its pitch, not copied.  Page-locked frames are kept referenced until
+        the ticket is collected."""
+        formats = [format] * len(frames) if isinstance(format, str) else list(format)
+        if len(formats) != len(frames) or any(fmt not in PIXEL_FORMATS for fmt in formats):
+            raise HyperposeError(HP_ERR_ARG, f"format {format!r}: expected one of {sorted(PIXEL_FORMATS)}, or one per frame")
+        for i, (f, fmt) in enumerate(zip(frames, formats)):
+            ch = PIXEL_CHANNELS[fmt]
+            shape = "(H, W)" if ch is None else f"(H, W, {ch})"
+            if not isinstance(f, np.ndarray) or f.dtype != np.uint8 or f.ndim != (2 if ch is None else 3) or (ch and f.shape[2] != ch):
+                raise HyperposeError(HP_ERR_ARG, f"frame {i}: expected a uint8 {shape} {fmt} array, got "
+                                                 f"{getattr(f, 'dtype', type(f).__name__)} {getattr(f, 'shape', '')}")
+            row = f.shape[1] * (ch or 1)
+            if f.strides[-1] != 1 or (ch and f.strides[1] != ch) or f.strides[0] < row or f.strides[0] >= 1 << 31:
+                raise HyperposeError(HP_ERR_ARG, f"frame {i}: the bytes of each row must be contiguous, rows at least {row} bytes apart "
+                                                 f"(strides {f.strides})")
+        table = (FrameInterleaved * len(frames))(*[interleaved_record(f, fmt) for f, fmt in zip(frames, formats)])
+        t = self._submit_frame_table(parser, table, keep_ratio, device=False, fmt="interleaved")
+        self._ticket_frames = getattr(self, "_ticket_frames", {})
+        self._ticket_frames[t] = list(frames)
+        return t
+
+    def submit_pose_interleaved_device(self, parser, frames, keep_ratio: bool = False) -> int:
+        """the same for interleaved frames in device memory, given as FrameInterleaved records (device pointer, size, pitch, format:
+        a cudaMallocPitch allocation, an NvBufSurface, a crop of either).  The resize kernel reads them in place: they must stay valid
+        and unchanged until the ticket is collected."""
+        for i, f in enumerate(frames):
+            if not isinstance(f, FrameInterleaved):
+                raise HyperposeError(HP_ERR_ARG, f"frame {i}: expected a FrameInterleaved, got {type(f).__name__}")
+        table = (FrameInterleaved * len(frames))(*frames)
+        return self._submit_frame_table(parser, table, keep_ratio, device=True, fmt="interleaved")
 
     def debug_read_slot_frames(self, ticket: int, n: int) -> np.ndarray:
         """the first n resized network-size frames u8[n,in_h,in_w,3] of a ticket in flight or collected"""

@@ -118,6 +118,19 @@ struct YuvFrameDesc {
 };
 static_assert(sizeof(YuvFrameDesc) == 64, "YuvFrameDesc is uploaded as raw bytes");
 
+// One interleaved frame of a resize launch (hp_frame_interleaved: BGR, RGB, BGRA, RGBA, gray, YUYV, UYVY, YVYU), rows pitched;
+// converted to BGR per source pixel as cv::cvtColor does, then resized exactly as a FrameDesc frame of the same size.
+struct InterleavedFrameDesc {
+    const uint8_t* src;
+    int sh, sw;     // source size
+    int rh, rw;     // resized region
+    int mode;       // RZ_*
+    int pitch;      // bytes from one row to the next
+    int format;     // hp_pixel_format
+    int pad;
+};
+static_assert(sizeof(InterleavedFrameDesc) == 40, "InterleavedFrameDesc is uploaded as raw bytes");
+
 // Source fetches of the resize: byte c (B, G, R) of source pixel x of one source row.
 struct BgrRow {
     const uint8_t* p;
@@ -126,18 +139,23 @@ struct BgrRow {
 };
 __device__ __forceinline__ BgrRow src_row(const FrameDesc& d, int sy) { return BgrRow{ d.src + (size_t)sy * d.sw * 3 }; }
 
-// OpenCV's YUV420sp2RGB / YUV420p2RGB fixed point (color_yuv.simd.hpp: ITUR_BT_601_CY .. _CVR, ITUR_BT_601_SHIFT = 20), BT.601
-// limited range.  Every sum stays below 2^30 in magnitude.
+// Byte c (B, G, R) of one pixel from its luma and chroma bytes: OpenCV's YUV420sp2RGB / YUV420p2RGB / YUV422toRGB fixed point
+// (color_yuv.simd.hpp: ITUR_BT_601_CY .. _CVR, ITUR_BT_601_SHIFT = 20), BT.601 limited range.  Every sum stays below 2^30 in magnitude.
+__device__ __forceinline__ int bt601_bgr(int y, int u, int v, int c)
+{
+    const int yy = max(y - 16, 0) * 1220542 + (1 << 19);
+    const int cu = u - 128, cv = v - 128;
+    const int s = c == 0 ? yy + 2116026 * cu : (c == 1 ? yy - 852492 * cv - 409993 * cu : yy + 1673527 * cv);
+    return min(max(s >> 20, 0), 255);
+}
+
 struct YuvRow {
     const uint8_t *y, *u, *v;
     int step;
     __device__ __forceinline__ int px(int x, int c) const
     {
-        const int yy = max(y[x] - 16, 0) * 1220542 + (1 << 19);
         const int k = (x >> 1) * step;
-        const int cu = u[k] - 128, cv = v[k] - 128;
-        const int s = c == 0 ? yy + 2116026 * cu : (c == 1 ? yy - 852492 * cv - 409993 * cu : yy + 1673527 * cv);
-        return min(max(s >> 20, 0), 255);
+        return bt601_bgr(y[x], u[k], v[k], c);
     }
     __device__ __forceinline__ int byte(int b) const { const int x = b / 3; return px(x, b - 3 * x); }
 };
@@ -145,6 +163,35 @@ __device__ __forceinline__ YuvRow src_row(const YuvFrameDesc& d, int sy)
 {
     const size_t c = (size_t)(sy >> 1) * d.pitch_uv;
     return YuvRow{ d.y + (size_t)sy * d.pitch_y, d.u + c, d.v + c, d.uv_step };
+}
+
+// cv::cvtColor's COLOR_RGB2BGR, _BGRA2BGR, _RGBA2BGR, _GRAY2BGR and _YUV2BGR_YUYV / _UYVY / _YVYU on one row; BGR is the identity.
+// The format is the frame's, so it is uniform across a CTA.
+struct InterleavedRow {
+    const uint8_t* p;
+    int format;
+    __device__ __forceinline__ int px(int x, int c) const
+    {
+        switch (format) {
+        case HP_PIX_BGR: return p[3 * x + c];
+        case HP_PIX_RGB: return p[3 * x + 2 - c];
+        case HP_PIX_BGRA: return p[4 * x + c];
+        case HP_PIX_RGBA: return p[4 * x + 2 - c];
+        case HP_PIX_GRAY: return p[x];
+        default: {   // 4:2:2: the 4 bytes of pixel pair x / 2 hold its two luma bytes and one U, V pair
+            const uint8_t* q = p + 4 * (x >> 1);
+            const int odd = 2 * (x & 1);
+            if (format == HP_PIX_YUYV) return bt601_bgr(q[odd], q[1], q[3], c);
+            if (format == HP_PIX_UYVY) return bt601_bgr(q[1 + odd], q[0], q[2], c);
+            return bt601_bgr(q[odd], q[3], q[1], c);   // YVYU
+        }
+        }
+    }
+    __device__ __forceinline__ int byte(int b) const { const int x = b / 3; return px(x, b - 3 * x); }
+};
+__device__ __forceinline__ InterleavedRow src_row(const InterleavedFrameDesc& d, int sy)
+{
+    return InterleavedRow{ d.src + (size_t)sy * d.pitch, d.format };
 }
 
 // cv::resize(INTER_LINEAR) on CV_8UC3 frames (src/tensorrt.cpp:451) for the N frames of a batch in one launch, each frame read
@@ -221,6 +268,16 @@ __global__ void __launch_bounds__(256) resize_frames_u8c3_kernel(const FrameDesc
 __global__ void __launch_bounds__(256, 6) resize_frames_yuv420_kernel(const YuvFrameDesc* __restrict__ desc, uint8_t* __restrict__ dst, int dh, int dw)
 {
     const YuvFrameDesc d = desc[blockIdx.y];
+    resize_frames(d, dst, dh, dw);
+}
+
+// interleaved frames with a row pitch (hp_frame_interleaved): the conversion is fused into the fetch as for YUV 4:2:0 frames; one
+// launch may mix formats, each CTA serving one frame.  One row pointer and the format per source row fit the 32 registers of 8 CTAs
+// per SM with no spills.
+__global__ void __launch_bounds__(256, 8) resize_frames_interleaved_kernel(const InterleavedFrameDesc* __restrict__ desc,
+                                                                           uint8_t* __restrict__ dst, int dh, int dw)
+{
+    const InterleavedFrameDesc d = desc[blockIdx.y];
     resize_frames(d, dst, dh, dw);
 }
 
@@ -899,6 +956,7 @@ struct hp_engine {
         uint8_t* pin_src = nullptr; size_t pin_src_bytes = 0;
         FrameDesc* d_desc = nullptr; FrameDesc* pin_desc = nullptr;   // [max_batch]
         YuvFrameDesc* d_ydesc = nullptr; YuvFrameDesc* pin_ydesc = nullptr;   // [max_batch] (hp_pose_submit_*frames_yuv420_*)
+        InterleavedFrameDesc* d_idesc = nullptr; InterleavedFrameDesc* pin_idesc = nullptr;   // [max_batch] (*frames_interleaved_*)
         hp_human* pin_humans = nullptr; size_t pin_humans_n = 0;
         int* pin_counts = nullptr; size_t pin_counts_n = 0;   // [N counts | N flags]
         cudaEvent_t h2d_done = nullptr, done = nullptr;
@@ -1535,6 +1593,8 @@ void free_engine(hp_engine* e)
         if (sl.pin_desc) cudaFreeHost(sl.pin_desc);
         if (sl.d_ydesc) cudaFree(sl.d_ydesc);
         if (sl.pin_ydesc) cudaFreeHost(sl.pin_ydesc);
+        if (sl.d_idesc) cudaFree(sl.d_idesc);
+        if (sl.pin_idesc) cudaFreeHost(sl.pin_idesc);
         if (sl.pin_humans) cudaFreeHost(sl.pin_humans);
         if (sl.pin_counts) cudaFreeHost(sl.pin_counts);
         if (sl.h2d_done) cudaEventDestroy(sl.h2d_done);
@@ -2035,6 +2095,15 @@ static int launch_resize_yuv(hp_engine* e, const YuvFrameDesc* d_desc, uint8_t* 
 {
     const dim3 grid((e->in_h + RZ_ROWS - 1) / RZ_ROWS, N);
     resize_frames_yuv420_kernel<<<grid, 256, (size_t)e->in_w * sizeof(int2), e->stream>>>(d_desc, dst, e->in_h, e->in_w);
+    e->launches++;
+    HP_CUDA_TRY(cudaGetLastError());
+    return HP_OK;
+}
+
+static int launch_resize_interleaved(hp_engine* e, const InterleavedFrameDesc* d_desc, uint8_t* dst, int N)
+{
+    const dim3 grid((e->in_h + RZ_ROWS - 1) / RZ_ROWS, N);
+    resize_frames_interleaved_kernel<<<grid, 256, (size_t)e->in_w * sizeof(int2), e->stream>>>(d_desc, dst, e->in_h, e->in_w);
     e->launches++;
     HP_CUDA_TRY(cudaGetLastError());
     return HP_OK;
@@ -2582,6 +2651,41 @@ int slot_upload_frames(hp_engine* e, hp_engine::PoseSlot& sl, FrameDesc* descs, 
     return launch_resize(e, sl.d_desc, sl.d_frames, N);
 }
 
+// the slot's source buffer for `bytes` of row-compacted host frames (grown here: the slot is idle, it has been collected)
+int slot_src_reserve(hp_engine::PoseSlot& sl, size_t bytes)
+{
+    if (sl.d_src_bytes < bytes) {
+        if (sl.d_src) cudaFree(sl.d_src);
+        sl.d_src = nullptr; sl.d_src_bytes = 0;
+        HP_CUDA_TRY(cudaMalloc(&sl.d_src, bytes));
+        sl.d_src_bytes = bytes;
+    }
+    return HP_OK;
+}
+
+// one plane of a host frame on the copy stream: rows x width bytes at `src` with pitch `pitch` into the slot's source buffer at byte
+// offset `at`, row-compacted.  By a pitched DMA from the caller when it is page-locked, else through the slot's pinned staging, which
+// grows to `total` bytes (the whole batch) on the first pageable plane that needs it.
+int upload_plane(hp_engine* e, hp_engine::PoseSlot& sl, const uint8_t* src, int pitch, int rows, int width, size_t at, size_t total)
+{
+    cudaPointerAttributes attr;
+    const bool pinned = cudaPointerGetAttributes(&attr, src) == cudaSuccess && attr.type == cudaMemoryTypeHost;
+    if (pinned) {
+        HP_CUDA_TRY(cudaMemcpy2DAsync(sl.d_src + at, width, src, pitch, width, rows, cudaMemcpyHostToDevice, e->copy_stream));
+        return HP_OK;
+    }
+    cudaGetLastError();
+    if (sl.pin_src_bytes < total) {
+        if (sl.pin_src) cudaFreeHost(sl.pin_src);
+        sl.pin_src = nullptr; sl.pin_src_bytes = 0;
+        HP_CUDA_TRY(cudaMallocHost(&sl.pin_src, total));
+        sl.pin_src_bytes = total;
+    }
+    for (int r = 0; r < rows; ++r) memcpy(sl.pin_src + at + (size_t)r * width, src + (size_t)r * pitch, width);
+    HP_CUDA_TRY(cudaMemcpyAsync(sl.d_src + at, sl.pin_src + at, (size_t)rows * width, cudaMemcpyHostToDevice, e->copy_stream));
+    return HP_OK;
+}
+
 // The same for YUV 4:2:0 frames.  A host frame is copied row-compacted into the slot's source buffer: its luma plane with pitch
 // width, then the interleaved UV plane (semi-planar, copied once) or the U and V planes (planar), 1.5 bytes per pixel.  Each plane goes
 // by a pitched DMA from the caller when it is page-locked, else through the slot's pinned staging.  Device frames are read in place.
@@ -2594,36 +2698,15 @@ int slot_upload_yuv(hp_engine* e, hp_engine::PoseSlot& sl, YuvFrameDesc* descs, 
     if (!device_src) {
         std::vector<size_t> off(N + 1, 0);
         for (int f = 0; f < N; ++f) off[f + 1] = off[f] + (((size_t)descs[f].sh * descs[f].sw * 3 / 2 + 255) & ~(size_t)255);
-        if (sl.d_src_bytes < off[N]) {
-            if (sl.d_src) cudaFree(sl.d_src);
-            sl.d_src = nullptr; sl.d_src_bytes = 0;
-            HP_CUDA_TRY(cudaMalloc(&sl.d_src, off[N]));
-            sl.d_src_bytes = off[N];
-        }
-        // one plane: rows x width bytes at `src` with pitch `pitch` into the compacted region at byte offset `at`
-        auto copy_plane = [&](const uint8_t* src, int pitch, int rows, int width, size_t at) -> int {
-            cudaPointerAttributes attr;
-            const bool pinned = cudaPointerGetAttributes(&attr, src) == cudaSuccess && attr.type == cudaMemoryTypeHost;
-            if (pinned) {
-                HP_CUDA_TRY(cudaMemcpy2DAsync(sl.d_src + at, width, src, pitch, width, rows, cudaMemcpyHostToDevice, e->copy_stream));
-                return HP_OK;
-            }
-            cudaGetLastError();
-            if (sl.pin_src_bytes < off[N]) {
-                if (sl.pin_src) cudaFreeHost(sl.pin_src);
-                sl.pin_src = nullptr; sl.pin_src_bytes = 0;
-                HP_CUDA_TRY(cudaMallocHost(&sl.pin_src, off[N]));
-                sl.pin_src_bytes = off[N];
-            }
-            for (int r = 0; r < rows; ++r) memcpy(sl.pin_src + at + (size_t)r * width, src + (size_t)r * pitch, width);
-            HP_CUDA_TRY(cudaMemcpyAsync(sl.d_src + at, sl.pin_src + at, (size_t)rows * width, cudaMemcpyHostToDevice, e->copy_stream));
-            return HP_OK;
+        int rc = slot_src_reserve(sl, off[N]);
+        if (rc) return rc;
+        auto copy_plane = [&](const uint8_t* src, int pitch, int rows, int width, size_t at) {
+            return upload_plane(e, sl, src, pitch, rows, width, at, off[N]);
         };
         for (int f = 0; f < N; ++f) {
             YuvFrameDesc& d = descs[f];
             const size_t luma = (size_t)d.sh * d.sw, at = off[f] + luma;
-            int rc = copy_plane(d.y, d.pitch_y, d.sh, d.sw, off[f]);
-            if (rc) return rc;
+            if ((rc = copy_plane(d.y, d.pitch_y, d.sh, d.sw, off[f]))) return rc;
             if (d.uv_step == 2) {   // one interleaved plane starting at the lower of u, v
                 const uint8_t* base = d.u < d.v ? d.u : d.v;
                 if ((rc = copy_plane(base, d.pitch_uv, d.sh / 2, d.sw, at))) return rc;
@@ -2649,9 +2732,54 @@ int slot_upload_yuv(hp_engine* e, hp_engine::PoseSlot& sl, YuvFrameDesc* descs, 
     return launch_resize_yuv(e, sl.d_ydesc, sl.d_frames, N);
 }
 
-// a submitted batch into the slot's device buffer: network-size frames, or frames of any size (BGR descs or YUV ydescs) resized there
-int slot_upload_batch(hp_engine* e, hp_engine::PoseSlot& sl, const uint8_t* frames, FrameDesc* descs, YuvFrameDesc* ydescs, int N, bool device_src)
+// bytes per pixel of an hp_pixel_format, 0 for an unknown one
+int pixel_bytes(int format)
 {
+    switch (format) {
+    case HP_PIX_BGR: case HP_PIX_RGB: return 3;
+    case HP_PIX_BGRA: case HP_PIX_RGBA: return 4;
+    case HP_PIX_GRAY: return 1;
+    case HP_PIX_YUYV: case HP_PIX_UYVY: case HP_PIX_YVYU: return 2;
+    default: return 0;
+    }
+}
+
+// The same for interleaved frames.  A host frame is copied row-compacted into the slot's source buffer (width * bytes per pixel per
+// row), by a pitched DMA from the caller when it is page-locked, else through the slot's pinned staging.  Device frames are read in
+// place with their pitch.
+int slot_upload_interleaved(hp_engine* e, hp_engine::PoseSlot& sl, InterleavedFrameDesc* descs, int N, bool device_src)
+{
+    if (!sl.d_idesc) {
+        HP_CUDA_TRY(cudaMalloc(&sl.d_idesc, e->max_batch * sizeof(InterleavedFrameDesc)));
+        HP_CUDA_TRY(cudaMallocHost(&sl.pin_idesc, e->max_batch * sizeof(InterleavedFrameDesc)));
+    }
+    if (!device_src) {
+        std::vector<size_t> off(N + 1, 0);
+        for (int f = 0; f < N; ++f)
+            off[f + 1] = off[f] + (((size_t)descs[f].sh * descs[f].sw * pixel_bytes(descs[f].format) + 255) & ~(size_t)255);
+        int rc = slot_src_reserve(sl, off[N]);
+        if (rc) return rc;
+        for (int f = 0; f < N; ++f) {
+            InterleavedFrameDesc& d = descs[f];
+            const int row = d.sw * pixel_bytes(d.format);
+            if ((rc = upload_plane(e, sl, d.src, d.pitch, d.sh, row, off[f], off[N]))) return rc;
+            d.src = sl.d_src + off[f];
+            d.pitch = row;
+        }
+    }
+    memcpy(sl.pin_idesc, descs, N * sizeof(InterleavedFrameDesc));
+    HP_CUDA_TRY(cudaMemcpyAsync(sl.d_idesc, sl.pin_idesc, N * sizeof(InterleavedFrameDesc), cudaMemcpyHostToDevice, e->copy_stream));
+    HP_CUDA_TRY(cudaEventRecord(sl.h2d_done, e->copy_stream));
+    HP_CUDA_TRY(cudaStreamWaitEvent(e->stream, sl.h2d_done, 0));
+    return launch_resize_interleaved(e, sl.d_idesc, sl.d_frames, N);
+}
+
+// a submitted batch into the slot's device buffer: network-size frames, or frames of any size (BGR descs, YUV 4:2:0 ydescs or
+// interleaved idescs) resized there
+int slot_upload_batch(hp_engine* e, hp_engine::PoseSlot& sl, const uint8_t* frames, FrameDesc* descs, YuvFrameDesc* ydescs,
+                      InterleavedFrameDesc* idescs, int N, bool device_src)
+{
+    if (idescs) return slot_upload_interleaved(e, sl, idescs, N, device_src);
     if (ydescs) return slot_upload_yuv(e, sl, ydescs, N, device_src);
     return descs ? slot_upload_frames(e, sl, descs, N, device_src) : slot_upload(e, sl, frames, N, device_src);
 }
@@ -2750,12 +2878,12 @@ static int pifpaf_enqueue(hp_engine* e, hp_engine::PoseSlot& sl)
     return HP_OK;
 }
 
-// frames: N network-size frames, or -- descs / ydescs != NULL -- N BGR / YUV 4:2:0 frames of any size described by them (their
-// sources are rewritten to the slot's copies of host frames)
-static int pose_submit_pifpaf(hp_engine* e, hp_pifpaf* dec, const uint8_t* frames, FrameDesc* descs, YuvFrameDesc* ydescs, int N, int* ticket,
-                              bool device_src)
+// frames: N network-size frames, or -- descs / ydescs / idescs != NULL -- N BGR / YUV 4:2:0 / interleaved frames of any size
+// described by them (their sources are rewritten to the slot's copies of host frames)
+static int pose_submit_pifpaf(hp_engine* e, hp_pifpaf* dec, const uint8_t* frames, FrameDesc* descs, YuvFrameDesc* ydescs,
+                              InterleavedFrameDesc* idescs, int N, int* ticket, bool device_src)
 {
-    if (!e || !dec || (!frames && !descs && !ydescs) || !ticket) { set_error("hp_pose_submit_pifpaf: null argument"); return HP_ERR_ARG; }
+    if (!e || !dec || (!frames && !descs && !ydescs && !idescs) || !ticket) { set_error("hp_pose_submit_pifpaf: null argument"); return HP_ERR_ARG; }
     if (N <= 0 || N > e->max_batch) { set_error("Input batch size overflow: Yours@%d Max@%d", N, e->max_batch); return HP_ERR_BATCH; }
     if (e->hdr.head_type != 1) { set_error("hp_pose_submit_pifpaf: the model pack has no OpenPifPaf heads (head_type %u)", e->hdr.head_type); return HP_ERR_UNSUPPORTED; }
     HP_CUDA_TRY(cudaSetDevice(e->device));
@@ -2765,7 +2893,7 @@ static int pose_submit_pifpaf(hp_engine* e, hp_pifpaf* dec, const uint8_t* frame
     int rc = pifpaf_slot_prepare(e, sl, dec, N);
     if (rc) return rc;
     e->reserve_sms = e->opt.pifpaf_reserve_sms;   // the decoder's growth kernel (one warp per frame) runs underneath the next batch's convolutions
-    rc = slot_upload_batch(e, sl, frames, descs, ydescs, N, device_src);
+    rc = slot_upload_batch(e, sl, frames, descs, ydescs, idescs, N, device_src);
     if (rc) return rc;
     rc = pifpaf_enqueue(e, sl);
     if (rc) return rc;
@@ -2776,11 +2904,11 @@ static int pose_submit_pifpaf(hp_engine* e, hp_pifpaf* dec, const uint8_t* frame
 }
 
 // the PAF-parser calls (ppn_call false: `parser` is an hp_paf) and the Pose Proposal Network calls (true: an hp_ppn)
-static int pose_submit(hp_engine* e, void* parser, bool ppn_call, const uint8_t* frames, FrameDesc* descs, YuvFrameDesc* ydescs, int N,
-                       int* ticket, bool device_src)
+static int pose_submit(hp_engine* e, void* parser, bool ppn_call, const uint8_t* frames, FrameDesc* descs, YuvFrameDesc* ydescs,
+                       InterleavedFrameDesc* idescs, int N, int* ticket, bool device_src)
 {
     const char* fn = ppn_call ? "hp_pose_submit_ppn" : "hp_pose_submit";
-    if (!e || !parser || (!frames && !descs && !ydescs) || !ticket) { set_error("%s: null argument", fn); return HP_ERR_ARG; }
+    if (!e || !parser || (!frames && !descs && !ydescs && !idescs) || !ticket) { set_error("%s: null argument", fn); return HP_ERR_ARG; }
     if (N <= 0 || N > e->max_batch) { set_error("Input batch size overflow: Yours@%d Max@%d", N, e->max_batch); return HP_ERR_BATCH; }
     hp_paf* paf = ppn_call ? nullptr : (hp_paf*)parser;
     hp_ppn* ppn = ppn_call ? (hp_ppn*)parser : nullptr;
@@ -2805,7 +2933,7 @@ static int pose_submit(hp_engine* e, void* parser, bool ppn_call, const uint8_t*
     if (sl.busy) { set_error("%s: two batches are already in flight -- collect ticket %d first", fn, idx); return HP_ERR_ARG; }
     int rc = pose_slot_prepare(e, sl, paf, ppn, N);
     if (rc) return rc;
-    rc = slot_upload_batch(e, sl, frames, descs, ydescs, N, device_src);   // (the captured graph reads the slot's buffer)
+    rc = slot_upload_batch(e, sl, frames, descs, ydescs, idescs, N, device_src);   // (the captured graph reads the slot's buffer)
     if (rc) return rc;
     rc = pose_launch(e, sl);
     if (rc) return rc;
@@ -2818,23 +2946,23 @@ static int pose_submit(hp_engine* e, void* parser, bool ppn_call, const uint8_t*
 
 int hp_pose_submit_u8_host(hp_engine* e, hp_paf* parser, const uint8_t* frames, int N, int* ticket)
 {
-    return pose_submit(e, parser, false, frames, nullptr, nullptr, N, ticket, false);
+    return pose_submit(e, parser, false, frames, nullptr, nullptr, nullptr, N, ticket, false);
 }
 
 // the same with the frames already resident in device memory (what a decoder / capture pipeline on the GPU hands over)
 int hp_pose_submit_u8_device(hp_engine* e, hp_paf* parser, const uint8_t* d_frames, int N, int* ticket)
 {
-    return pose_submit(e, parser, false, d_frames, nullptr, nullptr, N, ticket, true);
+    return pose_submit(e, parser, false, d_frames, nullptr, nullptr, nullptr, N, ticket, true);
 }
 
 int hp_pose_submit_pifpaf_u8_host(hp_engine* e, hp_pifpaf* decoder, const uint8_t* frames, int N, int* ticket)
 {
-    return pose_submit_pifpaf(e, decoder, frames, nullptr, nullptr, N, ticket, false);
+    return pose_submit_pifpaf(e, decoder, frames, nullptr, nullptr, nullptr, N, ticket, false);
 }
 
 int hp_pose_submit_pifpaf_u8_device(hp_engine* e, hp_pifpaf* decoder, const uint8_t* d_frames, int N, int* ticket)
 {
-    return pose_submit_pifpaf(e, decoder, d_frames, nullptr, nullptr, N, ticket, true);
+    return pose_submit_pifpaf(e, decoder, d_frames, nullptr, nullptr, nullptr, N, ticket, true);
 }
 
 // the resize descriptors of a frame list, refused before any work is enqueued
@@ -2858,53 +2986,53 @@ int hp_pose_submit_frames_u8_host(hp_engine* e, hp_paf* parser, const hp_frame_u
 {
     std::vector<FrameDesc> d;
     const int rc = frame_descs(e, frames, N, keep_ratio, d);
-    return rc ? rc : pose_submit(e, parser, false, nullptr, d.data(), nullptr, N, ticket, false);
+    return rc ? rc : pose_submit(e, parser, false, nullptr, d.data(), nullptr, nullptr, N, ticket, false);
 }
 
 int hp_pose_submit_frames_u8_device(hp_engine* e, hp_paf* parser, const hp_frame_u8* frames, int N, int keep_ratio, int* ticket)
 {
     std::vector<FrameDesc> d;
     const int rc = frame_descs(e, frames, N, keep_ratio, d);
-    return rc ? rc : pose_submit(e, parser, false, nullptr, d.data(), nullptr, N, ticket, true);
+    return rc ? rc : pose_submit(e, parser, false, nullptr, d.data(), nullptr, nullptr, N, ticket, true);
 }
 
 int hp_pose_submit_pifpaf_frames_u8_host(hp_engine* e, hp_pifpaf* decoder, const hp_frame_u8* frames, int N, int keep_ratio, int* ticket)
 {
     std::vector<FrameDesc> d;
     const int rc = frame_descs(e, frames, N, keep_ratio, d);
-    return rc ? rc : pose_submit_pifpaf(e, decoder, nullptr, d.data(), nullptr, N, ticket, false);
+    return rc ? rc : pose_submit_pifpaf(e, decoder, nullptr, d.data(), nullptr, nullptr, N, ticket, false);
 }
 
 int hp_pose_submit_pifpaf_frames_u8_device(hp_engine* e, hp_pifpaf* decoder, const hp_frame_u8* frames, int N, int keep_ratio, int* ticket)
 {
     std::vector<FrameDesc> d;
     const int rc = frame_descs(e, frames, N, keep_ratio, d);
-    return rc ? rc : pose_submit_pifpaf(e, decoder, nullptr, d.data(), nullptr, N, ticket, true);
+    return rc ? rc : pose_submit_pifpaf(e, decoder, nullptr, d.data(), nullptr, nullptr, N, ticket, true);
 }
 
 // ---- Pose Proposal Network packs: network, parse and record D2H in one captured graph on the engine stream, as for the PAF parser ----
 int hp_pose_submit_ppn_u8_host(hp_engine* e, hp_ppn* parser, const uint8_t* frames, int N, int* ticket)
 {
-    return pose_submit(e, parser, true, frames, nullptr, nullptr, N, ticket, false);
+    return pose_submit(e, parser, true, frames, nullptr, nullptr, nullptr, N, ticket, false);
 }
 
 int hp_pose_submit_ppn_u8_device(hp_engine* e, hp_ppn* parser, const uint8_t* d_frames, int N, int* ticket)
 {
-    return pose_submit(e, parser, true, d_frames, nullptr, nullptr, N, ticket, true);
+    return pose_submit(e, parser, true, d_frames, nullptr, nullptr, nullptr, N, ticket, true);
 }
 
 int hp_pose_submit_ppn_frames_u8_host(hp_engine* e, hp_ppn* parser, const hp_frame_u8* frames, int N, int keep_ratio, int* ticket)
 {
     std::vector<FrameDesc> d;
     const int rc = frame_descs(e, frames, N, keep_ratio, d);
-    return rc ? rc : pose_submit(e, parser, true, nullptr, d.data(), nullptr, N, ticket, false);
+    return rc ? rc : pose_submit(e, parser, true, nullptr, d.data(), nullptr, nullptr, N, ticket, false);
 }
 
 int hp_pose_submit_ppn_frames_u8_device(hp_engine* e, hp_ppn* parser, const hp_frame_u8* frames, int N, int keep_ratio, int* ticket)
 {
     std::vector<FrameDesc> d;
     const int rc = frame_descs(e, frames, N, keep_ratio, d);
-    return rc ? rc : pose_submit(e, parser, true, nullptr, d.data(), nullptr, N, ticket, true);
+    return rc ? rc : pose_submit(e, parser, true, nullptr, d.data(), nullptr, nullptr, N, ticket, true);
 }
 
 // the resize descriptors of a YUV 4:2:0 frame list, refused before any work is enqueued; the regime comes from the luma size
@@ -2938,42 +3066,113 @@ int hp_pose_submit_frames_yuv420_host(hp_engine* e, hp_paf* parser, const hp_fra
 {
     std::vector<YuvFrameDesc> d;
     const int rc = yuv_frame_descs(e, frames, N, keep_ratio, d);
-    return rc ? rc : pose_submit(e, parser, false, nullptr, nullptr, d.data(), N, ticket, false);
+    return rc ? rc : pose_submit(e, parser, false, nullptr, nullptr, d.data(), nullptr, N, ticket, false);
 }
 
 int hp_pose_submit_frames_yuv420_device(hp_engine* e, hp_paf* parser, const hp_frame_yuv420* frames, int N, int keep_ratio, int* ticket)
 {
     std::vector<YuvFrameDesc> d;
     const int rc = yuv_frame_descs(e, frames, N, keep_ratio, d);
-    return rc ? rc : pose_submit(e, parser, false, nullptr, nullptr, d.data(), N, ticket, true);
+    return rc ? rc : pose_submit(e, parser, false, nullptr, nullptr, d.data(), nullptr, N, ticket, true);
 }
 
 int hp_pose_submit_pifpaf_frames_yuv420_host(hp_engine* e, hp_pifpaf* decoder, const hp_frame_yuv420* frames, int N, int keep_ratio, int* ticket)
 {
     std::vector<YuvFrameDesc> d;
     const int rc = yuv_frame_descs(e, frames, N, keep_ratio, d);
-    return rc ? rc : pose_submit_pifpaf(e, decoder, nullptr, nullptr, d.data(), N, ticket, false);
+    return rc ? rc : pose_submit_pifpaf(e, decoder, nullptr, nullptr, d.data(), nullptr, N, ticket, false);
 }
 
 int hp_pose_submit_pifpaf_frames_yuv420_device(hp_engine* e, hp_pifpaf* decoder, const hp_frame_yuv420* frames, int N, int keep_ratio, int* ticket)
 {
     std::vector<YuvFrameDesc> d;
     const int rc = yuv_frame_descs(e, frames, N, keep_ratio, d);
-    return rc ? rc : pose_submit_pifpaf(e, decoder, nullptr, nullptr, d.data(), N, ticket, true);
+    return rc ? rc : pose_submit_pifpaf(e, decoder, nullptr, nullptr, d.data(), nullptr, N, ticket, true);
 }
 
 int hp_pose_submit_ppn_frames_yuv420_host(hp_engine* e, hp_ppn* parser, const hp_frame_yuv420* frames, int N, int keep_ratio, int* ticket)
 {
     std::vector<YuvFrameDesc> d;
     const int rc = yuv_frame_descs(e, frames, N, keep_ratio, d);
-    return rc ? rc : pose_submit(e, parser, true, nullptr, nullptr, d.data(), N, ticket, false);
+    return rc ? rc : pose_submit(e, parser, true, nullptr, nullptr, d.data(), nullptr, N, ticket, false);
 }
 
 int hp_pose_submit_ppn_frames_yuv420_device(hp_engine* e, hp_ppn* parser, const hp_frame_yuv420* frames, int N, int keep_ratio, int* ticket)
 {
     std::vector<YuvFrameDesc> d;
     const int rc = yuv_frame_descs(e, frames, N, keep_ratio, d);
-    return rc ? rc : pose_submit(e, parser, true, nullptr, nullptr, d.data(), N, ticket, true);
+    return rc ? rc : pose_submit(e, parser, true, nullptr, nullptr, d.data(), nullptr, N, ticket, true);
+}
+
+// the resize descriptors of an interleaved frame list, refused before any work is enqueued; the regime comes from the pixel size
+static int interleaved_frame_descs(const hp_engine* e, const hp_frame_interleaved* frames, int N, int keep_ratio,
+                                   std::vector<InterleavedFrameDesc>& descs)
+{
+    if (!e || !frames) { set_error("hp_pose_submit_frames_interleaved: null argument"); return HP_ERR_ARG; }
+    if (N <= 0 || N > e->max_batch) { set_error("Input batch size overflow: Yours@%d Max@%d", N, e->max_batch); return HP_ERR_BATCH; }
+    descs.resize(N);
+    for (int f = 0; f < N; ++f) {
+        const hp_frame_interleaved& fr = frames[f];
+        const int bpp = pixel_bytes(fr.format);
+        const char* bad = nullptr;
+        if (!fr.data) bad = "is null";
+        else if (fr.height <= 0 || fr.width <= 0) bad = "has a size that is not positive";
+        else if (!bpp) bad = "has an unknown format";
+        else if (bpp == 2 && (fr.width & 1)) bad = "is 4:2:2 of odd width";
+        else if ((long long)fr.pitch < (long long)fr.width * bpp) bad = "has a pitch shorter than its row";
+        if (bad) {
+            set_error("hp_pose_submit_frames_interleaved: frame %d %s (%dx%d, pitch %d, format %d)", f, bad, fr.height, fr.width, fr.pitch,
+                      fr.format);
+            return HP_ERR_ARG;
+        }
+        FrameDesc d;
+        const int rc = frame_desc(e, nullptr, fr.height, fr.width, keep_ratio, d);
+        if (rc) return rc;
+        descs[f] = InterleavedFrameDesc{ fr.data, fr.height, fr.width, d.rh, d.rw, d.mode, fr.pitch, fr.format, 0 };
+    }
+    return HP_OK;
+}
+
+int hp_pose_submit_frames_interleaved_host(hp_engine* e, hp_paf* parser, const hp_frame_interleaved* frames, int N, int keep_ratio, int* ticket)
+{
+    std::vector<InterleavedFrameDesc> d;
+    const int rc = interleaved_frame_descs(e, frames, N, keep_ratio, d);
+    return rc ? rc : pose_submit(e, parser, false, nullptr, nullptr, nullptr, d.data(), N, ticket, false);
+}
+
+int hp_pose_submit_frames_interleaved_device(hp_engine* e, hp_paf* parser, const hp_frame_interleaved* frames, int N, int keep_ratio, int* ticket)
+{
+    std::vector<InterleavedFrameDesc> d;
+    const int rc = interleaved_frame_descs(e, frames, N, keep_ratio, d);
+    return rc ? rc : pose_submit(e, parser, false, nullptr, nullptr, nullptr, d.data(), N, ticket, true);
+}
+
+int hp_pose_submit_pifpaf_frames_interleaved_host(hp_engine* e, hp_pifpaf* decoder, const hp_frame_interleaved* frames, int N, int keep_ratio, int* ticket)
+{
+    std::vector<InterleavedFrameDesc> d;
+    const int rc = interleaved_frame_descs(e, frames, N, keep_ratio, d);
+    return rc ? rc : pose_submit_pifpaf(e, decoder, nullptr, nullptr, nullptr, d.data(), N, ticket, false);
+}
+
+int hp_pose_submit_pifpaf_frames_interleaved_device(hp_engine* e, hp_pifpaf* decoder, const hp_frame_interleaved* frames, int N, int keep_ratio, int* ticket)
+{
+    std::vector<InterleavedFrameDesc> d;
+    const int rc = interleaved_frame_descs(e, frames, N, keep_ratio, d);
+    return rc ? rc : pose_submit_pifpaf(e, decoder, nullptr, nullptr, nullptr, d.data(), N, ticket, true);
+}
+
+int hp_pose_submit_ppn_frames_interleaved_host(hp_engine* e, hp_ppn* parser, const hp_frame_interleaved* frames, int N, int keep_ratio, int* ticket)
+{
+    std::vector<InterleavedFrameDesc> d;
+    const int rc = interleaved_frame_descs(e, frames, N, keep_ratio, d);
+    return rc ? rc : pose_submit(e, parser, true, nullptr, nullptr, nullptr, d.data(), N, ticket, false);
+}
+
+int hp_pose_submit_ppn_frames_interleaved_device(hp_engine* e, hp_ppn* parser, const hp_frame_interleaved* frames, int N, int keep_ratio, int* ticket)
+{
+    std::vector<InterleavedFrameDesc> d;
+    const int rc = interleaved_frame_descs(e, frames, N, keep_ratio, d);
+    return rc ? rc : pose_submit(e, parser, true, nullptr, nullptr, nullptr, d.data(), N, ticket, true);
 }
 
 // test hook: the first N resized network-size frames of ticket `ticket` (in flight or collected)

@@ -344,6 +344,35 @@ int hp_pose_submit_pifpaf_frames_yuv420_host(hp_engine* e, hp_pifpaf* decoder, c
 int hp_pose_submit_pifpaf_frames_yuv420_device(hp_engine* e, hp_pifpaf* decoder, const hp_frame_yuv420* frames, int N, int keep_ratio, int* ticket);
 int hp_pose_submit_ppn_frames_yuv420_host(hp_engine* e, hp_ppn* parser, const hp_frame_yuv420* frames, int N, int keep_ratio, int* ticket);
 int hp_pose_submit_ppn_frames_yuv420_device(hp_engine* e, hp_ppn* parser, const hp_frame_yuv420* frames, int N, int keep_ratio, int* ticket);
+/* The same calls for interleaved frames with a row pitch: webcams' YUYV (the V4L2 / UVC default), capture cards' UYVY, YVYU, 4-byte
+ * surfaces (GStreamer BGRx / RGBx, DeepStream's RGBA NvBufSurface, desktop capture's BGRA), RGB (PIL, torchvision, PyAV), gray (IR
+ * and industrial cameras) and BGR, for all three head types.  Each source pixel is converted to BGR as cv::cvtColor does --
+ * COLOR_RGB2BGR, _BGRA2BGR, _RGBA2BGR (alpha / x ignored), _GRAY2BGR (replicated), _YUV2BGR_YUYV / _UYVY / _YVYU (one U, V pair per
+ * 2x1 pixel pair, BT.601 limited range in OpenCV's 20-bit fixed point, as the 4:2:0 calls) -- inside the batched resize's fetch,
+ * before any interpolation: the network-size frame is byte-identical to cv::resize(cv::cvtColor(src, code), ...) (or
+ * non_scaling_resize of it), the regime chosen from the pixel size as for hp_frame_u8.  HP_PIX_BGR with pitch = 3 * width is the
+ * hp_frame_u8 call.  The frames of a batch may mix formats and sizes.  N > max_batch is HP_ERR_BATCH.  HP_ERR_ARG, before anything
+ * is enqueued: a null data, a height or width <= 0, an unknown format, a 4:2:2 frame of odd width, pitch < width * bytes per pixel.
+ * _host: each frame is copied row-compacted (width * bytes per pixel per row: 2 for 4:2:2, 1 for gray), by a pitched DMA from
+ * page-locked frames (keep them alive until collect), through pinned staging from pageable ones before submit returns.  _device: the
+ * frames are read in place with their pitch (a cudaMallocPitch / NvBufSurface / cropped surface as it stands) and must stay valid and
+ * unchanged until the ticket is collected; the bytes between a row's end and the pitch are never read. */
+typedef enum hp_pixel_format {
+    HP_PIX_BGR = 0, HP_PIX_RGB, HP_PIX_BGRA, HP_PIX_RGBA, HP_PIX_GRAY,   /* 3, 3, 4, 4, 1 bytes per pixel */
+    HP_PIX_YUYV, HP_PIX_UYVY, HP_PIX_YVYU                               /* 4:2:2, 2 bytes per pixel: Y0 U Y1 V, U Y0 V Y1, Y0 V Y1 U */
+} hp_pixel_format;
+typedef struct hp_frame_interleaved {
+    const uint8_t* data;
+    int32_t height, width;
+    int32_t pitch;    /* bytes from one row to the next */
+    int32_t format;   /* hp_pixel_format */
+} hp_frame_interleaved;
+int hp_pose_submit_frames_interleaved_host(hp_engine* e, hp_paf* parser, const hp_frame_interleaved* frames, int N, int keep_ratio, int* ticket);
+int hp_pose_submit_frames_interleaved_device(hp_engine* e, hp_paf* parser, const hp_frame_interleaved* frames, int N, int keep_ratio, int* ticket);
+int hp_pose_submit_pifpaf_frames_interleaved_host(hp_engine* e, hp_pifpaf* decoder, const hp_frame_interleaved* frames, int N, int keep_ratio, int* ticket);
+int hp_pose_submit_pifpaf_frames_interleaved_device(hp_engine* e, hp_pifpaf* decoder, const hp_frame_interleaved* frames, int N, int keep_ratio, int* ticket);
+int hp_pose_submit_ppn_frames_interleaved_host(hp_engine* e, hp_ppn* parser, const hp_frame_interleaved* frames, int N, int keep_ratio, int* ticket);
+int hp_pose_submit_ppn_frames_interleaved_device(hp_engine* e, hp_ppn* parser, const hp_frame_interleaved* frames, int N, int keep_ratio, int* ticket);
 /* test hook: the first N resized network-size frames [N,in_h,in_w,3] of an in-flight or collected ticket */
 int hp_pose_debug_read_slot_frames(hp_engine* e, int ticket, uint8_t* out, int N);
 int hp_pifpaf_pipeline_info(hp_pifpaf* p, void** stream, void** inputs_free_event, int* hcap);
