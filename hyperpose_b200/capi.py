@@ -221,7 +221,8 @@ EXPORTS += [
     "hp_pose_submit_frames_interleaved_host", "hp_pose_submit_frames_interleaved_device", "hp_pose_submit_pifpaf_frames_interleaved_host",
     "hp_pose_submit_pifpaf_frames_interleaved_device", "hp_pose_submit_ppn_frames_interleaved_host",
     "hp_pose_submit_ppn_frames_interleaved_device",
-]
+] + [f"hp_pose_submit{head}_frames_{fmt}_rotated_{where}" for head in ("", "_pifpaf", "_ppn") for fmt in ("yuv420", "interleaved")
+     for where in ("host", "device")]
 
 
 class FrameU8(C.Structure):
@@ -263,6 +264,26 @@ PIXEL_CHANNELS = {"bgr": 3, "rgb": 3, "bgra": 4, "rgba": 4, "gray": None, "yuyv"
 def interleaved_record(frame: np.ndarray, fmt: str) -> FrameInterleaved:
     """the FrameInterleaved of a host frame: uint8 (H, W, C) or (H, W) for gray, each row's bytes contiguous; the pitch is strides[0]"""
     return FrameInterleaved(frame.ctypes.data, frame.shape[0], frame.shape[1], frame.strides[0], PIXEL_FORMATS[fmt])
+
+
+# cv::rotate's clockwise rotations, in degrees: ROTATE_90_CLOCKWISE, ROTATE_180, ROTATE_90_COUNTERCLOCKWISE, and upright
+ROTATIONS = (0, 90, 180, 270)
+
+
+def rotation_table(rotation, n: int):
+    """the int32[n] per-frame clockwise degrees of the _rotated_ calls, from one int for the whole batch or one per frame; anything else,
+    or a value outside ROTATIONS, is refused before the library is called"""
+    rots = None
+    if isinstance(rotation, (int, np.integer)):
+        rots = [rotation] * n
+    elif isinstance(rotation, (list, tuple, np.ndarray)):
+        rots = list(rotation)
+    if rots is None or len(rots) != n:
+        raise HyperposeError(HP_ERR_ARG, f"rotation {rotation!r}: expected one of {ROTATIONS} degrees, or one per frame ({n})")
+    for i, r in enumerate(rots):
+        if isinstance(r, (bool, np.bool_)) or not isinstance(r, (int, np.integer)) or int(r) not in ROTATIONS:
+            raise HyperposeError(HP_ERR_ARG, f"frame {i}: rotation {r!r} is not one of {ROTATIONS} clockwise degrees")
+    return (C.c_int32 * n)(*[int(r) for r in rots])
 
 
 def _bind_engine(L):
@@ -317,6 +338,11 @@ def _bind_engine(L):
               L.hp_pose_submit_pifpaf_frames_interleaved_host, L.hp_pose_submit_pifpaf_frames_interleaved_device,
               L.hp_pose_submit_ppn_frames_interleaved_host, L.hp_pose_submit_ppn_frames_interleaved_device):
         f.argtypes = [vp, vp, C.POINTER(FrameInterleaved), C.c_int, C.c_int, ip]
+    for head in ("", "_pifpaf", "_ppn"):
+        for fmt, rec in (("yuv420", FrameYUV420), ("interleaved", FrameInterleaved)):
+            for where in ("host", "device"):
+                getattr(L, f"hp_pose_submit{head}_frames_{fmt}_rotated_{where}").argtypes = \
+                    [vp, vp, C.POINTER(rec), C.POINTER(C.c_int32), C.c_int, C.c_int, ip]
     L.hp_pose_submit_ppn_u8_host.argtypes = [vp, vp, vp, C.c_int, ip]
     L.hp_pose_submit_ppn_u8_device.argtypes = [vp, vp, vp, C.c_int, ip]
     L.hp_pose_debug_read_slot_frames.argtypes = [vp, C.c_int, vp, C.c_int]
@@ -572,12 +598,18 @@ class Engine:
         self._ticket_n[t.value] = n
         return t.value
 
-    def _submit_frame_table(self, parser, table, keep_ratio, device: bool, fmt: str = "u8") -> int:
-        """hp_pose_submit{,_pifpaf,_ppn}_frames_{fmt}_{host,device}, chosen by the parser's type"""
+    def _submit_frame_table(self, parser, table, keep_ratio, device: bool, fmt: str = "u8", rotation=None) -> int:
+        """hp_pose_submit{,_pifpaf,_ppn}_frames_{fmt}_{host,device}, chosen by the parser's type; with a rotation table (rotation_table)
+        the _rotated_ form"""
         t = C.c_int(-1)
         head = "_pifpaf" if isinstance(parser, PifPafParser) else "_ppn" if isinstance(parser, PoseProposalParser) else ""
-        fn = getattr(lib(), f"hp_pose_submit{head}_frames_{fmt}_{'device' if device else 'host'}")
-        check(fn(self._h, parser._h, table, len(table), 1 if keep_ratio else 0, C.byref(t)))
+        where = "device" if device else "host"
+        if rotation is None:
+            fn = getattr(lib(), f"hp_pose_submit{head}_frames_{fmt}_{where}")
+            check(fn(self._h, parser._h, table, len(table), 1 if keep_ratio else 0, C.byref(t)))
+        else:
+            fn = getattr(lib(), f"hp_pose_submit{head}_frames_{fmt}_rotated_{where}")
+            check(fn(self._h, parser._h, table, rotation, len(table), 1 if keep_ratio else 0, C.byref(t)))
         self._ticket_n = getattr(self, "_ticket_n", {})
         self._ticket_n[t.value] = len(table)
         return t.value
@@ -604,11 +636,13 @@ class Engine:
         table = (FrameU8 * len(frames))(*[FrameU8(int(p), int(h), int(w)) for p, h, w in frames])
         return self._submit_frame_table(parser, table, keep_ratio, device=True)
 
-    def submit_pose_yuv420(self, parser, frames, layout, keep_ratio: bool = False) -> int:
+    def submit_pose_yuv420(self, parser, frames, layout, keep_ratio: bool = False, rotation=None) -> int:
         """hp_pose_submit{,_pifpaf,_ppn}_frames_yuv420_host, by the parser's type: a list of YUV 4:2:0 frames, each uint8 (3H/2, W) in
         cv2's packed layout for `layout` (nv12, nv21, i420 or yv12; or a list of those, one per frame), converted as cv::cvtColor does
         and resized on the GPU as submit_pose_frames resizes BGR frames; returns the ticket for collect_pose.  Page-locked frames are
-        kept referenced until the ticket is collected."""
+        kept referenced until the ticket is collected.  rotation: clockwise degrees (0, 90, 180, 270), one for the batch or one per
+        frame, applied as cv::rotate after the conversion (the _rotated_ call); None: upright."""
+        rot = {} if rotation is None else {"rotation": rotation_table(rotation, len(frames))}
         layouts = [layout] * len(frames) if isinstance(layout, str) else list(layout)
         if len(layouts) != len(frames) or any(lay not in YUV420_LAYOUTS for lay in layouts):
             raise HyperposeError(HP_ERR_ARG, f"layout {layout!r}: expected one of {sorted(YUV420_LAYOUTS)}, or one per frame")
@@ -618,27 +652,29 @@ class Engine:
                                                  f"{getattr(f, 'dtype', type(f).__name__)} {getattr(f, 'shape', '')}")
         frames = [np.ascontiguousarray(f) for f in frames]
         table = (FrameYUV420 * len(frames))(*[yuv420_record(f, lay) for f, lay in zip(frames, layouts)])
-        t = self._submit_frame_table(parser, table, keep_ratio, device=False, fmt="yuv420")
+        t = self._submit_frame_table(parser, table, keep_ratio, device=False, fmt="yuv420", **rot)
         self._ticket_frames = getattr(self, "_ticket_frames", {})
         self._ticket_frames[t] = frames
         return t
 
-    def submit_pose_yuv420_device(self, parser, frames, keep_ratio: bool = False) -> int:
+    def submit_pose_yuv420_device(self, parser, frames, keep_ratio: bool = False, rotation=None) -> int:
         """the same for YUV 4:2:0 frames in device memory, given as FrameYUV420 records (device plane pointers and pitches, e.g. an
         NVDEC surface).  The resize kernel reads them in place: they must stay valid and unchanged until the ticket is collected."""
+        rot = {} if rotation is None else {"rotation": rotation_table(rotation, len(frames))}
         for i, f in enumerate(frames):
             if not isinstance(f, FrameYUV420):
                 raise HyperposeError(HP_ERR_ARG, f"frame {i}: expected a FrameYUV420, got {type(f).__name__}")
         table = (FrameYUV420 * len(frames))(*frames)
-        return self._submit_frame_table(parser, table, keep_ratio, device=True, fmt="yuv420")
+        return self._submit_frame_table(parser, table, keep_ratio, device=True, fmt="yuv420", **rot)
 
-    def submit_pose_interleaved(self, parser, frames, format, keep_ratio: bool = False) -> int:
+    def submit_pose_interleaved(self, parser, frames, format, keep_ratio: bool = False, rotation=None) -> int:
         """hp_pose_submit{,_pifpaf,_ppn}_frames_interleaved_host, by the parser's type: a list of uint8 frames, (H, W, 3) for bgr / rgb,
         (H, W, 4) for bgra / rgba, (H, W) for gray, (H, W, 2) for yuyv / uyvy / yvyu; `format` is one of those names or a list of them,
         one per frame.  Each frame is converted as cv::cvtColor(..., COLOR_<format>2BGR) does and resized on the GPU as
         submit_pose_frames resizes BGR frames; returns the ticket for collect_pose.  A frame whose rows are contiguous but strided (a
         crop view of a larger frame) is passed with strides[0] as its pitch, not copied.  Page-locked frames are kept referenced until
-        the ticket is collected."""
+        the ticket is collected.  rotation as for submit_pose_yuv420."""
+        rot = {} if rotation is None else {"rotation": rotation_table(rotation, len(frames))}
         formats = [format] * len(frames) if isinstance(format, str) else list(format)
         if len(formats) != len(frames) or any(fmt not in PIXEL_FORMATS for fmt in formats):
             raise HyperposeError(HP_ERR_ARG, f"format {format!r}: expected one of {sorted(PIXEL_FORMATS)}, or one per frame")
@@ -653,20 +689,21 @@ class Engine:
                 raise HyperposeError(HP_ERR_ARG, f"frame {i}: the bytes of each row must be contiguous, rows at least {row} bytes apart "
                                                  f"(strides {f.strides})")
         table = (FrameInterleaved * len(frames))(*[interleaved_record(f, fmt) for f, fmt in zip(frames, formats)])
-        t = self._submit_frame_table(parser, table, keep_ratio, device=False, fmt="interleaved")
+        t = self._submit_frame_table(parser, table, keep_ratio, device=False, fmt="interleaved", **rot)
         self._ticket_frames = getattr(self, "_ticket_frames", {})
         self._ticket_frames[t] = list(frames)
         return t
 
-    def submit_pose_interleaved_device(self, parser, frames, keep_ratio: bool = False) -> int:
+    def submit_pose_interleaved_device(self, parser, frames, keep_ratio: bool = False, rotation=None) -> int:
         """the same for interleaved frames in device memory, given as FrameInterleaved records (device pointer, size, pitch, format:
         a cudaMallocPitch allocation, an NvBufSurface, a crop of either).  The resize kernel reads them in place: they must stay valid
         and unchanged until the ticket is collected."""
+        rot = {} if rotation is None else {"rotation": rotation_table(rotation, len(frames))}
         for i, f in enumerate(frames):
             if not isinstance(f, FrameInterleaved):
                 raise HyperposeError(HP_ERR_ARG, f"frame {i}: expected a FrameInterleaved, got {type(f).__name__}")
         table = (FrameInterleaved * len(frames))(*frames)
-        return self._submit_frame_table(parser, table, keep_ratio, device=True, fmt="interleaved")
+        return self._submit_frame_table(parser, table, keep_ratio, device=True, fmt="interleaved", **rot)
 
     def debug_read_slot_frames(self, ticket: int, n: int) -> np.ndarray:
         """the first n resized network-size frames u8[n,in_h,in_w,3] of a ticket in flight or collected"""

@@ -114,7 +114,8 @@ struct YuvFrameDesc {
     int mode;                      // RZ_*
     int pitch_y, pitch_uv;         // bytes from one row to the next
     int uv_step;                   // bytes from one chroma sample to the next: 2 semi-planar, 1 planar
-    int pad[2];
+    int rot;                       // clockwise degrees: 0, 90, 180, 270 (read only by the rotated instantiation)
+    int pad;
 };
 static_assert(sizeof(YuvFrameDesc) == 64, "YuvFrameDesc is uploaded as raw bytes");
 
@@ -127,7 +128,7 @@ struct InterleavedFrameDesc {
     int mode;       // RZ_*
     int pitch;      // bytes from one row to the next
     int format;     // hp_pixel_format
-    int pad;
+    int rot;        // clockwise degrees: 0, 90, 180, 270 (read only by the rotated instantiation)
 };
 static_assert(sizeof(InterleavedFrameDesc) == 40, "InterleavedFrameDesc is uploaded as raw bytes");
 
@@ -193,6 +194,34 @@ __device__ __forceinline__ InterleavedRow src_row(const InterleavedFrameDesc& d,
 {
     return InterleavedRow{ d.src + (size_t)sy * d.pitch, d.format };
 }
+
+// A stored frame as the resize sees it after cv::rotate by d.rot clockwise degrees: sh, sw are the rotated size (which the regime,
+// scales and rh / rw were chosen from), and a rotated row is a row (180) or a column (90, 270) of the stored frame.  Each fetch maps
+// (rotated x, rotated y) to stored coordinates and reads there through the stored frame's own row fetch, so a 4:2:0 pixel keeps the
+// chroma of its 2x2 block and a 4:2:2 pixel the U, V pair of its pixel pair in the stored grid: cvtColor first, then rotate.
+template <class Desc>
+struct RotatedFrame {
+    const Desc& f;
+    int sh, sw, rh, rw, mode;
+    __device__ __forceinline__ explicit RotatedFrame(const Desc& d)
+        : f(d), sh(d.rot % 180 ? d.sw : d.sh), sw(d.rot % 180 ? d.sh : d.sw), rh(d.rh), rw(d.rw), mode(d.mode) {}
+};
+template <class Desc>
+struct RotatedRow {
+    const Desc& f;
+    int ry, sh, sw;   // rotated row and rotated size
+    __device__ __forceinline__ int px(int rx, int c) const
+    {
+        int x = rx, y = ry;   // ROTATE_90_CLOCKWISE: dst(y, x) = src(H-1-x, y); ROTATE_180; ROTATE_90_COUNTERCLOCKWISE: src(x, W-1-y)
+        if (f.rot == 90) { x = ry; y = sw - 1 - rx; }
+        else if (f.rot == 180) { x = sw - 1 - rx; y = sh - 1 - ry; }
+        else if (f.rot == 270) { x = sh - 1 - ry; y = rx; }
+        return src_row(f, y).px(x, c);
+    }
+    __device__ __forceinline__ int byte(int b) const { const int x = b / 3; return px(x, b - 3 * x); }
+};
+template <class Desc>
+__device__ __forceinline__ RotatedRow<Desc> src_row(const RotatedFrame<Desc>& d, int ry) { return RotatedRow<Desc>{ d.f, ry, d.sh, d.sw }; }
 
 // cv::resize(INTER_LINEAR) on CV_8UC3 frames (src/tensorrt.cpp:451) for the N frames of a batch in one launch, each frame read
 // through its own descriptor (blockIdx.y), RZ_ROWS destination rows per CTA (blockIdx.x).  OpenCV's 11-bit fixed-point bilinear:
@@ -265,20 +294,25 @@ __global__ void __launch_bounds__(256) resize_frames_u8c3_kernel(const FrameDesc
 
 // YUV 4:2:0 frames (hp_frame_yuv420): the conversion is fused into the fetch, so nothing is ever interpolated in YUV.  Two rows of
 // three plane pointers need more than the 32 registers of 8 CTAs per SM: 6 CTAs leave it 40, with no spills.
+// kRotated: the instantiation launched for a batch with a rotated frame (RotatedFrame), so upright batches keep their code.
+template <bool kRotated>
 __global__ void __launch_bounds__(256, 6) resize_frames_yuv420_kernel(const YuvFrameDesc* __restrict__ desc, uint8_t* __restrict__ dst, int dh, int dw)
 {
     const YuvFrameDesc d = desc[blockIdx.y];
-    resize_frames(d, dst, dh, dw);
+    if constexpr (kRotated) resize_frames(RotatedFrame<YuvFrameDesc>(d), dst, dh, dw);
+    else resize_frames(d, dst, dh, dw);
 }
 
 // interleaved frames with a row pitch (hp_frame_interleaved): the conversion is fused into the fetch as for YUV 4:2:0 frames; one
 // launch may mix formats, each CTA serving one frame.  One row pointer and the format per source row fit the 32 registers of 8 CTAs
-// per SM with no spills.
+// per SM with no spills.  kRotated as for YUV 4:2:0 frames.
+template <bool kRotated>
 __global__ void __launch_bounds__(256, 8) resize_frames_interleaved_kernel(const InterleavedFrameDesc* __restrict__ desc,
                                                                            uint8_t* __restrict__ dst, int dh, int dw)
 {
     const InterleavedFrameDesc d = desc[blockIdx.y];
-    resize_frames(d, dst, dh, dw);
+    if constexpr (kRotated) resize_frames(RotatedFrame<InterleavedFrameDesc>(d), dst, dh, dw);
+    else resize_frames(d, dst, dh, dw);
 }
 
 // depthwise KxK conv (K in {1,3}) + bias + PReLU on fp16 NHWC, 8 channels per thread (one 16-byte load per tap),
@@ -2091,19 +2125,22 @@ static int launch_resize(hp_engine* e, const FrameDesc* d_desc, uint8_t* dst, in
     return HP_OK;
 }
 
-static int launch_resize_yuv(hp_engine* e, const YuvFrameDesc* d_desc, uint8_t* dst, int N)
+// rotated: some frame of the batch has a rotation (the rotated instantiation serves the upright frames of such a batch too)
+static int launch_resize_yuv(hp_engine* e, const YuvFrameDesc* d_desc, uint8_t* dst, int N, bool rotated)
 {
     const dim3 grid((e->in_h + RZ_ROWS - 1) / RZ_ROWS, N);
-    resize_frames_yuv420_kernel<<<grid, 256, (size_t)e->in_w * sizeof(int2), e->stream>>>(d_desc, dst, e->in_h, e->in_w);
+    const auto kernel = rotated ? resize_frames_yuv420_kernel<true> : resize_frames_yuv420_kernel<false>;
+    kernel<<<grid, 256, (size_t)e->in_w * sizeof(int2), e->stream>>>(d_desc, dst, e->in_h, e->in_w);
     e->launches++;
     HP_CUDA_TRY(cudaGetLastError());
     return HP_OK;
 }
 
-static int launch_resize_interleaved(hp_engine* e, const InterleavedFrameDesc* d_desc, uint8_t* dst, int N)
+static int launch_resize_interleaved(hp_engine* e, const InterleavedFrameDesc* d_desc, uint8_t* dst, int N, bool rotated)
 {
     const dim3 grid((e->in_h + RZ_ROWS - 1) / RZ_ROWS, N);
-    resize_frames_interleaved_kernel<<<grid, 256, (size_t)e->in_w * sizeof(int2), e->stream>>>(d_desc, dst, e->in_h, e->in_w);
+    const auto kernel = rotated ? resize_frames_interleaved_kernel<true> : resize_frames_interleaved_kernel<false>;
+    kernel<<<grid, 256, (size_t)e->in_w * sizeof(int2), e->stream>>>(d_desc, dst, e->in_h, e->in_w);
     e->launches++;
     HP_CUDA_TRY(cudaGetLastError());
     return HP_OK;
@@ -2729,7 +2766,7 @@ int slot_upload_yuv(hp_engine* e, hp_engine::PoseSlot& sl, YuvFrameDesc* descs, 
     HP_CUDA_TRY(cudaMemcpyAsync(sl.d_ydesc, sl.pin_ydesc, N * sizeof(YuvFrameDesc), cudaMemcpyHostToDevice, e->copy_stream));
     HP_CUDA_TRY(cudaEventRecord(sl.h2d_done, e->copy_stream));
     HP_CUDA_TRY(cudaStreamWaitEvent(e->stream, sl.h2d_done, 0));
-    return launch_resize_yuv(e, sl.d_ydesc, sl.d_frames, N);
+    return launch_resize_yuv(e, sl.d_ydesc, sl.d_frames, N, std::any_of(descs, descs + N, [](const YuvFrameDesc& d) { return d.rot != 0; }));
 }
 
 // bytes per pixel of an hp_pixel_format, 0 for an unknown one
@@ -2771,7 +2808,8 @@ int slot_upload_interleaved(hp_engine* e, hp_engine::PoseSlot& sl, InterleavedFr
     HP_CUDA_TRY(cudaMemcpyAsync(sl.d_idesc, sl.pin_idesc, N * sizeof(InterleavedFrameDesc), cudaMemcpyHostToDevice, e->copy_stream));
     HP_CUDA_TRY(cudaEventRecord(sl.h2d_done, e->copy_stream));
     HP_CUDA_TRY(cudaStreamWaitEvent(e->stream, sl.h2d_done, 0));
-    return launch_resize_interleaved(e, sl.d_idesc, sl.d_frames, N);
+    return launch_resize_interleaved(e, sl.d_idesc, sl.d_frames, N,
+                                     std::any_of(descs, descs + N, [](const InterleavedFrameDesc& d) { return d.rot != 0; }));
 }
 
 // a submitted batch into the slot's device buffer: network-size frames, or frames of any size (BGR descs, YUV 4:2:0 ydescs or
@@ -3035,77 +3073,122 @@ int hp_pose_submit_ppn_frames_u8_device(hp_engine* e, hp_ppn* parser, const hp_f
     return rc ? rc : pose_submit(e, parser, true, nullptr, d.data(), nullptr, nullptr, N, ticket, true);
 }
 
-// the resize descriptors of a YUV 4:2:0 frame list, refused before any work is enqueued; the regime comes from the luma size
-static int yuv_frame_descs(const hp_engine* e, const hp_frame_yuv420* frames, int N, int keep_ratio, std::vector<YuvFrameDesc>& descs)
+// cv::rotate's clockwise rotations: ROTATE_90_CLOCKWISE, ROTATE_180, ROTATE_90_COUNTERCLOCKWISE, and upright
+static bool valid_rotation(int r) { return r == 0 || r == 90 || r == 180 || r == 270; }
+
+// the resize descriptors of a YUV 4:2:0 frame list, refused before any work is enqueued; the regime comes from the luma size after the
+// frame's rotation (rotation NULL: every frame upright)
+static int yuv_frame_descs(const hp_engine* e, const hp_frame_yuv420* frames, const int32_t* rotation, int N, int keep_ratio,
+                           std::vector<YuvFrameDesc>& descs)
 {
     if (!e || !frames) { set_error("hp_pose_submit_frames_yuv420: null argument"); return HP_ERR_ARG; }
     if (N <= 0 || N > e->max_batch) { set_error("Input batch size overflow: Yours@%d Max@%d", N, e->max_batch); return HP_ERR_BATCH; }
     descs.resize(N);
     for (int f = 0; f < N; ++f) {
         const hp_frame_yuv420& fr = frames[f];
+        const int rot = rotation ? rotation[f] : 0;
         const char* bad = nullptr;
         if (!fr.y || !fr.u || !fr.v) bad = "has a null plane";
         else if (fr.height <= 0 || fr.width <= 0 || (fr.height & 1) || (fr.width & 1)) bad = "has a size that is not positive and even";
         else if (fr.uv_step != 1 && fr.uv_step != 2) bad = "has a uv_step other than 1 (planar) or 2 (semi-planar)";
         else if (fr.pitch_y < fr.width || fr.pitch_uv < fr.width / 2 * fr.uv_step) bad = "has a pitch shorter than its row";
         else if (fr.uv_step == 2 && fr.u - fr.v != 1 && fr.v - fr.u != 1) bad = "is semi-planar but its u and v are not one byte apart";
+        else if (!valid_rotation(rot)) bad = "has a rotation other than 0, 90, 180 or 270 degrees";
         if (bad) {
-            set_error("hp_pose_submit_frames_yuv420: frame %d %s (%dx%d, pitches %d / %d, uv_step %d)", f, bad, fr.height, fr.width,
-                      fr.pitch_y, fr.pitch_uv, fr.uv_step);
+            set_error("hp_pose_submit_frames_yuv420: frame %d %s (%dx%d, pitches %d / %d, uv_step %d, rotation %d)", f, bad, fr.height,
+                      fr.width, fr.pitch_y, fr.pitch_uv, fr.uv_step, rot);
             return HP_ERR_ARG;
         }
         FrameDesc d;
-        const int rc = frame_desc(e, nullptr, fr.height, fr.width, keep_ratio, d);
+        const int rc = frame_desc(e, nullptr, rot % 180 ? fr.width : fr.height, rot % 180 ? fr.height : fr.width, keep_ratio, d);
         if (rc) return rc;
-        descs[f] = YuvFrameDesc{ fr.y, fr.u, fr.v, fr.height, fr.width, d.rh, d.rw, d.mode, fr.pitch_y, fr.pitch_uv, fr.uv_step, { 0, 0 } };
+        descs[f] = YuvFrameDesc{ fr.y, fr.u, fr.v, fr.height, fr.width, d.rh, d.rw, d.mode, fr.pitch_y, fr.pitch_uv, fr.uv_step, rot, 0 };
     }
     return HP_OK;
 }
 
-int hp_pose_submit_frames_yuv420_host(hp_engine* e, hp_paf* parser, const hp_frame_yuv420* frames, int N, int keep_ratio, int* ticket)
+int hp_pose_submit_frames_yuv420_rotated_host(hp_engine* e, hp_paf* parser, const hp_frame_yuv420* frames, const int32_t* rotation, int N,
+                                              int keep_ratio, int* ticket)
 {
     std::vector<YuvFrameDesc> d;
-    const int rc = yuv_frame_descs(e, frames, N, keep_ratio, d);
+    const int rc = yuv_frame_descs(e, frames, rotation, N, keep_ratio, d);
     return rc ? rc : pose_submit(e, parser, false, nullptr, nullptr, d.data(), nullptr, N, ticket, false);
+}
+
+int hp_pose_submit_frames_yuv420_rotated_device(hp_engine* e, hp_paf* parser, const hp_frame_yuv420* frames, const int32_t* rotation, int N,
+                                                int keep_ratio, int* ticket)
+{
+    std::vector<YuvFrameDesc> d;
+    const int rc = yuv_frame_descs(e, frames, rotation, N, keep_ratio, d);
+    return rc ? rc : pose_submit(e, parser, false, nullptr, nullptr, d.data(), nullptr, N, ticket, true);
+}
+
+int hp_pose_submit_pifpaf_frames_yuv420_rotated_host(hp_engine* e, hp_pifpaf* decoder, const hp_frame_yuv420* frames, const int32_t* rotation,
+                                                     int N, int keep_ratio, int* ticket)
+{
+    std::vector<YuvFrameDesc> d;
+    const int rc = yuv_frame_descs(e, frames, rotation, N, keep_ratio, d);
+    return rc ? rc : pose_submit_pifpaf(e, decoder, nullptr, nullptr, d.data(), nullptr, N, ticket, false);
+}
+
+int hp_pose_submit_pifpaf_frames_yuv420_rotated_device(hp_engine* e, hp_pifpaf* decoder, const hp_frame_yuv420* frames, const int32_t* rotation,
+                                                       int N, int keep_ratio, int* ticket)
+{
+    std::vector<YuvFrameDesc> d;
+    const int rc = yuv_frame_descs(e, frames, rotation, N, keep_ratio, d);
+    return rc ? rc : pose_submit_pifpaf(e, decoder, nullptr, nullptr, d.data(), nullptr, N, ticket, true);
+}
+
+int hp_pose_submit_ppn_frames_yuv420_rotated_host(hp_engine* e, hp_ppn* parser, const hp_frame_yuv420* frames, const int32_t* rotation, int N,
+                                                  int keep_ratio, int* ticket)
+{
+    std::vector<YuvFrameDesc> d;
+    const int rc = yuv_frame_descs(e, frames, rotation, N, keep_ratio, d);
+    return rc ? rc : pose_submit(e, parser, true, nullptr, nullptr, d.data(), nullptr, N, ticket, false);
+}
+
+int hp_pose_submit_ppn_frames_yuv420_rotated_device(hp_engine* e, hp_ppn* parser, const hp_frame_yuv420* frames, const int32_t* rotation, int N,
+                                                    int keep_ratio, int* ticket)
+{
+    std::vector<YuvFrameDesc> d;
+    const int rc = yuv_frame_descs(e, frames, rotation, N, keep_ratio, d);
+    return rc ? rc : pose_submit(e, parser, true, nullptr, nullptr, d.data(), nullptr, N, ticket, true);
+}
+
+// the upright calls: the rotated ones with every frame upright
+int hp_pose_submit_frames_yuv420_host(hp_engine* e, hp_paf* parser, const hp_frame_yuv420* frames, int N, int keep_ratio, int* ticket)
+{
+    return hp_pose_submit_frames_yuv420_rotated_host(e, parser, frames, nullptr, N, keep_ratio, ticket);
 }
 
 int hp_pose_submit_frames_yuv420_device(hp_engine* e, hp_paf* parser, const hp_frame_yuv420* frames, int N, int keep_ratio, int* ticket)
 {
-    std::vector<YuvFrameDesc> d;
-    const int rc = yuv_frame_descs(e, frames, N, keep_ratio, d);
-    return rc ? rc : pose_submit(e, parser, false, nullptr, nullptr, d.data(), nullptr, N, ticket, true);
+    return hp_pose_submit_frames_yuv420_rotated_device(e, parser, frames, nullptr, N, keep_ratio, ticket);
 }
 
 int hp_pose_submit_pifpaf_frames_yuv420_host(hp_engine* e, hp_pifpaf* decoder, const hp_frame_yuv420* frames, int N, int keep_ratio, int* ticket)
 {
-    std::vector<YuvFrameDesc> d;
-    const int rc = yuv_frame_descs(e, frames, N, keep_ratio, d);
-    return rc ? rc : pose_submit_pifpaf(e, decoder, nullptr, nullptr, d.data(), nullptr, N, ticket, false);
+    return hp_pose_submit_pifpaf_frames_yuv420_rotated_host(e, decoder, frames, nullptr, N, keep_ratio, ticket);
 }
 
 int hp_pose_submit_pifpaf_frames_yuv420_device(hp_engine* e, hp_pifpaf* decoder, const hp_frame_yuv420* frames, int N, int keep_ratio, int* ticket)
 {
-    std::vector<YuvFrameDesc> d;
-    const int rc = yuv_frame_descs(e, frames, N, keep_ratio, d);
-    return rc ? rc : pose_submit_pifpaf(e, decoder, nullptr, nullptr, d.data(), nullptr, N, ticket, true);
+    return hp_pose_submit_pifpaf_frames_yuv420_rotated_device(e, decoder, frames, nullptr, N, keep_ratio, ticket);
 }
 
 int hp_pose_submit_ppn_frames_yuv420_host(hp_engine* e, hp_ppn* parser, const hp_frame_yuv420* frames, int N, int keep_ratio, int* ticket)
 {
-    std::vector<YuvFrameDesc> d;
-    const int rc = yuv_frame_descs(e, frames, N, keep_ratio, d);
-    return rc ? rc : pose_submit(e, parser, true, nullptr, nullptr, d.data(), nullptr, N, ticket, false);
+    return hp_pose_submit_ppn_frames_yuv420_rotated_host(e, parser, frames, nullptr, N, keep_ratio, ticket);
 }
 
 int hp_pose_submit_ppn_frames_yuv420_device(hp_engine* e, hp_ppn* parser, const hp_frame_yuv420* frames, int N, int keep_ratio, int* ticket)
 {
-    std::vector<YuvFrameDesc> d;
-    const int rc = yuv_frame_descs(e, frames, N, keep_ratio, d);
-    return rc ? rc : pose_submit(e, parser, true, nullptr, nullptr, d.data(), nullptr, N, ticket, true);
+    return hp_pose_submit_ppn_frames_yuv420_rotated_device(e, parser, frames, nullptr, N, keep_ratio, ticket);
 }
 
-// the resize descriptors of an interleaved frame list, refused before any work is enqueued; the regime comes from the pixel size
-static int interleaved_frame_descs(const hp_engine* e, const hp_frame_interleaved* frames, int N, int keep_ratio,
+// the resize descriptors of an interleaved frame list, refused before any work is enqueued; the regime comes from the pixel size after
+// the frame's rotation (rotation NULL: every frame upright)
+static int interleaved_frame_descs(const hp_engine* e, const hp_frame_interleaved* frames, const int32_t* rotation, int N, int keep_ratio,
                                    std::vector<InterleavedFrameDesc>& descs)
 {
     if (!e || !frames) { set_error("hp_pose_submit_frames_interleaved: null argument"); return HP_ERR_ARG; }
@@ -3114,65 +3197,104 @@ static int interleaved_frame_descs(const hp_engine* e, const hp_frame_interleave
     for (int f = 0; f < N; ++f) {
         const hp_frame_interleaved& fr = frames[f];
         const int bpp = pixel_bytes(fr.format);
+        const int rot = rotation ? rotation[f] : 0;
         const char* bad = nullptr;
         if (!fr.data) bad = "is null";
         else if (fr.height <= 0 || fr.width <= 0) bad = "has a size that is not positive";
         else if (!bpp) bad = "has an unknown format";
         else if (bpp == 2 && (fr.width & 1)) bad = "is 4:2:2 of odd width";
         else if ((long long)fr.pitch < (long long)fr.width * bpp) bad = "has a pitch shorter than its row";
+        else if (!valid_rotation(rot)) bad = "has a rotation other than 0, 90, 180 or 270 degrees";
         if (bad) {
-            set_error("hp_pose_submit_frames_interleaved: frame %d %s (%dx%d, pitch %d, format %d)", f, bad, fr.height, fr.width, fr.pitch,
-                      fr.format);
+            set_error("hp_pose_submit_frames_interleaved: frame %d %s (%dx%d, pitch %d, format %d, rotation %d)", f, bad, fr.height, fr.width,
+                      fr.pitch, fr.format, rot);
             return HP_ERR_ARG;
         }
         FrameDesc d;
-        const int rc = frame_desc(e, nullptr, fr.height, fr.width, keep_ratio, d);
+        const int rc = frame_desc(e, nullptr, rot % 180 ? fr.width : fr.height, rot % 180 ? fr.height : fr.width, keep_ratio, d);
         if (rc) return rc;
-        descs[f] = InterleavedFrameDesc{ fr.data, fr.height, fr.width, d.rh, d.rw, d.mode, fr.pitch, fr.format, 0 };
+        descs[f] = InterleavedFrameDesc{ fr.data, fr.height, fr.width, d.rh, d.rw, d.mode, fr.pitch, fr.format, rot };
     }
     return HP_OK;
 }
 
-int hp_pose_submit_frames_interleaved_host(hp_engine* e, hp_paf* parser, const hp_frame_interleaved* frames, int N, int keep_ratio, int* ticket)
+int hp_pose_submit_frames_interleaved_rotated_host(hp_engine* e, hp_paf* parser, const hp_frame_interleaved* frames, const int32_t* rotation,
+                                                   int N, int keep_ratio, int* ticket)
 {
     std::vector<InterleavedFrameDesc> d;
-    const int rc = interleaved_frame_descs(e, frames, N, keep_ratio, d);
+    const int rc = interleaved_frame_descs(e, frames, rotation, N, keep_ratio, d);
     return rc ? rc : pose_submit(e, parser, false, nullptr, nullptr, nullptr, d.data(), N, ticket, false);
+}
+
+int hp_pose_submit_frames_interleaved_rotated_device(hp_engine* e, hp_paf* parser, const hp_frame_interleaved* frames, const int32_t* rotation,
+                                                     int N, int keep_ratio, int* ticket)
+{
+    std::vector<InterleavedFrameDesc> d;
+    const int rc = interleaved_frame_descs(e, frames, rotation, N, keep_ratio, d);
+    return rc ? rc : pose_submit(e, parser, false, nullptr, nullptr, nullptr, d.data(), N, ticket, true);
+}
+
+int hp_pose_submit_pifpaf_frames_interleaved_rotated_host(hp_engine* e, hp_pifpaf* decoder, const hp_frame_interleaved* frames,
+                                                          const int32_t* rotation, int N, int keep_ratio, int* ticket)
+{
+    std::vector<InterleavedFrameDesc> d;
+    const int rc = interleaved_frame_descs(e, frames, rotation, N, keep_ratio, d);
+    return rc ? rc : pose_submit_pifpaf(e, decoder, nullptr, nullptr, nullptr, d.data(), N, ticket, false);
+}
+
+int hp_pose_submit_pifpaf_frames_interleaved_rotated_device(hp_engine* e, hp_pifpaf* decoder, const hp_frame_interleaved* frames,
+                                                            const int32_t* rotation, int N, int keep_ratio, int* ticket)
+{
+    std::vector<InterleavedFrameDesc> d;
+    const int rc = interleaved_frame_descs(e, frames, rotation, N, keep_ratio, d);
+    return rc ? rc : pose_submit_pifpaf(e, decoder, nullptr, nullptr, nullptr, d.data(), N, ticket, true);
+}
+
+int hp_pose_submit_ppn_frames_interleaved_rotated_host(hp_engine* e, hp_ppn* parser, const hp_frame_interleaved* frames, const int32_t* rotation,
+                                                       int N, int keep_ratio, int* ticket)
+{
+    std::vector<InterleavedFrameDesc> d;
+    const int rc = interleaved_frame_descs(e, frames, rotation, N, keep_ratio, d);
+    return rc ? rc : pose_submit(e, parser, true, nullptr, nullptr, nullptr, d.data(), N, ticket, false);
+}
+
+int hp_pose_submit_ppn_frames_interleaved_rotated_device(hp_engine* e, hp_ppn* parser, const hp_frame_interleaved* frames,
+                                                         const int32_t* rotation, int N, int keep_ratio, int* ticket)
+{
+    std::vector<InterleavedFrameDesc> d;
+    const int rc = interleaved_frame_descs(e, frames, rotation, N, keep_ratio, d);
+    return rc ? rc : pose_submit(e, parser, true, nullptr, nullptr, nullptr, d.data(), N, ticket, true);
+}
+
+// the upright calls: the rotated ones with every frame upright
+int hp_pose_submit_frames_interleaved_host(hp_engine* e, hp_paf* parser, const hp_frame_interleaved* frames, int N, int keep_ratio, int* ticket)
+{
+    return hp_pose_submit_frames_interleaved_rotated_host(e, parser, frames, nullptr, N, keep_ratio, ticket);
 }
 
 int hp_pose_submit_frames_interleaved_device(hp_engine* e, hp_paf* parser, const hp_frame_interleaved* frames, int N, int keep_ratio, int* ticket)
 {
-    std::vector<InterleavedFrameDesc> d;
-    const int rc = interleaved_frame_descs(e, frames, N, keep_ratio, d);
-    return rc ? rc : pose_submit(e, parser, false, nullptr, nullptr, nullptr, d.data(), N, ticket, true);
+    return hp_pose_submit_frames_interleaved_rotated_device(e, parser, frames, nullptr, N, keep_ratio, ticket);
 }
 
 int hp_pose_submit_pifpaf_frames_interleaved_host(hp_engine* e, hp_pifpaf* decoder, const hp_frame_interleaved* frames, int N, int keep_ratio, int* ticket)
 {
-    std::vector<InterleavedFrameDesc> d;
-    const int rc = interleaved_frame_descs(e, frames, N, keep_ratio, d);
-    return rc ? rc : pose_submit_pifpaf(e, decoder, nullptr, nullptr, nullptr, d.data(), N, ticket, false);
+    return hp_pose_submit_pifpaf_frames_interleaved_rotated_host(e, decoder, frames, nullptr, N, keep_ratio, ticket);
 }
 
 int hp_pose_submit_pifpaf_frames_interleaved_device(hp_engine* e, hp_pifpaf* decoder, const hp_frame_interleaved* frames, int N, int keep_ratio, int* ticket)
 {
-    std::vector<InterleavedFrameDesc> d;
-    const int rc = interleaved_frame_descs(e, frames, N, keep_ratio, d);
-    return rc ? rc : pose_submit_pifpaf(e, decoder, nullptr, nullptr, nullptr, d.data(), N, ticket, true);
+    return hp_pose_submit_pifpaf_frames_interleaved_rotated_device(e, decoder, frames, nullptr, N, keep_ratio, ticket);
 }
 
 int hp_pose_submit_ppn_frames_interleaved_host(hp_engine* e, hp_ppn* parser, const hp_frame_interleaved* frames, int N, int keep_ratio, int* ticket)
 {
-    std::vector<InterleavedFrameDesc> d;
-    const int rc = interleaved_frame_descs(e, frames, N, keep_ratio, d);
-    return rc ? rc : pose_submit(e, parser, true, nullptr, nullptr, nullptr, d.data(), N, ticket, false);
+    return hp_pose_submit_ppn_frames_interleaved_rotated_host(e, parser, frames, nullptr, N, keep_ratio, ticket);
 }
 
 int hp_pose_submit_ppn_frames_interleaved_device(hp_engine* e, hp_ppn* parser, const hp_frame_interleaved* frames, int N, int keep_ratio, int* ticket)
 {
-    std::vector<InterleavedFrameDesc> d;
-    const int rc = interleaved_frame_descs(e, frames, N, keep_ratio, d);
-    return rc ? rc : pose_submit(e, parser, true, nullptr, nullptr, nullptr, d.data(), N, ticket, true);
+    return hp_pose_submit_ppn_frames_interleaved_rotated_device(e, parser, frames, nullptr, N, keep_ratio, ticket);
 }
 
 // test hook: the first N resized network-size frames of ticket `ticket` (in flight or collected)

@@ -373,6 +373,41 @@ int hp_pose_submit_pifpaf_frames_interleaved_host(hp_engine* e, hp_pifpaf* decod
 int hp_pose_submit_pifpaf_frames_interleaved_device(hp_engine* e, hp_pifpaf* decoder, const hp_frame_interleaved* frames, int N, int keep_ratio, int* ticket);
 int hp_pose_submit_ppn_frames_interleaved_host(hp_engine* e, hp_ppn* parser, const hp_frame_interleaved* frames, int N, int keep_ratio, int* ticket);
 int hp_pose_submit_ppn_frames_interleaved_device(hp_engine* e, hp_ppn* parser, const hp_frame_interleaved* frames, int N, int keep_ratio, int* ticket);
+/* The YUV 4:2:0 and interleaved calls for rotated frames: phone video stored landscape with a rotation in its display matrix, cameras
+ * mounted sideways or upside down.  rotation[f] is frame f's clockwise rotation in degrees: 0, 90 (cv::ROTATE_90_CLOCKWISE), 180
+ * (cv::ROTATE_180) or 270 (cv::ROTATE_90_COUNTERCLOCKWISE); rotation NULL is every frame upright, the calls above.  The network-size
+ * frame is byte-identical to cv::resize(cv::rotate(cv::cvtColor(src, code), rotate_code), ...) (or non_scaling_resize of it): the
+ * conversion happens in the stored grid (a 4:2:0 pixel takes the chroma of its 2x2 block, a 4:2:2 pixel the U, V pair of its pixel
+ * pair, as stored), the rotation is a permutation of the fetch inside the same batched resize (no extra pass, no extra buffer), and
+ * the regime and the letterbox come from the rotated size (height and width swapped for 90 and 270).  The records describe the
+ * rotated frame: they are what the calls above return for the frame rotated beforehand.  A rotation other than 0, 90, 180 or 270 is
+ * HP_ERR_ARG before anything is enqueued, as is everything the calls above refuse.  _host frames are copied in their stored
+ * orientation, as above; _device frames are read in place with their pitch (a rotated NVDEC surface as it stands).  For hp_frame_u8,
+ * use HP_PIX_BGR with pitch = 3 * width. */
+int hp_pose_submit_frames_yuv420_rotated_host(hp_engine* e, hp_paf* parser, const hp_frame_yuv420* frames, const int32_t* rotation, int N,
+                                              int keep_ratio, int* ticket);
+int hp_pose_submit_frames_yuv420_rotated_device(hp_engine* e, hp_paf* parser, const hp_frame_yuv420* frames, const int32_t* rotation, int N,
+                                                int keep_ratio, int* ticket);
+int hp_pose_submit_pifpaf_frames_yuv420_rotated_host(hp_engine* e, hp_pifpaf* decoder, const hp_frame_yuv420* frames, const int32_t* rotation,
+                                                     int N, int keep_ratio, int* ticket);
+int hp_pose_submit_pifpaf_frames_yuv420_rotated_device(hp_engine* e, hp_pifpaf* decoder, const hp_frame_yuv420* frames, const int32_t* rotation,
+                                                       int N, int keep_ratio, int* ticket);
+int hp_pose_submit_ppn_frames_yuv420_rotated_host(hp_engine* e, hp_ppn* parser, const hp_frame_yuv420* frames, const int32_t* rotation, int N,
+                                                  int keep_ratio, int* ticket);
+int hp_pose_submit_ppn_frames_yuv420_rotated_device(hp_engine* e, hp_ppn* parser, const hp_frame_yuv420* frames, const int32_t* rotation, int N,
+                                                    int keep_ratio, int* ticket);
+int hp_pose_submit_frames_interleaved_rotated_host(hp_engine* e, hp_paf* parser, const hp_frame_interleaved* frames, const int32_t* rotation,
+                                                   int N, int keep_ratio, int* ticket);
+int hp_pose_submit_frames_interleaved_rotated_device(hp_engine* e, hp_paf* parser, const hp_frame_interleaved* frames, const int32_t* rotation,
+                                                     int N, int keep_ratio, int* ticket);
+int hp_pose_submit_pifpaf_frames_interleaved_rotated_host(hp_engine* e, hp_pifpaf* decoder, const hp_frame_interleaved* frames,
+                                                          const int32_t* rotation, int N, int keep_ratio, int* ticket);
+int hp_pose_submit_pifpaf_frames_interleaved_rotated_device(hp_engine* e, hp_pifpaf* decoder, const hp_frame_interleaved* frames,
+                                                            const int32_t* rotation, int N, int keep_ratio, int* ticket);
+int hp_pose_submit_ppn_frames_interleaved_rotated_host(hp_engine* e, hp_ppn* parser, const hp_frame_interleaved* frames,
+                                                       const int32_t* rotation, int N, int keep_ratio, int* ticket);
+int hp_pose_submit_ppn_frames_interleaved_rotated_device(hp_engine* e, hp_ppn* parser, const hp_frame_interleaved* frames,
+                                                         const int32_t* rotation, int N, int keep_ratio, int* ticket);
 /* test hook: the first N resized network-size frames [N,in_h,in_w,3] of an in-flight or collected ticket */
 int hp_pose_debug_read_slot_frames(hp_engine* e, int ticket, uint8_t* out, int N);
 int hp_pifpaf_pipeline_info(hp_pifpaf* p, void** stream, void** inputs_free_event, int* hcap);
