@@ -222,7 +222,8 @@ EXPORTS += [
     "hp_pose_submit_pifpaf_frames_interleaved_device", "hp_pose_submit_ppn_frames_interleaved_host",
     "hp_pose_submit_ppn_frames_interleaved_device",
 ] + [f"hp_pose_submit{head}_frames_{fmt}_rotated_{where}" for head in ("", "_pifpaf", "_ppn") for fmt in ("yuv420", "interleaved")
-     for where in ("host", "device")]
+     for where in ("host", "device")] + [f"hp_pose_submit{head}_frames_{fmt}_{where}" for head in ("", "_pifpaf", "_ppn")
+                                         for fmt in ("yuv420_16", "interleaved16") for where in ("host", "device")]
 
 
 class FrameU8(C.Structure):
@@ -264,6 +265,56 @@ PIXEL_CHANNELS = {"bgr": 3, "rgb": 3, "bgra": 4, "rgba": 4, "gray": None, "yuyv"
 def interleaved_record(frame: np.ndarray, fmt: str) -> FrameInterleaved:
     """the FrameInterleaved of a host frame: uint8 (H, W, C) or (H, W) for gray, each row's bytes contiguous; the pitch is strides[0]"""
     return FrameInterleaved(frame.ctypes.data, frame.shape[0], frame.shape[1], frame.strides[0], PIXEL_FORMATS[fmt])
+
+
+class FrameYUV420_16(C.Structure):
+    """hp_frame_yuv420_16: FrameYUV420 with 16-bit samples holding `bits` significant bits, LSB-aligned (9..16; 16 for P010 /
+    P016).  Pitches in bytes, uv_step in samples: 2 semi-planar (P010 / P016: v = u + 1 sample; V first: u = v + 1), 1 planar"""
+    _fields_ = [("y", C.c_void_p), ("u", C.c_void_p), ("v", C.c_void_p), ("height", C.c_int32), ("width", C.c_int32),
+                ("pitch_y", C.c_int32), ("pitch_uv", C.c_int32), ("uv_step", C.c_int32), ("bits", C.c_int32)]
+
+
+# the uint16 (3H/2, W) layouts of submit_pose_yuv420_16, as cv2's packed 8-bit layouts with 16-bit samples: P010 / P016 (U V, NV12's
+# order), the same with V first (NV21's), planar U then V (I420's: yuv420p10le / p12le / p16le) and planar V then U (YV12's)
+YUV420_16_LAYOUTS = {"p016": "nv12", "p016_vu": "nv21", "i420": "i420", "yv12": "yv12"}
+
+
+def yuv420_16_record(frame: np.ndarray, layout: str, bits: int) -> FrameYUV420_16:
+    """the FrameYUV420_16 of a host frame: uint16 (3H/2, W) in a YUV420_16_LAYOUTS layout, C-contiguous"""
+    H, W = frame.shape[0] * 2 // 3, frame.shape[1]
+    u, v, pitch_uv, step = YUV420_LAYOUTS[YUV420_16_LAYOUTS[layout]](H, W)   # in samples
+    p = frame.ctypes.data
+    return FrameYUV420_16(p, p + 2 * u, p + 2 * v, H, W, 2 * W, 2 * pitch_uv, step, bits)
+
+
+class FrameInterleaved16(C.Structure):
+    """hp_frame_interleaved16: FrameInterleaved with 16-bit samples holding `bits` significant bits, LSB-aligned (9..16); `format` is
+    a PIXEL_FORMATS value of bgr, rgb, bgra, rgba or gray (INTERLEAVED16_FORMATS), rows `pitch` bytes apart"""
+    _fields_ = [("data", C.c_void_p), ("height", C.c_int32), ("width", C.c_int32), ("pitch", C.c_int32), ("format", C.c_int32),
+                ("bits", C.c_int32)]
+
+
+# the formats of submit_pose_interleaved16: the 8-bit format each one is, with 16-bit samples
+INTERLEAVED16_FORMATS = {"bgr48": "bgr", "rgb48": "rgb", "bgra64": "bgra", "rgba64": "rgba", "gray16": "gray"}
+
+
+def interleaved16_record(frame: np.ndarray, fmt: str, bits: int) -> FrameInterleaved16:
+    """the FrameInterleaved16 of a host frame: uint16 (H, W, C) or (H, W) for gray16, each row's samples contiguous; the pitch is
+    strides[0]"""
+    return FrameInterleaved16(frame.ctypes.data, frame.shape[0], frame.shape[1], frame.strides[0],
+                              PIXEL_FORMATS[INTERLEAVED16_FORMATS[fmt]], bits)
+
+
+def bits_list(bits, n: int) -> list:
+    """the per-frame significant bits of a 16-bit batch, from one int or one per frame, each 9..16; anything else is refused before
+    the library is called"""
+    bl = [bits] * n if isinstance(bits, (int, np.integer)) else list(bits) if isinstance(bits, (list, tuple, np.ndarray)) else None
+    if bl is None or len(bl) != n:
+        raise HyperposeError(HP_ERR_ARG, f"bits {bits!r}: expected an int in 9..16, or one per frame ({n})")
+    for i, b in enumerate(bl):
+        if isinstance(b, (bool, np.bool_)) or not isinstance(b, (int, np.integer)) or not 9 <= int(b) <= 16:
+            raise HyperposeError(HP_ERR_ARG, f"frame {i}: bits {b!r} is not an int in 9..16")
+    return [int(b) for b in bl]
 
 
 # cv::rotate's clockwise rotations, in degrees: ROTATE_90_CLOCKWISE, ROTATE_180, ROTATE_90_COUNTERCLOCKWISE, and upright
@@ -342,6 +393,10 @@ def _bind_engine(L):
         for fmt, rec in (("yuv420", FrameYUV420), ("interleaved", FrameInterleaved)):
             for where in ("host", "device"):
                 getattr(L, f"hp_pose_submit{head}_frames_{fmt}_rotated_{where}").argtypes = \
+                    [vp, vp, C.POINTER(rec), C.POINTER(C.c_int32), C.c_int, C.c_int, ip]
+        for fmt, rec in (("yuv420_16", FrameYUV420_16), ("interleaved16", FrameInterleaved16)):
+            for where in ("host", "device"):
+                getattr(L, f"hp_pose_submit{head}_frames_{fmt}_{where}").argtypes = \
                     [vp, vp, C.POINTER(rec), C.POINTER(C.c_int32), C.c_int, C.c_int, ip]
     L.hp_pose_submit_ppn_u8_host.argtypes = [vp, vp, vp, C.c_int, ip]
     L.hp_pose_submit_ppn_u8_device.argtypes = [vp, vp, vp, C.c_int, ip]
@@ -600,11 +655,14 @@ class Engine:
 
     def _submit_frame_table(self, parser, table, keep_ratio, device: bool, fmt: str = "u8", rotation=None) -> int:
         """hp_pose_submit{,_pifpaf,_ppn}_frames_{fmt}_{host,device}, chosen by the parser's type; with a rotation table (rotation_table)
-        the _rotated_ form"""
+        the _rotated_ form.  The 16-bit calls (yuv420_16, interleaved16) take the table, or NULL for None, themselves."""
         t = C.c_int(-1)
         head = "_pifpaf" if isinstance(parser, PifPafParser) else "_ppn" if isinstance(parser, PoseProposalParser) else ""
         where = "device" if device else "host"
-        if rotation is None:
+        if fmt in ("yuv420_16", "interleaved16"):
+            fn = getattr(lib(), f"hp_pose_submit{head}_frames_{fmt}_{where}")
+            check(fn(self._h, parser._h, table, rotation, len(table), 1 if keep_ratio else 0, C.byref(t)))
+        elif rotation is None:
             fn = getattr(lib(), f"hp_pose_submit{head}_frames_{fmt}_{where}")
             check(fn(self._h, parser._h, table, len(table), 1 if keep_ratio else 0, C.byref(t)))
         else:
@@ -704,6 +762,74 @@ class Engine:
                 raise HyperposeError(HP_ERR_ARG, f"frame {i}: expected a FrameInterleaved, got {type(f).__name__}")
         table = (FrameInterleaved * len(frames))(*frames)
         return self._submit_frame_table(parser, table, keep_ratio, device=True, fmt="interleaved", **rot)
+
+    def submit_pose_yuv420_16(self, parser, frames, layout, bits, keep_ratio: bool = False, rotation=None) -> int:
+        """hp_pose_submit{,_pifpaf,_ppn}_frames_yuv420_16_host, by the parser's type: submit_pose_yuv420 for YUV 4:2:0 frames of 16-bit
+        samples, each uint16 (3H/2, W) in a YUV420_16_LAYOUTS layout (p016, p016_vu, i420 or yv12; or one per frame).  bits: the
+        significant bits of the samples, LSB-aligned, 9..16, one for the batch or one per frame (16 for P010 / P016, 10 for
+        yuv420p10le).  Each sample is reduced as src.convertTo(CV_8U, 2^-(bits-8)) does, then converted, rotated and resized as by
+        submit_pose_yuv420."""
+        rot = rotation_table(rotation, len(frames)) if rotation is not None else None
+        bl = bits_list(bits, len(frames))
+        layouts = [layout] * len(frames) if isinstance(layout, str) else list(layout)
+        if len(layouts) != len(frames) or any(lay not in YUV420_16_LAYOUTS for lay in layouts):
+            raise HyperposeError(HP_ERR_ARG, f"layout {layout!r}: expected one of {sorted(YUV420_16_LAYOUTS)}, or one per frame")
+        for i, f in enumerate(frames):
+            if not isinstance(f, np.ndarray) or f.dtype != np.uint16 or f.ndim != 2 or f.shape[0] % 3 or f.shape[0] == 0:
+                raise HyperposeError(HP_ERR_ARG, f"frame {i}: expected a uint16 (3H/2, W) YUV 4:2:0 array, got "
+                                                 f"{getattr(f, 'dtype', type(f).__name__)} {getattr(f, 'shape', '')}")
+        frames = [np.ascontiguousarray(f) for f in frames]
+        table = (FrameYUV420_16 * len(frames))(*[yuv420_16_record(f, lay, b) for f, lay, b in zip(frames, layouts, bl)])
+        t = self._submit_frame_table(parser, table, keep_ratio, device=False, fmt="yuv420_16", rotation=rot)
+        self._ticket_frames = getattr(self, "_ticket_frames", {})
+        self._ticket_frames[t] = frames
+        return t
+
+    def submit_pose_yuv420_16_device(self, parser, frames, keep_ratio: bool = False, rotation=None) -> int:
+        """the same for 16-bit YUV 4:2:0 frames in device memory, given as FrameYUV420_16 records, each with its bits (a P010 / P016
+        NVDEC surface).  The resize kernel reads them in place: they must stay valid and unchanged until the ticket is collected."""
+        rot = rotation_table(rotation, len(frames)) if rotation is not None else None
+        for i, f in enumerate(frames):
+            if not isinstance(f, FrameYUV420_16):
+                raise HyperposeError(HP_ERR_ARG, f"frame {i}: expected a FrameYUV420_16, got {type(f).__name__}")
+        table = (FrameYUV420_16 * len(frames))(*frames)
+        return self._submit_frame_table(parser, table, keep_ratio, device=True, fmt="yuv420_16", rotation=rot)
+
+    def submit_pose_interleaved16(self, parser, frames, format, bits, keep_ratio: bool = False, rotation=None) -> int:
+        """hp_pose_submit{,_pifpaf,_ppn}_frames_interleaved16_host, by the parser's type: submit_pose_interleaved for frames of 16-bit
+        samples, uint16 (H, W, 3) for bgr48 / rgb48, (H, W, 4) for bgra64 / rgba64, (H, W) for gray16; `format` is one of those names
+        or one per frame.  bits as for submit_pose_yuv420_16.  A frame whose rows are contiguous but strided is passed with
+        strides[0] as its pitch, not copied."""
+        rot = rotation_table(rotation, len(frames)) if rotation is not None else None
+        bl = bits_list(bits, len(frames))
+        formats = [format] * len(frames) if isinstance(format, str) else list(format)
+        if len(formats) != len(frames) or any(fmt not in INTERLEAVED16_FORMATS for fmt in formats):
+            raise HyperposeError(HP_ERR_ARG, f"format {format!r}: expected one of {sorted(INTERLEAVED16_FORMATS)}, or one per frame")
+        for i, (f, fmt) in enumerate(zip(frames, formats)):
+            ch = PIXEL_CHANNELS[INTERLEAVED16_FORMATS[fmt]]
+            shape = "(H, W)" if ch is None else f"(H, W, {ch})"
+            if not isinstance(f, np.ndarray) or f.dtype != np.uint16 or f.ndim != (2 if ch is None else 3) or (ch and f.shape[2] != ch):
+                raise HyperposeError(HP_ERR_ARG, f"frame {i}: expected a uint16 {shape} {fmt} array, got "
+                                                 f"{getattr(f, 'dtype', type(f).__name__)} {getattr(f, 'shape', '')}")
+            row = 2 * f.shape[1] * (ch or 1)
+            if f.strides[-1] != 2 or (ch and f.strides[1] != 2 * ch) or f.strides[0] < row or f.strides[0] % 2 or f.strides[0] >= 1 << 31:
+                raise HyperposeError(HP_ERR_ARG, f"frame {i}: the samples of each row must be contiguous, rows at least {row} bytes "
+                                                 f"apart (strides {f.strides})")
+        table = (FrameInterleaved16 * len(frames))(*[interleaved16_record(f, fmt, b) for f, fmt, b in zip(frames, formats, bl)])
+        t = self._submit_frame_table(parser, table, keep_ratio, device=False, fmt="interleaved16", rotation=rot)
+        self._ticket_frames = getattr(self, "_ticket_frames", {})
+        self._ticket_frames[t] = list(frames)
+        return t
+
+    def submit_pose_interleaved16_device(self, parser, frames, keep_ratio: bool = False, rotation=None) -> int:
+        """the same for 16-bit interleaved frames in device memory, given as FrameInterleaved16 records, each with its bits.  The
+        resize kernel reads them in place: they must stay valid and unchanged until the ticket is collected."""
+        rot = rotation_table(rotation, len(frames)) if rotation is not None else None
+        for i, f in enumerate(frames):
+            if not isinstance(f, FrameInterleaved16):
+                raise HyperposeError(HP_ERR_ARG, f"frame {i}: expected a FrameInterleaved16, got {type(f).__name__}")
+        table = (FrameInterleaved16 * len(frames))(*frames)
+        return self._submit_frame_table(parser, table, keep_ratio, device=True, fmt="interleaved16", rotation=rot)
 
     def debug_read_slot_frames(self, ticket: int, n: int) -> np.ndarray:
         """the first n resized network-size frames u8[n,in_h,in_w,3] of a ticket in flight or collected"""

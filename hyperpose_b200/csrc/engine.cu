@@ -19,8 +19,10 @@
 #include <string.h>
 
 #include <algorithm>
+#include <initializer_list>
 #include <memory>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "../../include/hyperpose_b200.h"
@@ -132,6 +134,33 @@ struct InterleavedFrameDesc {
 };
 static_assert(sizeof(InterleavedFrameDesc) == 40, "InterleavedFrameDesc is uploaded as raw bytes");
 
+// The same two for frames of 16-bit samples holding `bits` significant bits (hp_frame_yuv420_16, hp_frame_interleaved16): every sample
+// is reduced to a byte (reduce_depth) in the fetch, then converted and resized exactly as its 8-bit counterpart.  Pitches in bytes.
+struct Yuv16FrameDesc {
+    const uint16_t *y, *u, *v;
+    int sh, sw;                    // luma size (both even)
+    int rh, rw;                    // resized region
+    int mode;                      // RZ_*
+    int pitch_y, pitch_uv;         // bytes from one row to the next
+    int uv_step;                   // samples from one chroma sample to the next: 2 semi-planar, 1 planar
+    int rot;                       // clockwise degrees: 0, 90, 180, 270 (read only by the rotated instantiation)
+    int bits;                      // 9..16
+};
+static_assert(sizeof(Yuv16FrameDesc) == 64, "Yuv16FrameDesc is uploaded as raw bytes");
+
+struct Interleaved16FrameDesc {
+    const uint16_t* src;
+    int sh, sw;     // source size
+    int rh, rw;     // resized region
+    int mode;       // RZ_*
+    int pitch;      // bytes from one row to the next
+    int format;     // HP_PIX_BGR, _RGB, _BGRA, _RGBA, _GRAY
+    int rot;        // clockwise degrees: 0, 90, 180, 270 (read only by the rotated instantiation)
+    int bits;       // 9..16
+    int pad;
+};
+static_assert(sizeof(Interleaved16FrameDesc) == 48, "Interleaved16FrameDesc is uploaded as raw bytes");
+
 // Source fetches of the resize: byte c (B, G, R) of source pixel x of one source row.
 struct BgrRow {
     const uint8_t* p;
@@ -193,6 +222,55 @@ struct InterleavedRow {
 __device__ __forceinline__ InterleavedRow src_row(const InterleavedFrameDesc& d, int sy)
 {
     return InterleavedRow{ d.src + (size_t)sy * d.pitch, d.format };
+}
+
+// 2^-(bits - 8), exactly: the scale of cv::Mat::convertTo(CV_8U) from `bits` significant bits
+__device__ __forceinline__ float depth_scale(int bits) { return __int_as_float((127 + 8 - bits) << 23); }
+
+// The byte src.convertTo(dst, CV_8U, 2^-(bits - 8)) makes of a 16-bit sample: saturate(rint_half_even(v * scale)).  The product of an
+// integer below 2^16 and a power of two is exact in fp32, and both roundings are explicit, so no contraction can change the result.
+__device__ __forceinline__ int reduce_depth(int v, float scale) { return min(__float2int_rn(__fmul_rn((float)v, scale)), 255); }
+
+struct Yuv16Row {
+    const uint16_t *y, *u, *v;
+    int step;
+    float scale;
+    __device__ __forceinline__ int px(int x, int c) const
+    {
+        const int k = (x >> 1) * step;
+        return bt601_bgr(reduce_depth(y[x], scale), reduce_depth(u[k], scale), reduce_depth(v[k], scale), c);
+    }
+    __device__ __forceinline__ int byte(int b) const { const int x = b / 3; return px(x, b - 3 * x); }
+};
+__device__ __forceinline__ Yuv16Row src_row(const Yuv16FrameDesc& d, int sy)
+{
+    const size_t c = (size_t)(sy >> 1) * d.pitch_uv;
+    return Yuv16Row{ (const uint16_t*)((const uint8_t*)d.y + (size_t)sy * d.pitch_y), (const uint16_t*)((const uint8_t*)d.u + c),
+                     (const uint16_t*)((const uint8_t*)d.v + c), d.uv_step, depth_scale(d.bits) };
+}
+
+// BGR48, RGB48, BGRA64, RGBA64, GRAY16: the sample InterleavedRow reads as a byte, reduced
+struct Interleaved16Row {
+    const uint16_t* p;
+    int format;
+    float scale;
+    __device__ __forceinline__ int px(int x, int c) const
+    {
+        int i;
+        switch (format) {
+        case HP_PIX_BGR: i = 3 * x + c; break;
+        case HP_PIX_RGB: i = 3 * x + 2 - c; break;
+        case HP_PIX_BGRA: i = 4 * x + c; break;
+        case HP_PIX_RGBA: i = 4 * x + 2 - c; break;
+        default: i = x;   // HP_PIX_GRAY
+        }
+        return reduce_depth(p[i], scale);
+    }
+    __device__ __forceinline__ int byte(int b) const { const int x = b / 3; return px(x, b - 3 * x); }
+};
+__device__ __forceinline__ Interleaved16Row src_row(const Interleaved16FrameDesc& d, int sy)
+{
+    return Interleaved16Row{ (const uint16_t*)((const uint8_t*)d.src + (size_t)sy * d.pitch), d.format, depth_scale(d.bits) };
 }
 
 // A stored frame as the resize sees it after cv::rotate by d.rot clockwise degrees: sh, sw are the rotated size (which the regime,
@@ -312,6 +390,27 @@ __global__ void __launch_bounds__(256, 8) resize_frames_interleaved_kernel(const
 {
     const InterleavedFrameDesc d = desc[blockIdx.y];
     if constexpr (kRotated) resize_frames(RotatedFrame<InterleavedFrameDesc>(d), dst, dh, dw);
+    else resize_frames(d, dst, dh, dw);
+}
+
+// YUV 4:2:0 and interleaved frames of 16-bit samples: their 8-bit kernels with each sample reduced in the fetch (reduce_depth).  The
+// three reductions per 4:2:0 pixel spill at the 40 registers of 6 CTAs per SM: 5 CTAs leave it 48, with no spills.  The interleaved
+// fetch keeps 8 CTAs at 32 registers with no spills.  kRotated as for YUV 4:2:0 frames.
+template <bool kRotated>
+__global__ void __launch_bounds__(256, 5) resize_frames_yuv420_16_kernel(const Yuv16FrameDesc* __restrict__ desc, uint8_t* __restrict__ dst,
+                                                                          int dh, int dw)
+{
+    const Yuv16FrameDesc d = desc[blockIdx.y];
+    if constexpr (kRotated) resize_frames(RotatedFrame<Yuv16FrameDesc>(d), dst, dh, dw);
+    else resize_frames(d, dst, dh, dw);
+}
+
+template <bool kRotated>
+__global__ void __launch_bounds__(256, 8) resize_frames_interleaved16_kernel(const Interleaved16FrameDesc* __restrict__ desc,
+                                                                             uint8_t* __restrict__ dst, int dh, int dw)
+{
+    const Interleaved16FrameDesc d = desc[blockIdx.y];
+    if constexpr (kRotated) resize_frames(RotatedFrame<Interleaved16FrameDesc>(d), dst, dh, dw);
     else resize_frames(d, dst, dh, dw);
 }
 
@@ -991,6 +1090,8 @@ struct hp_engine {
         FrameDesc* d_desc = nullptr; FrameDesc* pin_desc = nullptr;   // [max_batch]
         YuvFrameDesc* d_ydesc = nullptr; YuvFrameDesc* pin_ydesc = nullptr;   // [max_batch] (hp_pose_submit_*frames_yuv420_*)
         InterleavedFrameDesc* d_idesc = nullptr; InterleavedFrameDesc* pin_idesc = nullptr;   // [max_batch] (*frames_interleaved_*)
+        Yuv16FrameDesc* d_y16desc = nullptr; Yuv16FrameDesc* pin_y16desc = nullptr;   // [max_batch] (*frames_yuv420_16_*)
+        Interleaved16FrameDesc* d_i16desc = nullptr; Interleaved16FrameDesc* pin_i16desc = nullptr;   // [max_batch] (*frames_interleaved16_*)
         hp_human* pin_humans = nullptr; size_t pin_humans_n = 0;
         int* pin_counts = nullptr; size_t pin_counts_n = 0;   // [N counts | N flags]
         cudaEvent_t h2d_done = nullptr, done = nullptr;
@@ -1629,6 +1730,10 @@ void free_engine(hp_engine* e)
         if (sl.pin_ydesc) cudaFreeHost(sl.pin_ydesc);
         if (sl.d_idesc) cudaFree(sl.d_idesc);
         if (sl.pin_idesc) cudaFreeHost(sl.pin_idesc);
+        if (sl.d_y16desc) cudaFree(sl.d_y16desc);
+        if (sl.pin_y16desc) cudaFreeHost(sl.pin_y16desc);
+        if (sl.d_i16desc) cudaFree(sl.d_i16desc);
+        if (sl.pin_i16desc) cudaFreeHost(sl.pin_i16desc);
         if (sl.pin_humans) cudaFreeHost(sl.pin_humans);
         if (sl.pin_counts) cudaFreeHost(sl.pin_counts);
         if (sl.h2d_done) cudaEventDestroy(sl.h2d_done);
@@ -2125,26 +2230,34 @@ static int launch_resize(hp_engine* e, const FrameDesc* d_desc, uint8_t* dst, in
     return HP_OK;
 }
 
+extern "C++" {   // overloads and templates, inside the C ABI block
+// the resize kernel of a fused-conversion descriptor type; rotated: the instantiation for a batch with a rotated frame
+static auto resize_kernel(const YuvFrameDesc*, bool rotated) { return rotated ? resize_frames_yuv420_kernel<true> : resize_frames_yuv420_kernel<false>; }
+static auto resize_kernel(const InterleavedFrameDesc*, bool rotated)
+{
+    return rotated ? resize_frames_interleaved_kernel<true> : resize_frames_interleaved_kernel<false>;
+}
+static auto resize_kernel(const Yuv16FrameDesc*, bool rotated)
+{
+    return rotated ? resize_frames_yuv420_16_kernel<true> : resize_frames_yuv420_16_kernel<false>;
+}
+static auto resize_kernel(const Interleaved16FrameDesc*, bool rotated)
+{
+    return rotated ? resize_frames_interleaved16_kernel<true> : resize_frames_interleaved16_kernel<false>;
+}
+
 // rotated: some frame of the batch has a rotation (the rotated instantiation serves the upright frames of such a batch too)
-static int launch_resize_yuv(hp_engine* e, const YuvFrameDesc* d_desc, uint8_t* dst, int N, bool rotated)
+template <class Desc>
+static int launch_resize_fused(hp_engine* e, const Desc* d_desc, uint8_t* dst, int N, bool rotated)
 {
     const dim3 grid((e->in_h + RZ_ROWS - 1) / RZ_ROWS, N);
-    const auto kernel = rotated ? resize_frames_yuv420_kernel<true> : resize_frames_yuv420_kernel<false>;
-    kernel<<<grid, 256, (size_t)e->in_w * sizeof(int2), e->stream>>>(d_desc, dst, e->in_h, e->in_w);
+    resize_kernel(d_desc, rotated)<<<grid, 256, (size_t)e->in_w * sizeof(int2), e->stream>>>(d_desc, dst, e->in_h, e->in_w);
     e->launches++;
     HP_CUDA_TRY(cudaGetLastError());
     return HP_OK;
 }
 
-static int launch_resize_interleaved(hp_engine* e, const InterleavedFrameDesc* d_desc, uint8_t* dst, int N, bool rotated)
-{
-    const dim3 grid((e->in_h + RZ_ROWS - 1) / RZ_ROWS, N);
-    const auto kernel = rotated ? resize_frames_interleaved_kernel<true> : resize_frames_interleaved_kernel<false>;
-    kernel<<<grid, 256, (size_t)e->in_w * sizeof(int2), e->stream>>>(d_desc, dst, e->in_h, e->in_w);
-    e->launches++;
-    HP_CUDA_TRY(cudaGetLastError());
-    return HP_OK;
-}
+}   // extern "C++"
 
 // Stages ONE host frame of arbitrary size into batch slot `slot`: H2D of the original pixels, then the reference's
 // resize step on the GPU -- cv::resize(INTER_LINEAR) or, with keep_ratio, non_scaling_resize (src/tensorrt.cpp:446-451).
@@ -2723,50 +2836,62 @@ int upload_plane(hp_engine* e, hp_engine::PoseSlot& sl, const uint8_t* src, int 
     return HP_OK;
 }
 
-// The same for YUV 4:2:0 frames.  A host frame is copied row-compacted into the slot's source buffer: its luma plane with pitch
-// width, then the interleaved UV plane (semi-planar, copied once) or the U and V planes (planar), 1.5 bytes per pixel.  Each plane goes
-// by a pitched DMA from the caller when it is page-locked, else through the slot's pinned staging.  Device frames are read in place.
-int slot_upload_yuv(hp_engine* e, hp_engine::PoseSlot& sl, YuvFrameDesc* descs, int N, bool device_src)
+// A batch's fused-conversion descriptors to the slot's device array for them (d_desc, allocated here with its pinned twin) on the copy
+// stream, ordered before the engine stream's next work, then the resize launch that reads them.
+template <class Desc>
+int slot_launch_fused(hp_engine* e, hp_engine::PoseSlot& sl, Desc*& d_desc, Desc*& pin_desc, const Desc* descs, int N)
 {
-    if (!sl.d_ydesc) {
-        HP_CUDA_TRY(cudaMalloc(&sl.d_ydesc, e->max_batch * sizeof(YuvFrameDesc)));
-        HP_CUDA_TRY(cudaMallocHost(&sl.pin_ydesc, e->max_batch * sizeof(YuvFrameDesc)));
+    if (!d_desc) {
+        HP_CUDA_TRY(cudaMalloc(&d_desc, e->max_batch * sizeof(Desc)));
+        HP_CUDA_TRY(cudaMallocHost(&pin_desc, e->max_batch * sizeof(Desc)));
     }
+    memcpy(pin_desc, descs, N * sizeof(Desc));
+    HP_CUDA_TRY(cudaMemcpyAsync(d_desc, pin_desc, N * sizeof(Desc), cudaMemcpyHostToDevice, e->copy_stream));
+    HP_CUDA_TRY(cudaEventRecord(sl.h2d_done, e->copy_stream));
+    HP_CUDA_TRY(cudaStreamWaitEvent(e->stream, sl.h2d_done, 0));
+    return launch_resize_fused(e, d_desc, sl.d_frames, N, std::any_of(descs, descs + N, [](const Desc& d) { return d.rot != 0; }));
+}
+
+// The same for YUV 4:2:0 frames (YuvFrameDesc, or Yuv16FrameDesc of 16-bit samples).  A host frame is copied row-compacted into the
+// slot's source buffer: its luma plane with pitch width, then the interleaved UV plane (semi-planar, copied once) or the U and V planes
+// (planar), 1.5 samples per pixel.  Each plane goes by a pitched DMA from the caller when it is page-locked, else through the slot's
+// pinned staging.  Device frames are read in place.
+template <class Desc>
+int slot_upload_yuv(hp_engine* e, hp_engine::PoseSlot& sl, Desc*& d_desc, Desc*& pin_desc, Desc* descs, int N, bool device_src)
+{
+    using Sample = std::remove_pointer_t<decltype(Desc::y)>;   // const uint8_t or const uint16_t
+    constexpr size_t S = sizeof(Sample);
     if (!device_src) {
         std::vector<size_t> off(N + 1, 0);
-        for (int f = 0; f < N; ++f) off[f + 1] = off[f] + (((size_t)descs[f].sh * descs[f].sw * 3 / 2 + 255) & ~(size_t)255);
+        for (int f = 0; f < N; ++f) off[f + 1] = off[f] + (((size_t)descs[f].sh * descs[f].sw * 3 / 2 * S + 255) & ~(size_t)255);
         int rc = slot_src_reserve(sl, off[N]);
         if (rc) return rc;
-        auto copy_plane = [&](const uint8_t* src, int pitch, int rows, int width, size_t at) {
-            return upload_plane(e, sl, src, pitch, rows, width, at, off[N]);
+        auto copy_plane = [&](const Sample* src, int pitch, int rows, int width, size_t at) {
+            return upload_plane(e, sl, (const uint8_t*)src, pitch, rows, width * (int)S, at, off[N]);
         };
         for (int f = 0; f < N; ++f) {
-            YuvFrameDesc& d = descs[f];
-            const size_t luma = (size_t)d.sh * d.sw, at = off[f] + luma;
+            Desc& d = descs[f];
+            const size_t luma = (size_t)d.sh * d.sw * S, at = off[f] + luma;
             if ((rc = copy_plane(d.y, d.pitch_y, d.sh, d.sw, off[f]))) return rc;
             if (d.uv_step == 2) {   // one interleaved plane starting at the lower of u, v
-                const uint8_t* base = d.u < d.v ? d.u : d.v;
+                const Sample* base = d.u < d.v ? d.u : d.v;
                 if ((rc = copy_plane(base, d.pitch_uv, d.sh / 2, d.sw, at))) return rc;
-                d.u = sl.d_src + at + (d.u - base);
-                d.v = sl.d_src + at + (d.v - base);
-                d.pitch_uv = d.sw;
+                d.u = (const Sample*)(sl.d_src + at) + (d.u - base);
+                d.v = (const Sample*)(sl.d_src + at) + (d.v - base);
+                d.pitch_uv = d.sw * S;
             } else {
                 const size_t chroma = luma / 4;
                 if ((rc = copy_plane(d.u, d.pitch_uv, d.sh / 2, d.sw / 2, at))) return rc;
                 if ((rc = copy_plane(d.v, d.pitch_uv, d.sh / 2, d.sw / 2, at + chroma))) return rc;
-                d.u = sl.d_src + at;
-                d.v = sl.d_src + at + chroma;
-                d.pitch_uv = d.sw / 2;
+                d.u = (const Sample*)(sl.d_src + at);
+                d.v = (const Sample*)(sl.d_src + at + chroma);
+                d.pitch_uv = d.sw / 2 * S;
             }
-            d.y = sl.d_src + off[f];
-            d.pitch_y = d.sw;
+            d.y = (const Sample*)(sl.d_src + off[f]);
+            d.pitch_y = d.sw * S;
         }
     }
-    memcpy(sl.pin_ydesc, descs, N * sizeof(YuvFrameDesc));
-    HP_CUDA_TRY(cudaMemcpyAsync(sl.d_ydesc, sl.pin_ydesc, N * sizeof(YuvFrameDesc), cudaMemcpyHostToDevice, e->copy_stream));
-    HP_CUDA_TRY(cudaEventRecord(sl.h2d_done, e->copy_stream));
-    HP_CUDA_TRY(cudaStreamWaitEvent(e->stream, sl.h2d_done, 0));
-    return launch_resize_yuv(e, sl.d_ydesc, sl.d_frames, N, std::any_of(descs, descs + N, [](const YuvFrameDesc& d) { return d.rot != 0; }));
+    return slot_launch_fused(e, sl, d_desc, pin_desc, descs, N);
 }
 
 // bytes per pixel of an hp_pixel_format, 0 for an unknown one
@@ -2781,45 +2906,57 @@ int pixel_bytes(int format)
     }
 }
 
-// The same for interleaved frames.  A host frame is copied row-compacted into the slot's source buffer (width * bytes per pixel per
-// row), by a pitched DMA from the caller when it is page-locked, else through the slot's pinned staging.  Device frames are read in
-// place with their pitch.
-int slot_upload_interleaved(hp_engine* e, hp_engine::PoseSlot& sl, InterleavedFrameDesc* descs, int N, bool device_src)
+// The same for interleaved frames (InterleavedFrameDesc, or Interleaved16FrameDesc of 16-bit samples).  A host frame is copied
+// row-compacted into the slot's source buffer (width * bytes per pixel per row), by a pitched DMA from the caller when it is
+// page-locked, else through the slot's pinned staging.  Device frames are read in place with their pitch.
+template <class Desc>
+int slot_upload_interleaved(hp_engine* e, hp_engine::PoseSlot& sl, Desc*& d_desc, Desc*& pin_desc, Desc* descs, int N, bool device_src)
 {
-    if (!sl.d_idesc) {
-        HP_CUDA_TRY(cudaMalloc(&sl.d_idesc, e->max_batch * sizeof(InterleavedFrameDesc)));
-        HP_CUDA_TRY(cudaMallocHost(&sl.pin_idesc, e->max_batch * sizeof(InterleavedFrameDesc)));
-    }
+    using Sample = std::remove_pointer_t<decltype(Desc::src)>;   // const uint8_t or const uint16_t
+    auto row_bytes = [](const Desc& d) { return d.sw * pixel_bytes(d.format) * (int)sizeof(Sample); };
     if (!device_src) {
         std::vector<size_t> off(N + 1, 0);
-        for (int f = 0; f < N; ++f)
-            off[f + 1] = off[f] + (((size_t)descs[f].sh * descs[f].sw * pixel_bytes(descs[f].format) + 255) & ~(size_t)255);
+        for (int f = 0; f < N; ++f) off[f + 1] = off[f] + (((size_t)descs[f].sh * row_bytes(descs[f]) + 255) & ~(size_t)255);
         int rc = slot_src_reserve(sl, off[N]);
         if (rc) return rc;
         for (int f = 0; f < N; ++f) {
-            InterleavedFrameDesc& d = descs[f];
-            const int row = d.sw * pixel_bytes(d.format);
-            if ((rc = upload_plane(e, sl, d.src, d.pitch, d.sh, row, off[f], off[N]))) return rc;
-            d.src = sl.d_src + off[f];
+            Desc& d = descs[f];
+            const int row = row_bytes(d);
+            if ((rc = upload_plane(e, sl, (const uint8_t*)d.src, d.pitch, d.sh, row, off[f], off[N]))) return rc;
+            d.src = (const Sample*)(sl.d_src + off[f]);
             d.pitch = row;
         }
     }
-    memcpy(sl.pin_idesc, descs, N * sizeof(InterleavedFrameDesc));
-    HP_CUDA_TRY(cudaMemcpyAsync(sl.d_idesc, sl.pin_idesc, N * sizeof(InterleavedFrameDesc), cudaMemcpyHostToDevice, e->copy_stream));
-    HP_CUDA_TRY(cudaEventRecord(sl.h2d_done, e->copy_stream));
-    HP_CUDA_TRY(cudaStreamWaitEvent(e->stream, sl.h2d_done, 0));
-    return launch_resize_interleaved(e, sl.d_idesc, sl.d_frames, N,
-                                     std::any_of(descs, descs + N, [](const InterleavedFrameDesc& d) { return d.rot != 0; }));
+    return slot_launch_fused(e, sl, d_desc, pin_desc, descs, N);
 }
 
-// a submitted batch into the slot's device buffer: network-size frames, or frames of any size (BGR descs, YUV 4:2:0 ydescs or
-// interleaved idescs) resized there
-int slot_upload_batch(hp_engine* e, hp_engine::PoseSlot& sl, const uint8_t* frames, FrameDesc* descs, YuvFrameDesc* ydescs,
-                      InterleavedFrameDesc* idescs, int N, bool device_src)
+// the frames of a submitted batch, one kind set by the constructor: network-size frames, or frames of any size described by resize
+// descriptors (BGR, YUV 4:2:0, interleaved, and the 16-bit YUV 4:2:0 and interleaved ones) whose sources are rewritten to the slot's
+// copies of host frames
+struct BatchFrames {
+    const uint8_t* frames = nullptr;
+    FrameDesc* descs = nullptr;
+    YuvFrameDesc* ydescs = nullptr;
+    InterleavedFrameDesc* idescs = nullptr;
+    Yuv16FrameDesc* y16descs = nullptr;
+    Interleaved16FrameDesc* i16descs = nullptr;
+    BatchFrames(const uint8_t* p) : frames(p) {}
+    BatchFrames(FrameDesc* p) : descs(p) {}
+    BatchFrames(YuvFrameDesc* p) : ydescs(p) {}
+    BatchFrames(InterleavedFrameDesc* p) : idescs(p) {}
+    BatchFrames(Yuv16FrameDesc* p) : y16descs(p) {}
+    BatchFrames(Interleaved16FrameDesc* p) : i16descs(p) {}
+    bool empty() const { return !frames && !descs && !ydescs && !idescs && !y16descs && !i16descs; }
+};
+
+// a submitted batch into the slot's device buffer: network-size frames copied, frames of any size resized there
+int slot_upload_batch(hp_engine* e, hp_engine::PoseSlot& sl, const BatchFrames& b, int N, bool device_src)
 {
-    if (idescs) return slot_upload_interleaved(e, sl, idescs, N, device_src);
-    if (ydescs) return slot_upload_yuv(e, sl, ydescs, N, device_src);
-    return descs ? slot_upload_frames(e, sl, descs, N, device_src) : slot_upload(e, sl, frames, N, device_src);
+    if (b.i16descs) return slot_upload_interleaved(e, sl, sl.d_i16desc, sl.pin_i16desc, b.i16descs, N, device_src);
+    if (b.y16descs) return slot_upload_yuv(e, sl, sl.d_y16desc, sl.pin_y16desc, b.y16descs, N, device_src);
+    if (b.idescs) return slot_upload_interleaved(e, sl, sl.d_idesc, sl.pin_idesc, b.idescs, N, device_src);
+    if (b.ydescs) return slot_upload_yuv(e, sl, sl.d_ydesc, sl.pin_ydesc, b.ydescs, N, device_src);
+    return b.descs ? slot_upload_frames(e, sl, b.descs, N, device_src) : slot_upload(e, sl, b.frames, N, device_src);
 }
 
 // the parser's state a captured graph bakes in (hp_paf_state / hp_ppn_state), and the capacity of records per frame in it
@@ -2916,12 +3053,10 @@ static int pifpaf_enqueue(hp_engine* e, hp_engine::PoseSlot& sl)
     return HP_OK;
 }
 
-// frames: N network-size frames, or -- descs / ydescs / idescs != NULL -- N BGR / YUV 4:2:0 / interleaved frames of any size
-// described by them (their sources are rewritten to the slot's copies of host frames)
-static int pose_submit_pifpaf(hp_engine* e, hp_pifpaf* dec, const uint8_t* frames, FrameDesc* descs, YuvFrameDesc* ydescs,
-                              InterleavedFrameDesc* idescs, int N, int* ticket, bool device_src)
+// frames: the N frames of the batch (BatchFrames)
+static int pose_submit_pifpaf(hp_engine* e, hp_pifpaf* dec, const BatchFrames& frames, int N, int* ticket, bool device_src)
 {
-    if (!e || !dec || (!frames && !descs && !ydescs && !idescs) || !ticket) { set_error("hp_pose_submit_pifpaf: null argument"); return HP_ERR_ARG; }
+    if (!e || !dec || frames.empty() || !ticket) { set_error("hp_pose_submit_pifpaf: null argument"); return HP_ERR_ARG; }
     if (N <= 0 || N > e->max_batch) { set_error("Input batch size overflow: Yours@%d Max@%d", N, e->max_batch); return HP_ERR_BATCH; }
     if (e->hdr.head_type != 1) { set_error("hp_pose_submit_pifpaf: the model pack has no OpenPifPaf heads (head_type %u)", e->hdr.head_type); return HP_ERR_UNSUPPORTED; }
     HP_CUDA_TRY(cudaSetDevice(e->device));
@@ -2931,7 +3066,7 @@ static int pose_submit_pifpaf(hp_engine* e, hp_pifpaf* dec, const uint8_t* frame
     int rc = pifpaf_slot_prepare(e, sl, dec, N);
     if (rc) return rc;
     e->reserve_sms = e->opt.pifpaf_reserve_sms;   // the decoder's growth kernel (one warp per frame) runs underneath the next batch's convolutions
-    rc = slot_upload_batch(e, sl, frames, descs, ydescs, idescs, N, device_src);
+    rc = slot_upload_batch(e, sl, frames, N, device_src);
     if (rc) return rc;
     rc = pifpaf_enqueue(e, sl);
     if (rc) return rc;
@@ -2942,11 +3077,10 @@ static int pose_submit_pifpaf(hp_engine* e, hp_pifpaf* dec, const uint8_t* frame
 }
 
 // the PAF-parser calls (ppn_call false: `parser` is an hp_paf) and the Pose Proposal Network calls (true: an hp_ppn)
-static int pose_submit(hp_engine* e, void* parser, bool ppn_call, const uint8_t* frames, FrameDesc* descs, YuvFrameDesc* ydescs,
-                       InterleavedFrameDesc* idescs, int N, int* ticket, bool device_src)
+static int pose_submit(hp_engine* e, void* parser, bool ppn_call, const BatchFrames& frames, int N, int* ticket, bool device_src)
 {
     const char* fn = ppn_call ? "hp_pose_submit_ppn" : "hp_pose_submit";
-    if (!e || !parser || (!frames && !descs && !ydescs && !idescs) || !ticket) { set_error("%s: null argument", fn); return HP_ERR_ARG; }
+    if (!e || !parser || frames.empty() || !ticket) { set_error("%s: null argument", fn); return HP_ERR_ARG; }
     if (N <= 0 || N > e->max_batch) { set_error("Input batch size overflow: Yours@%d Max@%d", N, e->max_batch); return HP_ERR_BATCH; }
     hp_paf* paf = ppn_call ? nullptr : (hp_paf*)parser;
     hp_ppn* ppn = ppn_call ? (hp_ppn*)parser : nullptr;
@@ -2971,7 +3105,7 @@ static int pose_submit(hp_engine* e, void* parser, bool ppn_call, const uint8_t*
     if (sl.busy) { set_error("%s: two batches are already in flight -- collect ticket %d first", fn, idx); return HP_ERR_ARG; }
     int rc = pose_slot_prepare(e, sl, paf, ppn, N);
     if (rc) return rc;
-    rc = slot_upload_batch(e, sl, frames, descs, ydescs, idescs, N, device_src);   // (the captured graph reads the slot's buffer)
+    rc = slot_upload_batch(e, sl, frames, N, device_src);   // (the captured graph reads the slot's buffer)
     if (rc) return rc;
     rc = pose_launch(e, sl);
     if (rc) return rc;
@@ -2984,23 +3118,23 @@ static int pose_submit(hp_engine* e, void* parser, bool ppn_call, const uint8_t*
 
 int hp_pose_submit_u8_host(hp_engine* e, hp_paf* parser, const uint8_t* frames, int N, int* ticket)
 {
-    return pose_submit(e, parser, false, frames, nullptr, nullptr, nullptr, N, ticket, false);
+    return pose_submit(e, parser, false, frames, N, ticket, false);
 }
 
 // the same with the frames already resident in device memory (what a decoder / capture pipeline on the GPU hands over)
 int hp_pose_submit_u8_device(hp_engine* e, hp_paf* parser, const uint8_t* d_frames, int N, int* ticket)
 {
-    return pose_submit(e, parser, false, d_frames, nullptr, nullptr, nullptr, N, ticket, true);
+    return pose_submit(e, parser, false, d_frames, N, ticket, true);
 }
 
 int hp_pose_submit_pifpaf_u8_host(hp_engine* e, hp_pifpaf* decoder, const uint8_t* frames, int N, int* ticket)
 {
-    return pose_submit_pifpaf(e, decoder, frames, nullptr, nullptr, nullptr, N, ticket, false);
+    return pose_submit_pifpaf(e, decoder, frames, N, ticket, false);
 }
 
 int hp_pose_submit_pifpaf_u8_device(hp_engine* e, hp_pifpaf* decoder, const uint8_t* d_frames, int N, int* ticket)
 {
-    return pose_submit_pifpaf(e, decoder, d_frames, nullptr, nullptr, nullptr, N, ticket, true);
+    return pose_submit_pifpaf(e, decoder, d_frames, N, ticket, true);
 }
 
 // the resize descriptors of a frame list, refused before any work is enqueued
@@ -3024,95 +3158,116 @@ int hp_pose_submit_frames_u8_host(hp_engine* e, hp_paf* parser, const hp_frame_u
 {
     std::vector<FrameDesc> d;
     const int rc = frame_descs(e, frames, N, keep_ratio, d);
-    return rc ? rc : pose_submit(e, parser, false, nullptr, d.data(), nullptr, nullptr, N, ticket, false);
+    return rc ? rc : pose_submit(e, parser, false, d.data(), N, ticket, false);
 }
 
 int hp_pose_submit_frames_u8_device(hp_engine* e, hp_paf* parser, const hp_frame_u8* frames, int N, int keep_ratio, int* ticket)
 {
     std::vector<FrameDesc> d;
     const int rc = frame_descs(e, frames, N, keep_ratio, d);
-    return rc ? rc : pose_submit(e, parser, false, nullptr, d.data(), nullptr, nullptr, N, ticket, true);
+    return rc ? rc : pose_submit(e, parser, false, d.data(), N, ticket, true);
 }
 
 int hp_pose_submit_pifpaf_frames_u8_host(hp_engine* e, hp_pifpaf* decoder, const hp_frame_u8* frames, int N, int keep_ratio, int* ticket)
 {
     std::vector<FrameDesc> d;
     const int rc = frame_descs(e, frames, N, keep_ratio, d);
-    return rc ? rc : pose_submit_pifpaf(e, decoder, nullptr, d.data(), nullptr, nullptr, N, ticket, false);
+    return rc ? rc : pose_submit_pifpaf(e, decoder, d.data(), N, ticket, false);
 }
 
 int hp_pose_submit_pifpaf_frames_u8_device(hp_engine* e, hp_pifpaf* decoder, const hp_frame_u8* frames, int N, int keep_ratio, int* ticket)
 {
     std::vector<FrameDesc> d;
     const int rc = frame_descs(e, frames, N, keep_ratio, d);
-    return rc ? rc : pose_submit_pifpaf(e, decoder, nullptr, d.data(), nullptr, nullptr, N, ticket, true);
+    return rc ? rc : pose_submit_pifpaf(e, decoder, d.data(), N, ticket, true);
 }
 
 // ---- Pose Proposal Network packs: network, parse and record D2H in one captured graph on the engine stream, as for the PAF parser ----
 int hp_pose_submit_ppn_u8_host(hp_engine* e, hp_ppn* parser, const uint8_t* frames, int N, int* ticket)
 {
-    return pose_submit(e, parser, true, frames, nullptr, nullptr, nullptr, N, ticket, false);
+    return pose_submit(e, parser, true, frames, N, ticket, false);
 }
 
 int hp_pose_submit_ppn_u8_device(hp_engine* e, hp_ppn* parser, const uint8_t* d_frames, int N, int* ticket)
 {
-    return pose_submit(e, parser, true, d_frames, nullptr, nullptr, nullptr, N, ticket, true);
+    return pose_submit(e, parser, true, d_frames, N, ticket, true);
 }
 
 int hp_pose_submit_ppn_frames_u8_host(hp_engine* e, hp_ppn* parser, const hp_frame_u8* frames, int N, int keep_ratio, int* ticket)
 {
     std::vector<FrameDesc> d;
     const int rc = frame_descs(e, frames, N, keep_ratio, d);
-    return rc ? rc : pose_submit(e, parser, true, nullptr, d.data(), nullptr, nullptr, N, ticket, false);
+    return rc ? rc : pose_submit(e, parser, true, d.data(), N, ticket, false);
 }
 
 int hp_pose_submit_ppn_frames_u8_device(hp_engine* e, hp_ppn* parser, const hp_frame_u8* frames, int N, int keep_ratio, int* ticket)
 {
     std::vector<FrameDesc> d;
     const int rc = frame_descs(e, frames, N, keep_ratio, d);
-    return rc ? rc : pose_submit(e, parser, true, nullptr, d.data(), nullptr, nullptr, N, ticket, true);
+    return rc ? rc : pose_submit(e, parser, true, d.data(), N, ticket, true);
 }
 
 // cv::rotate's clockwise rotations: ROTATE_90_CLOCKWISE, ROTATE_180, ROTATE_90_COUNTERCLOCKWISE, and upright
 static bool valid_rotation(int r) { return r == 0 || r == 90 || r == 180 || r == 270; }
 
-// the resize descriptors of a YUV 4:2:0 frame list, refused before any work is enqueued; the regime comes from the luma size after the
-// frame's rotation (rotation NULL: every frame upright)
-static int yuv_frame_descs(const hp_engine* e, const hp_frame_yuv420* frames, const int32_t* rotation, int N, int keep_ratio,
-                           std::vector<YuvFrameDesc>& descs)
+extern "C++" {   // overloads and templates, inside the C ABI block
+// what the 16-bit records add to the 8-bit refusals: bits outside 9..16, and a pointer or a pitch that is not 2-byte aligned
+static const char* sample_refusal(int bits, std::initializer_list<const void*> ptrs, std::initializer_list<int> pitches)
 {
-    if (!e || !frames) { set_error("hp_pose_submit_frames_yuv420: null argument"); return HP_ERR_ARG; }
+    if (bits < 9 || bits > 16) return "has bits outside 9..16";
+    for (const void* p : ptrs) if ((uintptr_t)p & 1) return "has a plane that is not 2-byte aligned";
+    for (int p : pitches) if (p & 1) return "has a pitch that is not a whole number of 16-bit samples";
+    return nullptr;
+}
+
+// the resize descriptors of a YUV 4:2:0 frame list (hp_frame_yuv420 -> YuvFrameDesc, hp_frame_yuv420_16 -> Yuv16FrameDesc), refused
+// before any work is enqueued; the regime comes from the luma size after the frame's rotation (rotation NULL: every frame upright)
+template <class Frame, class Desc>
+static int yuv_frame_descs(const hp_engine* e, const Frame* frames, const int32_t* rotation, int N, int keep_ratio, std::vector<Desc>& descs)
+{
+    constexpr bool k16 = std::is_same_v<Frame, hp_frame_yuv420_16>;
+    constexpr long long S = k16 ? 2 : 1;   // bytes per sample
+    const char* fn = k16 ? "hp_pose_submit_frames_yuv420_16" : "hp_pose_submit_frames_yuv420";
+    if (!e || !frames) { set_error("%s: null argument", fn); return HP_ERR_ARG; }
     if (N <= 0 || N > e->max_batch) { set_error("Input batch size overflow: Yours@%d Max@%d", N, e->max_batch); return HP_ERR_BATCH; }
     descs.resize(N);
     for (int f = 0; f < N; ++f) {
-        const hp_frame_yuv420& fr = frames[f];
+        const Frame& fr = frames[f];
         const int rot = rotation ? rotation[f] : 0;
+        int bits = 8;
+        if constexpr (k16) bits = fr.bits;
         const char* bad = nullptr;
         if (!fr.y || !fr.u || !fr.v) bad = "has a null plane";
         else if (fr.height <= 0 || fr.width <= 0 || (fr.height & 1) || (fr.width & 1)) bad = "has a size that is not positive and even";
         else if (fr.uv_step != 1 && fr.uv_step != 2) bad = "has a uv_step other than 1 (planar) or 2 (semi-planar)";
-        else if (fr.pitch_y < fr.width || fr.pitch_uv < fr.width / 2 * fr.uv_step) bad = "has a pitch shorter than its row";
-        else if (fr.uv_step == 2 && fr.u - fr.v != 1 && fr.v - fr.u != 1) bad = "is semi-planar but its u and v are not one byte apart";
+        else if (fr.pitch_y < fr.width * S || fr.pitch_uv < fr.width / 2 * fr.uv_step * S) bad = "has a pitch shorter than its row";
+        else if (fr.uv_step == 2 && fr.u - fr.v != 1 && fr.v - fr.u != 1)
+            bad = k16 ? "is semi-planar but its u and v are not one sample apart" : "is semi-planar but its u and v are not one byte apart";
         else if (!valid_rotation(rot)) bad = "has a rotation other than 0, 90, 180 or 270 degrees";
+        else if (k16) bad = sample_refusal(bits, { fr.y, fr.u, fr.v }, { fr.pitch_y, fr.pitch_uv });
         if (bad) {
-            set_error("hp_pose_submit_frames_yuv420: frame %d %s (%dx%d, pitches %d / %d, uv_step %d, rotation %d)", f, bad, fr.height,
-                      fr.width, fr.pitch_y, fr.pitch_uv, fr.uv_step, rot);
+            if (k16) set_error("%s: frame %d %s (%dx%d, pitches %d / %d, uv_step %d, rotation %d, bits %d)", fn, f, bad, fr.height, fr.width,
+                               fr.pitch_y, fr.pitch_uv, fr.uv_step, rot, bits);
+            else set_error("%s: frame %d %s (%dx%d, pitches %d / %d, uv_step %d, rotation %d)", fn, f, bad, fr.height, fr.width,
+                           fr.pitch_y, fr.pitch_uv, fr.uv_step, rot);
             return HP_ERR_ARG;
         }
         FrameDesc d;
         const int rc = frame_desc(e, nullptr, rot % 180 ? fr.width : fr.height, rot % 180 ? fr.height : fr.width, keep_ratio, d);
         if (rc) return rc;
-        descs[f] = YuvFrameDesc{ fr.y, fr.u, fr.v, fr.height, fr.width, d.rh, d.rw, d.mode, fr.pitch_y, fr.pitch_uv, fr.uv_step, rot, 0 };
+        descs[f] = Desc{ fr.y, fr.u, fr.v, fr.height, fr.width, d.rh, d.rw, d.mode, fr.pitch_y, fr.pitch_uv, fr.uv_step, rot, k16 ? bits : 0 };
     }
     return HP_OK;
 }
+
+}   // extern "C++"
 
 int hp_pose_submit_frames_yuv420_rotated_host(hp_engine* e, hp_paf* parser, const hp_frame_yuv420* frames, const int32_t* rotation, int N,
                                               int keep_ratio, int* ticket)
 {
     std::vector<YuvFrameDesc> d;
     const int rc = yuv_frame_descs(e, frames, rotation, N, keep_ratio, d);
-    return rc ? rc : pose_submit(e, parser, false, nullptr, nullptr, d.data(), nullptr, N, ticket, false);
+    return rc ? rc : pose_submit(e, parser, false, d.data(), N, ticket, false);
 }
 
 int hp_pose_submit_frames_yuv420_rotated_device(hp_engine* e, hp_paf* parser, const hp_frame_yuv420* frames, const int32_t* rotation, int N,
@@ -3120,7 +3275,7 @@ int hp_pose_submit_frames_yuv420_rotated_device(hp_engine* e, hp_paf* parser, co
 {
     std::vector<YuvFrameDesc> d;
     const int rc = yuv_frame_descs(e, frames, rotation, N, keep_ratio, d);
-    return rc ? rc : pose_submit(e, parser, false, nullptr, nullptr, d.data(), nullptr, N, ticket, true);
+    return rc ? rc : pose_submit(e, parser, false, d.data(), N, ticket, true);
 }
 
 int hp_pose_submit_pifpaf_frames_yuv420_rotated_host(hp_engine* e, hp_pifpaf* decoder, const hp_frame_yuv420* frames, const int32_t* rotation,
@@ -3128,7 +3283,7 @@ int hp_pose_submit_pifpaf_frames_yuv420_rotated_host(hp_engine* e, hp_pifpaf* de
 {
     std::vector<YuvFrameDesc> d;
     const int rc = yuv_frame_descs(e, frames, rotation, N, keep_ratio, d);
-    return rc ? rc : pose_submit_pifpaf(e, decoder, nullptr, nullptr, d.data(), nullptr, N, ticket, false);
+    return rc ? rc : pose_submit_pifpaf(e, decoder, d.data(), N, ticket, false);
 }
 
 int hp_pose_submit_pifpaf_frames_yuv420_rotated_device(hp_engine* e, hp_pifpaf* decoder, const hp_frame_yuv420* frames, const int32_t* rotation,
@@ -3136,7 +3291,7 @@ int hp_pose_submit_pifpaf_frames_yuv420_rotated_device(hp_engine* e, hp_pifpaf* 
 {
     std::vector<YuvFrameDesc> d;
     const int rc = yuv_frame_descs(e, frames, rotation, N, keep_ratio, d);
-    return rc ? rc : pose_submit_pifpaf(e, decoder, nullptr, nullptr, d.data(), nullptr, N, ticket, true);
+    return rc ? rc : pose_submit_pifpaf(e, decoder, d.data(), N, ticket, true);
 }
 
 int hp_pose_submit_ppn_frames_yuv420_rotated_host(hp_engine* e, hp_ppn* parser, const hp_frame_yuv420* frames, const int32_t* rotation, int N,
@@ -3144,7 +3299,7 @@ int hp_pose_submit_ppn_frames_yuv420_rotated_host(hp_engine* e, hp_ppn* parser, 
 {
     std::vector<YuvFrameDesc> d;
     const int rc = yuv_frame_descs(e, frames, rotation, N, keep_ratio, d);
-    return rc ? rc : pose_submit(e, parser, true, nullptr, nullptr, d.data(), nullptr, N, ticket, false);
+    return rc ? rc : pose_submit(e, parser, true, d.data(), N, ticket, false);
 }
 
 int hp_pose_submit_ppn_frames_yuv420_rotated_device(hp_engine* e, hp_ppn* parser, const hp_frame_yuv420* frames, const int32_t* rotation, int N,
@@ -3152,7 +3307,7 @@ int hp_pose_submit_ppn_frames_yuv420_rotated_device(hp_engine* e, hp_ppn* parser
 {
     std::vector<YuvFrameDesc> d;
     const int rc = yuv_frame_descs(e, frames, rotation, N, keep_ratio, d);
-    return rc ? rc : pose_submit(e, parser, true, nullptr, nullptr, d.data(), nullptr, N, ticket, true);
+    return rc ? rc : pose_submit(e, parser, true, d.data(), N, ticket, true);
 }
 
 // the upright calls: the rotated ones with every frame upright
@@ -3186,44 +3341,59 @@ int hp_pose_submit_ppn_frames_yuv420_device(hp_engine* e, hp_ppn* parser, const 
     return hp_pose_submit_ppn_frames_yuv420_rotated_device(e, parser, frames, nullptr, N, keep_ratio, ticket);
 }
 
-// the resize descriptors of an interleaved frame list, refused before any work is enqueued; the regime comes from the pixel size after
-// the frame's rotation (rotation NULL: every frame upright)
-static int interleaved_frame_descs(const hp_engine* e, const hp_frame_interleaved* frames, const int32_t* rotation, int N, int keep_ratio,
-                                   std::vector<InterleavedFrameDesc>& descs)
+extern "C++" {   // overloads and templates, inside the C ABI block
+// the resize descriptors of an interleaved frame list (hp_frame_interleaved -> InterleavedFrameDesc, hp_frame_interleaved16 ->
+// Interleaved16FrameDesc), refused before any work is enqueued; the regime comes from the pixel size after the frame's rotation
+// (rotation NULL: every frame upright)
+template <class Frame, class Desc>
+static int interleaved_frame_descs(const hp_engine* e, const Frame* frames, const int32_t* rotation, int N, int keep_ratio,
+                                   std::vector<Desc>& descs)
 {
-    if (!e || !frames) { set_error("hp_pose_submit_frames_interleaved: null argument"); return HP_ERR_ARG; }
+    constexpr bool k16 = std::is_same_v<Frame, hp_frame_interleaved16>;
+    constexpr long long S = k16 ? 2 : 1;   // bytes per sample
+    const char* fn = k16 ? "hp_pose_submit_frames_interleaved16" : "hp_pose_submit_frames_interleaved";
+    if (!e || !frames) { set_error("%s: null argument", fn); return HP_ERR_ARG; }
     if (N <= 0 || N > e->max_batch) { set_error("Input batch size overflow: Yours@%d Max@%d", N, e->max_batch); return HP_ERR_BATCH; }
     descs.resize(N);
     for (int f = 0; f < N; ++f) {
-        const hp_frame_interleaved& fr = frames[f];
-        const int bpp = pixel_bytes(fr.format);
+        const Frame& fr = frames[f];
+        const int bpp = pixel_bytes(fr.format);   // samples per pixel but for 4:2:2
         const int rot = rotation ? rotation[f] : 0;
+        int bits = 8;
+        if constexpr (k16) bits = fr.bits;
         const char* bad = nullptr;
         if (!fr.data) bad = "is null";
         else if (fr.height <= 0 || fr.width <= 0) bad = "has a size that is not positive";
         else if (!bpp) bad = "has an unknown format";
+        else if (k16 && bpp == 2) bad = "is 4:2:2, which has no 16-bit form";
         else if (bpp == 2 && (fr.width & 1)) bad = "is 4:2:2 of odd width";
-        else if ((long long)fr.pitch < (long long)fr.width * bpp) bad = "has a pitch shorter than its row";
+        else if ((long long)fr.pitch < (long long)fr.width * bpp * S) bad = "has a pitch shorter than its row";
         else if (!valid_rotation(rot)) bad = "has a rotation other than 0, 90, 180 or 270 degrees";
+        else if (k16) bad = sample_refusal(bits, { fr.data }, { fr.pitch });
         if (bad) {
-            set_error("hp_pose_submit_frames_interleaved: frame %d %s (%dx%d, pitch %d, format %d, rotation %d)", f, bad, fr.height, fr.width,
-                      fr.pitch, fr.format, rot);
+            if (k16) set_error("%s: frame %d %s (%dx%d, pitch %d, format %d, rotation %d, bits %d)", fn, f, bad, fr.height, fr.width, fr.pitch,
+                               fr.format, rot, bits);
+            else set_error("%s: frame %d %s (%dx%d, pitch %d, format %d, rotation %d)", fn, f, bad, fr.height, fr.width, fr.pitch,
+                           fr.format, rot);
             return HP_ERR_ARG;
         }
         FrameDesc d;
         const int rc = frame_desc(e, nullptr, rot % 180 ? fr.width : fr.height, rot % 180 ? fr.height : fr.width, keep_ratio, d);
         if (rc) return rc;
-        descs[f] = InterleavedFrameDesc{ fr.data, fr.height, fr.width, d.rh, d.rw, d.mode, fr.pitch, fr.format, rot };
+        if constexpr (k16) descs[f] = Desc{ fr.data, fr.height, fr.width, d.rh, d.rw, d.mode, fr.pitch, fr.format, rot, bits, 0 };
+        else descs[f] = Desc{ fr.data, fr.height, fr.width, d.rh, d.rw, d.mode, fr.pitch, fr.format, rot };
     }
     return HP_OK;
 }
+
+}   // extern "C++"
 
 int hp_pose_submit_frames_interleaved_rotated_host(hp_engine* e, hp_paf* parser, const hp_frame_interleaved* frames, const int32_t* rotation,
                                                    int N, int keep_ratio, int* ticket)
 {
     std::vector<InterleavedFrameDesc> d;
     const int rc = interleaved_frame_descs(e, frames, rotation, N, keep_ratio, d);
-    return rc ? rc : pose_submit(e, parser, false, nullptr, nullptr, nullptr, d.data(), N, ticket, false);
+    return rc ? rc : pose_submit(e, parser, false, d.data(), N, ticket, false);
 }
 
 int hp_pose_submit_frames_interleaved_rotated_device(hp_engine* e, hp_paf* parser, const hp_frame_interleaved* frames, const int32_t* rotation,
@@ -3231,7 +3401,7 @@ int hp_pose_submit_frames_interleaved_rotated_device(hp_engine* e, hp_paf* parse
 {
     std::vector<InterleavedFrameDesc> d;
     const int rc = interleaved_frame_descs(e, frames, rotation, N, keep_ratio, d);
-    return rc ? rc : pose_submit(e, parser, false, nullptr, nullptr, nullptr, d.data(), N, ticket, true);
+    return rc ? rc : pose_submit(e, parser, false, d.data(), N, ticket, true);
 }
 
 int hp_pose_submit_pifpaf_frames_interleaved_rotated_host(hp_engine* e, hp_pifpaf* decoder, const hp_frame_interleaved* frames,
@@ -3239,7 +3409,7 @@ int hp_pose_submit_pifpaf_frames_interleaved_rotated_host(hp_engine* e, hp_pifpa
 {
     std::vector<InterleavedFrameDesc> d;
     const int rc = interleaved_frame_descs(e, frames, rotation, N, keep_ratio, d);
-    return rc ? rc : pose_submit_pifpaf(e, decoder, nullptr, nullptr, nullptr, d.data(), N, ticket, false);
+    return rc ? rc : pose_submit_pifpaf(e, decoder, d.data(), N, ticket, false);
 }
 
 int hp_pose_submit_pifpaf_frames_interleaved_rotated_device(hp_engine* e, hp_pifpaf* decoder, const hp_frame_interleaved* frames,
@@ -3247,7 +3417,7 @@ int hp_pose_submit_pifpaf_frames_interleaved_rotated_device(hp_engine* e, hp_pif
 {
     std::vector<InterleavedFrameDesc> d;
     const int rc = interleaved_frame_descs(e, frames, rotation, N, keep_ratio, d);
-    return rc ? rc : pose_submit_pifpaf(e, decoder, nullptr, nullptr, nullptr, d.data(), N, ticket, true);
+    return rc ? rc : pose_submit_pifpaf(e, decoder, d.data(), N, ticket, true);
 }
 
 int hp_pose_submit_ppn_frames_interleaved_rotated_host(hp_engine* e, hp_ppn* parser, const hp_frame_interleaved* frames, const int32_t* rotation,
@@ -3255,7 +3425,7 @@ int hp_pose_submit_ppn_frames_interleaved_rotated_host(hp_engine* e, hp_ppn* par
 {
     std::vector<InterleavedFrameDesc> d;
     const int rc = interleaved_frame_descs(e, frames, rotation, N, keep_ratio, d);
-    return rc ? rc : pose_submit(e, parser, true, nullptr, nullptr, nullptr, d.data(), N, ticket, false);
+    return rc ? rc : pose_submit(e, parser, true, d.data(), N, ticket, false);
 }
 
 int hp_pose_submit_ppn_frames_interleaved_rotated_device(hp_engine* e, hp_ppn* parser, const hp_frame_interleaved* frames,
@@ -3263,7 +3433,7 @@ int hp_pose_submit_ppn_frames_interleaved_rotated_device(hp_engine* e, hp_ppn* p
 {
     std::vector<InterleavedFrameDesc> d;
     const int rc = interleaved_frame_descs(e, frames, rotation, N, keep_ratio, d);
-    return rc ? rc : pose_submit(e, parser, true, nullptr, nullptr, nullptr, d.data(), N, ticket, true);
+    return rc ? rc : pose_submit(e, parser, true, d.data(), N, ticket, true);
 }
 
 // the upright calls: the rotated ones with every frame upright
@@ -3295,6 +3465,103 @@ int hp_pose_submit_ppn_frames_interleaved_host(hp_engine* e, hp_ppn* parser, con
 int hp_pose_submit_ppn_frames_interleaved_device(hp_engine* e, hp_ppn* parser, const hp_frame_interleaved* frames, int N, int keep_ratio, int* ticket)
 {
     return hp_pose_submit_ppn_frames_interleaved_rotated_device(e, parser, frames, nullptr, N, keep_ratio, ticket);
+}
+
+// 16-bit samples: the 8-bit calls' descriptors and resize, each sample reduced in the fetch
+int hp_pose_submit_frames_yuv420_16_host(hp_engine* e, hp_paf* parser, const hp_frame_yuv420_16* frames, const int32_t* rotation,
+                                         int N, int keep_ratio, int* ticket)
+{
+    std::vector<Yuv16FrameDesc> d;
+    const int rc = yuv_frame_descs(e, frames, rotation, N, keep_ratio, d);
+    return rc ? rc : pose_submit(e, parser, false, d.data(), N, ticket, false);
+}
+
+int hp_pose_submit_frames_yuv420_16_device(hp_engine* e, hp_paf* parser, const hp_frame_yuv420_16* frames, const int32_t* rotation,
+                                           int N, int keep_ratio, int* ticket)
+{
+    std::vector<Yuv16FrameDesc> d;
+    const int rc = yuv_frame_descs(e, frames, rotation, N, keep_ratio, d);
+    return rc ? rc : pose_submit(e, parser, false, d.data(), N, ticket, true);
+}
+
+int hp_pose_submit_pifpaf_frames_yuv420_16_host(hp_engine* e, hp_pifpaf* decoder, const hp_frame_yuv420_16* frames, const int32_t* rotation,
+                                                int N, int keep_ratio, int* ticket)
+{
+    std::vector<Yuv16FrameDesc> d;
+    const int rc = yuv_frame_descs(e, frames, rotation, N, keep_ratio, d);
+    return rc ? rc : pose_submit_pifpaf(e, decoder, d.data(), N, ticket, false);
+}
+
+int hp_pose_submit_pifpaf_frames_yuv420_16_device(hp_engine* e, hp_pifpaf* decoder, const hp_frame_yuv420_16* frames, const int32_t* rotation,
+                                                  int N, int keep_ratio, int* ticket)
+{
+    std::vector<Yuv16FrameDesc> d;
+    const int rc = yuv_frame_descs(e, frames, rotation, N, keep_ratio, d);
+    return rc ? rc : pose_submit_pifpaf(e, decoder, d.data(), N, ticket, true);
+}
+
+int hp_pose_submit_ppn_frames_yuv420_16_host(hp_engine* e, hp_ppn* parser, const hp_frame_yuv420_16* frames, const int32_t* rotation,
+                                             int N, int keep_ratio, int* ticket)
+{
+    std::vector<Yuv16FrameDesc> d;
+    const int rc = yuv_frame_descs(e, frames, rotation, N, keep_ratio, d);
+    return rc ? rc : pose_submit(e, parser, true, d.data(), N, ticket, false);
+}
+
+int hp_pose_submit_ppn_frames_yuv420_16_device(hp_engine* e, hp_ppn* parser, const hp_frame_yuv420_16* frames, const int32_t* rotation,
+                                               int N, int keep_ratio, int* ticket)
+{
+    std::vector<Yuv16FrameDesc> d;
+    const int rc = yuv_frame_descs(e, frames, rotation, N, keep_ratio, d);
+    return rc ? rc : pose_submit(e, parser, true, d.data(), N, ticket, true);
+}
+
+int hp_pose_submit_frames_interleaved16_host(hp_engine* e, hp_paf* parser, const hp_frame_interleaved16* frames, const int32_t* rotation,
+                                             int N, int keep_ratio, int* ticket)
+{
+    std::vector<Interleaved16FrameDesc> d;
+    const int rc = interleaved_frame_descs(e, frames, rotation, N, keep_ratio, d);
+    return rc ? rc : pose_submit(e, parser, false, d.data(), N, ticket, false);
+}
+
+int hp_pose_submit_frames_interleaved16_device(hp_engine* e, hp_paf* parser, const hp_frame_interleaved16* frames, const int32_t* rotation,
+                                               int N, int keep_ratio, int* ticket)
+{
+    std::vector<Interleaved16FrameDesc> d;
+    const int rc = interleaved_frame_descs(e, frames, rotation, N, keep_ratio, d);
+    return rc ? rc : pose_submit(e, parser, false, d.data(), N, ticket, true);
+}
+
+int hp_pose_submit_pifpaf_frames_interleaved16_host(hp_engine* e, hp_pifpaf* decoder, const hp_frame_interleaved16* frames, const int32_t* rotation,
+                                                    int N, int keep_ratio, int* ticket)
+{
+    std::vector<Interleaved16FrameDesc> d;
+    const int rc = interleaved_frame_descs(e, frames, rotation, N, keep_ratio, d);
+    return rc ? rc : pose_submit_pifpaf(e, decoder, d.data(), N, ticket, false);
+}
+
+int hp_pose_submit_pifpaf_frames_interleaved16_device(hp_engine* e, hp_pifpaf* decoder, const hp_frame_interleaved16* frames, const int32_t* rotation,
+                                                      int N, int keep_ratio, int* ticket)
+{
+    std::vector<Interleaved16FrameDesc> d;
+    const int rc = interleaved_frame_descs(e, frames, rotation, N, keep_ratio, d);
+    return rc ? rc : pose_submit_pifpaf(e, decoder, d.data(), N, ticket, true);
+}
+
+int hp_pose_submit_ppn_frames_interleaved16_host(hp_engine* e, hp_ppn* parser, const hp_frame_interleaved16* frames, const int32_t* rotation,
+                                                 int N, int keep_ratio, int* ticket)
+{
+    std::vector<Interleaved16FrameDesc> d;
+    const int rc = interleaved_frame_descs(e, frames, rotation, N, keep_ratio, d);
+    return rc ? rc : pose_submit(e, parser, true, d.data(), N, ticket, false);
+}
+
+int hp_pose_submit_ppn_frames_interleaved16_device(hp_engine* e, hp_ppn* parser, const hp_frame_interleaved16* frames, const int32_t* rotation,
+                                                   int N, int keep_ratio, int* ticket)
+{
+    std::vector<Interleaved16FrameDesc> d;
+    const int rc = interleaved_frame_descs(e, frames, rotation, N, keep_ratio, d);
+    return rc ? rc : pose_submit(e, parser, true, d.data(), N, ticket, true);
 }
 
 // test hook: the first N resized network-size frames of ticket `ticket` (in flight or collected)

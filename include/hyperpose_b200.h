@@ -408,6 +408,58 @@ int hp_pose_submit_ppn_frames_interleaved_rotated_host(hp_engine* e, hp_ppn* par
                                                        const int32_t* rotation, int N, int keep_ratio, int* ticket);
 int hp_pose_submit_ppn_frames_interleaved_rotated_device(hp_engine* e, hp_ppn* parser, const hp_frame_interleaved* frames,
                                                          const int32_t* rotation, int N, int keep_ratio, int* ticket);
+/* The YUV 4:2:0 and interleaved calls for frames whose samples are 16-bit words: 10 / 12-bit video (NVDEC's P010 / P016, FFmpeg's
+ * p010le / p016le, yuv420p10le / p12le / p16le), 16-bit images (Mono12 / Mono16 cameras, 16-bit PNG / TIFF gray, RGB, RGBA).  Each
+ * sample v, holding `bits` significant bits LSB-aligned (9 <= bits <= 16), is first reduced to the byte that OpenCV's
+ * src.convertTo(dst, CV_8U, 1.0 / (1 << (bits - 8))) gives: saturate(rint_half_even(v * 2^-(bits - 8))).  P010 / P016 are
+ * MSB-aligned: pass bits = 16; yuv420p10le is bits = 10 (1023 saturates to 255).  The 8-bit calls above then run on the reduced
+ * bytes, unchanged, inside the same batched resize's fetch: the network-size frame is byte-identical to
+ * cv::resize(cv::rotate(cv::cvtColor(convertTo(src16, CV_8U, 2^-(bits-8)), code), rotate_code), ...) (or non_scaling_resize of it).
+ * rotation as for the _rotated_ calls (NULL: every frame upright).  No extra pass and no extra buffer.  The frames of a batch may mix
+ * layouts, formats, sizes, bits and rotations.  Every pointer, pitch and uv_step is as in the 8-bit records, but counted over 16-bit
+ * samples where the 8-bit ones count bytes: pitches stay in bytes, uv_step is in samples.  HP_ERR_ARG, before anything is enqueued:
+ * everything the 8-bit calls refuse, bits outside 9..16, a pointer or pitch that is not 2-byte aligned, semi-planar u and v not one
+ * sample apart, and in the interleaved call a 4:2:2 format (only HP_PIX_BGR, _RGB, _BGRA, _RGBA, _GRAY: BGR48, RGB48, BGRA64,
+ * RGBA64, GRAY16).  _host: copied row-compacted at 2 bytes per sample, by a pitched DMA from page-locked frames, through pinned
+ * staging from pageable ones.  _device: read in place with their pitch; the bytes between a row's end and the pitch are never read. */
+typedef struct hp_frame_yuv420_16 {
+    const uint16_t *y, *u, *v;
+    int32_t height, width;       /* luma size, both even */
+    int32_t pitch_y, pitch_uv;   /* bytes from one row to the next, even */
+    int32_t uv_step;             /* samples: 2 semi-planar (P010 / P016 v = u + 1, V-first u = v + 1); 1 planar (I420, YV12 order) */
+    int32_t bits;                /* significant bits per sample, LSB-aligned: 9..16 (16 for P010 / P016) */
+} hp_frame_yuv420_16;
+typedef struct hp_frame_interleaved16 {
+    const uint16_t* data;
+    int32_t height, width;
+    int32_t pitch;    /* bytes from one row to the next, even */
+    int32_t format;   /* HP_PIX_BGR, _RGB, _BGRA, _RGBA or _GRAY: 3, 3, 4, 4, 1 samples per pixel */
+    int32_t bits;     /* as in hp_frame_yuv420_16 */
+} hp_frame_interleaved16;
+int hp_pose_submit_frames_yuv420_16_host(hp_engine* e, hp_paf* parser, const hp_frame_yuv420_16* frames, const int32_t* rotation, int N,
+                                         int keep_ratio, int* ticket);
+int hp_pose_submit_frames_yuv420_16_device(hp_engine* e, hp_paf* parser, const hp_frame_yuv420_16* frames, const int32_t* rotation, int N,
+                                           int keep_ratio, int* ticket);
+int hp_pose_submit_pifpaf_frames_yuv420_16_host(hp_engine* e, hp_pifpaf* decoder, const hp_frame_yuv420_16* frames, const int32_t* rotation,
+                                                int N, int keep_ratio, int* ticket);
+int hp_pose_submit_pifpaf_frames_yuv420_16_device(hp_engine* e, hp_pifpaf* decoder, const hp_frame_yuv420_16* frames, const int32_t* rotation,
+                                                  int N, int keep_ratio, int* ticket);
+int hp_pose_submit_ppn_frames_yuv420_16_host(hp_engine* e, hp_ppn* parser, const hp_frame_yuv420_16* frames, const int32_t* rotation, int N,
+                                             int keep_ratio, int* ticket);
+int hp_pose_submit_ppn_frames_yuv420_16_device(hp_engine* e, hp_ppn* parser, const hp_frame_yuv420_16* frames, const int32_t* rotation, int N,
+                                               int keep_ratio, int* ticket);
+int hp_pose_submit_frames_interleaved16_host(hp_engine* e, hp_paf* parser, const hp_frame_interleaved16* frames, const int32_t* rotation,
+                                             int N, int keep_ratio, int* ticket);
+int hp_pose_submit_frames_interleaved16_device(hp_engine* e, hp_paf* parser, const hp_frame_interleaved16* frames, const int32_t* rotation,
+                                               int N, int keep_ratio, int* ticket);
+int hp_pose_submit_pifpaf_frames_interleaved16_host(hp_engine* e, hp_pifpaf* decoder, const hp_frame_interleaved16* frames,
+                                                    const int32_t* rotation, int N, int keep_ratio, int* ticket);
+int hp_pose_submit_pifpaf_frames_interleaved16_device(hp_engine* e, hp_pifpaf* decoder, const hp_frame_interleaved16* frames,
+                                                      const int32_t* rotation, int N, int keep_ratio, int* ticket);
+int hp_pose_submit_ppn_frames_interleaved16_host(hp_engine* e, hp_ppn* parser, const hp_frame_interleaved16* frames, const int32_t* rotation,
+                                                 int N, int keep_ratio, int* ticket);
+int hp_pose_submit_ppn_frames_interleaved16_device(hp_engine* e, hp_ppn* parser, const hp_frame_interleaved16* frames,
+                                                   const int32_t* rotation, int N, int keep_ratio, int* ticket);
 /* test hook: the first N resized network-size frames [N,in_h,in_w,3] of an in-flight or collected ticket */
 int hp_pose_debug_read_slot_frames(hp_engine* e, int ticket, uint8_t* out, int N);
 int hp_pifpaf_pipeline_info(hp_pifpaf* p, void** stream, void** inputs_free_event, int* hcap);
