@@ -213,17 +213,8 @@ EXPORTS += [
     "hp_engine_create_ex", "hp_engine_dtype", "hp_pose_submit_u8_device", "hp_engine_debug_op_kernel",
     "hp_engine_debug_op_epilogue", "hp_engine_debug_op_conv_epilogue", "hp_engine_debug_uses_pdl",
     "hp_engine_debug_read_buffer_raw", "hp_engine_debug_write_outputs",
-    "hp_engine_calibrate_u8", "hp_pack_int8_calibrated",
-    "hp_pose_submit_frames_u8_host", "hp_pose_submit_frames_u8_device", "hp_pose_submit_pifpaf_frames_u8_host",
-    "hp_pose_submit_pifpaf_frames_u8_device", "hp_pose_debug_read_slot_frames",
-    "hp_pose_submit_frames_yuv420_host", "hp_pose_submit_frames_yuv420_device", "hp_pose_submit_pifpaf_frames_yuv420_host",
-    "hp_pose_submit_pifpaf_frames_yuv420_device", "hp_pose_submit_ppn_frames_yuv420_host", "hp_pose_submit_ppn_frames_yuv420_device",
-    "hp_pose_submit_frames_interleaved_host", "hp_pose_submit_frames_interleaved_device", "hp_pose_submit_pifpaf_frames_interleaved_host",
-    "hp_pose_submit_pifpaf_frames_interleaved_device", "hp_pose_submit_ppn_frames_interleaved_host",
-    "hp_pose_submit_ppn_frames_interleaved_device",
-] + [f"hp_pose_submit{head}_frames_{fmt}_rotated_{where}" for head in ("", "_pifpaf", "_ppn") for fmt in ("yuv420", "interleaved")
-     for where in ("host", "device")] + [f"hp_pose_submit{head}_frames_{fmt}_{where}" for head in ("", "_pifpaf", "_ppn")
-                                         for fmt in ("yuv420_16", "interleaved16") for where in ("host", "device")]
+    "hp_engine_calibrate_u8", "hp_pack_int8_calibrated", "hp_pose_debug_read_slot_frames",
+]   # (+ the frame calls of FRAME_CALLS, below)
 
 
 class FrameU8(C.Structure):
@@ -305,6 +296,30 @@ def interleaved16_record(frame: np.ndarray, fmt: str, bits: int) -> FrameInterle
                               PIXEL_FORMATS[INTERLEAVED16_FORMATS[fmt]], bits)
 
 
+# The frame calls hp_pose_submit{,_pifpaf,_ppn}_frames_<format>_{host,device}: each format's record type, and the form of its calls
+# that takes a per-frame rotation table (int32[N], or NULL for upright): "_rotated" names a twin of each upright call, "" the call
+# itself (16-bit frames), None none (BGR frames).
+FRAME_CALLS = {"u8": (FrameU8, None), "yuv420": (FrameYUV420, "_rotated"), "interleaved": (FrameInterleaved, "_rotated"),
+               "yuv420_16": (FrameYUV420_16, ""), "interleaved16": (FrameInterleaved16, "")}
+
+
+def frame_call(head: str, fmt: str, device: bool, rotated: bool) -> str:
+    """the symbol of a frame call: head "", "_pifpaf" or "_ppn"; rotated: the form that takes a rotation table"""
+    return f"hp_pose_submit{head}_frames_{fmt}{FRAME_CALLS[fmt][1] if rotated else ''}_{'device' if device else 'host'}"
+
+
+def frame_calls():
+    """(symbol, record type, takes a rotation table) of every frame call"""
+    for fmt, (rec, rot) in FRAME_CALLS.items():
+        for head in ("", "_pifpaf", "_ppn"):
+            for device in (False, True):
+                for rotated in ((False,) if rot is None else (True,) if rot == "" else (False, True)):
+                    yield frame_call(head, fmt, device, rotated), rec, rotated
+
+
+EXPORTS += [name for name, _, _ in frame_calls()]
+
+
 def bits_list(bits, n: int) -> list:
     """the per-frame significant bits of a 16-bit batch, from one int or one per frame, each 9..16; anything else is refused before
     the library is called"""
@@ -335,6 +350,33 @@ def rotation_table(rotation, n: int):
         if isinstance(r, (bool, np.bool_)) or not isinstance(r, (int, np.integer)) or int(r) not in ROTATIONS:
             raise HyperposeError(HP_ERR_ARG, f"frame {i}: rotation {r!r} is not one of {ROTATIONS} clockwise degrees")
     return (C.c_int32 * n)(*[int(r) for r in rots])
+
+
+def _rotation_arg(rotation, n: int) -> dict:
+    """the rotation= of _submit_frame_table: nothing for None (upright), else rotation_table's int32[n]"""
+    return {} if rotation is None else {"rotation": rotation_table(rotation, n)}
+
+
+def _per_frame(value, n: int, allowed, what: str) -> list:
+    """a per-batch layout or format as one per frame: one name for the batch or a list of n names, each in `allowed`; anything else
+    is refused before the library is called"""
+    values = [value] * n if isinstance(value, str) else list(value)
+    if len(values) != n or any(v not in allowed for v in values):
+        raise HyperposeError(HP_ERR_ARG, f"{what} {value!r}: expected one of {sorted(allowed)}, or one per frame")
+    return values
+
+
+def _record_table(frames, rec):
+    """the ctypes array of a device call's frame records, each of which must be a `rec`"""
+    for i, f in enumerate(frames):
+        if not isinstance(f, rec):
+            raise HyperposeError(HP_ERR_ARG, f"frame {i}: expected a {rec.__name__}, got {type(f).__name__}")
+    return (rec * len(frames))(*frames)
+
+
+def _head(parser) -> str:
+    """the infix of the pose calls for a parser's head: _pifpaf for OpenPifPaf packs, _ppn for Pose Proposal Network packs"""
+    return "_pifpaf" if isinstance(parser, PifPafParser) else "_ppn" if isinstance(parser, PoseProposalParser) else ""
 
 
 def _bind_engine(L):
@@ -379,25 +421,10 @@ def _bind_engine(L):
     L.hp_pose_submit_u8_host.argtypes = [vp, vp, vp, C.c_int, ip]
     L.hp_pose_submit_u8_device.argtypes = [vp, vp, vp, C.c_int, ip]
     L.hp_pose_collect.argtypes = [vp, C.c_int, vp, C.c_int, ip]
-    for f in (L.hp_pose_submit_frames_u8_host, L.hp_pose_submit_frames_u8_device, L.hp_pose_submit_pifpaf_frames_u8_host,
-              L.hp_pose_submit_pifpaf_frames_u8_device, L.hp_pose_submit_ppn_frames_u8_host, L.hp_pose_submit_ppn_frames_u8_device):
-        f.argtypes = [vp, vp, C.POINTER(FrameU8), C.c_int, C.c_int, ip]
-    for f in (L.hp_pose_submit_frames_yuv420_host, L.hp_pose_submit_frames_yuv420_device, L.hp_pose_submit_pifpaf_frames_yuv420_host,
-              L.hp_pose_submit_pifpaf_frames_yuv420_device, L.hp_pose_submit_ppn_frames_yuv420_host, L.hp_pose_submit_ppn_frames_yuv420_device):
-        f.argtypes = [vp, vp, C.POINTER(FrameYUV420), C.c_int, C.c_int, ip]
-    for f in (L.hp_pose_submit_frames_interleaved_host, L.hp_pose_submit_frames_interleaved_device,
-              L.hp_pose_submit_pifpaf_frames_interleaved_host, L.hp_pose_submit_pifpaf_frames_interleaved_device,
-              L.hp_pose_submit_ppn_frames_interleaved_host, L.hp_pose_submit_ppn_frames_interleaved_device):
-        f.argtypes = [vp, vp, C.POINTER(FrameInterleaved), C.c_int, C.c_int, ip]
-    for head in ("", "_pifpaf", "_ppn"):
-        for fmt, rec in (("yuv420", FrameYUV420), ("interleaved", FrameInterleaved)):
-            for where in ("host", "device"):
-                getattr(L, f"hp_pose_submit{head}_frames_{fmt}_rotated_{where}").argtypes = \
-                    [vp, vp, C.POINTER(rec), C.POINTER(C.c_int32), C.c_int, C.c_int, ip]
-        for fmt, rec in (("yuv420_16", FrameYUV420_16), ("interleaved16", FrameInterleaved16)):
-            for where in ("host", "device"):
-                getattr(L, f"hp_pose_submit{head}_frames_{fmt}_{where}").argtypes = \
-                    [vp, vp, C.POINTER(rec), C.POINTER(C.c_int32), C.c_int, C.c_int, ip]
+    L.hp_pose_submit_pifpaf_u8_host.argtypes = [vp, vp, vp, C.c_int, ip]
+    L.hp_pose_submit_pifpaf_u8_device.argtypes = [vp, vp, vp, C.c_int, ip]
+    for name, rec, rotated in frame_calls():
+        getattr(L, name).argtypes = [vp, vp, C.POINTER(rec)] + [C.POINTER(C.c_int32)] * rotated + [C.c_int, C.c_int, ip]
     L.hp_pose_submit_ppn_u8_host.argtypes = [vp, vp, vp, C.c_int, ip]
     L.hp_pose_submit_ppn_u8_device.argtypes = [vp, vp, vp, C.c_int, ip]
     L.hp_pose_debug_read_slot_frames.argtypes = [vp, C.c_int, vp, C.c_int]
@@ -622,55 +649,39 @@ class Engine:
         return [out[i, :n[i]].copy() for i in range(N)]
 
 
-    def submit_pose(self, parser: "PafParser", frames: np.ndarray) -> int:
-        """hp_pose_submit_u8_host (the _pifpaf_ / _ppn_ form for a PifPafParser / PoseProposalParser): enqueue one batch (H2D on the
-        copy stream, graph replay, record D2H); returns the ticket.
-        `frames` must stay alive until collect_pose when it is page-locked memory (DMA reads it directly)."""
-        assert frames.dtype == np.uint8 and frames.flags["C_CONTIGUOUS"]
+    def _submit(self, name: str, parser, *args, n: int) -> int:
+        """lib().<name>(engine, parser, *args, &ticket) for a batch of n frames; returns the ticket for collect_pose"""
         t = C.c_int(-1)
-        if isinstance(parser, PifPafParser):   # OpenPifPaf pack: decoder on its own stream underneath the next batch's convs
-            lib().hp_pose_submit_pifpaf_u8_host.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.POINTER(C.c_int)]
-            check(lib().hp_pose_submit_pifpaf_u8_host(self._h, parser._h, frames.ctypes.data, frames.shape[0], C.byref(t)))
-        elif isinstance(parser, PoseProposalParser):   # PPN pack: the parse is part of the captured graph on the engine stream
-            check(lib().hp_pose_submit_ppn_u8_host(self._h, parser._h, frames.ctypes.data, frames.shape[0], C.byref(t)))
-        else:
-            check(lib().hp_pose_submit_u8_host(self._h, parser._h, frames.ctypes.data, frames.shape[0], C.byref(t)))
-        self._ticket_n = getattr(self, "_ticket_n", {})
-        self._ticket_n[t.value] = frames.shape[0]
-        return t.value
-
-    def submit_pose_device(self, parser: "PafParser", d_frames_ptr: int, n: int) -> int:
-        """hp_pose_submit_u8_device: the frames are already in device memory"""
-        t = C.c_int(-1)
-        if isinstance(parser, PifPafParser):
-            lib().hp_pose_submit_pifpaf_u8_device.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.POINTER(C.c_int)]
-            check(lib().hp_pose_submit_pifpaf_u8_device(self._h, parser._h, d_frames_ptr, n, C.byref(t)))
-        elif isinstance(parser, PoseProposalParser):
-            check(lib().hp_pose_submit_ppn_u8_device(self._h, parser._h, d_frames_ptr, n, C.byref(t)))
-        else:
-            check(lib().hp_pose_submit_u8_device(self._h, parser._h, d_frames_ptr, n, C.byref(t)))
+        check(getattr(lib(), name)(self._h, parser._h, *args, C.byref(t)))
         self._ticket_n = getattr(self, "_ticket_n", {})
         self._ticket_n[t.value] = n
         return t.value
 
+    def _keep_until_collect(self, ticket: int, frames: list) -> int:
+        """host frames stay referenced until their ticket is collected: page-locked ones are read by DMA after submit returns"""
+        self._ticket_frames = getattr(self, "_ticket_frames", {})
+        self._ticket_frames[ticket] = frames
+        return ticket
+
+    def submit_pose(self, parser: "PafParser", frames: np.ndarray) -> int:
+        """hp_pose_submit_u8_host (the _pifpaf_ / _ppn_ form for a PifPafParser / PoseProposalParser): enqueue one batch (H2D on the
+        copy stream, graph replay, record D2H); returns the ticket.  An OpenPifPaf pack decodes on the decoder's own stream underneath
+        the next batch's convs; a PPN pack parses inside the captured graph on the engine stream.
+        `frames` must stay alive until collect_pose when it is page-locked memory (DMA reads it directly)."""
+        assert frames.dtype == np.uint8 and frames.flags["C_CONTIGUOUS"]
+        return self._submit(f"hp_pose_submit{_head(parser)}_u8_host", parser, frames.ctypes.data, frames.shape[0], n=frames.shape[0])
+
+    def submit_pose_device(self, parser: "PafParser", d_frames_ptr: int, n: int) -> int:
+        """hp_pose_submit_u8_device: the frames are already in device memory"""
+        return self._submit(f"hp_pose_submit{_head(parser)}_u8_device", parser, d_frames_ptr, n, n=n)
+
     def _submit_frame_table(self, parser, table, keep_ratio, device: bool, fmt: str = "u8", rotation=None) -> int:
         """hp_pose_submit{,_pifpaf,_ppn}_frames_{fmt}_{host,device}, chosen by the parser's type; with a rotation table (rotation_table)
-        the _rotated_ form.  The 16-bit calls (yuv420_16, interleaved16) take the table, or NULL for None, themselves."""
-        t = C.c_int(-1)
-        head = "_pifpaf" if isinstance(parser, PifPafParser) else "_ppn" if isinstance(parser, PoseProposalParser) else ""
-        where = "device" if device else "host"
-        if fmt in ("yuv420_16", "interleaved16"):
-            fn = getattr(lib(), f"hp_pose_submit{head}_frames_{fmt}_{where}")
-            check(fn(self._h, parser._h, table, rotation, len(table), 1 if keep_ratio else 0, C.byref(t)))
-        elif rotation is None:
-            fn = getattr(lib(), f"hp_pose_submit{head}_frames_{fmt}_{where}")
-            check(fn(self._h, parser._h, table, len(table), 1 if keep_ratio else 0, C.byref(t)))
-        else:
-            fn = getattr(lib(), f"hp_pose_submit{head}_frames_{fmt}_rotated_{where}")
-            check(fn(self._h, parser._h, table, rotation, len(table), 1 if keep_ratio else 0, C.byref(t)))
-        self._ticket_n = getattr(self, "_ticket_n", {})
-        self._ticket_n[t.value] = len(table)
-        return t.value
+        the form of FRAME_CALLS that takes one.  The 16-bit calls (yuv420_16, interleaved16) take the table, or NULL for None, themselves."""
+        rotated = rotation is not None or FRAME_CALLS[fmt][1] == ""
+        rot = (rotation,) if rotated else ()
+        return self._submit(frame_call(_head(parser), fmt, device, rotated), parser, table, *rot, len(table), 1 if keep_ratio else 0,
+                            n=len(table))
 
     def submit_pose_frames(self, parser, frames, keep_ratio: bool = False) -> int:
         """hp_pose_submit_frames_u8_host (hp_pose_submit_pifpaf_frames_u8_host for a PifPafParser, hp_pose_submit_ppn_frames_u8_host for a
@@ -683,10 +694,7 @@ class Engine:
                                                  f"{getattr(f, 'dtype', type(f).__name__)} {getattr(f, 'shape', '')}")
         frames = [np.ascontiguousarray(f) for f in frames]
         table = (FrameU8 * len(frames))(*[FrameU8(f.ctypes.data, f.shape[0], f.shape[1]) for f in frames])
-        t = self._submit_frame_table(parser, table, keep_ratio, device=False)
-        self._ticket_frames = getattr(self, "_ticket_frames", {})
-        self._ticket_frames[t] = frames
-        return t
+        return self._keep_until_collect(self._submit_frame_table(parser, table, keep_ratio, device=False), frames)
 
     def submit_pose_frames_device(self, parser, frames, keep_ratio: bool = False) -> int:
         """the same for frames in device memory, given as [(ptr, h, w), ...] (u8 HWC3, rows packed).  The resize kernel reads them in
@@ -700,30 +708,21 @@ class Engine:
         and resized on the GPU as submit_pose_frames resizes BGR frames; returns the ticket for collect_pose.  Page-locked frames are
         kept referenced until the ticket is collected.  rotation: clockwise degrees (0, 90, 180, 270), one for the batch or one per
         frame, applied as cv::rotate after the conversion (the _rotated_ call); None: upright."""
-        rot = {} if rotation is None else {"rotation": rotation_table(rotation, len(frames))}
-        layouts = [layout] * len(frames) if isinstance(layout, str) else list(layout)
-        if len(layouts) != len(frames) or any(lay not in YUV420_LAYOUTS for lay in layouts):
-            raise HyperposeError(HP_ERR_ARG, f"layout {layout!r}: expected one of {sorted(YUV420_LAYOUTS)}, or one per frame")
+        rot = _rotation_arg(rotation, len(frames))
+        layouts = _per_frame(layout, len(frames), YUV420_LAYOUTS, "layout")
         for i, f in enumerate(frames):
             if not isinstance(f, np.ndarray) or f.dtype != np.uint8 or f.ndim != 2 or f.shape[0] % 3 or f.shape[0] == 0:
                 raise HyperposeError(HP_ERR_ARG, f"frame {i}: expected a uint8 (3H/2, W) YUV 4:2:0 array, got "
                                                  f"{getattr(f, 'dtype', type(f).__name__)} {getattr(f, 'shape', '')}")
         frames = [np.ascontiguousarray(f) for f in frames]
         table = (FrameYUV420 * len(frames))(*[yuv420_record(f, lay) for f, lay in zip(frames, layouts)])
-        t = self._submit_frame_table(parser, table, keep_ratio, device=False, fmt="yuv420", **rot)
-        self._ticket_frames = getattr(self, "_ticket_frames", {})
-        self._ticket_frames[t] = frames
-        return t
+        return self._keep_until_collect(self._submit_frame_table(parser, table, keep_ratio, device=False, fmt="yuv420", **rot), frames)
 
     def submit_pose_yuv420_device(self, parser, frames, keep_ratio: bool = False, rotation=None) -> int:
         """the same for YUV 4:2:0 frames in device memory, given as FrameYUV420 records (device plane pointers and pitches, e.g. an
         NVDEC surface).  The resize kernel reads them in place: they must stay valid and unchanged until the ticket is collected."""
-        rot = {} if rotation is None else {"rotation": rotation_table(rotation, len(frames))}
-        for i, f in enumerate(frames):
-            if not isinstance(f, FrameYUV420):
-                raise HyperposeError(HP_ERR_ARG, f"frame {i}: expected a FrameYUV420, got {type(f).__name__}")
-        table = (FrameYUV420 * len(frames))(*frames)
-        return self._submit_frame_table(parser, table, keep_ratio, device=True, fmt="yuv420", **rot)
+        rot = _rotation_arg(rotation, len(frames))
+        return self._submit_frame_table(parser, _record_table(frames, FrameYUV420), keep_ratio, device=True, fmt="yuv420", **rot)
 
     def submit_pose_interleaved(self, parser, frames, format, keep_ratio: bool = False, rotation=None) -> int:
         """hp_pose_submit{,_pifpaf,_ppn}_frames_interleaved_host, by the parser's type: a list of uint8 frames, (H, W, 3) for bgr / rgb,
@@ -732,10 +731,8 @@ class Engine:
         submit_pose_frames resizes BGR frames; returns the ticket for collect_pose.  A frame whose rows are contiguous but strided (a
         crop view of a larger frame) is passed with strides[0] as its pitch, not copied.  Page-locked frames are kept referenced until
         the ticket is collected.  rotation as for submit_pose_yuv420."""
-        rot = {} if rotation is None else {"rotation": rotation_table(rotation, len(frames))}
-        formats = [format] * len(frames) if isinstance(format, str) else list(format)
-        if len(formats) != len(frames) or any(fmt not in PIXEL_FORMATS for fmt in formats):
-            raise HyperposeError(HP_ERR_ARG, f"format {format!r}: expected one of {sorted(PIXEL_FORMATS)}, or one per frame")
+        rot = _rotation_arg(rotation, len(frames))
+        formats = _per_frame(format, len(frames), PIXEL_FORMATS, "format")
         for i, (f, fmt) in enumerate(zip(frames, formats)):
             ch = PIXEL_CHANNELS[fmt]
             shape = "(H, W)" if ch is None else f"(H, W, {ch})"
@@ -747,21 +744,15 @@ class Engine:
                 raise HyperposeError(HP_ERR_ARG, f"frame {i}: the bytes of each row must be contiguous, rows at least {row} bytes apart "
                                                  f"(strides {f.strides})")
         table = (FrameInterleaved * len(frames))(*[interleaved_record(f, fmt) for f, fmt in zip(frames, formats)])
-        t = self._submit_frame_table(parser, table, keep_ratio, device=False, fmt="interleaved", **rot)
-        self._ticket_frames = getattr(self, "_ticket_frames", {})
-        self._ticket_frames[t] = list(frames)
-        return t
+        return self._keep_until_collect(self._submit_frame_table(parser, table, keep_ratio, device=False, fmt="interleaved", **rot),
+                                        list(frames))
 
     def submit_pose_interleaved_device(self, parser, frames, keep_ratio: bool = False, rotation=None) -> int:
         """the same for interleaved frames in device memory, given as FrameInterleaved records (device pointer, size, pitch, format:
         a cudaMallocPitch allocation, an NvBufSurface, a crop of either).  The resize kernel reads them in place: they must stay valid
         and unchanged until the ticket is collected."""
-        rot = {} if rotation is None else {"rotation": rotation_table(rotation, len(frames))}
-        for i, f in enumerate(frames):
-            if not isinstance(f, FrameInterleaved):
-                raise HyperposeError(HP_ERR_ARG, f"frame {i}: expected a FrameInterleaved, got {type(f).__name__}")
-        table = (FrameInterleaved * len(frames))(*frames)
-        return self._submit_frame_table(parser, table, keep_ratio, device=True, fmt="interleaved", **rot)
+        rot = _rotation_arg(rotation, len(frames))
+        return self._submit_frame_table(parser, _record_table(frames, FrameInterleaved), keep_ratio, device=True, fmt="interleaved", **rot)
 
     def submit_pose_yuv420_16(self, parser, frames, layout, bits, keep_ratio: bool = False, rotation=None) -> int:
         """hp_pose_submit{,_pifpaf,_ppn}_frames_yuv420_16_host, by the parser's type: submit_pose_yuv420 for YUV 4:2:0 frames of 16-bit
@@ -769,42 +760,31 @@ class Engine:
         significant bits of the samples, LSB-aligned, 9..16, one for the batch or one per frame (16 for P010 / P016, 10 for
         yuv420p10le).  Each sample is reduced as src.convertTo(CV_8U, 2^-(bits-8)) does, then converted, rotated and resized as by
         submit_pose_yuv420."""
-        rot = rotation_table(rotation, len(frames)) if rotation is not None else None
+        rot = _rotation_arg(rotation, len(frames))
         bl = bits_list(bits, len(frames))
-        layouts = [layout] * len(frames) if isinstance(layout, str) else list(layout)
-        if len(layouts) != len(frames) or any(lay not in YUV420_16_LAYOUTS for lay in layouts):
-            raise HyperposeError(HP_ERR_ARG, f"layout {layout!r}: expected one of {sorted(YUV420_16_LAYOUTS)}, or one per frame")
+        layouts = _per_frame(layout, len(frames), YUV420_16_LAYOUTS, "layout")
         for i, f in enumerate(frames):
             if not isinstance(f, np.ndarray) or f.dtype != np.uint16 or f.ndim != 2 or f.shape[0] % 3 or f.shape[0] == 0:
                 raise HyperposeError(HP_ERR_ARG, f"frame {i}: expected a uint16 (3H/2, W) YUV 4:2:0 array, got "
                                                  f"{getattr(f, 'dtype', type(f).__name__)} {getattr(f, 'shape', '')}")
         frames = [np.ascontiguousarray(f) for f in frames]
         table = (FrameYUV420_16 * len(frames))(*[yuv420_16_record(f, lay, b) for f, lay, b in zip(frames, layouts, bl)])
-        t = self._submit_frame_table(parser, table, keep_ratio, device=False, fmt="yuv420_16", rotation=rot)
-        self._ticket_frames = getattr(self, "_ticket_frames", {})
-        self._ticket_frames[t] = frames
-        return t
+        return self._keep_until_collect(self._submit_frame_table(parser, table, keep_ratio, device=False, fmt="yuv420_16", **rot), frames)
 
     def submit_pose_yuv420_16_device(self, parser, frames, keep_ratio: bool = False, rotation=None) -> int:
         """the same for 16-bit YUV 4:2:0 frames in device memory, given as FrameYUV420_16 records, each with its bits (a P010 / P016
         NVDEC surface).  The resize kernel reads them in place: they must stay valid and unchanged until the ticket is collected."""
-        rot = rotation_table(rotation, len(frames)) if rotation is not None else None
-        for i, f in enumerate(frames):
-            if not isinstance(f, FrameYUV420_16):
-                raise HyperposeError(HP_ERR_ARG, f"frame {i}: expected a FrameYUV420_16, got {type(f).__name__}")
-        table = (FrameYUV420_16 * len(frames))(*frames)
-        return self._submit_frame_table(parser, table, keep_ratio, device=True, fmt="yuv420_16", rotation=rot)
+        rot = _rotation_arg(rotation, len(frames))
+        return self._submit_frame_table(parser, _record_table(frames, FrameYUV420_16), keep_ratio, device=True, fmt="yuv420_16", **rot)
 
     def submit_pose_interleaved16(self, parser, frames, format, bits, keep_ratio: bool = False, rotation=None) -> int:
         """hp_pose_submit{,_pifpaf,_ppn}_frames_interleaved16_host, by the parser's type: submit_pose_interleaved for frames of 16-bit
         samples, uint16 (H, W, 3) for bgr48 / rgb48, (H, W, 4) for bgra64 / rgba64, (H, W) for gray16; `format` is one of those names
         or one per frame.  bits as for submit_pose_yuv420_16.  A frame whose rows are contiguous but strided is passed with
         strides[0] as its pitch, not copied."""
-        rot = rotation_table(rotation, len(frames)) if rotation is not None else None
+        rot = _rotation_arg(rotation, len(frames))
         bl = bits_list(bits, len(frames))
-        formats = [format] * len(frames) if isinstance(format, str) else list(format)
-        if len(formats) != len(frames) or any(fmt not in INTERLEAVED16_FORMATS for fmt in formats):
-            raise HyperposeError(HP_ERR_ARG, f"format {format!r}: expected one of {sorted(INTERLEAVED16_FORMATS)}, or one per frame")
+        formats = _per_frame(format, len(frames), INTERLEAVED16_FORMATS, "format")
         for i, (f, fmt) in enumerate(zip(frames, formats)):
             ch = PIXEL_CHANNELS[INTERLEAVED16_FORMATS[fmt]]
             shape = "(H, W)" if ch is None else f"(H, W, {ch})"
@@ -816,20 +796,15 @@ class Engine:
                 raise HyperposeError(HP_ERR_ARG, f"frame {i}: the samples of each row must be contiguous, rows at least {row} bytes "
                                                  f"apart (strides {f.strides})")
         table = (FrameInterleaved16 * len(frames))(*[interleaved16_record(f, fmt, b) for f, fmt, b in zip(frames, formats, bl)])
-        t = self._submit_frame_table(parser, table, keep_ratio, device=False, fmt="interleaved16", rotation=rot)
-        self._ticket_frames = getattr(self, "_ticket_frames", {})
-        self._ticket_frames[t] = list(frames)
-        return t
+        return self._keep_until_collect(self._submit_frame_table(parser, table, keep_ratio, device=False, fmt="interleaved16", **rot),
+                                        list(frames))
 
     def submit_pose_interleaved16_device(self, parser, frames, keep_ratio: bool = False, rotation=None) -> int:
         """the same for 16-bit interleaved frames in device memory, given as FrameInterleaved16 records, each with its bits.  The
         resize kernel reads them in place: they must stay valid and unchanged until the ticket is collected."""
-        rot = rotation_table(rotation, len(frames)) if rotation is not None else None
-        for i, f in enumerate(frames):
-            if not isinstance(f, FrameInterleaved16):
-                raise HyperposeError(HP_ERR_ARG, f"frame {i}: expected a FrameInterleaved16, got {type(f).__name__}")
-        table = (FrameInterleaved16 * len(frames))(*frames)
-        return self._submit_frame_table(parser, table, keep_ratio, device=True, fmt="interleaved16", rotation=rot)
+        rot = _rotation_arg(rotation, len(frames))
+        return self._submit_frame_table(parser, _record_table(frames, FrameInterleaved16), keep_ratio, device=True, fmt="interleaved16",
+                                        **rot)
 
     def debug_read_slot_frames(self, ticket: int, n: int) -> np.ndarray:
         """the first n resized network-size frames u8[n,in_h,in_w,3] of a ticket in flight or collected"""
@@ -983,8 +958,7 @@ class PifPafParser:
 EXPORTS += ["hp_ppn_create", "hp_ppn_destroy", "hp_ppn_set_point_thresh", "hp_ppn_set_limb_thresh", "hp_ppn_set_nms_thresh",
             "hp_ppn_process_host", "hp_ppn_process_device", "hp_ppn_process_device_strided", "hp_ppn_fetch", "hp_ppn_launch_count",
             "hp_ppn_prepare", "hp_ppn_state", "hp_ppn_copy_results_host_async", "hp_ppn_grow_capacity",
-            "hp_pose_submit_ppn_u8_host", "hp_pose_submit_ppn_u8_device", "hp_pose_submit_ppn_frames_u8_host",
-            "hp_pose_submit_ppn_frames_u8_device"]
+            "hp_pose_submit_ppn_u8_host", "hp_pose_submit_ppn_u8_device"]
 
 
 class PoseProposalParser:

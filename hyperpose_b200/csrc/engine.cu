@@ -161,6 +161,15 @@ struct Interleaved16FrameDesc {
 };
 static_assert(sizeof(Interleaved16FrameDesc) == 48, "Interleaved16FrameDesc is uploaded as raw bytes");
 
+// A pipelined slot keeps one descriptor buffer for whichever frame type its batch has: max_batch of the largest descriptor, in
+// cudaMalloc / cudaMallocHost memory (256-byte aligned at least).  Reusing it across types is safe: a slot is only refilled after it
+// has been collected, and collecting waits for its `done` event, which follows the resize that reads the descriptors.
+constexpr size_t FRAME_DESC_BYTES = 64;
+template <class... Desc>
+constexpr bool fits_desc_buffer = ((sizeof(Desc) <= FRAME_DESC_BYTES && 256 % alignof(Desc) == 0) && ...);
+static_assert(fits_desc_buffer<FrameDesc, YuvFrameDesc, InterleavedFrameDesc, Yuv16FrameDesc, Interleaved16FrameDesc>,
+              "every resize descriptor fits a slot's descriptor buffer");
+
 // Source fetches of the resize: byte c (B, G, R) of source pixel x of one source row.
 struct BgrRow {
     const uint8_t* p;
@@ -1087,11 +1096,7 @@ struct hp_engine {
         // camera-size frames (hp_pose_submit_frames_u8_*): their source pixels, pinned staging for pageable ones, resize descriptors
         uint8_t* d_src = nullptr; size_t d_src_bytes = 0;
         uint8_t* pin_src = nullptr; size_t pin_src_bytes = 0;
-        FrameDesc* d_desc = nullptr; FrameDesc* pin_desc = nullptr;   // [max_batch]
-        YuvFrameDesc* d_ydesc = nullptr; YuvFrameDesc* pin_ydesc = nullptr;   // [max_batch] (hp_pose_submit_*frames_yuv420_*)
-        InterleavedFrameDesc* d_idesc = nullptr; InterleavedFrameDesc* pin_idesc = nullptr;   // [max_batch] (*frames_interleaved_*)
-        Yuv16FrameDesc* d_y16desc = nullptr; Yuv16FrameDesc* pin_y16desc = nullptr;   // [max_batch] (*frames_yuv420_16_*)
-        Interleaved16FrameDesc* d_i16desc = nullptr; Interleaved16FrameDesc* pin_i16desc = nullptr;   // [max_batch] (*frames_interleaved16_*)
+        void* d_desc = nullptr; void* pin_desc = nullptr;   // [max_batch * FRAME_DESC_BYTES]: the batch's resize descriptors, any type
         hp_human* pin_humans = nullptr; size_t pin_humans_n = 0;
         int* pin_counts = nullptr; size_t pin_counts_n = 0;   // [N counts | N flags]
         cudaEvent_t h2d_done = nullptr, done = nullptr;
@@ -1726,14 +1731,6 @@ void free_engine(hp_engine* e)
         if (sl.pin_src) cudaFreeHost(sl.pin_src);
         if (sl.d_desc) cudaFree(sl.d_desc);
         if (sl.pin_desc) cudaFreeHost(sl.pin_desc);
-        if (sl.d_ydesc) cudaFree(sl.d_ydesc);
-        if (sl.pin_ydesc) cudaFreeHost(sl.pin_ydesc);
-        if (sl.d_idesc) cudaFree(sl.d_idesc);
-        if (sl.pin_idesc) cudaFreeHost(sl.pin_idesc);
-        if (sl.d_y16desc) cudaFree(sl.d_y16desc);
-        if (sl.pin_y16desc) cudaFreeHost(sl.pin_y16desc);
-        if (sl.d_i16desc) cudaFree(sl.d_i16desc);
-        if (sl.pin_i16desc) cudaFreeHost(sl.pin_i16desc);
         if (sl.pin_humans) cudaFreeHost(sl.pin_humans);
         if (sl.pin_counts) cudaFreeHost(sl.pin_counts);
         if (sl.h2d_done) cudaEventDestroy(sl.h2d_done);
@@ -2220,18 +2217,9 @@ static int frame_desc(const hp_engine* e, const uint8_t* src, int src_h, int src
     return HP_OK;
 }
 
-// N network-size frames into dst on the engine stream, frame i read through d_desc[i]
-static int launch_resize(hp_engine* e, const FrameDesc* d_desc, uint8_t* dst, int N)
-{
-    const dim3 grid((e->in_h + RZ_ROWS - 1) / RZ_ROWS, N);
-    resize_frames_u8c3_kernel<<<grid, 256, (size_t)e->in_w * sizeof(int2), e->stream>>>(d_desc, dst, e->in_h, e->in_w);
-    e->launches++;
-    HP_CUDA_TRY(cudaGetLastError());
-    return HP_OK;
-}
-
 extern "C++" {   // overloads and templates, inside the C ABI block
-// the resize kernel of a fused-conversion descriptor type; rotated: the instantiation for a batch with a rotated frame
+// the resize kernel of a descriptor type; rotated: the instantiation for a batch with a rotated frame (BGR frames have none)
+static auto resize_kernel(const FrameDesc*, bool) { return resize_frames_u8c3_kernel; }
 static auto resize_kernel(const YuvFrameDesc*, bool rotated) { return rotated ? resize_frames_yuv420_kernel<true> : resize_frames_yuv420_kernel<false>; }
 static auto resize_kernel(const InterleavedFrameDesc*, bool rotated)
 {
@@ -2246,9 +2234,10 @@ static auto resize_kernel(const Interleaved16FrameDesc*, bool rotated)
     return rotated ? resize_frames_interleaved16_kernel<true> : resize_frames_interleaved16_kernel<false>;
 }
 
-// rotated: some frame of the batch has a rotation (the rotated instantiation serves the upright frames of such a batch too)
+// N network-size frames into dst on the engine stream, frame i read through d_desc[i].  rotated: some frame of the batch has a
+// rotation (the rotated instantiation serves the upright frames of such a batch too)
 template <class Desc>
-static int launch_resize_fused(hp_engine* e, const Desc* d_desc, uint8_t* dst, int N, bool rotated)
+static int launch_resize(hp_engine* e, const Desc* d_desc, uint8_t* dst, int N, bool rotated = false)
 {
     const dim3 grid((e->in_h + RZ_ROWS - 1) / RZ_ROWS, N);
     resize_kernel(d_desc, rotated)<<<grid, 256, (size_t)e->in_w * sizeof(int2), e->stream>>>(d_desc, dst, e->in_h, e->in_w);
@@ -2725,10 +2714,10 @@ int slot_alloc(hp_engine* e, hp_engine::PoseSlot& sl, int hcap)
     return HP_OK;
 }
 
-// the N frames of a submitted batch into the slot's device buffer, ordered before the engine stream's next work: frames already in
-// HBM by a D2D copy on the engine stream, host frames by an H2D on the copy stream (pageable ones through the slot's pinned staging,
-// free since the slot was collected)
-int slot_upload(hp_engine* e, hp_engine::PoseSlot& sl, const uint8_t* frames, int N, bool device_src)
+// the N network-size frames of a submitted batch into the slot's device buffer, ordered before the engine stream's next work: frames
+// already in HBM by a D2D copy on the engine stream, host frames by an H2D on the copy stream (pageable ones through the slot's pinned
+// staging, free since the slot was collected)
+int slot_upload(hp_engine* e, hp_engine::PoseSlot& sl, const void* frames, int N, bool device_src)
 {
     const size_t bytes = (size_t)N * e->in_h * e->in_w * 3;
     if (device_src) {
@@ -2738,7 +2727,7 @@ int slot_upload(hp_engine* e, hp_engine::PoseSlot& sl, const uint8_t* frames, in
     cudaPointerAttributes attr;
     const bool pinned = (cudaPointerGetAttributes(&attr, frames) == cudaSuccess && attr.type == cudaMemoryTypeHost);
     if (!pinned) cudaGetLastError();
-    const uint8_t* src = frames;
+    const void* src = frames;
     if (!pinned) {
         if (!sl.pin_frames) HP_CUDA_TRY(cudaMallocHost(&sl.pin_frames, (size_t)e->max_batch * e->in_h * e->in_w * 3));
         memcpy(sl.pin_frames, frames, bytes);
@@ -2750,78 +2739,34 @@ int slot_upload(hp_engine* e, hp_engine::PoseSlot& sl, const uint8_t* frames, in
     return HP_OK;
 }
 
-// The N frames of any size of a submitted batch, resized into the slot's device buffer by one launch on the engine stream, ahead of
-// the batch's network.  Host frames reach the slot's source buffer (256-byte aligned per frame) by H2Ds on the copy stream: page-locked
-// ones straight from the caller, pageable ones through the slot's pinned staging.  Device frames are read in place.  The descriptors
-// travel on the copy stream too.  Source buffer and staging grow here: the slot is idle, it has been collected.  The resize stays
-// outside the captured graph, so the graph never sees a frame geometry or a source address and new sizes never recapture it.
-int slot_upload_frames(hp_engine* e, hp_engine::PoseSlot& sl, FrameDesc* descs, int N, bool device_src)
+// Byte offsets in the slot's source buffer of the N host frames of a batch, each row-compacted (host_bytes(f) bytes) and 256-byte
+// aligned: off[N] is the whole batch.  The buffer grows here to hold them: the slot is idle, it has been collected.
+template <class HostBytes>
+int slot_src_layout(hp_engine::PoseSlot& sl, int N, HostBytes host_bytes, std::vector<size_t>& off)
 {
-    if (!sl.d_desc) {
-        HP_CUDA_TRY(cudaMalloc(&sl.d_desc, e->max_batch * sizeof(FrameDesc)));
-        HP_CUDA_TRY(cudaMallocHost(&sl.pin_desc, e->max_batch * sizeof(FrameDesc)));
-    }
-    if (!device_src) {
-        std::vector<size_t> off(N + 1, 0);
-        std::vector<char> pinned(N, 0);
-        bool any_pageable = false;
-        for (int f = 0; f < N; ++f) {
-            off[f + 1] = off[f] + (((size_t)descs[f].sh * descs[f].sw * 3 + 255) & ~(size_t)255);
-            cudaPointerAttributes attr;
-            pinned[f] = cudaPointerGetAttributes(&attr, descs[f].src) == cudaSuccess && attr.type == cudaMemoryTypeHost;
-            if (!pinned[f]) { cudaGetLastError(); any_pageable = true; }
-        }
-        if (sl.d_src_bytes < off[N]) {
-            if (sl.d_src) cudaFree(sl.d_src);
-            sl.d_src = nullptr; sl.d_src_bytes = 0;
-            HP_CUDA_TRY(cudaMalloc(&sl.d_src, off[N]));
-            sl.d_src_bytes = off[N];
-        }
-        if (any_pageable && sl.pin_src_bytes < off[N]) {
-            if (sl.pin_src) cudaFreeHost(sl.pin_src);
-            sl.pin_src = nullptr; sl.pin_src_bytes = 0;
-            HP_CUDA_TRY(cudaMallocHost(&sl.pin_src, off[N]));
-            sl.pin_src_bytes = off[N];
-        }
-        for (int f = 0; f < N; ++f) {
-            const size_t bytes = (size_t)descs[f].sh * descs[f].sw * 3;
-            const uint8_t* src = descs[f].src;
-            if (!pinned[f]) {
-                memcpy(sl.pin_src + off[f], src, bytes);
-                src = sl.pin_src + off[f];
-            }
-            HP_CUDA_TRY(cudaMemcpyAsync(sl.d_src + off[f], src, bytes, cudaMemcpyHostToDevice, e->copy_stream));
-            descs[f].src = sl.d_src + off[f];
-        }
-    }
-    memcpy(sl.pin_desc, descs, N * sizeof(FrameDesc));
-    HP_CUDA_TRY(cudaMemcpyAsync(sl.d_desc, sl.pin_desc, N * sizeof(FrameDesc), cudaMemcpyHostToDevice, e->copy_stream));
-    HP_CUDA_TRY(cudaEventRecord(sl.h2d_done, e->copy_stream));
-    HP_CUDA_TRY(cudaStreamWaitEvent(e->stream, sl.h2d_done, 0));
-    return launch_resize(e, sl.d_desc, sl.d_frames, N);
-}
-
-// the slot's source buffer for `bytes` of row-compacted host frames (grown here: the slot is idle, it has been collected)
-int slot_src_reserve(hp_engine::PoseSlot& sl, size_t bytes)
-{
-    if (sl.d_src_bytes < bytes) {
+    off.assign(N + 1, 0);
+    for (int f = 0; f < N; ++f) off[f + 1] = off[f] + ((host_bytes(f) + 255) & ~(size_t)255);
+    if (sl.d_src_bytes < off[N]) {
         if (sl.d_src) cudaFree(sl.d_src);
         sl.d_src = nullptr; sl.d_src_bytes = 0;
-        HP_CUDA_TRY(cudaMalloc(&sl.d_src, bytes));
-        sl.d_src_bytes = bytes;
+        HP_CUDA_TRY(cudaMalloc(&sl.d_src, off[N]));
+        sl.d_src_bytes = off[N];
     }
     return HP_OK;
 }
 
 // one plane of a host frame on the copy stream: rows x width bytes at `src` with pitch `pitch` into the slot's source buffer at byte
-// offset `at`, row-compacted.  By a pitched DMA from the caller when it is page-locked, else through the slot's pinned staging, which
-// grows to `total` bytes (the whole batch) on the first pageable plane that needs it.
+// offset `at`, row-compacted.  By DMA from the caller when it is page-locked, else through the slot's pinned staging, which grows to
+// `total` bytes (the whole batch) on the first pageable plane that needs it.  A plane of packed rows (pitch = width) goes as one
+// contiguous copy; a pitched one by a pitched DMA, or row by row into the staging.
 int upload_plane(hp_engine* e, hp_engine::PoseSlot& sl, const uint8_t* src, int pitch, int rows, int width, size_t at, size_t total)
 {
+    const bool packed = pitch == width;
     cudaPointerAttributes attr;
     const bool pinned = cudaPointerGetAttributes(&attr, src) == cudaSuccess && attr.type == cudaMemoryTypeHost;
     if (pinned) {
-        HP_CUDA_TRY(cudaMemcpy2DAsync(sl.d_src + at, width, src, pitch, width, rows, cudaMemcpyHostToDevice, e->copy_stream));
+        if (packed) HP_CUDA_TRY(cudaMemcpyAsync(sl.d_src + at, src, (size_t)rows * width, cudaMemcpyHostToDevice, e->copy_stream));
+        else HP_CUDA_TRY(cudaMemcpy2DAsync(sl.d_src + at, width, src, pitch, width, rows, cudaMemcpyHostToDevice, e->copy_stream));
         return HP_OK;
     }
     cudaGetLastError();
@@ -2831,68 +2776,66 @@ int upload_plane(hp_engine* e, hp_engine::PoseSlot& sl, const uint8_t* src, int 
         HP_CUDA_TRY(cudaMallocHost(&sl.pin_src, total));
         sl.pin_src_bytes = total;
     }
-    for (int r = 0; r < rows; ++r) memcpy(sl.pin_src + at + (size_t)r * width, src + (size_t)r * pitch, width);
+    if (packed) memcpy(sl.pin_src + at, src, (size_t)rows * width);
+    else for (int r = 0; r < rows; ++r) memcpy(sl.pin_src + at + (size_t)r * width, src + (size_t)r * pitch, width);
     HP_CUDA_TRY(cudaMemcpyAsync(sl.d_src + at, sl.pin_src + at, (size_t)rows * width, cudaMemcpyHostToDevice, e->copy_stream));
     return HP_OK;
 }
 
-// A batch's fused-conversion descriptors to the slot's device array for them (d_desc, allocated here with its pinned twin) on the copy
-// stream, ordered before the engine stream's next work, then the resize launch that reads them.
-template <class Desc>
-int slot_launch_fused(hp_engine* e, hp_engine::PoseSlot& sl, Desc*& d_desc, Desc*& pin_desc, const Desc* descs, int N)
+// upload_host_frames: the N host frames of a batch into the slot's source buffer (slot_src_layout, upload_plane), each descriptor
+// pointed at its frame's copy there.  One overload per descriptor type.
+
+// BGR frames (FrameDesc): one plane of packed rows each
+int upload_host_frames(hp_engine* e, hp_engine::PoseSlot& sl, FrameDesc* descs, int N)
 {
-    if (!d_desc) {
-        HP_CUDA_TRY(cudaMalloc(&d_desc, e->max_batch * sizeof(Desc)));
-        HP_CUDA_TRY(cudaMallocHost(&pin_desc, e->max_batch * sizeof(Desc)));
+    std::vector<size_t> off;
+    int rc = slot_src_layout(sl, N, [&](int f) { return (size_t)descs[f].sh * descs[f].sw * 3; }, off);
+    for (int f = 0; f < N && !rc; ++f) {
+        FrameDesc& d = descs[f];
+        rc = upload_plane(e, sl, d.src, 3 * d.sw, d.sh, 3 * d.sw, off[f], off[N]);
+        d.src = sl.d_src + off[f];
     }
-    memcpy(pin_desc, descs, N * sizeof(Desc));
-    HP_CUDA_TRY(cudaMemcpyAsync(d_desc, pin_desc, N * sizeof(Desc), cudaMemcpyHostToDevice, e->copy_stream));
-    HP_CUDA_TRY(cudaEventRecord(sl.h2d_done, e->copy_stream));
-    HP_CUDA_TRY(cudaStreamWaitEvent(e->stream, sl.h2d_done, 0));
-    return launch_resize_fused(e, d_desc, sl.d_frames, N, std::any_of(descs, descs + N, [](const Desc& d) { return d.rot != 0; }));
+    return rc;
 }
 
-// The same for YUV 4:2:0 frames (YuvFrameDesc, or Yuv16FrameDesc of 16-bit samples).  A host frame is copied row-compacted into the
-// slot's source buffer: its luma plane with pitch width, then the interleaved UV plane (semi-planar, copied once) or the U and V planes
-// (planar), 1.5 samples per pixel.  Each plane goes by a pitched DMA from the caller when it is page-locked, else through the slot's
-// pinned staging.  Device frames are read in place.
+// YUV 4:2:0 frames (YuvFrameDesc, or Yuv16FrameDesc of 16-bit samples): the luma plane with pitch width, then the interleaved UV plane
+// (semi-planar, copied once) or the U and V planes (planar), 1.5 samples per pixel
 template <class Desc>
-int slot_upload_yuv(hp_engine* e, hp_engine::PoseSlot& sl, Desc*& d_desc, Desc*& pin_desc, Desc* descs, int N, bool device_src)
+int upload_yuv_frames(hp_engine* e, hp_engine::PoseSlot& sl, Desc* descs, int N)
 {
     using Sample = std::remove_pointer_t<decltype(Desc::y)>;   // const uint8_t or const uint16_t
     constexpr size_t S = sizeof(Sample);
-    if (!device_src) {
-        std::vector<size_t> off(N + 1, 0);
-        for (int f = 0; f < N; ++f) off[f + 1] = off[f] + (((size_t)descs[f].sh * descs[f].sw * 3 / 2 * S + 255) & ~(size_t)255);
-        int rc = slot_src_reserve(sl, off[N]);
-        if (rc) return rc;
-        auto copy_plane = [&](const Sample* src, int pitch, int rows, int width, size_t at) {
-            return upload_plane(e, sl, (const uint8_t*)src, pitch, rows, width * (int)S, at, off[N]);
-        };
-        for (int f = 0; f < N; ++f) {
-            Desc& d = descs[f];
-            const size_t luma = (size_t)d.sh * d.sw * S, at = off[f] + luma;
-            if ((rc = copy_plane(d.y, d.pitch_y, d.sh, d.sw, off[f]))) return rc;
-            if (d.uv_step == 2) {   // one interleaved plane starting at the lower of u, v
-                const Sample* base = d.u < d.v ? d.u : d.v;
-                if ((rc = copy_plane(base, d.pitch_uv, d.sh / 2, d.sw, at))) return rc;
-                d.u = (const Sample*)(sl.d_src + at) + (d.u - base);
-                d.v = (const Sample*)(sl.d_src + at) + (d.v - base);
-                d.pitch_uv = d.sw * S;
-            } else {
-                const size_t chroma = luma / 4;
-                if ((rc = copy_plane(d.u, d.pitch_uv, d.sh / 2, d.sw / 2, at))) return rc;
-                if ((rc = copy_plane(d.v, d.pitch_uv, d.sh / 2, d.sw / 2, at + chroma))) return rc;
-                d.u = (const Sample*)(sl.d_src + at);
-                d.v = (const Sample*)(sl.d_src + at + chroma);
-                d.pitch_uv = d.sw / 2 * S;
-            }
-            d.y = (const Sample*)(sl.d_src + off[f]);
-            d.pitch_y = d.sw * S;
+    std::vector<size_t> off;
+    int rc = slot_src_layout(sl, N, [&](int f) { return (size_t)descs[f].sh * descs[f].sw * 3 / 2 * S; }, off);
+    if (rc) return rc;
+    auto copy_plane = [&](const Sample* src, int pitch, int rows, int width, size_t at) {
+        return upload_plane(e, sl, (const uint8_t*)src, pitch, rows, width * (int)S, at, off[N]);
+    };
+    for (int f = 0; f < N; ++f) {
+        Desc& d = descs[f];
+        const size_t luma = (size_t)d.sh * d.sw * S, at = off[f] + luma;
+        if ((rc = copy_plane(d.y, d.pitch_y, d.sh, d.sw, off[f]))) return rc;
+        if (d.uv_step == 2) {   // one interleaved plane starting at the lower of u, v
+            const Sample* base = d.u < d.v ? d.u : d.v;
+            if ((rc = copy_plane(base, d.pitch_uv, d.sh / 2, d.sw, at))) return rc;
+            d.u = (const Sample*)(sl.d_src + at) + (d.u - base);
+            d.v = (const Sample*)(sl.d_src + at) + (d.v - base);
+            d.pitch_uv = d.sw * S;
+        } else {
+            const size_t chroma = luma / 4;
+            if ((rc = copy_plane(d.u, d.pitch_uv, d.sh / 2, d.sw / 2, at))) return rc;
+            if ((rc = copy_plane(d.v, d.pitch_uv, d.sh / 2, d.sw / 2, at + chroma))) return rc;
+            d.u = (const Sample*)(sl.d_src + at);
+            d.v = (const Sample*)(sl.d_src + at + chroma);
+            d.pitch_uv = d.sw / 2 * S;
         }
+        d.y = (const Sample*)(sl.d_src + off[f]);
+        d.pitch_y = d.sw * S;
     }
-    return slot_launch_fused(e, sl, d_desc, pin_desc, descs, N);
+    return HP_OK;
 }
+int upload_host_frames(hp_engine* e, hp_engine::PoseSlot& sl, YuvFrameDesc* descs, int N) { return upload_yuv_frames(e, sl, descs, N); }
+int upload_host_frames(hp_engine* e, hp_engine::PoseSlot& sl, Yuv16FrameDesc* descs, int N) { return upload_yuv_frames(e, sl, descs, N); }
 
 // bytes per pixel of an hp_pixel_format, 0 for an unknown one
 int pixel_bytes(int format)
@@ -2906,58 +2849,68 @@ int pixel_bytes(int format)
     }
 }
 
-// The same for interleaved frames (InterleavedFrameDesc, or Interleaved16FrameDesc of 16-bit samples).  A host frame is copied
-// row-compacted into the slot's source buffer (width * bytes per pixel per row), by a pitched DMA from the caller when it is
-// page-locked, else through the slot's pinned staging.  Device frames are read in place with their pitch.
+// interleaved frames (InterleavedFrameDesc, or Interleaved16FrameDesc of 16-bit samples): one plane of width * bytes per pixel per row
 template <class Desc>
-int slot_upload_interleaved(hp_engine* e, hp_engine::PoseSlot& sl, Desc*& d_desc, Desc*& pin_desc, Desc* descs, int N, bool device_src)
+int upload_interleaved_frames(hp_engine* e, hp_engine::PoseSlot& sl, Desc* descs, int N)
 {
     using Sample = std::remove_pointer_t<decltype(Desc::src)>;   // const uint8_t or const uint16_t
     auto row_bytes = [](const Desc& d) { return d.sw * pixel_bytes(d.format) * (int)sizeof(Sample); };
-    if (!device_src) {
-        std::vector<size_t> off(N + 1, 0);
-        for (int f = 0; f < N; ++f) off[f + 1] = off[f] + (((size_t)descs[f].sh * row_bytes(descs[f]) + 255) & ~(size_t)255);
-        int rc = slot_src_reserve(sl, off[N]);
-        if (rc) return rc;
-        for (int f = 0; f < N; ++f) {
-            Desc& d = descs[f];
-            const int row = row_bytes(d);
-            if ((rc = upload_plane(e, sl, (const uint8_t*)d.src, d.pitch, d.sh, row, off[f], off[N]))) return rc;
-            d.src = (const Sample*)(sl.d_src + off[f]);
-            d.pitch = row;
-        }
+    std::vector<size_t> off;
+    int rc = slot_src_layout(sl, N, [&](int f) { return (size_t)descs[f].sh * row_bytes(descs[f]); }, off);
+    for (int f = 0; f < N && !rc; ++f) {
+        Desc& d = descs[f];
+        const int row = row_bytes(d);
+        rc = upload_plane(e, sl, (const uint8_t*)d.src, d.pitch, d.sh, row, off[f], off[N]);
+        d.src = (const Sample*)(sl.d_src + off[f]);
+        d.pitch = row;
     }
-    return slot_launch_fused(e, sl, d_desc, pin_desc, descs, N);
+    return rc;
 }
-
-// the frames of a submitted batch, one kind set by the constructor: network-size frames, or frames of any size described by resize
-// descriptors (BGR, YUV 4:2:0, interleaved, and the 16-bit YUV 4:2:0 and interleaved ones) whose sources are rewritten to the slot's
-// copies of host frames
-struct BatchFrames {
-    const uint8_t* frames = nullptr;
-    FrameDesc* descs = nullptr;
-    YuvFrameDesc* ydescs = nullptr;
-    InterleavedFrameDesc* idescs = nullptr;
-    Yuv16FrameDesc* y16descs = nullptr;
-    Interleaved16FrameDesc* i16descs = nullptr;
-    BatchFrames(const uint8_t* p) : frames(p) {}
-    BatchFrames(FrameDesc* p) : descs(p) {}
-    BatchFrames(YuvFrameDesc* p) : ydescs(p) {}
-    BatchFrames(InterleavedFrameDesc* p) : idescs(p) {}
-    BatchFrames(Yuv16FrameDesc* p) : y16descs(p) {}
-    BatchFrames(Interleaved16FrameDesc* p) : i16descs(p) {}
-    bool empty() const { return !frames && !descs && !ydescs && !idescs && !y16descs && !i16descs; }
-};
-
-// a submitted batch into the slot's device buffer: network-size frames copied, frames of any size resized there
-int slot_upload_batch(hp_engine* e, hp_engine::PoseSlot& sl, const BatchFrames& b, int N, bool device_src)
+int upload_host_frames(hp_engine* e, hp_engine::PoseSlot& sl, InterleavedFrameDesc* descs, int N)
 {
-    if (b.i16descs) return slot_upload_interleaved(e, sl, sl.d_i16desc, sl.pin_i16desc, b.i16descs, N, device_src);
-    if (b.y16descs) return slot_upload_yuv(e, sl, sl.d_y16desc, sl.pin_y16desc, b.y16descs, N, device_src);
-    if (b.idescs) return slot_upload_interleaved(e, sl, sl.d_idesc, sl.pin_idesc, b.idescs, N, device_src);
-    if (b.ydescs) return slot_upload_yuv(e, sl, sl.d_ydesc, sl.pin_ydesc, b.ydescs, N, device_src);
-    return b.descs ? slot_upload_frames(e, sl, b.descs, N, device_src) : slot_upload(e, sl, b.frames, N, device_src);
+    return upload_interleaved_frames(e, sl, descs, N);
 }
+int upload_host_frames(hp_engine* e, hp_engine::PoseSlot& sl, Interleaved16FrameDesc* descs, int N)
+{
+    return upload_interleaved_frames(e, sl, descs, N);
+}
+
+bool is_rotated(const FrameDesc&) { return false; }
+template <class Desc> bool is_rotated(const Desc& d) { return d.rot != 0; }
+
+// The N frames of any size of a submitted batch, resized into the slot's device buffer by one launch on the engine stream, ahead of
+// the batch's network.  The descriptors are copied into the slot's pinned descriptor buffer; host frames are uploaded into the
+// slot's source buffer (upload_host_frames) and their descriptors pointed there, device frames are read in place.  The descriptors
+// then travel on the copy stream, ordered before the engine stream's next work.  The resize stays outside the captured graph, so the
+// graph never sees a frame geometry or a source address and new sizes never recapture it.
+template <class Desc>
+int slot_upload_resized(hp_engine* e, hp_engine::PoseSlot& sl, const void* batch, int N, bool device_src)
+{
+    if (!sl.d_desc) {
+        HP_CUDA_TRY(cudaMalloc(&sl.d_desc, e->max_batch * FRAME_DESC_BYTES));
+        HP_CUDA_TRY(cudaMallocHost(&sl.pin_desc, e->max_batch * FRAME_DESC_BYTES));
+    }
+    Desc* descs = (Desc*)sl.pin_desc;
+    memcpy(descs, batch, N * sizeof(Desc));
+    if (!device_src) {
+        const int rc = upload_host_frames(e, sl, descs, N);
+        if (rc) return rc;
+    }
+    HP_CUDA_TRY(cudaMemcpyAsync(sl.d_desc, descs, N * sizeof(Desc), cudaMemcpyHostToDevice, e->copy_stream));
+    HP_CUDA_TRY(cudaEventRecord(sl.h2d_done, e->copy_stream));
+    HP_CUDA_TRY(cudaStreamWaitEvent(e->stream, sl.h2d_done, 0));
+    return launch_resize(e, (const Desc*)sl.d_desc, sl.d_frames, N, std::any_of(descs, descs + N, [](const Desc& d) { return is_rotated(d); }));
+}
+
+// the frames of a submitted batch and the upload that puts them into the slot's device buffer: network-size frames copied
+// (slot_upload), or the resize descriptors of frames of any size, one type per batch, resized there (slot_upload_resized)
+struct BatchFrames {
+    const void* data;
+    int (*upload)(hp_engine* e, hp_engine::PoseSlot& sl, const void* data, int N, bool device_src);
+    BatchFrames(const uint8_t* frames) : data(frames), upload(slot_upload) {}
+    template <class Desc>
+    BatchFrames(const Desc* descs) : data(descs), upload(slot_upload_resized<Desc>) {}
+};
 
 // the parser's state a captured graph bakes in (hp_paf_state / hp_ppn_state), and the capacity of records per frame in it
 void parser_state(const hp_paf* parser, const hp_ppn* ppn, float kf[3], int ki[6], int* hcap)
@@ -3053,46 +3006,30 @@ static int pifpaf_enqueue(hp_engine* e, hp_engine::PoseSlot& sl)
     return HP_OK;
 }
 
-// frames: the N frames of the batch (BatchFrames)
-static int pose_submit_pifpaf(hp_engine* e, hp_pifpaf* dec, const BatchFrames& frames, int N, int* ticket, bool device_src)
-{
-    if (!e || !dec || frames.empty() || !ticket) { set_error("hp_pose_submit_pifpaf: null argument"); return HP_ERR_ARG; }
-    if (N <= 0 || N > e->max_batch) { set_error("Input batch size overflow: Yours@%d Max@%d", N, e->max_batch); return HP_ERR_BATCH; }
-    if (e->hdr.head_type != 1) { set_error("hp_pose_submit_pifpaf: the model pack has no OpenPifPaf heads (head_type %u)", e->hdr.head_type); return HP_ERR_UNSUPPORTED; }
-    HP_CUDA_TRY(cudaSetDevice(e->device));
-    const int idx = e->next_slot;
-    hp_engine::PoseSlot& sl = e->slots[idx];
-    if (sl.busy) { set_error("hp_pose_submit_pifpaf: two batches are already in flight -- collect ticket %d first", idx); return HP_ERR_ARG; }
-    int rc = pifpaf_slot_prepare(e, sl, dec, N);
-    if (rc) return rc;
-    e->reserve_sms = e->opt.pifpaf_reserve_sms;   // the decoder's growth kernel (one warp per frame) runs underneath the next batch's convolutions
-    rc = slot_upload_batch(e, sl, frames, N, device_src);
-    if (rc) return rc;
-    rc = pifpaf_enqueue(e, sl);
-    if (rc) return rc;
-    sl.busy = true;
-    e->next_slot = idx ^ 1;
-    *ticket = idx;
-    return HP_OK;
-}
+// the head a pipelined pose call parses with: its parser handle is an hp_paf, an hp_pifpaf or an hp_ppn
+enum class PoseHead { Paf, PifPaf, Ppn };
 
-// the PAF-parser calls (ppn_call false: `parser` is an hp_paf) and the Pose Proposal Network calls (true: an hp_ppn)
-static int pose_submit(hp_engine* e, void* parser, bool ppn_call, const BatchFrames& frames, int N, int* ticket, bool device_src)
+// One batch of a pipelined pose call, whatever its head and frames: the checks, the slot (refused while busy), the head's prepare, the
+// upload of the frames into the slot (the captured graph reads the slot's buffer), the head's enqueue, and the ticket.
+static int pose_submit(hp_engine* e, PoseHead head, void* parser, const BatchFrames& frames, int N, int* ticket, bool device_src)
 {
-    const char* fn = ppn_call ? "hp_pose_submit_ppn" : "hp_pose_submit";
-    if (!e || !parser || frames.empty() || !ticket) { set_error("%s: null argument", fn); return HP_ERR_ARG; }
+    const char* fn = head == PoseHead::PifPaf ? "hp_pose_submit_pifpaf" : head == PoseHead::Ppn ? "hp_pose_submit_ppn" : "hp_pose_submit";
+    if (!e || !parser || !frames.data || !ticket) { set_error("%s: null argument", fn); return HP_ERR_ARG; }
     if (N <= 0 || N > e->max_batch) { set_error("Input batch size overflow: Yours@%d Max@%d", N, e->max_batch); return HP_ERR_BATCH; }
-    hp_paf* paf = ppn_call ? nullptr : (hp_paf*)parser;
-    hp_ppn* ppn = ppn_call ? (hp_ppn*)parser : nullptr;
-    if (ppn) {
+    if (head == PoseHead::PifPaf && e->hdr.head_type != 1) {
+        set_error("hp_pose_submit_pifpaf: the model pack has no OpenPifPaf heads (head_type %u)", e->hdr.head_type);
+        return HP_ERR_UNSUPPORTED;
+    }
+    if (head == PoseHead::Ppn) {
         if (e->hdr.head_type != 2) {
             set_error("hp_pose_submit_ppn: the model pack has no Pose Proposal Network heads (head_type %u)", e->hdr.head_type);
             return HP_ERR_UNSUPPORTED;
         }
         int ki[6];
-        hp_ppn_state(ppn, nullptr, ki);
+        hp_ppn_state((hp_ppn*)parser, nullptr, ki);
         if (ki[5] != e->device) { set_error("hp_pose_submit_ppn: the parser is on device %d but the engine on device %d", ki[5], e->device); return HP_ERR_ARG; }
-    } else {
+    }
+    if (head == PoseHead::Paf) {
         if (e->hdr.head_type == 1) { set_error("hp_pose_submit: the model pack has OpenPifPaf heads (use hp_engine_infer_u8_host + hp_pifpaf_process_device)"); return HP_ERR_UNSUPPORTED; }
         if (e->hdr.head_type != 0) {
             set_error("hp_pose_submit: the model pack has Pose Proposal Network heads (use hp_pose_submit_ppn_* with a Pose Proposal Network parser)");
@@ -3103,42 +3040,36 @@ static int pose_submit(hp_engine* e, void* parser, bool ppn_call, const BatchFra
     const int idx = e->next_slot;
     hp_engine::PoseSlot& sl = e->slots[idx];
     if (sl.busy) { set_error("%s: two batches are already in flight -- collect ticket %d first", fn, idx); return HP_ERR_ARG; }
-    int rc = pose_slot_prepare(e, sl, paf, ppn, N);
+    int rc = head == PoseHead::PifPaf ? pifpaf_slot_prepare(e, sl, (hp_pifpaf*)parser, N)
+                                      : pose_slot_prepare(e, sl, head == PoseHead::Paf ? (hp_paf*)parser : nullptr,
+                                                          head == PoseHead::Ppn ? (hp_ppn*)parser : nullptr, N);
     if (rc) return rc;
-    rc = slot_upload_batch(e, sl, frames, N, device_src);   // (the captured graph reads the slot's buffer)
+    // the decoder's growth kernel (one warp per frame) runs underneath the next batch's convolutions
+    if (head == PoseHead::PifPaf) e->reserve_sms = e->opt.pifpaf_reserve_sms;
+    rc = frames.upload(e, sl, frames.data, N, device_src);
     if (rc) return rc;
-    rc = pose_launch(e, sl);
-    if (rc) return rc;
-    HP_CUDA_TRY(cudaEventRecord(sl.done, e->stream));
+    if (head == PoseHead::PifPaf) {
+        rc = pifpaf_enqueue(e, sl);
+        if (rc) return rc;
+    } else {
+        rc = pose_launch(e, sl);
+        if (rc) return rc;
+        HP_CUDA_TRY(cudaEventRecord(sl.done, e->stream));
+    }
     sl.busy = true;
     e->next_slot = idx ^ 1;
     *ticket = idx;
     return HP_OK;
 }
 
-int hp_pose_submit_u8_host(hp_engine* e, hp_paf* parser, const uint8_t* frames, int N, int* ticket)
-{
-    return pose_submit(e, parser, false, frames, N, ticket, false);
-}
+// cv::rotate's clockwise rotations: ROTATE_90_CLOCKWISE, ROTATE_180, ROTATE_90_COUNTERCLOCKWISE, and upright
+static bool valid_rotation(int r) { return r == 0 || r == 90 || r == 180 || r == 270; }
 
-// the same with the frames already resident in device memory (what a decoder / capture pipeline on the GPU hands over)
-int hp_pose_submit_u8_device(hp_engine* e, hp_paf* parser, const uint8_t* d_frames, int N, int* ticket)
-{
-    return pose_submit(e, parser, false, d_frames, N, ticket, true);
-}
+extern "C++" {   // overloads and templates, inside the C ABI block
+// frame_descs: the resize descriptors of a frame list, refused before any work is enqueued; one overload per frame record type
 
-int hp_pose_submit_pifpaf_u8_host(hp_engine* e, hp_pifpaf* decoder, const uint8_t* frames, int N, int* ticket)
-{
-    return pose_submit_pifpaf(e, decoder, frames, N, ticket, false);
-}
-
-int hp_pose_submit_pifpaf_u8_device(hp_engine* e, hp_pifpaf* decoder, const uint8_t* d_frames, int N, int* ticket)
-{
-    return pose_submit_pifpaf(e, decoder, d_frames, N, ticket, true);
-}
-
-// the resize descriptors of a frame list, refused before any work is enqueued
-static int frame_descs(const hp_engine* e, const hp_frame_u8* frames, int N, int keep_ratio, std::vector<FrameDesc>& descs)
+// BGR frames (hp_frame_u8), which have no rotated calls: rotation is always NULL
+static int frame_descs(const hp_engine* e, const hp_frame_u8* frames, const int32_t*, int N, int keep_ratio, std::vector<FrameDesc>& descs)
 {
     if (!e || !frames) { set_error("hp_pose_submit_frames: null argument"); return HP_ERR_ARG; }
     if (N <= 0 || N > e->max_batch) { set_error("Input batch size overflow: Yours@%d Max@%d", N, e->max_batch); return HP_ERR_BATCH; }
@@ -3154,63 +3085,6 @@ static int frame_descs(const hp_engine* e, const hp_frame_u8* frames, int N, int
     return HP_OK;
 }
 
-int hp_pose_submit_frames_u8_host(hp_engine* e, hp_paf* parser, const hp_frame_u8* frames, int N, int keep_ratio, int* ticket)
-{
-    std::vector<FrameDesc> d;
-    const int rc = frame_descs(e, frames, N, keep_ratio, d);
-    return rc ? rc : pose_submit(e, parser, false, d.data(), N, ticket, false);
-}
-
-int hp_pose_submit_frames_u8_device(hp_engine* e, hp_paf* parser, const hp_frame_u8* frames, int N, int keep_ratio, int* ticket)
-{
-    std::vector<FrameDesc> d;
-    const int rc = frame_descs(e, frames, N, keep_ratio, d);
-    return rc ? rc : pose_submit(e, parser, false, d.data(), N, ticket, true);
-}
-
-int hp_pose_submit_pifpaf_frames_u8_host(hp_engine* e, hp_pifpaf* decoder, const hp_frame_u8* frames, int N, int keep_ratio, int* ticket)
-{
-    std::vector<FrameDesc> d;
-    const int rc = frame_descs(e, frames, N, keep_ratio, d);
-    return rc ? rc : pose_submit_pifpaf(e, decoder, d.data(), N, ticket, false);
-}
-
-int hp_pose_submit_pifpaf_frames_u8_device(hp_engine* e, hp_pifpaf* decoder, const hp_frame_u8* frames, int N, int keep_ratio, int* ticket)
-{
-    std::vector<FrameDesc> d;
-    const int rc = frame_descs(e, frames, N, keep_ratio, d);
-    return rc ? rc : pose_submit_pifpaf(e, decoder, d.data(), N, ticket, true);
-}
-
-// ---- Pose Proposal Network packs: network, parse and record D2H in one captured graph on the engine stream, as for the PAF parser ----
-int hp_pose_submit_ppn_u8_host(hp_engine* e, hp_ppn* parser, const uint8_t* frames, int N, int* ticket)
-{
-    return pose_submit(e, parser, true, frames, N, ticket, false);
-}
-
-int hp_pose_submit_ppn_u8_device(hp_engine* e, hp_ppn* parser, const uint8_t* d_frames, int N, int* ticket)
-{
-    return pose_submit(e, parser, true, d_frames, N, ticket, true);
-}
-
-int hp_pose_submit_ppn_frames_u8_host(hp_engine* e, hp_ppn* parser, const hp_frame_u8* frames, int N, int keep_ratio, int* ticket)
-{
-    std::vector<FrameDesc> d;
-    const int rc = frame_descs(e, frames, N, keep_ratio, d);
-    return rc ? rc : pose_submit(e, parser, true, d.data(), N, ticket, false);
-}
-
-int hp_pose_submit_ppn_frames_u8_device(hp_engine* e, hp_ppn* parser, const hp_frame_u8* frames, int N, int keep_ratio, int* ticket)
-{
-    std::vector<FrameDesc> d;
-    const int rc = frame_descs(e, frames, N, keep_ratio, d);
-    return rc ? rc : pose_submit(e, parser, true, d.data(), N, ticket, true);
-}
-
-// cv::rotate's clockwise rotations: ROTATE_90_CLOCKWISE, ROTATE_180, ROTATE_90_COUNTERCLOCKWISE, and upright
-static bool valid_rotation(int r) { return r == 0 || r == 90 || r == 180 || r == 270; }
-
-extern "C++" {   // overloads and templates, inside the C ABI block
 // what the 16-bit records add to the 8-bit refusals: bits outside 9..16, and a pointer or a pitch that is not 2-byte aligned
 static const char* sample_refusal(int bits, std::initializer_list<const void*> ptrs, std::initializer_list<int> pitches)
 {
@@ -3220,8 +3094,8 @@ static const char* sample_refusal(int bits, std::initializer_list<const void*> p
     return nullptr;
 }
 
-// the resize descriptors of a YUV 4:2:0 frame list (hp_frame_yuv420 -> YuvFrameDesc, hp_frame_yuv420_16 -> Yuv16FrameDesc), refused
-// before any work is enqueued; the regime comes from the luma size after the frame's rotation (rotation NULL: every frame upright)
+// YUV 4:2:0 frames (hp_frame_yuv420 -> YuvFrameDesc, hp_frame_yuv420_16 -> Yuv16FrameDesc): the regime comes from the luma size after
+// the frame's rotation (rotation NULL: every frame upright)
 template <class Frame, class Desc>
 static int yuv_frame_descs(const hp_engine* e, const Frame* frames, const int32_t* rotation, int N, int keep_ratio, std::vector<Desc>& descs)
 {
@@ -3260,91 +3134,8 @@ static int yuv_frame_descs(const hp_engine* e, const Frame* frames, const int32_
     return HP_OK;
 }
 
-}   // extern "C++"
-
-int hp_pose_submit_frames_yuv420_rotated_host(hp_engine* e, hp_paf* parser, const hp_frame_yuv420* frames, const int32_t* rotation, int N,
-                                              int keep_ratio, int* ticket)
-{
-    std::vector<YuvFrameDesc> d;
-    const int rc = yuv_frame_descs(e, frames, rotation, N, keep_ratio, d);
-    return rc ? rc : pose_submit(e, parser, false, d.data(), N, ticket, false);
-}
-
-int hp_pose_submit_frames_yuv420_rotated_device(hp_engine* e, hp_paf* parser, const hp_frame_yuv420* frames, const int32_t* rotation, int N,
-                                                int keep_ratio, int* ticket)
-{
-    std::vector<YuvFrameDesc> d;
-    const int rc = yuv_frame_descs(e, frames, rotation, N, keep_ratio, d);
-    return rc ? rc : pose_submit(e, parser, false, d.data(), N, ticket, true);
-}
-
-int hp_pose_submit_pifpaf_frames_yuv420_rotated_host(hp_engine* e, hp_pifpaf* decoder, const hp_frame_yuv420* frames, const int32_t* rotation,
-                                                     int N, int keep_ratio, int* ticket)
-{
-    std::vector<YuvFrameDesc> d;
-    const int rc = yuv_frame_descs(e, frames, rotation, N, keep_ratio, d);
-    return rc ? rc : pose_submit_pifpaf(e, decoder, d.data(), N, ticket, false);
-}
-
-int hp_pose_submit_pifpaf_frames_yuv420_rotated_device(hp_engine* e, hp_pifpaf* decoder, const hp_frame_yuv420* frames, const int32_t* rotation,
-                                                       int N, int keep_ratio, int* ticket)
-{
-    std::vector<YuvFrameDesc> d;
-    const int rc = yuv_frame_descs(e, frames, rotation, N, keep_ratio, d);
-    return rc ? rc : pose_submit_pifpaf(e, decoder, d.data(), N, ticket, true);
-}
-
-int hp_pose_submit_ppn_frames_yuv420_rotated_host(hp_engine* e, hp_ppn* parser, const hp_frame_yuv420* frames, const int32_t* rotation, int N,
-                                                  int keep_ratio, int* ticket)
-{
-    std::vector<YuvFrameDesc> d;
-    const int rc = yuv_frame_descs(e, frames, rotation, N, keep_ratio, d);
-    return rc ? rc : pose_submit(e, parser, true, d.data(), N, ticket, false);
-}
-
-int hp_pose_submit_ppn_frames_yuv420_rotated_device(hp_engine* e, hp_ppn* parser, const hp_frame_yuv420* frames, const int32_t* rotation, int N,
-                                                    int keep_ratio, int* ticket)
-{
-    std::vector<YuvFrameDesc> d;
-    const int rc = yuv_frame_descs(e, frames, rotation, N, keep_ratio, d);
-    return rc ? rc : pose_submit(e, parser, true, d.data(), N, ticket, true);
-}
-
-// the upright calls: the rotated ones with every frame upright
-int hp_pose_submit_frames_yuv420_host(hp_engine* e, hp_paf* parser, const hp_frame_yuv420* frames, int N, int keep_ratio, int* ticket)
-{
-    return hp_pose_submit_frames_yuv420_rotated_host(e, parser, frames, nullptr, N, keep_ratio, ticket);
-}
-
-int hp_pose_submit_frames_yuv420_device(hp_engine* e, hp_paf* parser, const hp_frame_yuv420* frames, int N, int keep_ratio, int* ticket)
-{
-    return hp_pose_submit_frames_yuv420_rotated_device(e, parser, frames, nullptr, N, keep_ratio, ticket);
-}
-
-int hp_pose_submit_pifpaf_frames_yuv420_host(hp_engine* e, hp_pifpaf* decoder, const hp_frame_yuv420* frames, int N, int keep_ratio, int* ticket)
-{
-    return hp_pose_submit_pifpaf_frames_yuv420_rotated_host(e, decoder, frames, nullptr, N, keep_ratio, ticket);
-}
-
-int hp_pose_submit_pifpaf_frames_yuv420_device(hp_engine* e, hp_pifpaf* decoder, const hp_frame_yuv420* frames, int N, int keep_ratio, int* ticket)
-{
-    return hp_pose_submit_pifpaf_frames_yuv420_rotated_device(e, decoder, frames, nullptr, N, keep_ratio, ticket);
-}
-
-int hp_pose_submit_ppn_frames_yuv420_host(hp_engine* e, hp_ppn* parser, const hp_frame_yuv420* frames, int N, int keep_ratio, int* ticket)
-{
-    return hp_pose_submit_ppn_frames_yuv420_rotated_host(e, parser, frames, nullptr, N, keep_ratio, ticket);
-}
-
-int hp_pose_submit_ppn_frames_yuv420_device(hp_engine* e, hp_ppn* parser, const hp_frame_yuv420* frames, int N, int keep_ratio, int* ticket)
-{
-    return hp_pose_submit_ppn_frames_yuv420_rotated_device(e, parser, frames, nullptr, N, keep_ratio, ticket);
-}
-
-extern "C++" {   // overloads and templates, inside the C ABI block
-// the resize descriptors of an interleaved frame list (hp_frame_interleaved -> InterleavedFrameDesc, hp_frame_interleaved16 ->
-// Interleaved16FrameDesc), refused before any work is enqueued; the regime comes from the pixel size after the frame's rotation
-// (rotation NULL: every frame upright)
+// interleaved frames (hp_frame_interleaved -> InterleavedFrameDesc, hp_frame_interleaved16 -> Interleaved16FrameDesc): the regime comes
+// from the pixel size after the frame's rotation (rotation NULL: every frame upright)
 template <class Frame, class Desc>
 static int interleaved_frame_descs(const hp_engine* e, const Frame* frames, const int32_t* rotation, int N, int keep_ratio,
                                    std::vector<Desc>& descs)
@@ -3386,182 +3177,308 @@ static int interleaved_frame_descs(const hp_engine* e, const Frame* frames, cons
     return HP_OK;
 }
 
+static int frame_descs(const hp_engine* e, const hp_frame_yuv420* frames, const int32_t* rotation, int N, int keep_ratio,
+                       std::vector<YuvFrameDesc>& descs)
+{
+    return yuv_frame_descs(e, frames, rotation, N, keep_ratio, descs);
+}
+static int frame_descs(const hp_engine* e, const hp_frame_yuv420_16* frames, const int32_t* rotation, int N, int keep_ratio,
+                       std::vector<Yuv16FrameDesc>& descs)
+{
+    return yuv_frame_descs(e, frames, rotation, N, keep_ratio, descs);
+}
+static int frame_descs(const hp_engine* e, const hp_frame_interleaved* frames, const int32_t* rotation, int N, int keep_ratio,
+                       std::vector<InterleavedFrameDesc>& descs)
+{
+    return interleaved_frame_descs(e, frames, rotation, N, keep_ratio, descs);
+}
+static int frame_descs(const hp_engine* e, const hp_frame_interleaved16* frames, const int32_t* rotation, int N, int keep_ratio,
+                       std::vector<Interleaved16FrameDesc>& descs)
+{
+    return interleaved_frame_descs(e, frames, rotation, N, keep_ratio, descs);
+}
+
+// a frame call of any record type: the frame list validated and described (frame_descs), then submitted.  rotation: N clockwise
+// degrees, or NULL for every frame upright.
+template <class Desc, class Frame>
+static int pose_submit_frames(hp_engine* e, PoseHead head, void* parser, const Frame* frames, const int32_t* rotation, int N, int keep_ratio,
+                              int* ticket, bool device_src)
+{
+    std::vector<Desc> d;
+    const int rc = frame_descs(e, frames, rotation, N, keep_ratio, d);
+    return rc ? rc : pose_submit(e, head, parser, d.data(), N, ticket, device_src);
+}
+
 }   // extern "C++"
+
+// ---- the exported calls: network-size frames, then frames of any size by record type.  PAF parser and Pose Proposal Network packs run
+// network, parse and record D2H in one captured graph on the engine stream; OpenPifPaf packs decode on the decoder's stream. ----
+int hp_pose_submit_u8_host(hp_engine* e, hp_paf* parser, const uint8_t* frames, int N, int* ticket)
+{
+    return pose_submit(e, PoseHead::Paf, parser, frames, N, ticket, false);
+}
+
+// the same with the frames already resident in device memory (what a decoder / capture pipeline on the GPU hands over)
+int hp_pose_submit_u8_device(hp_engine* e, hp_paf* parser, const uint8_t* d_frames, int N, int* ticket)
+{
+    return pose_submit(e, PoseHead::Paf, parser, d_frames, N, ticket, true);
+}
+
+int hp_pose_submit_pifpaf_u8_host(hp_engine* e, hp_pifpaf* decoder, const uint8_t* frames, int N, int* ticket)
+{
+    return pose_submit(e, PoseHead::PifPaf, decoder, frames, N, ticket, false);
+}
+
+int hp_pose_submit_pifpaf_u8_device(hp_engine* e, hp_pifpaf* decoder, const uint8_t* d_frames, int N, int* ticket)
+{
+    return pose_submit(e, PoseHead::PifPaf, decoder, d_frames, N, ticket, true);
+}
+
+int hp_pose_submit_ppn_u8_host(hp_engine* e, hp_ppn* parser, const uint8_t* frames, int N, int* ticket)
+{
+    return pose_submit(e, PoseHead::Ppn, parser, frames, N, ticket, false);
+}
+
+int hp_pose_submit_ppn_u8_device(hp_engine* e, hp_ppn* parser, const uint8_t* d_frames, int N, int* ticket)
+{
+    return pose_submit(e, PoseHead::Ppn, parser, d_frames, N, ticket, true);
+}
+
+int hp_pose_submit_frames_u8_host(hp_engine* e, hp_paf* parser, const hp_frame_u8* frames, int N, int keep_ratio, int* ticket)
+{
+    return pose_submit_frames<FrameDesc>(e, PoseHead::Paf, parser, frames, nullptr, N, keep_ratio, ticket, false);
+}
+
+int hp_pose_submit_frames_u8_device(hp_engine* e, hp_paf* parser, const hp_frame_u8* frames, int N, int keep_ratio, int* ticket)
+{
+    return pose_submit_frames<FrameDesc>(e, PoseHead::Paf, parser, frames, nullptr, N, keep_ratio, ticket, true);
+}
+
+int hp_pose_submit_pifpaf_frames_u8_host(hp_engine* e, hp_pifpaf* decoder, const hp_frame_u8* frames, int N, int keep_ratio, int* ticket)
+{
+    return pose_submit_frames<FrameDesc>(e, PoseHead::PifPaf, decoder, frames, nullptr, N, keep_ratio, ticket, false);
+}
+
+int hp_pose_submit_pifpaf_frames_u8_device(hp_engine* e, hp_pifpaf* decoder, const hp_frame_u8* frames, int N, int keep_ratio, int* ticket)
+{
+    return pose_submit_frames<FrameDesc>(e, PoseHead::PifPaf, decoder, frames, nullptr, N, keep_ratio, ticket, true);
+}
+
+int hp_pose_submit_ppn_frames_u8_host(hp_engine* e, hp_ppn* parser, const hp_frame_u8* frames, int N, int keep_ratio, int* ticket)
+{
+    return pose_submit_frames<FrameDesc>(e, PoseHead::Ppn, parser, frames, nullptr, N, keep_ratio, ticket, false);
+}
+
+int hp_pose_submit_ppn_frames_u8_device(hp_engine* e, hp_ppn* parser, const hp_frame_u8* frames, int N, int keep_ratio, int* ticket)
+{
+    return pose_submit_frames<FrameDesc>(e, PoseHead::Ppn, parser, frames, nullptr, N, keep_ratio, ticket, true);
+}
+
+int hp_pose_submit_frames_yuv420_rotated_host(hp_engine* e, hp_paf* parser, const hp_frame_yuv420* frames, const int32_t* rotation, int N,
+                                              int keep_ratio, int* ticket)
+{
+    return pose_submit_frames<YuvFrameDesc>(e, PoseHead::Paf, parser, frames, rotation, N, keep_ratio, ticket, false);
+}
+
+int hp_pose_submit_frames_yuv420_rotated_device(hp_engine* e, hp_paf* parser, const hp_frame_yuv420* frames, const int32_t* rotation, int N,
+                                                int keep_ratio, int* ticket)
+{
+    return pose_submit_frames<YuvFrameDesc>(e, PoseHead::Paf, parser, frames, rotation, N, keep_ratio, ticket, true);
+}
+
+int hp_pose_submit_pifpaf_frames_yuv420_rotated_host(hp_engine* e, hp_pifpaf* decoder, const hp_frame_yuv420* frames, const int32_t* rotation,
+                                                     int N, int keep_ratio, int* ticket)
+{
+    return pose_submit_frames<YuvFrameDesc>(e, PoseHead::PifPaf, decoder, frames, rotation, N, keep_ratio, ticket, false);
+}
+
+int hp_pose_submit_pifpaf_frames_yuv420_rotated_device(hp_engine* e, hp_pifpaf* decoder, const hp_frame_yuv420* frames, const int32_t* rotation,
+                                                       int N, int keep_ratio, int* ticket)
+{
+    return pose_submit_frames<YuvFrameDesc>(e, PoseHead::PifPaf, decoder, frames, rotation, N, keep_ratio, ticket, true);
+}
+
+int hp_pose_submit_ppn_frames_yuv420_rotated_host(hp_engine* e, hp_ppn* parser, const hp_frame_yuv420* frames, const int32_t* rotation, int N,
+                                                  int keep_ratio, int* ticket)
+{
+    return pose_submit_frames<YuvFrameDesc>(e, PoseHead::Ppn, parser, frames, rotation, N, keep_ratio, ticket, false);
+}
+
+int hp_pose_submit_ppn_frames_yuv420_rotated_device(hp_engine* e, hp_ppn* parser, const hp_frame_yuv420* frames, const int32_t* rotation, int N,
+                                                    int keep_ratio, int* ticket)
+{
+    return pose_submit_frames<YuvFrameDesc>(e, PoseHead::Ppn, parser, frames, rotation, N, keep_ratio, ticket, true);
+}
+
+// the upright calls: the rotated ones with every frame upright
+int hp_pose_submit_frames_yuv420_host(hp_engine* e, hp_paf* parser, const hp_frame_yuv420* frames, int N, int keep_ratio, int* ticket)
+{
+    return pose_submit_frames<YuvFrameDesc>(e, PoseHead::Paf, parser, frames, nullptr, N, keep_ratio, ticket, false);
+}
+
+int hp_pose_submit_frames_yuv420_device(hp_engine* e, hp_paf* parser, const hp_frame_yuv420* frames, int N, int keep_ratio, int* ticket)
+{
+    return pose_submit_frames<YuvFrameDesc>(e, PoseHead::Paf, parser, frames, nullptr, N, keep_ratio, ticket, true);
+}
+
+int hp_pose_submit_pifpaf_frames_yuv420_host(hp_engine* e, hp_pifpaf* decoder, const hp_frame_yuv420* frames, int N, int keep_ratio, int* ticket)
+{
+    return pose_submit_frames<YuvFrameDesc>(e, PoseHead::PifPaf, decoder, frames, nullptr, N, keep_ratio, ticket, false);
+}
+
+int hp_pose_submit_pifpaf_frames_yuv420_device(hp_engine* e, hp_pifpaf* decoder, const hp_frame_yuv420* frames, int N, int keep_ratio, int* ticket)
+{
+    return pose_submit_frames<YuvFrameDesc>(e, PoseHead::PifPaf, decoder, frames, nullptr, N, keep_ratio, ticket, true);
+}
+
+int hp_pose_submit_ppn_frames_yuv420_host(hp_engine* e, hp_ppn* parser, const hp_frame_yuv420* frames, int N, int keep_ratio, int* ticket)
+{
+    return pose_submit_frames<YuvFrameDesc>(e, PoseHead::Ppn, parser, frames, nullptr, N, keep_ratio, ticket, false);
+}
+
+int hp_pose_submit_ppn_frames_yuv420_device(hp_engine* e, hp_ppn* parser, const hp_frame_yuv420* frames, int N, int keep_ratio, int* ticket)
+{
+    return pose_submit_frames<YuvFrameDesc>(e, PoseHead::Ppn, parser, frames, nullptr, N, keep_ratio, ticket, true);
+}
 
 int hp_pose_submit_frames_interleaved_rotated_host(hp_engine* e, hp_paf* parser, const hp_frame_interleaved* frames, const int32_t* rotation,
                                                    int N, int keep_ratio, int* ticket)
 {
-    std::vector<InterleavedFrameDesc> d;
-    const int rc = interleaved_frame_descs(e, frames, rotation, N, keep_ratio, d);
-    return rc ? rc : pose_submit(e, parser, false, d.data(), N, ticket, false);
+    return pose_submit_frames<InterleavedFrameDesc>(e, PoseHead::Paf, parser, frames, rotation, N, keep_ratio, ticket, false);
 }
 
 int hp_pose_submit_frames_interleaved_rotated_device(hp_engine* e, hp_paf* parser, const hp_frame_interleaved* frames, const int32_t* rotation,
                                                      int N, int keep_ratio, int* ticket)
 {
-    std::vector<InterleavedFrameDesc> d;
-    const int rc = interleaved_frame_descs(e, frames, rotation, N, keep_ratio, d);
-    return rc ? rc : pose_submit(e, parser, false, d.data(), N, ticket, true);
+    return pose_submit_frames<InterleavedFrameDesc>(e, PoseHead::Paf, parser, frames, rotation, N, keep_ratio, ticket, true);
 }
 
 int hp_pose_submit_pifpaf_frames_interleaved_rotated_host(hp_engine* e, hp_pifpaf* decoder, const hp_frame_interleaved* frames,
                                                           const int32_t* rotation, int N, int keep_ratio, int* ticket)
 {
-    std::vector<InterleavedFrameDesc> d;
-    const int rc = interleaved_frame_descs(e, frames, rotation, N, keep_ratio, d);
-    return rc ? rc : pose_submit_pifpaf(e, decoder, d.data(), N, ticket, false);
+    return pose_submit_frames<InterleavedFrameDesc>(e, PoseHead::PifPaf, decoder, frames, rotation, N, keep_ratio, ticket, false);
 }
 
 int hp_pose_submit_pifpaf_frames_interleaved_rotated_device(hp_engine* e, hp_pifpaf* decoder, const hp_frame_interleaved* frames,
                                                             const int32_t* rotation, int N, int keep_ratio, int* ticket)
 {
-    std::vector<InterleavedFrameDesc> d;
-    const int rc = interleaved_frame_descs(e, frames, rotation, N, keep_ratio, d);
-    return rc ? rc : pose_submit_pifpaf(e, decoder, d.data(), N, ticket, true);
+    return pose_submit_frames<InterleavedFrameDesc>(e, PoseHead::PifPaf, decoder, frames, rotation, N, keep_ratio, ticket, true);
 }
 
 int hp_pose_submit_ppn_frames_interleaved_rotated_host(hp_engine* e, hp_ppn* parser, const hp_frame_interleaved* frames, const int32_t* rotation,
                                                        int N, int keep_ratio, int* ticket)
 {
-    std::vector<InterleavedFrameDesc> d;
-    const int rc = interleaved_frame_descs(e, frames, rotation, N, keep_ratio, d);
-    return rc ? rc : pose_submit(e, parser, true, d.data(), N, ticket, false);
+    return pose_submit_frames<InterleavedFrameDesc>(e, PoseHead::Ppn, parser, frames, rotation, N, keep_ratio, ticket, false);
 }
 
 int hp_pose_submit_ppn_frames_interleaved_rotated_device(hp_engine* e, hp_ppn* parser, const hp_frame_interleaved* frames,
                                                          const int32_t* rotation, int N, int keep_ratio, int* ticket)
 {
-    std::vector<InterleavedFrameDesc> d;
-    const int rc = interleaved_frame_descs(e, frames, rotation, N, keep_ratio, d);
-    return rc ? rc : pose_submit(e, parser, true, d.data(), N, ticket, true);
+    return pose_submit_frames<InterleavedFrameDesc>(e, PoseHead::Ppn, parser, frames, rotation, N, keep_ratio, ticket, true);
 }
 
 // the upright calls: the rotated ones with every frame upright
 int hp_pose_submit_frames_interleaved_host(hp_engine* e, hp_paf* parser, const hp_frame_interleaved* frames, int N, int keep_ratio, int* ticket)
 {
-    return hp_pose_submit_frames_interleaved_rotated_host(e, parser, frames, nullptr, N, keep_ratio, ticket);
+    return pose_submit_frames<InterleavedFrameDesc>(e, PoseHead::Paf, parser, frames, nullptr, N, keep_ratio, ticket, false);
 }
 
 int hp_pose_submit_frames_interleaved_device(hp_engine* e, hp_paf* parser, const hp_frame_interleaved* frames, int N, int keep_ratio, int* ticket)
 {
-    return hp_pose_submit_frames_interleaved_rotated_device(e, parser, frames, nullptr, N, keep_ratio, ticket);
+    return pose_submit_frames<InterleavedFrameDesc>(e, PoseHead::Paf, parser, frames, nullptr, N, keep_ratio, ticket, true);
 }
 
 int hp_pose_submit_pifpaf_frames_interleaved_host(hp_engine* e, hp_pifpaf* decoder, const hp_frame_interleaved* frames, int N, int keep_ratio, int* ticket)
 {
-    return hp_pose_submit_pifpaf_frames_interleaved_rotated_host(e, decoder, frames, nullptr, N, keep_ratio, ticket);
+    return pose_submit_frames<InterleavedFrameDesc>(e, PoseHead::PifPaf, decoder, frames, nullptr, N, keep_ratio, ticket, false);
 }
 
 int hp_pose_submit_pifpaf_frames_interleaved_device(hp_engine* e, hp_pifpaf* decoder, const hp_frame_interleaved* frames, int N, int keep_ratio, int* ticket)
 {
-    return hp_pose_submit_pifpaf_frames_interleaved_rotated_device(e, decoder, frames, nullptr, N, keep_ratio, ticket);
+    return pose_submit_frames<InterleavedFrameDesc>(e, PoseHead::PifPaf, decoder, frames, nullptr, N, keep_ratio, ticket, true);
 }
 
 int hp_pose_submit_ppn_frames_interleaved_host(hp_engine* e, hp_ppn* parser, const hp_frame_interleaved* frames, int N, int keep_ratio, int* ticket)
 {
-    return hp_pose_submit_ppn_frames_interleaved_rotated_host(e, parser, frames, nullptr, N, keep_ratio, ticket);
+    return pose_submit_frames<InterleavedFrameDesc>(e, PoseHead::Ppn, parser, frames, nullptr, N, keep_ratio, ticket, false);
 }
 
 int hp_pose_submit_ppn_frames_interleaved_device(hp_engine* e, hp_ppn* parser, const hp_frame_interleaved* frames, int N, int keep_ratio, int* ticket)
 {
-    return hp_pose_submit_ppn_frames_interleaved_rotated_device(e, parser, frames, nullptr, N, keep_ratio, ticket);
+    return pose_submit_frames<InterleavedFrameDesc>(e, PoseHead::Ppn, parser, frames, nullptr, N, keep_ratio, ticket, true);
 }
 
 // 16-bit samples: the 8-bit calls' descriptors and resize, each sample reduced in the fetch
 int hp_pose_submit_frames_yuv420_16_host(hp_engine* e, hp_paf* parser, const hp_frame_yuv420_16* frames, const int32_t* rotation,
                                          int N, int keep_ratio, int* ticket)
 {
-    std::vector<Yuv16FrameDesc> d;
-    const int rc = yuv_frame_descs(e, frames, rotation, N, keep_ratio, d);
-    return rc ? rc : pose_submit(e, parser, false, d.data(), N, ticket, false);
+    return pose_submit_frames<Yuv16FrameDesc>(e, PoseHead::Paf, parser, frames, rotation, N, keep_ratio, ticket, false);
 }
 
 int hp_pose_submit_frames_yuv420_16_device(hp_engine* e, hp_paf* parser, const hp_frame_yuv420_16* frames, const int32_t* rotation,
                                            int N, int keep_ratio, int* ticket)
 {
-    std::vector<Yuv16FrameDesc> d;
-    const int rc = yuv_frame_descs(e, frames, rotation, N, keep_ratio, d);
-    return rc ? rc : pose_submit(e, parser, false, d.data(), N, ticket, true);
+    return pose_submit_frames<Yuv16FrameDesc>(e, PoseHead::Paf, parser, frames, rotation, N, keep_ratio, ticket, true);
 }
 
 int hp_pose_submit_pifpaf_frames_yuv420_16_host(hp_engine* e, hp_pifpaf* decoder, const hp_frame_yuv420_16* frames, const int32_t* rotation,
                                                 int N, int keep_ratio, int* ticket)
 {
-    std::vector<Yuv16FrameDesc> d;
-    const int rc = yuv_frame_descs(e, frames, rotation, N, keep_ratio, d);
-    return rc ? rc : pose_submit_pifpaf(e, decoder, d.data(), N, ticket, false);
+    return pose_submit_frames<Yuv16FrameDesc>(e, PoseHead::PifPaf, decoder, frames, rotation, N, keep_ratio, ticket, false);
 }
 
 int hp_pose_submit_pifpaf_frames_yuv420_16_device(hp_engine* e, hp_pifpaf* decoder, const hp_frame_yuv420_16* frames, const int32_t* rotation,
                                                   int N, int keep_ratio, int* ticket)
 {
-    std::vector<Yuv16FrameDesc> d;
-    const int rc = yuv_frame_descs(e, frames, rotation, N, keep_ratio, d);
-    return rc ? rc : pose_submit_pifpaf(e, decoder, d.data(), N, ticket, true);
+    return pose_submit_frames<Yuv16FrameDesc>(e, PoseHead::PifPaf, decoder, frames, rotation, N, keep_ratio, ticket, true);
 }
 
 int hp_pose_submit_ppn_frames_yuv420_16_host(hp_engine* e, hp_ppn* parser, const hp_frame_yuv420_16* frames, const int32_t* rotation,
                                              int N, int keep_ratio, int* ticket)
 {
-    std::vector<Yuv16FrameDesc> d;
-    const int rc = yuv_frame_descs(e, frames, rotation, N, keep_ratio, d);
-    return rc ? rc : pose_submit(e, parser, true, d.data(), N, ticket, false);
+    return pose_submit_frames<Yuv16FrameDesc>(e, PoseHead::Ppn, parser, frames, rotation, N, keep_ratio, ticket, false);
 }
 
 int hp_pose_submit_ppn_frames_yuv420_16_device(hp_engine* e, hp_ppn* parser, const hp_frame_yuv420_16* frames, const int32_t* rotation,
                                                int N, int keep_ratio, int* ticket)
 {
-    std::vector<Yuv16FrameDesc> d;
-    const int rc = yuv_frame_descs(e, frames, rotation, N, keep_ratio, d);
-    return rc ? rc : pose_submit(e, parser, true, d.data(), N, ticket, true);
+    return pose_submit_frames<Yuv16FrameDesc>(e, PoseHead::Ppn, parser, frames, rotation, N, keep_ratio, ticket, true);
 }
 
 int hp_pose_submit_frames_interleaved16_host(hp_engine* e, hp_paf* parser, const hp_frame_interleaved16* frames, const int32_t* rotation,
                                              int N, int keep_ratio, int* ticket)
 {
-    std::vector<Interleaved16FrameDesc> d;
-    const int rc = interleaved_frame_descs(e, frames, rotation, N, keep_ratio, d);
-    return rc ? rc : pose_submit(e, parser, false, d.data(), N, ticket, false);
+    return pose_submit_frames<Interleaved16FrameDesc>(e, PoseHead::Paf, parser, frames, rotation, N, keep_ratio, ticket, false);
 }
 
 int hp_pose_submit_frames_interleaved16_device(hp_engine* e, hp_paf* parser, const hp_frame_interleaved16* frames, const int32_t* rotation,
                                                int N, int keep_ratio, int* ticket)
 {
-    std::vector<Interleaved16FrameDesc> d;
-    const int rc = interleaved_frame_descs(e, frames, rotation, N, keep_ratio, d);
-    return rc ? rc : pose_submit(e, parser, false, d.data(), N, ticket, true);
+    return pose_submit_frames<Interleaved16FrameDesc>(e, PoseHead::Paf, parser, frames, rotation, N, keep_ratio, ticket, true);
 }
 
 int hp_pose_submit_pifpaf_frames_interleaved16_host(hp_engine* e, hp_pifpaf* decoder, const hp_frame_interleaved16* frames, const int32_t* rotation,
                                                     int N, int keep_ratio, int* ticket)
 {
-    std::vector<Interleaved16FrameDesc> d;
-    const int rc = interleaved_frame_descs(e, frames, rotation, N, keep_ratio, d);
-    return rc ? rc : pose_submit_pifpaf(e, decoder, d.data(), N, ticket, false);
+    return pose_submit_frames<Interleaved16FrameDesc>(e, PoseHead::PifPaf, decoder, frames, rotation, N, keep_ratio, ticket, false);
 }
 
 int hp_pose_submit_pifpaf_frames_interleaved16_device(hp_engine* e, hp_pifpaf* decoder, const hp_frame_interleaved16* frames, const int32_t* rotation,
                                                       int N, int keep_ratio, int* ticket)
 {
-    std::vector<Interleaved16FrameDesc> d;
-    const int rc = interleaved_frame_descs(e, frames, rotation, N, keep_ratio, d);
-    return rc ? rc : pose_submit_pifpaf(e, decoder, d.data(), N, ticket, true);
+    return pose_submit_frames<Interleaved16FrameDesc>(e, PoseHead::PifPaf, decoder, frames, rotation, N, keep_ratio, ticket, true);
 }
 
 int hp_pose_submit_ppn_frames_interleaved16_host(hp_engine* e, hp_ppn* parser, const hp_frame_interleaved16* frames, const int32_t* rotation,
                                                  int N, int keep_ratio, int* ticket)
 {
-    std::vector<Interleaved16FrameDesc> d;
-    const int rc = interleaved_frame_descs(e, frames, rotation, N, keep_ratio, d);
-    return rc ? rc : pose_submit(e, parser, true, d.data(), N, ticket, false);
+    return pose_submit_frames<Interleaved16FrameDesc>(e, PoseHead::Ppn, parser, frames, rotation, N, keep_ratio, ticket, false);
 }
 
 int hp_pose_submit_ppn_frames_interleaved16_device(hp_engine* e, hp_ppn* parser, const hp_frame_interleaved16* frames, const int32_t* rotation,
                                                    int N, int keep_ratio, int* ticket)
 {
-    std::vector<Interleaved16FrameDesc> d;
-    const int rc = interleaved_frame_descs(e, frames, rotation, N, keep_ratio, d);
-    return rc ? rc : pose_submit(e, parser, true, d.data(), N, ticket, true);
+    return pose_submit_frames<Interleaved16FrameDesc>(e, PoseHead::Ppn, parser, frames, rotation, N, keep_ratio, ticket, true);
 }
 
 // test hook: the first N resized network-size frames of ticket `ticket` (in flight or collected)
